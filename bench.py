@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """bench.py -- tokens/s of single-batch decode through libcalm_b200.so (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload NAME] [--engine E]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload NAME] [--dump-outputs DIR]
 
 One "step" = one token of single-sequence decode (one pass of the per-token forward() path).  The
 N = 1 workload is BASELINE.json configs[1]: Llama-3-8B shape, random-init fp8 (e5m2) weights, 4096-token
 context, the timed tokens sitting at the END of the context (the reference's own "last tokens" protocol,
 README.md:86) so attention reads the whole KV cache.  Every token streams all 7.5 GB of weights, far more
-than the 126 MB L2, so no L2 flush is needed between steps.
+than the 50 MB L2 of an H100, so no L2 flush is needed between steps.
 
 Printed JSON (one line, rank 0):
   value      tokens/s with everything resident in HBM: device-side greedy loop (forward + argmax feeding
@@ -19,6 +19,8 @@ Printed JSON (one line, rank 0):
   cpu_baseline  the reference's CPU implementation (oracle/_ref, or the oracle port) on this box's cores,
              bounded sample of the same workload.  Reported, not a target.
 With --impl reference the same metric is measured on the reference's CPU path only (no product code).
+--dump-outputs DIR writes what the timed device loop returned in its last step (rank 0): greedy_tokens.npy (the K tokens),
+last_logits.npy (float32 logits of the last timed token); the inputs are seeded, so two builds can be compared file by file.
 For N > 1 the N GPUs serve ONE token stream, tensor-parallel (--parallel tp, the default): every rank holds 1/N of the
 heads and FFN rows, the two partial projections per layer are summed inside k_matres over NVLink peer memory, the
 classifier is split by vocabulary; "scaling": "strong".  --parallel replicas runs N independent copies instead
@@ -49,11 +51,11 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi samples of SM clock / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi samples of SM clock / throttle reasons DURING the timed region."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -230,7 +232,7 @@ def workload_config(spec, pos0, args):
     return {"workload": f"{spec.name}: {spec.n_layers} layers, dim {spec.dim}, hidden {spec.hidden_dim}, heads {spec.n_heads}/{spec.n_kv_heads}x{spec.head_dim}, "
                         f"vocab {spec.vocab_size}, {spec.dtype} weights, {'fp16' if getattr(args, 'kvbits', 16) == 16 else 'e5m2'} KV cache, context 4096, batch 1",
             "positions": f"{pos0}..{pos0 + args.steps + args.warmup - 1} (KV cache pre-filled to pos0)",
-            "l2": f"inputs ({per_gpu / 1e9:.2f} GB of weights per step and GPU) exceed the 126 MB L2; no flush",
+            "l2": f"inputs ({per_gpu / 1e9:.2f} GB of weights per step and GPU) exceed the 50 MB L2; no flush",
             "parallelism": "single GPU" if args.gpus <= 1 else (f"tp{args.gpus}" if args.parallel == "tp" else "replicas")}
 
 
@@ -253,6 +255,7 @@ def main():
     ap.add_argument("--kvbits", type=int, default=16, choices=[16, 8], help="KV cache element: fp16 (what the reference uses up to 4096 positions) or e5m2 (its choice beyond, run.c:537-539)")
     ap.add_argument("--layers", type=int, default=None, help="(debug) override the layer count")
     ap.add_argument("--pos0", type=int, default=None, help="(debug) first timed position instead of the end of the context")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -326,6 +329,10 @@ def main():
     launches = int(L.calm_b200_launch_count() - l0)
     ms = max_over_ranks(ms)
     value = K / (ms / 1e3) if is_tp else agg.whole_job_rate(K, ms)  # TP: the N GPUs serve ONE token stream
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "greedy_tokens.npy"), toks.astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "last_logits.npy"), dm.device_logits())
 
     # ---- leg 2: end to end through forward_cuda with host buffers
     tok = 23
@@ -359,7 +366,7 @@ def main():
         "frac_of_peak_whole_token": per_gpu / 1e9 / (ms / K / 1e3) / peak, "tp_mode": {0: None, 1: "ncclAllReduce between kernels", 2: "all-reduce inside k_matres over peer memory"}[L.calm_b200_tp_mode()],
     }
     if world == 1 and not spec.n_experts:
-        # ---- the prompt pass (configs[2]: "2048-token prefill"): forward_prefill_cuda, tcgen05 GEMMs; timed with CUDA events on the library's stream
+        # ---- the prompt pass (configs[2]: "2048-token prefill"): forward_prefill_cuda, wgmma GEMMs; timed with CUDA events on the library's stream
         try:
             n_pf = min(2048, seq_len)
             ptoks = np.array(mg.teacher_tokens(spec.vocab_size, n_pf), np.int32)
@@ -374,9 +381,9 @@ def main():
             try:
                 tpeak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"])
             except Exception:
-                tpeak = 1400.0
+                tpeak = 989.0  # H100 SXM data sheet, dense BF16 (not measured)
             prefill = {"tokens": n_pf, "ms": pf_ms, "tok_s": n_pf / (pf_ms / 1e3), "tflops": tf, "frac_of_bf16_sustained": tf / tpeak,
-                       "path": "tcgen05 GEMMs (f16 hi + lo activations: two MMAs per k-step) + block-causal attention" if served else "fed token by token (shape not served by the batched pass)",
+                       "path": "wgmma GEMMs (f16 hi + lo activations: two MMAs per k-step) + block-causal attention" if served else "fed token by token (shape not served by the batched pass)",
                        "vs_serial_prompt": (n_pf / (pf_ms / 1e3)) / value}
         except Exception as e:
             prefill = {"unavailable": str(e)}
@@ -395,7 +402,7 @@ def main():
             if r.returncode == 0 and line:
                 rc = json.loads(line[-1])
                 out["ref_cuda"] = {"e2e_tok_s": rc["tok_s"], "ms_per_step": rc["ms_per_step"], "ours_e2e_over_ref": e2e / rc["tok_s"],
-                                   "what": "unmodified reference src/infer.cu (sm_100a build, oracle/_ref/libcalm_ref_cuda.so): forward_cuda per token, host argmax, same model and positions as e2e"}
+                                   "what": "unmodified reference src/infer.cu (sm_90a build, oracle/_ref/libcalm_ref_cuda.so): forward_cuda per token, host argmax, same model and positions as e2e"}
             else:
                 out["ref_cuda"] = {"unavailable": (r.stderr or r.stdout)[-300:]}
             tensors = None
@@ -436,8 +443,7 @@ def dm_roofline(dm, L, spec, pos, peak, peak_src, ms_per_tok, bytes_per_tok):
              for k, v in stats.items() if v[2] > 0}
     name, (ms, by, nl) = max(((k, v) for k, v in stats.items() if v[1] > 0), key=lambda kv: kv[1][0])
     achieved = by / 1e9 / (ms / 1e3) if ms > 0 else None
-    # dram__bytes_read.sum + dram__bytes_write.sum per launch: not measurable in-run; the figure of the committed ncu capture is quoted with its source
-    traffic, traffic_src = (117.53e6 + 3.41e6, "profiles/r02_ncu_full_one_layer.csv (k_ffn_up_ring<8,4,2>, Llama-3-8B fp8: dram__bytes_read.sum + dram__bytes_write.sum of one launch)") if (name == "matmul_ffn_up" and spec.name == "llama3-8b-fp8") else (None, None)
+    traffic, traffic_src = None, "not measured (DRAM byte counters are not readable in-run)"
     return {"bound": "hbm", "kernel": name, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak if achieved else None,
             "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "bytes_per_launch": by / max(nl, 1), "us_per_launch": ms / max(nl, 1) * 1e3,
             "timing": "in-kernel %globaltimer stamps, production graph", "token_span_us_profiled": span_ms * 1e3, "stages": table}

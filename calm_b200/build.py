@@ -1,4 +1,4 @@
-"""Build libcalm_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so ships to the GPU box)."""
+"""Build libcalm_b200.so in-tree with nvcc for sm_90a (no JIT cache: the library is built once, next to the sources)."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ LIB = os.path.join(HERE, "libcalm_b200.so")
 SOURCES = ["engine.cu"]
 HEADERS = ["common.cuh", "stages.cuh", os.path.join("..", "..", "include", "calm_b200.h"), os.path.join("..", "..", "include", "calm_model.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-ccbin", "/usr/bin/g++",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-ccbin", "/usr/bin/g++",
          "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared"]
 
 

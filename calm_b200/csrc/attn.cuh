@@ -51,13 +51,13 @@ __host__ __device__ inline size_t attn2_smem_bytes(int hg, int head_dim, int nbm
 	return kv + ((size_t)hg * head_dim + scratch + (size_t)hg * (head_dim + 2)) * sizeof(float);
 }
 
-// How the slices of a unit are folded (measured on the in-kernel timeline, profiles/README.md round 2: with global partials,
-// a grid-scope fence, an atomic counter and a last-CTA pass the fold cost the last CTA 5.5 us of a 15 us kernel):
+// How the slices of a unit are folded (with global partials, a grid-scope fence, an atomic counter and a last-CTA pass the
+// fold is a serial tail on the last CTA):
 //   CLUSTER = false (default): every CTA publishes its record as 8-byte {value, epoch} cells -- no fence, no atomic: a reader
 //     that sees the epoch sees the value -- and then normalises 1/nsplit of the unit's outputs itself, polling the cells
 //     of its peers (all CTAs of the grid are resident, so every cell arrives; a watchdog traps instead of hanging).
 //   CLUSTER = true: the nsplit CTAs of a unit are one thread-block cluster and read each other's records through
-//     distributed shared memory (measured slower: a 16-CTA cluster waits for 16 free SMs of one GPC; kept selectable).
+//     distributed shared memory (a 16-CTA cluster has to wait for 16 free SMs of one GPC; kept selectable, off by default).
 __device__ __forceinline__ float attn_cell_wait(const unsigned long long* cell, unsigned epoch, int* err) {
 	unsigned long long v;
 	unsigned spins = 0;
@@ -180,7 +180,7 @@ __global__ void __launch_bounds__(ATTN_THREADS) k_attn2(const AttnArgs a) {
 
 	// Steps are taken SC at a time: first ALL scores of the chunk (independent dot products and transposing reductions: no
 	// serial softmax state between them), then one max / exp / sum for the chunk, then the value pass.  With 8 warps per SM
-	// the per-step online softmax was a latency chain (5 us for 4 steps on the in-kernel timeline); this form rescales the
+	// the per-step online softmax is a latency chain (max / exp / rescale per step); this form rescales the
 	// accumulators once per chunk.
 	constexpr int SC = 4, STEP = NW * G * P;
 	const int gbase = grp * LPP;

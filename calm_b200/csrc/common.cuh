@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libcalm_b200 (sm_100a only).
+// common.cuh -- shared device/host helpers for libcalm_b200 (sm_90a only).
 #pragma once
 
 #include <cuda_fp16.h>
@@ -117,7 +117,7 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
 // (weights are immutable; the KV prefix of a layer only gains the slot k_qkv writes).  One lane per warp turns
 // its share into cp.async.bulk.prefetch.L2 requests, so HBM keeps streaming while this kernel is in a phase
 // that leaves it idle (activation staging, reductions, attention arithmetic, tails), and the consumer finds its
-// first bytes in the 126 MB L2 instead of paying a DRAM round trip behind a kernel boundary.
+// first bytes in the 50 MB L2 instead of paying a DRAM round trip behind a kernel boundary.
 #define PF_RANGES 3
 #define PF_CHUNK 8192
 struct Prefetch {

@@ -1,6 +1,6 @@
 // engine.cu -- host side of libcalm_b200.so: the reference's CUDA backend boundary
 // (upload_cuda / prepare_cuda / forward_cuda / perf_cuda, reference src/run.c:22-25 and
-// src/infer.cu:69-131, 651-801) implemented over the sm_100a kernels in stages.cuh.
+// src/infer.cu:69-131, 651-801) implemented over the sm_90a kernels in stages.cuh.
 //
 // The per-token kernel sequence is captured once into CUDA graphs and replayed; per-token scalars
 // live in a device-resident TokenParams record that the host (forward_cuda) or the device
@@ -59,7 +59,7 @@ struct Engine {
 	// attention launch shape
 	int attn_hg = 1, attn_qgroups = 1, attn_nsplit = 1, attn_lpp = 1;
 	// TMA-ring matvec kernels (ring.cuh): slots per warp / CTAs per SM for FFN-up and for wo / w2; u = 512-byte units per row and chunk (0: not used)
-	int ring_up_ns = 2, ring_up_cps = 2, ring_res_ns = 2, ring_res_warps = 16; // measured: 16 consuming warps per SM are needed (profiles/r02_sweep_ring_*.jsonl)
+	int ring_up_ns = 2, ring_up_cps = 2, ring_res_ns = 2, ring_res_warps = 16; // best of the H100 sweep in profiles/README.md
 	int ring_up_u = 0, ring_wo_u = 0, ring_down_u = 0, ring_wo_s = 1, ring_down_s = 1;
 	int grid_up_ring = 0, grid_wo_ring = 0, grid_down_ring = 0;
 	size_t smem_up_ring = 0, smem_wo_ring = 0, smem_down_ring = 0;
@@ -76,9 +76,8 @@ struct Engine {
 	int attn_nsplit_cap = 1 << 30;
 
 	// L2 prefetch schedule (common.cuh Prefetch): what each stage requests for the stages after it.  Bytes, or flags.
-	// Measured (profiles/r02_sweep_l2_prefetch_schedule.jsonl): no setting beats "off" -- the stage kernels are not waiting for
-	// DRAM behind their boundaries, and requests for later stages only compete with the running one -- so the default is off;
-	// CALM_B200_PF keeps the experiment reproducible.
+	// Off by default: on an H100 it did not beat "off" (profiles/README.md) -- the stage kernels are not waiting for DRAM behind
+	// their boundaries, and requests for later stages only compete with the running one; CALM_B200_PF keeps the experiment.
 	bool pf_kv = false;           // k_qkv / w2 request the KV prefix the next attention kernel reads
 	bool pf_attn_wo = false;      // k_attn requests wo
 	size_t pf_attn_up = 0;        // ... and this much of w1 + w3
@@ -756,18 +755,18 @@ void make_plan() {
 		for (int grid : {g.grid_wo, g.grid_down})
 			if (cdiv(c.dim / 2, grid * 8) > TP_MAX_ITERS) CALM_FATAL("tensor parallelism: grid %d outside the exchange tables for dim %d", grid, c.dim);
 	}
-	// (measured: for the long FFN-up stage a full 4-CTA/SM grid with uneven rounds beats a balanced 3-CTA/SM one)
+	// (the long FFN-up stage gets a full grid with uneven rounds rather than balanced_grid's even ones)
 	g.grid_up = imin(max_ctas(k_ffn_up<DBITS>, 256, g.smem_dim), cdiv(g.nact * c.hidden_dim, 8));
 	// TMA-ring kernels for the dense single-GPU stages whose rows are whole 1 KB / 2 KB chunks (ring.cuh)
 	g.ring_up_u = g.ring_wo_u = g.ring_down_u = 0;
-	{ // weights are read once per token: L2::evict_first on the ring's bulk copies measured 2 % faster than the default policy
+	{ // weights are read once per token: L2::evict_first on the ring's bulk copies
 		const int hint = getenv("CALM_B200_RING_HINT") ? atoi(getenv("CALM_B200_RING_HINT")) : 1;
 		CUDA_CHECK(cudaMemcpyToSymbol(d_ring_l2_hint, &hint, sizeof(int)));
 	}
 	if (const char* e = getenv("CALM_B200_RING")) sscanf(e, "%d,%d,%d,%d", &g.ring_up_ns, &g.ring_up_cps, &g.ring_res_ns, &g.ring_res_warps); // 0 slots: stage not ring-fed
 	const bool ring_ok = c.n_experts == 0; // MoE: the expert rows are known only after the router
 	const bool ring_up_on = ring_ok && g.ring_up_ns >= 2 && g.ring_up_ns <= RING_MAX_NS; // (row shards of w1 / w3 under tensor parallelism are fine)
-	const bool ring_res_on = ring_ok && (g.tp_world == 1 || g.tp_fused) /* the ring kernels carry the in-kernel exchange too */ && g.ring_res_ns >= 2 && g.ring_res_ns <= RING_MAX_NS && (g.ring_res_warps == 8 || g.ring_res_warps == 16); // (gf4 too: 2.384 vs 2.467 ms per Mistral-7B token, profiles/r02_sweep_gf4_rows_per_slot.jsonl)
+	const bool ring_res_on = ring_ok && (g.tp_world == 1 || g.tp_fused) /* the ring kernels carry the in-kernel exchange too */ && g.ring_res_ns >= 2 && g.ring_res_ns <= RING_MAX_NS && (g.ring_res_warps == 8 || g.ring_res_warps == 16); // (gf4 too)
 	auto chunk_units = [](size_t rowbytes) { return rowbytes % 2048 == 0 ? 4 : (rowbytes % 1024 == 0 ? 2 : 0); };
 	if (ring_up_on) {
 		const int u = chunk_units((size_t)c.dim * DBITS / 8);
@@ -912,7 +911,7 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 
 	cudaDeviceProp prop;
 	CUDA_CHECK(cudaGetDeviceProperties(&prop, g.device));
-	if (prop.major != 10) CALM_FATAL("device %s is sm_%d%d; this library contains sm_100a code only and has no fallback", prop.name, prop.major, prop.minor);
+	if (prop.major != 9 || prop.minor != 0) CALM_FATAL("device %s is sm_%d%d; this library contains sm_90a code only and has no fallback", prop.name, prop.major, prop.minor);
 	g.sms = prop.multiProcessorCount;
 	if (!getenv("CALM_B200_QUIET"))
 		printf("# CUDA: %s, compute %d.%d, %d SMs, %.1f GiB, peak bandwidth %.0f GB/s (ECC %d)\n", prop.name, prop.major, prop.minor, prop.multiProcessorCount,
@@ -1012,8 +1011,8 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 	int want = (split_mul > 1 ? split_mul : 1) * g.sms / units; // about one 256-thread CTA per SM
 	int maxsplit = cdiv(c.seq_len, 64);                 // at least 64 positions per slice at full context
 	g.attn_nsplit = want < 1 ? 1 : (want > maxsplit ? maxsplit : want);
-	// (measured 9 us per launch SLOWER than the global-partial fold: a 16-CTA cluster needs 16 SMs of one GPC at once, which the
-	// still-resident q/k/v CTAs delay; kept selectable for the record -- profiles/r02_sweep_ring_and_attention_variants.jsonl)
+	// (the cluster fold is off by default: a 16-CTA cluster needs 16 SMs of one GPC at once, which the still-resident q/k/v CTAs
+	// delay; kept selectable)
 	if (g.attn_nsplit > ATTN2_MAXB + 4) g.attn_nsplit = ATTN2_MAXB + 4; // k_attn2 keeps one (m, l) pair per slice in static shared memory
 	const bool want_cluster = getenv("CALM_B200_ATTN_CLUSTER") && atoi(getenv("CALM_B200_ATTN_CLUSTER")) != 0;
 	if (want_cluster && attn2_shape_ok(g.attn_hg, g.attn_lpp, c.head_dim) && !(getenv("CALM_B200_ATTN2") && atoi(getenv("CALM_B200_ATTN2")) == 0)) {

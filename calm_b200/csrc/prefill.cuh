@@ -1,17 +1,18 @@
 // prefill.cuh -- batched prompt pass (SURVEY.md s.8f row 1; reference behaviour replaced: run.c:206-209 feeds the prompt one
 // token at a time through forward(), README.md:80).  T prompt tokens go through every layer together, so each weight
 // matrix is read once per 128-token tile instead of once per token and the projections become real GEMMs on the
-// 5th-generation tensor cores:
+// Hopper tensor cores:
 //
-//   k_pf_gemm   D[128 weight rows][128 tokens] (+)= W_tile . X_tile^T with tcgen05.mma (kind::f16, cta_group::1), fp32
-//               accumulators in TMEM.  A = the weight tile, dequantised ON THE FLY by four warps from the model's own
-//               format (fp16 / e5m2 / gf4: all exact in f16) into the 128-byte-swizzled K-major shared-memory layout
-//               the MMA reads; B = the activations as TWO f16 matrices hi + lo (x = hi + lo to 22 bits, so the result
+//   k_pf_gemm   D[128 tokens][128 weight rows] (+)= X_tile . W_tile^T with wgmma.mma_async (m64n128k16, f16 in, fp32
+//               accumulators in registers).  B = the weight tile, dequantised ON THE FLY by one warpgroup from the model's
+//               own format (fp16 / e5m2 / gf4: all exact in f16) into the 128-byte-swizzled K-major shared-memory layout
+//               the MMA reads; A = the activations as TWO f16 matrices hi + lo (x = hi + lo to 22 bits, so the result
 //               carries fp32-grade inputs: two MMAs per k-step into the same accumulator), brought in by 2-D TMA
-//               (cp.async.bulk.tensor, SWIZZLE_128B).  One warp issues TMA, one thread issues MMAs, completion flows
-//               through mbarriers (tcgen05.commit), the epilogue reads TMEM with tcgen05.ld and applies what the
-//               decode kernels apply: bias / clip / RoPE / KV-cache append (QKV), residual add (wo, w2),
-//               act(w1 x) * (w3 x) with both accumulators side by side in TMEM (FFN up).
+//               (cp.async.bulk.tensor, SWIZZLE_128B).  Two consumer warpgroups own 64 tokens each; stages are handed
+//               over through mbarriers, and the epilogue works on the accumulator registers directly: bias / clip /
+//               RoPE / KV-cache append (QKV), residual add (wo, w2), act(w1 x) * (w3 x) with both accumulators held by
+//               the same thread (FFN up).  A thread holds adjacent weight rows (features 2c, 2c + 1) of a token, so a
+//               RoPE pair never leaves the thread and every store is a contiguous pair.
 //   k_pf_attn   causal attention of the block against the cache (fp32 math on the cached fp16 / e5m2 entries, online
 //               softmax; reference infer.c:238-267), one warp per query token, K/V tiles staged in shared memory.
 //   k_pf_norm   RMSNorm / LayerNorm per token (reference infer.c:183-207) -> hi / lo f16 rows.
@@ -24,52 +25,48 @@
 
 #include "stages.cuh"
 
-#define PF_BM 128 // weight rows per tile  (TMEM lanes)
-#define PF_BN 128 // tokens per tile       (TMEM columns per accumulator)
+#define PF_BM 128 // weight rows per tile  (the N of the MMA)
+#define PF_BN 128 // tokens per tile       (two consumer warpgroups of 64: the M of the MMA)
 #define PF_BK 64  // k per stage: 64 f16 = 128 bytes = one swizzle atom
-#define PF_THREADS 192
+#define PF_THREADS 384 // warpgroup 0: dequantising producers (thread 0 also issues the TMA); warpgroups 1, 2: MMA + epilogue
 enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3 };
 
-// ---------------------------------------------------------------- tcgen05 / TMA wrappers
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) { // one whole warp
-	asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-	asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma / TMA wrappers
+__device__ __forceinline__ void wgmma_fence() { // accumulator registers written by ordinary instructions -> visible to wgmma
+	asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) { // the allocating warp
-	asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+__device__ __forceinline__ void wgmma_commit() {
+	asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-	asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { // at most N committed groups of this warpgroup still in flight
+	asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-	asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] . B[smem]^T, f16 x f16 -> f32, issued by ONE thread
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-	asm volatile(
-	    "{\n\t.reg .pred p;\n\t"
-	    "setp.ne.b32 p, %4, 0;\n\t"
-	    "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-	    ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-	    : "memory");
-}
-// all MMAs issued so far by this thread arrive on `bar` when they have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 columns of 32-bit accumulators: thread t of the warp gets row (lane base + t), columns c .. c+31
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-	uint32_t r[32];
-	asm volatile(
-	    "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-	    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-	      "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-	      "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-	    : "r"(taddr)
-	    : "memory");
-	asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accesses to accumulator registers across wgmma_wait
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
 #pragma unroll
-	for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+	for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 128] += A[64 x 16] . B[128 x 16]^T, f16 x f16 -> f32, A and B K-major in shared memory; issued by the whole warpgroup
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
+	asm volatile(
+	    "{\n\t"
+	    "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+	    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+	    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+	    "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+	    "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+	    "%64, %65, 1, 1, 1, 0, 0;\n\t"
+	    "}"
+	    : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+	      "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+	      "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+	      "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+	      "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+	      "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+	      "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+	    : "l"(desc_a), "l"(desc_b)
+	    : "memory");
 }
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
 	asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(smem_u32(dst)), "l"(map),
@@ -92,13 +89,12 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void fence_async_smem() { // generic-proxy writes to shared memory -> visible to the async proxy (tensor core reads)
 	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-// shared-memory matrix descriptor: K-major tile, rows of 128 bytes (64 f16), SWIZZLE_128B, 8-row groups 1024 bytes apart, sm_100 version bit
-__device__ __forceinline__ uint64_t umma_desc_sw128(const void* tile) {
+// wgmma shared-memory matrix descriptor: K-major tile, rows of 128 bytes (64 f16), 128-byte swizzle (layout type 1),
+// 8-row groups 1024 bytes apart (stride byte offset); the leading byte offset is unused by swizzled K-major layouts
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(const void* tile) {
 	const uint64_t addr = (uint64_t)(smem_u32(tile) & 0x3FFFF) >> 4;
-	return addr | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+	return addr | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// instruction descriptor, kind::f16: D = f32, A = B = f16, both K-major, M = 128, N = 128
-#define PF_IDESC ((1u << 4) | ((uint32_t)(PF_BN >> 3) << 17) | ((uint32_t)(PF_BM >> 4) << 24))
 
 // ---------------------------------------------------------------- small kernels
 
@@ -178,7 +174,7 @@ struct PfGemmArgs {
 	int hidden, gelu;
 };
 
-// 64 weights of one row (one k-stage) -> 8 swizzled 16-byte chunks of f16 in the A tile
+// 64 weights of one row (one k-stage) -> 8 swizzled 16-byte chunks of f16 in the weight tile
 template <int DBITS>
 __device__ __forceinline__ void pf_load_raw(const unsigned char* row, int kb, uint4 (&raw)[DBITS / 2]) {
 	const uint4* p = reinterpret_cast<const uint4*>(row + (size_t)kb * (PF_BK * DBITS / 8));
@@ -234,65 +230,28 @@ __host__ __device__ constexpr size_t pf_smem_bytes() {
 template <int MODE, int DBITS, typename KVT>
 __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, const PfGemmArgs a) {
 	constexpr int STAGES = pf_stages<MODE>(), NA = MODE == PF_UP ? 2 : 1;
-	constexpr uint32_t TMEM_COLS = NA * PF_BN;
 	extern __shared__ unsigned char smem_dyn[];
-	__shared__ __align__(8) uint64_t full[STAGES], empty[STAGES], accum;
-	__shared__ uint32_t tmem_base_s;
+	__shared__ __align__(8) uint64_t full[STAGES], empty[STAGES];
 	unsigned char* smem = reinterpret_cast<unsigned char*>(((uintptr_t)smem_dyn + 1023) & ~(uintptr_t)1023);
-	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+	const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
 	const int row0 = blockIdx.x * PF_BM, tok0 = blockIdx.y * PF_BN;
 	const int nkb = a.K / PF_BK;
-	auto a_tile = [&](int s, int i) { return smem + (size_t)s * pf_stage_bytes<MODE>() + (size_t)i * PF_BM * 128; };
-	auto b_tile = [&](int s, int i) { return smem + (size_t)s * pf_stage_bytes<MODE>() + (size_t)NA * PF_BM * 128 + (size_t)i * PF_BN * 128; };
+	auto w_tile = [&](int s, int i) { return smem + (size_t)s * pf_stage_bytes<MODE>() + (size_t)i * PF_BM * 128; };
+	auto x_tile = [&](int s, int i) { return smem + (size_t)s * pf_stage_bytes<MODE>() + (size_t)NA * PF_BM * 128 + (size_t)i * PF_BN * 128; };
 
 	pdl_launch_next();
 	if (tid == 0) {
-		for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1 + 4), mbar_init(&empty[s], 1);
-		mbar_init(&accum, 1);
+		// full: the TMA thread's expect_tx arrival + one arrival per producer warp; empty: one arrival per consumer warp
+		for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1 + 4), mbar_init(&empty[s], 8);
 		mbar_init_fence();
 	}
-	if (warp == 1) tmem_alloc(&tmem_base_s, TMEM_COLS);
-	tc_fence_before();
 	__syncthreads();
-	tc_fence_after();
-	const uint32_t tmem_base = tmem_base_s;
 	pdl_wait_prev(); // activations (and, for the KV rows, the cache) come from the previous kernels of the layer
 
-	if (warp == 0) {
-		// ===== TMA producer: the two activation tiles of every k-stage
-		if (lane == 0) {
-			for (int kb = 0; kb < nkb; ++kb) {
-				const int s = kb % STAGES;
-				mbar_wait_guard(&empty[s], ((kb / STAGES) & 1) ^ 1);
-				mbar_expect_tx(&full[s], 2 * PF_BN * 128);
-				tma_load_2d(b_tile(s, 0), &tm_hi, kb * PF_BK, tok0, &full[s]);
-				tma_load_2d(b_tile(s, 1), &tm_lo, kb * PF_BK, tok0, &full[s]);
-			}
-		}
-	} else if (warp == 1) {
-		// ===== MMA issuer
-		if (lane == 0) {
-			for (int kb = 0; kb < nkb; ++kb) {
-				const int s = kb % STAGES;
-				mbar_wait_guard(&full[s], (kb / STAGES) & 1);
-				tc_fence_after();
-#pragma unroll
-				for (int k = 0; k < PF_BK / 16; ++k) { // 16 f16 = 32 bytes along K inside the swizzle atom: +2 in the 16-byte address field
-					const uint64_t db_hi = umma_desc_sw128(b_tile(s, 0)) + 2 * k, db_lo = umma_desc_sw128(b_tile(s, 1)) + 2 * k;
-#pragma unroll
-					for (int i = 0; i < NA; ++i) {
-						const uint64_t da = umma_desc_sw128(a_tile(s, i)) + 2 * k;
-						umma_f16(tmem_base + i * PF_BN, da, db_hi, PF_IDESC, (kb | k) ? 1u : 0u);
-						umma_f16(tmem_base + i * PF_BN, da, db_lo, PF_IDESC, 1u);
-					}
-				}
-				umma_commit(&empty[s]); // frees the stage when these MMAs have read it
-			}
-			umma_commit(&accum);
-		}
-	} else {
-		// ===== dequantising producers (one tile row per thread), then the epilogue (one accumulator row per thread)
-		const int r = tid - 64; // 0..127
+	if (wg == 0) {
+		// ===== producers: one weight-tile row per thread, dequantised into the swizzled layout; thread 0 also brings in the
+		// two activation tiles of every k-stage with TMA
+		const int r = tid; // 0..127
 		const unsigned char* rowp[NA];
 		{
 			const size_t rowbytes = (size_t)a.K * DBITS / 8;
@@ -314,8 +273,13 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 		for (int kb = 0; kb < nkb; ++kb) {
 			const int s = kb % STAGES;
 			mbar_wait_guard(&empty[s], ((kb / STAGES) & 1) ^ 1);
+			if (tid == 0) {
+				mbar_expect_tx(&full[s], 2 * PF_BN * 128);
+				tma_load_2d(x_tile(s, 0), &tm_hi, kb * PF_BK, tok0, &full[s]);
+				tma_load_2d(x_tile(s, 1), &tm_lo, kb * PF_BK, tok0, &full[s]);
+			}
 #pragma unroll
-			for (int i = 0; i < NA; ++i) pf_store_a<DBITS>(a_tile(s, i), r, raw[i]);
+			for (int i = 0; i < NA; ++i) pf_store_a<DBITS>(w_tile(s, i), r, raw[i]);
 			if (kb + 1 < nkb) { // the next stage's bytes travel while this one is being multiplied
 #pragma unroll
 				for (int i = 0; i < NA; ++i) pf_load_raw<DBITS>(rowp[i], kb + 1, raw[i]);
@@ -324,64 +288,80 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 			__syncwarp();
 			if (lane == 0) mbar_arrive(&full[s]);
 		}
+	} else {
+		// ===== consumers: warpgroup c = wg - 1 multiplies tokens 64 c .. 64 c + 63 of the tile against all 128 weight rows
+		const int c = wg - 1;
+		float acc[NA][64];
+#pragma unroll
+		for (int i = 0; i < NA; ++i)
+#pragma unroll
+			for (int j = 0; j < 64; ++j) acc[i][j] = 0.f;
+		for (int kb = 0; kb < nkb; ++kb) {
+			const int s = kb % STAGES;
+			mbar_wait_guard(&full[s], (kb / STAGES) & 1);
+			wgmma_fence();
+#pragma unroll
+			for (int k = 0; k < PF_BK / 16; ++k) { // 16 f16 = 32 bytes along K inside the swizzle atom: +2 in the 16-byte address field
+				const uint64_t dx_hi = wgmma_desc_sw128(x_tile(s, 0) + c * 64 * 128) + 2 * k, dx_lo = wgmma_desc_sw128(x_tile(s, 1) + c * 64 * 128) + 2 * k;
+#pragma unroll
+				for (int i = 0; i < NA; ++i) {
+					const uint64_t dw = wgmma_desc_sw128(w_tile(s, i)) + 2 * k;
+					wgmma_m64n128k16(acc[i], dx_hi, dw);
+					wgmma_m64n128k16(acc[i], dx_lo, dw);
+				}
+			}
+			wgmma_commit();
+			wgmma_wait<1>(); // the MMAs of the previous stage have finished reading it
+#pragma unroll
+			for (int i = 0; i < NA; ++i) acc_fence(acc[i]);
+			if (kb > 0 && lane == 0) mbar_arrive(&empty[(kb - 1) % STAGES]);
+		}
+		wgmma_wait<0>();
+#pragma unroll
+		for (int i = 0; i < NA; ++i) acc_fence(acc[i]);
 
-		mbar_wait_guard(&accum, 0);
-		tc_fence_after();
-		const int q4 = warp & 3; // the TMEM lane quarter this warp may read
-		const int lr = q4 * 32 + lane, gr = row0 + lr;
-		for (int c0 = 0; c0 < PF_BN; c0 += 32) {
-			float v[32];
-			tmem_ld32(tmem_base + ((uint32_t)(q4 * 32) << 16) + c0, v);
-			if constexpr (MODE == PF_QKV) {
-				const bool is_q = gr < a.q_dim, is_k = !is_q && gr < a.q_dim + a.kv_dim;
-				const int k = is_q ? gr : (is_k ? gr - a.q_dim : gr - a.q_dim - a.kv_dim);
-				const int d = k % a.head_dim, h = k / a.head_dim;
-				const float b = a.bias ? a.bias[gr] : 0.f;
+		// accumulator fragment of m64nN: register 4 j + 2 h + e holds token 16 w + lane / 4 + 8 h, weight row 8 j + 2 (lane % 4) + e
+		const int w4 = warp & 3;
+		const int tb = tok0 + c * 64 + w4 * 16 + (lane >> 2);
 #pragma unroll
-				for (int j = 0; j < 32; ++j) {
-					const int t = tok0 + c0 + j;
-					float x = fminf(fmaxf(v[j] + b, -a.clip), a.clip);
-					const float other = __shfl_xor_sync(0xffffffffu, x, 1); // the row pair a rotation mixes sits in adjacent lanes
-					if (t < a.n_tokens) {
-						if (is_q || is_k) {
-							const float2 cs = a.rope[(size_t)t * (a.head_dim / 2) + (d >> 1)];
-							x = (lane & 1) ? fmaf(other, cs.y, x * cs.x) : fmaf(-other, cs.y, x * cs.x);
-						}
-						if (is_q) {
-							a.Q[(size_t)t * a.q_dim + k] = x;
-						} else {
-							KVT* dst = reinterpret_cast<KVT*>(is_k ? a.kc : a.vc) + ((size_t)h * a.seq_len + a.pos0 + t) * a.head_dim + d;
-							kv_store(dst, x);
-						}
+		for (int j = 0; j < PF_BM / 8; ++j) {
+			const int gr = row0 + 8 * j + 2 * (lane & 3); // even: (gr, gr + 1) is a RoPE pair
+#pragma unroll
+			for (int h = 0; h < 2; ++h) {
+				const int t = tb + 8 * h;
+				if (t >= a.n_tokens) continue;
+				float x0 = acc[0][4 * j + 2 * h], x1 = acc[0][4 * j + 2 * h + 1];
+				if constexpr (MODE == PF_QKV) {
+					const bool is_q = gr < a.q_dim, is_k = !is_q && gr < a.q_dim + a.kv_dim;
+					const int k = is_q ? gr : (is_k ? gr - a.q_dim : gr - a.q_dim - a.kv_dim);
+					const int d = k % a.head_dim, hh = k / a.head_dim;
+					if (a.bias) x0 += a.bias[gr], x1 += a.bias[gr + 1];
+					x0 = fminf(fmaxf(x0, -a.clip), a.clip), x1 = fminf(fmaxf(x1, -a.clip), a.clip);
+					if (is_q || is_k) {
+						const float2 cs = a.rope[(size_t)t * (a.head_dim / 2) + (d >> 1)];
+						const float r0 = fmaf(-x1, cs.y, x0 * cs.x), r1 = fmaf(x0, cs.y, x1 * cs.x);
+						x0 = r0, x1 = r1;
 					}
-				}
-			} else if constexpr (MODE == PF_UP) {
-				float v3[32];
-				tmem_ld32(tmem_base + ((uint32_t)(q4 * 32) << 16) + PF_BN + c0, v3);
-#pragma unroll
-				for (int j = 0; j < 32; ++j) {
-					const int t = tok0 + c0 + j;
-					if (t < a.n_tokens) {
-						const float hv = (a.gelu ? act_gelu(v[j]) : act_silu(v[j])) * v3[j];
-						__half hh, hl;
-						split_hl(hv, hh, hl);
-						a.Hhi[(size_t)t * a.hidden + gr] = hh, a.Hlo[(size_t)t * a.hidden + gr] = hl;
+					if (is_q) {
+						*reinterpret_cast<float2*>(a.Q + (size_t)t * a.q_dim + k) = make_float2(x0, x1);
+					} else {
+						KVT* dst = reinterpret_cast<KVT*>(is_k ? a.kc : a.vc) + ((size_t)hh * a.seq_len + a.pos0 + t) * a.head_dim + d;
+						kv_store(dst, x0), kv_store(dst + 1, x1);
 					}
-				}
-			} else {
-#pragma unroll
-				for (int j = 0; j < 32; ++j) {
-					const int t = tok0 + c0 + j;
-					if (t < a.n_tokens) a.X[(size_t)t * a.dim + gr] += v[j];
+				} else if constexpr (MODE == PF_UP) {
+					const float g0 = acc[NA - 1][4 * j + 2 * h], g1 = acc[NA - 1][4 * j + 2 * h + 1];
+					const float h0 = (a.gelu ? act_gelu(x0) : act_silu(x0)) * g0, h1 = (a.gelu ? act_gelu(x1) : act_silu(x1)) * g1;
+					__half hh0, hl0, hh1, hl1;
+					split_hl(h0, hh0, hl0), split_hl(h1, hh1, hl1);
+					*reinterpret_cast<uint32_t*>(a.Hhi + (size_t)t * a.hidden + gr) = pack_h2(hh0, hh1);
+					*reinterpret_cast<uint32_t*>(a.Hlo + (size_t)t * a.hidden + gr) = pack_h2(hl0, hl1);
+				} else {
+					float2* dst = reinterpret_cast<float2*>(a.X + (size_t)t * a.dim + gr);
+					const float2 o = *dst;
+					*dst = make_float2(o.x + x0, o.y + x1);
 				}
 			}
 		}
-		tc_fence_before();
-	}
-	__syncthreads();
-	if (warp == 1) {
-		tc_fence_after();
-		tmem_dealloc(tmem_base, TMEM_COLS);
 	}
 }
 

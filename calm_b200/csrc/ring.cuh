@@ -1,6 +1,6 @@
 // ring.cuh -- the two largest matvec stages (FFN up, FFN down; and wo) fed by warp-private bulk-TMA rings.
 //
-// Why (profiles/README.md, round 1 + 2): the register-fed stage kernels keep their bytes in flight in registers --
+// Why: the register-fed stage kernels keep their bytes in flight in registers --
 // a warp requests one batch (8 x 16 B per lane), waits a DRAM round trip, consumes it, and only then requests the next --
 // so the bytes in flight per SM are duty-cycled, bounded by the register file, and nothing can be requested before the
 // dependency wait without costing a CTA of occupancy.  Here every warp owns a small ring of shared-memory slots that it

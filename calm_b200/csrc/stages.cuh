@@ -311,12 +311,12 @@ struct QkvArgs {
 };
 
 // Before waiting for the previous kernel a warp asks the L2 for its first row pair (cp.async.bulk.prefetch.L2: no registers;
-// weights are immutable, so this is always legal).  (Issuing the first loads into registers instead measured 25 % slower:
-// 32 more live registers across the staging cost a CTA per SM.)
+// weights are immutable, so this is always legal).  (Issuing the first loads into registers instead keeps 32 more registers
+// live across the staging, which costs a CTA per SM.)
 #define QKV_THREADS 256
 // One warp per row pair (the whole 2 x rowbytes pair is requested in one batch), 3 CTAs per SM.  (A one-CTA-per-SM form with
-// equal contiguous shares, meant to leave half the register file to an early attention CTA, measured 2.8 us slower per
-// launch: most warps then need a second DRAM round trip -- profiles/README.md, round 2.)
+// equal contiguous shares, meant to leave half the register file to an early attention CTA, makes most warps wait for a
+// second DRAM round trip.)
 template <int DBITS, typename KVT>
 __global__ void __launch_bounds__(QKV_THREADS, 3) k_qkv(const QkvArgs<KVT> a) {
 	pdl_launch_next();

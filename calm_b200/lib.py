@@ -3,7 +3,7 @@
 The function names, argument meaning and error behaviour are the reference's
 (run.c:22-25): upload_cuda / prepare_cuda / forward_cuda / perf_cuda.  There is
 no CPU path behind these calls: loading fails loudly when the library has not
-been built, and prepare_cuda aborts the process when no sm_100 device exists.
+been built, and prepare_cuda aborts the process when no sm_90 device exists.
 """
 from __future__ import annotations
 
@@ -200,6 +200,7 @@ class DeviceModel:
             for p in self._uploaded:
                 self.lib.calm_b200_free(p)
             self._uploaded = []
+            self._keep = None  # the caller's tensors (device weights of a large model) can be freed now
             self.transformer = None
 
     def __enter__(self):

@@ -117,7 +117,7 @@ SPECS.update({
     # records exceed the default 48 KB of dynamic shared memory)
     # (hidden >= dim >= q_dim: the reference CPU backend reuses xb2[dim] and hb[hidden] as scratch, infer.c:152-153, 404, 409)
     "tiny-hd256": replace(_T, name="tiny-hd256", dim=2048, n_layers=2, n_heads=8, n_kv_heads=1, head_dim=256, hidden_dim=2048),
-    # Llama-3-8B's attention geometry (32 query / 8 kv heads of 128, so 8 units x 18 slices on 148 SMs) at the full
+    # Llama-3-8B's attention geometry (32 query / 8 kv heads of 128, so 8 units x 16 slices on 132 SMs) at the full
     # 4096-token context, on widths the CPU oracle finishes in milliseconds per token
     "attn-l8": ModelSpec("attn-l8", 256, 512, 2, 32, 8, 128, 512, "fp8", rope_theta=5e5, max_seq_len=4096),
 })

@@ -1,5 +1,5 @@
 /*
- * calm_b200.h -- C ABI of libcalm_b200.so, a B200 (sm_100a) backend for calm's
+ * calm_b200.h -- C ABI of libcalm_b200.so, an H100 (sm_90a) backend for calm's
  * per-token forward() path.
  *
  * The first four functions ARE the reference's CUDA backend boundary: the
@@ -11,7 +11,7 @@
  *
  * Error behaviour follows the reference (infer.cu:12-20, 755): there are no
  * error codes; a CUDA failure or an unsupported configuration prints one line
- * to stderr and abort()s.  There is NO CPU fallback: without a usable sm_100
+ * to stderr and abort()s.  There is NO CPU fallback: without a usable sm_90
  * device prepare_cuda() aborts.
  *
  * Threading: one host thread, one model per process at a time (the reference

@@ -17,16 +17,16 @@ KV_ATOL = 2e-4
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a)")
 
 
 @pytest.fixture(scope="session")
 def oracle_pkg():
-    """Builds (if needed) and returns the oracle package.  /root/reference is only needed for the
-    'reference' checker, whose prebuilt .so travels to the GPU box in oracle/_ref/."""
+    """Builds (if needed) and returns the oracle package (our restatement; what the reference computed is stored
+    under tests/golden/)."""
     import oracle
 
-    oracle.build(ref=os.path.isdir("/root/reference"))
+    oracle.build(ref=False)
     return oracle
 
 

@@ -50,8 +50,7 @@ def test_no_oracle_in_product():
 
 
 def test_struct_layout_matches_reference_header(tmp_path):
-    """include/calm_model.h vs reference src/model.h, field by field (only where the reference is mounted);
-    the ctypes mirror vs include/calm_model.h everywhere."""
+    """include/calm_model.h vs reference src/model.h, field by field; the ctypes mirror vs include/calm_model.h."""
     prog = r'''
 #include <stdio.h>
 #include <stddef.h>
@@ -77,8 +76,8 @@ int main() {
         return subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout
 
     ours = layout(os.path.join(ROOT, "include", "calm_model.h"))
-    if os.path.exists("/root/reference/src/model.h"):
-        assert ours == layout("/root/reference/src/model.h")
+    # the same program's output for the reference's src/model.h (stored: the reference is not part of this repository)
+    assert ours == open(os.path.join(ROOT, "tests", "golden", "reference-model-h-layout.txt")).read()
     kv = dict(line.rsplit(" ", 1) for line in ours.strip().splitlines()[:-1])
     for name, cls in (("Config", cstructs.Config), ("Weights", cstructs.Weights), ("RunState", cstructs.RunState), ("Transformer", cstructs.Transformer)):
         assert int(kv[name]) == C.sizeof(cls)

@@ -1,6 +1,6 @@
-"""The JSON line bench.py prints (the driver's contract) checked on the committed round-2 lines: keys, types and the internal
-arithmetic (value <-> ms_per_step, roofline.frac = achieved / peak, e2e declares its copies).  CPU only: the lines were
-produced on the GPU box by the committed command and live under profiles/."""
+"""The JSON line bench.py prints checked on the committed lines: keys, types and the internal arithmetic (value <->
+ms_per_step, roofline.frac = achieved / peak, e2e declares its copies).  CPU only: the lines were produced on an H100 by
+the commands profiles/README.md lists and live under profiles/."""
 import json
 import os
 import sys
@@ -10,8 +10,7 @@ import pytest
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from conftest import ROOT  # noqa: E402
 
-LINES = ["r02_bench_llama3-8b-fp8_final.jsonl", "r02_bench_mistral-7b-gf4.jsonl", "r02_bench_mixtral-8x7b-fp8.jsonl", "r02_tp2_llama3-8b-fp8.jsonl",
-         "r02_tp8_llama3-70b-fp8.jsonl"]
+LINES = ["r02_bench_llama3-8b-fp8_final.jsonl", "r02_bench_mistral-7b-gf4.jsonl", "r02_bench_mixtral-8x7b-fp8.jsonl"]
 
 
 def _line(name):

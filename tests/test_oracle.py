@@ -1,7 +1,6 @@
 """CPU tests: the oracle (our restatement of reference infer.c) against the reference itself and against
 the committed golden fixtures; the synthetic-model writer against the reference loader."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -15,8 +14,6 @@ from calm_b200 import modelgen as mg  # noqa: E402
 
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 from make_golden import GOLDEN_SPECS, model_digest  # noqa: E402
-
-HAVE_REF = os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libcalm_ref_cpu.so")) or os.path.isdir("/root/reference")
 
 
 @pytest.mark.parametrize("name", GOLDEN_SPECS)
@@ -41,33 +38,28 @@ def test_oracle_matches_golden(oracle_pkg, name):
     ck.release(model)
 
 
-@pytest.mark.skipif(not HAVE_REF, reason="oracle/_ref not built and /root/reference absent")
 @pytest.mark.parametrize("name", ["tiny-fp8", "tiny-gf4", "tiny-qwen", "tiny-moe"])
 def test_oracle_matches_reference_live(oracle_pkg, name):
-    """Same comparison against the reference executed now, on a different seed and at a position offset."""
+    """Same comparison against reference logits stored from a run of the reference (tools/make_reference_golden.py), on a
+    different seed and at a position offset."""
     spec = mg.SPECS[name]
     toks = mg.teacher_tokens(spec.vocab_size, 12, start=100)
-    out = {}
-    for kind in ("reference", "port", "port_f64"):
+    ref = golden("reference-cpu")["live-" + name]
+    sigma = ref.std()
+    for kind in ("port", "port_f64"):
         model = mg.HostModel(spec, seed=3)
-        out[kind] = oracle_pkg.teacher_forced(oracle_pkg.Checker(kind), model, toks)
-    sigma = out["reference"].std()
-    assert np.abs(out["port"] - out["reference"]).max() <= TOL_SIGMA * sigma
-    assert np.abs(out["port_f64"] - out["reference"]).max() <= TOL_SIGMA * sigma
+        got = oracle_pkg.teacher_forced(oracle_pkg.Checker(kind), model, toks)
+        assert np.abs(got - ref).max() <= TOL_SIGMA * sigma, kind
 
 
 def test_oracle_rolling_cache(oracle_pkg):
     """Past seq_len the cache rolls with 2 pinned sinks (reference infer.c:330-332, 384-394)."""
-    if not HAVE_REF:
-        pytest.skip("needs oracle/_ref")
     spec = mg.SPECS["tiny-fp8"]
     toks = mg.teacher_tokens(spec.vocab_size, 40)
-    res = {}
-    for kind in ("reference", "port"):
-        model = mg.HostModel(spec, seed=1, seq_len=16)
-        res[kind] = oracle_pkg.teacher_forced(oracle_pkg.Checker(kind), model, toks)
-    sigma = res["reference"].std()
-    assert np.abs(res["port"] - res["reference"]).max() <= TOL_SIGMA * sigma
+    ref = golden("reference-cpu")["rolling-tiny-fp8"]
+    model = mg.HostModel(spec, seed=1, seq_len=16)
+    got = oracle_pkg.teacher_forced(oracle_pkg.Checker("port"), model, toks)
+    assert np.abs(got - ref).max() <= TOL_SIGMA * ref.std()
 
 
 def test_decoders_exact(oracle_pkg):
@@ -124,19 +116,18 @@ def test_algorithmic_bytes_table():
     assert abs(mg.kv_bytes(mg.SPECS["llama3-8b-fp8"], 4095, 4096) / 1e9 - 0.537) < 1e-3
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "run_ref")), reason="reference binary not built")
 def test_calm_file_loads_in_reference_driver(tmp_path, oracle_pkg):
-    """A .calm file written by modelgen.write_calm is accepted by the UNMODIFIED reference program
-    (tensors.c parser, run.c get_config/get_weights shape checks) and decodes on its CPU path."""
+    """modelgen.write_calm still writes the .calm file the UNMODIFIED reference program accepted (tensors.c parser, run.c
+    get_config/get_weights shape checks) and decoded on its CPU path, and the oracle continues the prompt as it did
+    (the program's output is stored in tests/golden/reference-cpu.npz by tools/make_reference_golden.py)."""
+    import hashlib
+
     spec = mg.SPECS["tiny-fp8"]
+    g = golden("reference-cpu")
     model = mg.HostModel(spec, seed=0)
     path = str(tmp_path / "tiny.calm")
     mg.write_calm(path, spec, model.tensors)
-    env = dict(os.environ, CALM_CPU="1", OMP_NUM_THREADS="2")
-    r = subprocess.run([os.path.join(ROOT, "oracle", "_ref", "run_ref"), path, "-n", "8", "-t", "0", "-i", "<|t7|><|t8|>"],
-                       capture_output=True, text=True, env=env, timeout=120)
-    assert r.returncode == 0, r.stderr
-    assert "tok/s" in r.stderr
+    assert hashlib.sha256(open(path, "rb").read()).hexdigest() == str(g["driver-tiny-fp8-sha256"])
     # same greedy continuation from the oracle: prompt = BOS, 7, 8
     ck = oracle_pkg.Checker("port")
     m2 = mg.HostModel(spec, seed=0)
@@ -151,8 +142,8 @@ def test_calm_file_loads_in_reference_driver(tmp_path, oracle_pkg):
         gen.append(nxt)
         logits = ck.forward(m2, nxt, pos)
         pos += 1
-    expect = "".join(f"<|t{t}|>" for t in gen)
-    assert expect in r.stdout, (expect, r.stdout)
+    driver = [int(t) for t in g["driver-tiny-fp8-tokens"]]
+    assert driver[:2] == [7, 8] and driver[2:2 + len(gen)] == gen[:len(driver) - 2], (driver, gen)
 
 
 def test_oracle_e5m2_cache_rounding_is_bit_exact(oracle_pkg):

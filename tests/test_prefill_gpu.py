@@ -1,4 +1,4 @@
-"""The batched prompt pass (forward_prefill_cuda: tcgen05 GEMMs + block-causal attention, SURVEY.md s.8f row 1) against
+"""The batched prompt pass (forward_prefill_cuda: wgmma GEMMs + block-causal attention, SURVEY.md s.8f row 1) against
 the path it replaces: n serial forward(FF_UPDATE_KV_ONLY) calls (reference run.c:206-209).  The parity contract is the
 KV cache -- every layer, positions across the block -- and the logits of the token that follows, also against the CPU
 oracle.  Shapes: the smallest the pass serves, all three weight formats, both cache types, a bias / wide-head variant,

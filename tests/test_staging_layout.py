@@ -1,8 +1,7 @@
 """Host-side model of the shared-memory layout of the staged activation vector (calm_b200/csrc/common.cuh: xs_index,
 xs_swz, xs_aux_floats).  The kernels' parity tests prove the values; this file pins the two properties the layout exists
 for -- the staging stores and the matvec loads are both free of shared-memory bank conflicts -- so that a later change of
-the permutation cannot silently bring back the 4-way (fp8) / 8-way (gf4) store conflicts ncu showed in round 2
-(profiles/README.md, r02_sweep_staging_bank_swizzle.jsonl)."""
+the permutation cannot silently bring back the 4-way (fp8) / 8-way (gf4) store conflicts of the unswizzled layout."""
 import numpy as np
 import pytest
 

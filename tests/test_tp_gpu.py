@@ -2,7 +2,7 @@
 reference boundary plus calm_b200_tp_init; every rank must return the full logits, equal to the single-device reference
 fixtures within the stated tolerance, and all ranks must agree bit for bit (they sample independently).  Covers the fused
 matvec -> all-reduce inside k_matres, the vocabulary-split classifier with its NVLink gather, and MoE expert slices.
-Cases whose world size exceeds the visible GPUs are skipped (run under `gpurun --gpus N`)."""
+Cases whose world size exceeds the visible GPUs are skipped (tools/tp_round.sh N runs them on N GPUs)."""
 import os
 import subprocess
 import sys
@@ -53,7 +53,7 @@ def test_ranks_match_single_device_reference(tmp_path, name, world, fused):
     """fused=1: partial sums exchanged inside k_matres over peer memory, classifier split by vocabulary;
     fused=0: ncclAllReduce between kernels, replicated classifier."""
     if _gpus() < world:
-        pytest.skip(f"needs {world} GPUs (gpurun --gpus {world})")
+        pytest.skip(f"needs {world} GPUs")
     spec = mg.SPECS[name]
     g = golden(name)
     res = _run_world(tmp_path, name, world, fused, len(g["tokens"]))

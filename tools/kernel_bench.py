@@ -2,7 +2,7 @@
 """Per-kernel roofline of the stand-alone matvec kernel (calm_b200_matvec) on matrices larger than L2.
 
   python tools/kernel_bench.py [--iters 20]            # prints one JSON line per (format, shape)
-Used under ncu for the per-kernel evidence in profiles/ (see profiles/README.md)."""
+Timed with CUDA events around the kernel over many launches."""
 import argparse
 import json
 import os

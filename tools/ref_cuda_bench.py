@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Same-box comparison through the REFERENCE DRIVER (unmodified run.c + tensors.c + tokenizer.c + sampler.c):
 
-  oracle/_ref/run_ref   reference program with its own CUDA backend (src/infer.cu, compiled for sm_100a)
+  oracle/_ref/run_ref   reference program with its own CUDA backend (src/infer.cu, compiled for sm_90a)
   oracle/_ref/run_b200  the same reference program linked against libcalm_b200.so (the drop-in)
 
 Writes the synthetic model as a .calm file (calm_b200.modelgen.write_calm) into /dev/shm, runs both binaries with

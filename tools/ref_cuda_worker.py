@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Run the UNMODIFIED reference CUDA backend (oracle/_ref/libcalm_ref_cuda.so = reference src/infer.cu compiled for
-sm_100a by oracle/Makefile) on a seeded synthetic model and save its logits: the at-scale oracle of the GPU parity
+sm_90a by oracle/Makefile) on a seeded synthetic model and save its logits: the at-scale oracle of the GPU parity
 tests (tests/test_scale_gpu.py).  TEST INFRASTRUCTURE ONLY; runs in its own process because the reference keeps global
 state and abort()s on errors.
 
