@@ -65,6 +65,12 @@ __device__ __forceinline__ void l2_prefetch_row(const void* row, int rowbytes) {
 	for (int off = 0; off < rowbytes; off += 16384) l2_prefetch((const char*)row + off, (uint32_t)min(16384, rowbytes - off));
 }
 
+// f32 -> (hi, lo) f16 pair with x = hi + lo up to 2^-22 |x|
+__device__ __forceinline__ void split_hl(float x, __half& hi, __half& lo) {
+	hi = __float2half_rn(x);
+	lo = __float2half_rn(x - __half2float(hi));
+}
+
 // ---------------------------------------------------------------- bulk async copies (TMA, 1-D) and mbarriers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 	return (uint32_t)__cvta_generic_to_shared(p);

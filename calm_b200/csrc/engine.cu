@@ -63,8 +63,7 @@ struct Engine {
 	int ring_up_u = 0, ring_wo_u = 0, ring_down_u = 0, ring_wo_s = 1, ring_down_s = 1;
 	int grid_up_ring = 0, grid_wo_ring = 0, grid_down_ring = 0;
 	size_t smem_up_ring = 0, smem_wo_ring = 0, smem_down_ring = 0;
-	bool attn2_cluster = false; // ... with the CTAs of a unit as one thread-block cluster (slices folded through distributed shared memory)
-	bool attn2 = false; // k_attn2 (attn.cuh): KV slice requested into shared memory ahead of the dependency wait
+	bool attn2 = false; // k_attn2 (attn.cuh): KV slice requested into shared memory ahead of the dependency wait, tensor-core passes
 	int attn_nbmax = 0;
 	size_t attn2_smem = 0;
 
@@ -399,46 +398,16 @@ void launch_attn(const AttnArgs& a, int nunits, int* nl) {
 	++*nl;
 }
 
-template <typename KVT, int HG, int LPP>
+template <typename KVT, int HG, int HD>
 void launch_attn2(const AttnArgs& a, int nunits, int* nl) {
-	if (!nl) { // prepare time: opt-ins, and whether the cluster form can be scheduled at all
-		smem_optin(k_attn2<KVT, HG, LPP, false>, g.attn2_smem);
-		{ // the cell fold polls its peers: the whole grid must fit on the device at once
-			int per_sm = 0;
-			CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_attn2<KVT, HG, LPP, false>, ATTN_THREADS, g.attn2_smem));
-			if (per_sm * g.sms < nunits * a.nsplit) g.attn2 = false; // k_attn (global partials, last-CTA fold) has no such requirement
-		}
-		if (g.attn2_cluster) {
-			smem_optin(k_attn2<KVT, HG, LPP, true>, g.attn2_smem);
-			if (a.nsplit > 8) CUDA_CHECK(cudaFuncSetAttribute(k_attn2<KVT, HG, LPP, true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-			cudaLaunchConfig_t cfg = {};
-			cfg.gridDim = dim3(nunits * a.nsplit), cfg.blockDim = dim3(ATTN_THREADS), cfg.dynamicSmemBytes = g.attn2_smem;
-			cudaLaunchAttribute at[1];
-			at[0].id = cudaLaunchAttributeClusterDimension;
-			at[0].val.clusterDim.x = a.nsplit, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
-			cfg.attrs = at, cfg.numAttrs = 1;
-			int nclusters = 0;
-			if (cudaOccupancyMaxActiveClusters(&nclusters, k_attn2<KVT, HG, LPP, true>, &cfg) != cudaSuccess || nclusters < 1) {
-				(void)cudaGetLastError();
-				g.attn2_cluster = false; // e.g. no GPC with nsplit free SMs: fold the slices through global partials instead
-			}
-		}
+	if (!nl) { // prepare time: opt-in, and the cell fold polls its peers: the whole grid must fit on the device at once
+		smem_optin(k_attn2<KVT, HG, HD>, g.attn2_smem);
+		int per_sm = 0;
+		CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_attn2<KVT, HG, HD>, ATTN_THREADS, g.attn2_smem));
+		if (per_sm * g.sms < nunits * a.nsplit) g.attn2 = false; // k_attn (global partials, last-CTA fold) has no such requirement
 		return;
 	}
-	if (g.attn2_cluster) {
-		same_carveout((const void*)k_attn2<KVT, HG, LPP, true>);
-		cudaLaunchConfig_t cfg = {};
-		cfg.gridDim = dim3(nunits * a.nsplit), cfg.blockDim = dim3(ATTN_THREADS), cfg.dynamicSmemBytes = g.attn2_smem, cfg.stream = g.stream;
-		cudaLaunchAttribute at[2];
-		at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-		at[0].val.programmaticStreamSerializationAllowed = g.use_pdl ? 1 : 0;
-		at[1].id = cudaLaunchAttributeClusterDimension;
-		at[1].val.clusterDim.x = a.nsplit, at[1].val.clusterDim.y = 1, at[1].val.clusterDim.z = 1;
-		cfg.attrs = at, cfg.numAttrs = 2;
-		CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_attn2<KVT, HG, LPP, true>, a));
-	} else {
-		launch_pdl(k_attn2<KVT, HG, LPP, false>, nunits * a.nsplit, ATTN_THREADS, g.attn2_smem, a);
-	}
+	launch_pdl(k_attn2<KVT, HG, HD>, nunits * a.nsplit, ATTN_THREADS, g.attn2_smem, a);
 	++*nl;
 }
 
@@ -451,11 +420,11 @@ template <typename KVT>
 void dispatch_attn(const AttnArgs& a, int nunits, int* nl) {
 	if (g.attn2) {
 		switch (g.attn_lpp * 100 + g.attn_hg) {
-		case 1604: launch_attn2<KVT, 4, 16>(a, nunits, nl); return;
-		case 1608: launch_attn2<KVT, 8, 16>(a, nunits, nl); return;
-		case 802: launch_attn2<KVT, 2, 8>(a, nunits, nl); return;
-		case 804: launch_attn2<KVT, 4, 8>(a, nunits, nl); return;
-		case 808: launch_attn2<KVT, 8, 8>(a, nunits, nl); return;
+		case 1604: launch_attn2<KVT, 4, 128>(a, nunits, nl); return;
+		case 1608: launch_attn2<KVT, 8, 128>(a, nunits, nl); return;
+		case 802: launch_attn2<KVT, 2, 64>(a, nunits, nl); return;
+		case 804: launch_attn2<KVT, 4, 64>(a, nunits, nl); return;
+		case 808: launch_attn2<KVT, 8, 64>(a, nunits, nl); return;
 		}
 	}
 	switch (g.attn_hg) {
@@ -740,10 +709,9 @@ void make_plan() {
 	{
 		// k_attn2 when the shape is instantiated and the CTA's share of the context fits in shared memory
 		g.attn_nbmax = cdiv(cdiv(c.seq_len, ATTN2_BP), g.attn_nsplit);
-		g.attn2_smem = attn2_smem_bytes<KVT>(g.attn_hg, c.head_dim, g.attn_nbmax, g.attn_nsplit);
+		g.attn2_smem = attn2_smem_bytes<KVT>(g.attn_hg, c.head_dim, g.attn_nbmax);
 		const bool want = !(getenv("CALM_B200_ATTN2") && atoi(getenv("CALM_B200_ATTN2")) == 0);
 		g.attn2 = want && attn2_shape_ok(g.attn_hg, g.attn_lpp, c.head_dim) && g.attn_nbmax <= ATTN2_MAXB && g.attn2_smem <= 200 * 1024;
-		g.attn2_cluster = g.attn2 && g.attn_nsplit <= ATTN2_MAX_CLUSTER && getenv("CALM_B200_ATTN_CLUSTER") && atoi(getenv("CALM_B200_ATTN_CLUSTER")) != 0;
 		AttnArgs aa = {};
 		aa.head_dim = c.head_dim, aa.nsplit = g.attn_nsplit;
 		dispatch_attn<KVT>(aa, c.n_kv_heads * g.attn_qgroups, nullptr);
@@ -1011,15 +979,7 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 	int want = (split_mul > 1 ? split_mul : 1) * g.sms / units; // about one 256-thread CTA per SM
 	int maxsplit = cdiv(c.seq_len, 64);                 // at least 64 positions per slice at full context
 	g.attn_nsplit = want < 1 ? 1 : (want > maxsplit ? maxsplit : want);
-	// (the cluster fold is off by default: a 16-CTA cluster needs 16 SMs of one GPC at once, which the still-resident q/k/v CTAs
-	// delay; kept selectable)
 	if (g.attn_nsplit > ATTN2_MAXB + 4) g.attn_nsplit = ATTN2_MAXB + 4; // k_attn2 keeps one (m, l) pair per slice in static shared memory
-	const bool want_cluster = getenv("CALM_B200_ATTN_CLUSTER") && atoi(getenv("CALM_B200_ATTN_CLUSTER")) != 0;
-	if (want_cluster && attn2_shape_ok(g.attn_hg, g.attn_lpp, c.head_dim) && !(getenv("CALM_B200_ATTN2") && atoi(getenv("CALM_B200_ATTN2")) == 0)) {
-		int ns = 1; // the slices of a unit will be one thread-block cluster: a power of two, at most 16 CTAs
-		while (ns * 2 <= g.attn_nsplit && ns * 2 <= ATTN2_MAX_CLUSTER) ns *= 2;
-		g.attn_nsplit = ns;
-	}
 	g.attn_partial = (float*)dev_alloc((size_t)units * g.attn_nsplit * g.attn_hg * (c.head_dim + 2) * sizeof(float));
 	{
 		const size_t cell_bytes = (size_t)units * (g.sms / units > g.attn_nsplit ? g.sms / units : g.attn_nsplit) * g.attn_hg * (c.head_dim + 2) * sizeof(unsigned long long);

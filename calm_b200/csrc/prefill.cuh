@@ -98,12 +98,6 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(const void* tile) {
 
 // ---------------------------------------------------------------- small kernels
 
-// f32 -> (hi, lo) f16 pair with x = hi + lo up to 2^-22 |x|
-__device__ __forceinline__ void split_hl(float x, __half& hi, __half& lo) {
-	hi = __float2half_rn(x);
-	lo = __float2half_rn(x - __half2float(hi));
-}
-
 // X[t][:] = decode(E[tokens[t]])  (reference infer.c:335-347)
 template <int DBITS>
 __global__ void k_pf_embed(float* X, const void* table, const int* tokens, int n, int dim) {

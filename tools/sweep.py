@@ -57,7 +57,8 @@ def main():
             dbg = (C.c_ulonglong * 16)()
             L.calm_b200_debug_stamps(dbg)
             d = [int(x) for x in dbg]
-            attn_dbg = {"entry->wait": d[1] - d[0], "wait->q": d[2] - d[1], "q->first_block": d[3] - d[2], "loop": d[4] - d[3], "tail": d[7] - d[4], "tail_merge_in_cta": d[5] - d[4], "tail_publish_wait_ml_coef": d[6] - d[5], "tail_outputs": d[7] - d[6],
+            attn_dbg = {"entry->wait": d[1] - d[0], "wait->q": d[2] - d[1], "q->first_block": d[3] - d[2], "loop": d[4] - d[3], "q->all_blocks_landed": d[8] - d[2], "loop_after_all_blocks": d[4] - d[8],
+                        "loop_scores_softmax": d[11] - d[3], "loop_values": d[4] - d[11], "tail": d[7] - d[4], "tail_publish_wait_ml_coef": d[6] - d[4], "tail_outputs": d[7] - d[6],
                         "first_start->last_end": d[9] - d[10], "cta0_start_after_first": d[1] - d[10]} if d[1] else None
             dm.close()
             row = {k: round(v[0] / max(v[2], 1) * 1e3, 2) for k, v in stats.items() if v[2]}
