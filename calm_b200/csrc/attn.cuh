@@ -142,7 +142,7 @@ __device__ __forceinline__ void attn2_fix_block(KVT* kb, KVT* vb, const KVT* kgl
 }
 
 template <typename KVT, int HG, int HD>
-__global__ void __launch_bounds__(ATTN_THREADS, 1) k_attn2(const AttnArgs a) {
+__global__ void __launch_bounds__(ATTN_THREADS, 1) k_attn2(__grid_constant__ const AttnArgs a) {
 	constexpr int NW = ATTN_THREADS / 32, KS = HD / 16, NVW = HD / 16, REC = HD + 2;
 	static_assert((HG == 2 || HG == 4 || HG == 8) && (HD == 64 || HD == 128) && NVW <= NW, "unsupported attention shape");
 	extern __shared__ __align__(128) unsigned char smem_raw[];

@@ -118,58 +118,6 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
 	return p;
 }
 
-// ---------------------------------------------------------------- L2 prefetch schedule
-// Every stage kernel of a token can be handed byte ranges that LATER kernels of the same token will stream
-// (weights are immutable; the KV prefix of a layer only gains the slot k_qkv writes).  One lane per warp turns
-// its share into cp.async.bulk.prefetch.L2 requests, so HBM keeps streaming while this kernel is in a phase
-// that leaves it idle (activation staging, reductions, attention arithmetic, tails), and the consumer finds its
-// first bytes in the 50 MB L2 instead of paying a DRAM round trip behind a kernel boundary.
-#define PF_RANGES 3
-#define PF_CHUNK 8192
-struct Prefetch {
-	const void* p[PF_RANGES];
-	unsigned long long bytes[PF_RANGES]; // multiples of 16
-	// KV prefix of one layer: K and V are [heads][seq_len][rowbytes]; kv_len rows per head are requested
-	const void* kc;
-	const void* vc;
-	int kv_rowbytes, kv_heads;
-	unsigned long long kv_head_stride; // bytes
-};
-
-__device__ __forceinline__ void prefetch_ranges(const Prefetch& pf) {
-	if ((threadIdx.x & 31) != 0) return;
-	const unsigned nw = gridDim.x * (blockDim.x >> 5);
-	unsigned gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-#pragma unroll
-	for (int r = 0; r < PF_RANGES; ++r) {
-		const unsigned long long bytes = pf.bytes[r];
-		if (bytes == 0) continue;
-		const unsigned nchunks = (unsigned)((bytes + PF_CHUNK - 1) / PF_CHUNK);
-		for (unsigned c = gw; c < nchunks; c += nw) {
-			const unsigned long long off = (unsigned long long)c * PF_CHUNK;
-			const unsigned long long left = bytes - off;
-			l2_prefetch((const char*)pf.p[r] + off, (uint32_t)(left < PF_CHUNK ? left : PF_CHUNK));
-		}
-		gw = (gw + nw - nchunks % nw) % nw; // the next range starts where this one stopped
-	}
-}
-
-__device__ __forceinline__ void prefetch_kv(const Prefetch& pf, int kv_len) {
-	if (pf.kc == nullptr || (threadIdx.x & 31) != 0 || (pf.kv_rowbytes & 15)) return; // bulk requests are 16-byte granular
-	const unsigned nw = gridDim.x * (blockDim.x >> 5);
-	const unsigned gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-	const unsigned long long per_head = (unsigned long long)kv_len * pf.kv_rowbytes; // multiple of 16 (head_dim % 8 == 0)
-	const unsigned cph = (unsigned)((per_head + PF_CHUNK - 1) / PF_CHUNK);
-	const unsigned total = 2u * pf.kv_heads * cph;
-	for (unsigned c = gw; c < total; c += nw) {
-		const unsigned which = c / (pf.kv_heads * cph), rem = c % (pf.kv_heads * cph);
-		const unsigned h = rem / cph, k = rem % cph;
-		const unsigned long long off = (unsigned long long)k * PF_CHUNK, left = per_head - off;
-		const char* base = (const char*)(which ? pf.vc : pf.kc) + h * pf.kv_head_stride + off;
-		l2_prefetch(base, (uint32_t)(left < PF_CHUNK ? left : PF_CHUNK));
-	}
-}
-
 // ---------------------------------------------------------------- in-kernel stage stamps (perf_cuda)
 // The reference times its stages INSIDE the running kernel with %globaltimer (infer.cu:390-402) so that the
 // table describes the production path.  Same here: when a kernel is handed a stamp slot, one thread per CTA

@@ -58,8 +58,7 @@ struct Engine {
 
 	// attention launch shape
 	int attn_hg = 1, attn_qgroups = 1, attn_nsplit = 1, attn_lpp = 1;
-	// TMA-ring matvec kernels (ring.cuh): slots per warp / CTAs per SM for FFN-up and for wo / w2; u = 512-byte units per row and chunk (0: not used)
-	int ring_up_ns = 2, ring_up_cps = 2, ring_res_ns = 2, ring_res_warps = 16; // best of the H100 sweep in profiles/README.md
+	// TMA-ring matvec kernels (ring.cuh): u = 512-byte units per row and chunk (0: not used)
 	int ring_up_u = 0, ring_wo_u = 0, ring_down_u = 0, ring_wo_s = 1, ring_down_s = 1;
 	int grid_up_ring = 0, grid_wo_ring = 0, grid_down_ring = 0;
 	size_t smem_up_ring = 0, smem_wo_ring = 0, smem_down_ring = 0;
@@ -72,18 +71,6 @@ struct Engine {
 	size_t smem_dim = 0, smem_qdim = 0, smem_hidden = 0;
 	int cur_kv_len = 0; // host copy, for the perf table only
 	int cur_pos = 0;
-	int attn_nsplit_cap = 1 << 30;
-
-	// L2 prefetch schedule (common.cuh Prefetch): what each stage requests for the stages after it.  Bytes, or flags.
-	// Off by default: on an H100 it did not beat "off" (profiles/README.md) -- the stage kernels are not waiting for DRAM behind
-	// their boundaries, and requests for later stages only compete with the running one; CALM_B200_PF keeps the experiment.
-	bool pf_kv = false;           // k_qkv / w2 request the KV prefix the next attention kernel reads
-	bool pf_attn_wo = false;      // k_attn requests wo
-	size_t pf_attn_up = 0;        // ... and this much of w1 + w3
-	size_t pf_wo_up = 0;          // wo requests this much more of w1 + w3
-	size_t pf_up_down = 0;        // k_ffn_up requests this much of w2
-	bool pf_down_qkv = false;     // w2 requests the next layer's wq / wk / wv
-
 
 	// tensor parallelism (staged engine): this process owns 1/tp_world of the heads and of the FFN rows
 	int tp_rank = 0, tp_world = 1;
@@ -112,7 +99,6 @@ struct Engine {
 	float* sample_prob = nullptr;
 	bool use_graph = true;
 	bool use_pdl = true;
-	int carveout = -1;   // cudaFuncAttributePreferredSharedMemoryCarveout applied to every kernel of the token, or -1
 
 	// profiling (perf_cuda): in-kernel %globaltimer stamps per launch of the production graph (stages.cuh stamp_begin/end)
 	bool perf = false;
@@ -299,35 +285,10 @@ void tp_fill(TpExchange& t, int idx) {
 
 // Launch on the library's stream with programmatic stream serialization (PDL), so that consecutive kernels
 // of a token overlap their launch latency (the kernels order themselves with griddepcontrol.wait).
-// One L1 / shared-memory split for every kernel of the token (env CALM_B200_CARVEOUT = percent of shared memory, unset:
-// the driver picks per kernel): kernels whose preferred splits differ cannot be co-resident on an SM, which serialises
-// exactly the hand-over that programmatic dependent launch is there to overlap.
-void same_carveout(const void* kernel) {
-	if (g.carveout < 0) return;
-	static std::vector<const void*> done;
-	for (const void* k : done)
-		if (k == kernel) return;
-	done.push_back(kernel);
-	CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, g.carveout));
-}
-
 template <typename... KArgs, typename... Args>
-void launch_pdl(void (*kernel)(KArgs...), int grid, int block, size_t smem, Args... args) {
-	same_carveout((const void*)kernel);
+void launch_pdl(void (*kernel)(KArgs...), dim3 grid, int block, size_t smem, Args... args) {
 	cudaLaunchConfig_t cfg = {};
-	cfg.gridDim = dim3(grid), cfg.blockDim = dim3(block), cfg.dynamicSmemBytes = smem, cfg.stream = g.stream;
-	cudaLaunchAttribute at[1];
-	at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-	at[0].val.programmaticStreamSerializationAllowed = g.use_pdl ? 1 : 0;
-	cfg.attrs = at, cfg.numAttrs = 1;
-	CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, args...));
-}
-
-template <typename... KArgs, typename... Args>
-void launch_pdl_grid(void (*kernel)(KArgs...), dim3 grid, int block, Args... args) {
-	same_carveout((const void*)kernel);
-	cudaLaunchConfig_t cfg = {};
-	cfg.gridDim = grid, cfg.blockDim = dim3(block), cfg.dynamicSmemBytes = 0, cfg.stream = g.stream;
+	cfg.gridDim = grid, cfg.blockDim = dim3(block), cfg.dynamicSmemBytes = smem, cfg.stream = g.stream;
 	cudaLaunchAttribute at[1];
 	at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
 	at[0].val.programmaticStreamSerializationAllowed = g.use_pdl ? 1 : 0;
@@ -439,47 +400,18 @@ void dispatch_attn(const AttnArgs& a, int nunits, int* nl) {
 	}
 }
 
-// ring kernels are instantiated for U in {2, 4} (1 KB / 2 KB per row and chunk) and NS in {2, 3, 4}
-template <int DBITS, int U, int NS>
-void ring_up_launch(const FfnUpArgs& a, bool attr_only) {
-	if (attr_only) return smem_optin(k_ffn_up_ring<DBITS, U, NS>, g.smem_up_ring);
-	launch_pdl(k_ffn_up_ring<DBITS, U, NS>, g.grid_up_ring, 256, g.smem_up_ring, a);
-}
-template <int DBITS, int U, int NS>
-void ring_res_launch(const MatResArgs& a, int S, int grid, size_t smem, bool attr_only) {
-	if (attr_only) return smem_optin(k_matres_ring<DBITS, U, NS>, smem);
-	launch_pdl(k_matres_ring<DBITS, U, NS>, grid, g.ring_res_warps * 32, smem, a, S);
-}
+// ring kernels are instantiated for u in {2, 4} (1 KB / 2 KB per row and chunk)
 template <int DBITS>
 void ring_up_dispatch(const FfnUpArgs& a, bool attr_only) {
-	switch (g.ring_up_u * 10 + g.ring_up_ns) {
-	case 22: return ring_up_launch<DBITS, 2, 2>(a, attr_only);
-	case 23: return ring_up_launch<DBITS, 2, 3>(a, attr_only);
-	case 24: return ring_up_launch<DBITS, 2, 4>(a, attr_only);
-	case 42: return ring_up_launch<DBITS, 4, 2>(a, attr_only);
-	case 43: return ring_up_launch<DBITS, 4, 3>(a, attr_only);
-	default: return ring_up_launch<DBITS, 4, 4>(a, attr_only);
-	}
+	auto kernel = g.ring_up_u == 2 ? k_ffn_up_ring<DBITS, 2> : k_ffn_up_ring<DBITS, 4>;
+	if (attr_only) return smem_optin(kernel, g.smem_up_ring);
+	launch_pdl(kernel, g.grid_up_ring, RING_UP_WARPS * 32, g.smem_up_ring, a);
 }
 template <int DBITS>
 void ring_res_dispatch(const MatResArgs& a, int u, int S, int grid, size_t smem, bool attr_only) {
-	switch (u * 10 + g.ring_res_ns) {
-	case 22: return ring_res_launch<DBITS, 2, 2>(a, S, grid, smem, attr_only);
-	case 23: return ring_res_launch<DBITS, 2, 3>(a, S, grid, smem, attr_only);
-	case 24: return ring_res_launch<DBITS, 2, 4>(a, S, grid, smem, attr_only);
-	case 42: return ring_res_launch<DBITS, 4, 2>(a, S, grid, smem, attr_only);
-	case 43: return ring_res_launch<DBITS, 4, 3>(a, S, grid, smem, attr_only);
-	default: return ring_res_launch<DBITS, 4, 4>(a, S, grid, smem, attr_only);
-	}
-}
-
-// first `budget` bytes of the (w1, w3) row interleave that k_ffn_up walks: half from each matrix (row prefixes)
-static void pf_up_prefix(Prefetch& pf, int slot, const void* w1, const void* w3, size_t skip, size_t budget, size_t matrix_bytes) {
-	size_t off = (skip / 2) & ~(size_t)15, len = (budget / 2) & ~(size_t)15;
-	if (off >= matrix_bytes) return;
-	if (off + len > matrix_bytes) len = matrix_bytes - off;
-	pf.p[slot] = (const char*)w1 + off, pf.bytes[slot] = len;
-	pf.p[slot + 1] = (const char*)w3 + off, pf.bytes[slot + 1] = len;
+	auto kernel = u == 2 ? k_matres_ring<DBITS, 2> : k_matres_ring<DBITS, 4>;
+	if (attr_only) return smem_optin(kernel, smem);
+	launch_pdl(kernel, grid, RING_RES_WARPS * 32, smem, a, S);
 }
 
 // mode: 0 kv only, 1 logits -> host, 2 logits -> device + advance (greedy loop), 3 logits -> host + argmax, 4 logits -> device + min-p sample + advance
@@ -492,16 +424,6 @@ int run_token(int mode) {
 	int nl = 0;
 	g.n_stamps = 0;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * hd; // elements per layer
-	const size_t qkv_bytes[3] = {(size_t)g.q_dim * dim * wb / 8, (size_t)g.kv_dim * dim * wb / 8, (size_t)g.kv_dim * dim * wb / 8};
-	const size_t wo_bytes = (size_t)dim * g.q_dim * wb / 8, up_bytes = (size_t)hidden * dim * wb / 8 /* per matrix (and expert) */, down_bytes = up_bytes;
-	const bool dense = c.n_experts == 0;
-	auto kv_prefix = [&](Prefetch& pf, int l) {
-		pf.kc = (KVT*)g.kc + l * kv_layer, pf.vc = (KVT*)g.vc + l * kv_layer;
-		pf.kv_rowbytes = hd * (int)sizeof(KVT), pf.kv_heads = c.n_kv_heads, pf.kv_head_stride = (unsigned long long)c.seq_len * hd * sizeof(KVT);
-	};
-	auto qkv_weights = [&](Prefetch& pf, int l) {
-		pf.p[0] = w.wq[l], pf.bytes[0] = qkv_bytes[0], pf.p[1] = w.wk[l], pf.bytes[1] = qkv_bytes[1], pf.p[2] = w.wv[l], pf.bytes[2] = qkv_bytes[2];
-	};
 
 	{
 		StageScope t(ST_EMBED, 0);
@@ -511,7 +433,6 @@ int run_token(int mode) {
 		a.key_cache = (KVT*)g.kc, a.rope_freq = g.rope_freq, a.rope_cs = g.rope_cs;
 		a.n_layers = c.n_layers, a.n_kv_heads = c.n_kv_heads, a.head_dim = hd, a.seq_len = c.seq_len;
 		a.stamp = nullptr, a.stamp_reset = g.perf ? g.stamps : nullptr, a.n_stamps = MAX_STAMPS + 8; // + the 16 debug stamps
-		if (g.pf_down_qkv) qkv_weights(a.pf, 0);
 		launch_pdl(k_embed<DBITS, KVT>, a.embed_blocks + 8, 256, 0, a);
 		++nl;
 	}
@@ -526,7 +447,6 @@ int run_token(int mode) {
 			a.dim = dim, a.q_dim = g.q_dim, a.kv_dim = g.kv_dim, a.head_dim = hd, a.seq_len = c.seq_len;
 			a.eps = c.norm_eps, a.clip = c.qkv_clip, a.ln = c.norm_ln;
 			a.stamp = t.slot;
-			if (g.pf_kv && (l == 0 || !g.pf_down_qkv)) kv_prefix(a.pf, l); // later layers: requested by the previous w2 kernel
 			launch_pdl(k_qkv<DBITS, KVT>, g.grid_qkv, QKV_THREADS, g.smem_dim, a);
 			++nl;
 		}
@@ -542,16 +462,13 @@ int run_token(int mode) {
 			a.cells = g.attn_cells, a.epoch_stride = (unsigned)c.n_layers + 1, a.epoch_idx = (unsigned)l + 1, a.err = g.dev_err;
 			a.dbg = (g.perf && l == c.n_layers / 2) ? g.stamps + 2 * (size_t)MAX_STAMPS : nullptr;
 			a.stamp = t.slot;
-			if (g.pf_attn_wo) a.pf.p[0] = w.wo[l], a.pf.bytes[0] = wo_bytes;
-			if (dense && g.pf_attn_up) pf_up_prefix(a.pf, 1, w.w1[l], w.w3[l], 0, g.pf_attn_up, up_bytes);
 			dispatch_attn<KVT>(a, c.n_kv_heads * g.attn_qgroups, &nl);
 		}
 		{
 			StageScope t(ST_WO, (double)dim * g.q_dim * wb / 8);
 			MatResArgs a = {};
-			a.xin = g.att, a.w = w.wo[l], a.y = g.x, a.sel = nullptr, a.n = g.q_dim, a.d = dim, a.nact = 1, a.accumulate = 1, a.tp = g.tp;
+			a.xin = g.att, a.w = w.wo[l], a.y = g.x, a.sel = nullptr, a.n = g.q_dim, a.d = dim, a.nact = 1, a.accumulate = 1;
 			a.stamp = t.slot;
-			if (dense && g.pf_wo_up) pf_up_prefix(a.pf, 0, w.w1[l], w.w3[l], g.pf_attn_up, g.pf_wo_up, up_bytes);
 			if (g.tp_fused) tp_fill(a.tpx, 2 * l); // partial over this rank's heads, summed over the ranks in the kernel
 			else if (g.tp_world > 1) a.y = g.xpart, a.accumulate = 0;
 			if (g.ring_wo_u) ring_res_dispatch<DBITS>(a, g.ring_wo_u, g.ring_wo_s, g.grid_wo_ring, g.smem_wo_ring, false);
@@ -572,22 +489,16 @@ int run_token(int mode) {
 			a.eps = c.norm_eps, a.ln = c.norm_ln, a.gelu = c.act_gelu;
 			a.expert_stride = g.up_expert_stride;
 			a.stamp = t.slot;
-			if (dense && g.pf_up_down) a.pf.p[0] = w.w2[l], a.pf.bytes[0] = (g.pf_up_down < down_bytes ? g.pf_up_down : down_bytes) & ~(size_t)15;
-			bool done = false;
-			if (g.ring_up_u) ring_up_dispatch<DBITS>(a, false), done = true;
-			if (!done) launch_pdl(k_ffn_up<DBITS>, g.grid_up, 256, g.smem_dim, a);
+			if (g.ring_up_u) ring_up_dispatch<DBITS>(a, false);
+			else launch_pdl(k_ffn_up<DBITS>, g.grid_up, 256, g.smem_dim, a);
 			++nl;
 		}
 		{
 			StageScope t(ST_FFN_DOWN, (double)g.nact * hidden * dim * wb / 8);
 			MatResArgs a = {};
 			a.xin = g.hb, a.w = w.w2[l], a.y = g.x, a.sel = c.n_experts ? g.moe_sel : nullptr;
-			a.n = hidden, a.d = dim, a.nact = g.nact, a.accumulate = 1, a.tp = g.tp;
+			a.n = hidden, a.d = dim, a.nact = g.nact, a.accumulate = 1;
 			a.stamp = t.slot;
-			if (l + 1 < c.n_layers && g.pf_down_qkv) {
-				qkv_weights(a.pf, l + 1);
-				if (g.pf_kv) kv_prefix(a.pf, l + 1);
-			}
 			if (g.tp_fused) tp_fill(a.tpx, 2 * l + 1); // partial over this rank's FFN rows
 			else if (g.tp_world > 1) a.y = g.xpart, a.accumulate = 0;
 			if (g.ring_down_u) ring_res_dispatch<DBITS>(a, g.ring_down_u, g.ring_down_s, g.grid_down_ring, g.smem_down_ring, false);
@@ -710,8 +621,7 @@ void make_plan() {
 		// k_attn2 when the shape is instantiated and the CTA's share of the context fits in shared memory
 		g.attn_nbmax = cdiv(cdiv(c.seq_len, ATTN2_BP), g.attn_nsplit);
 		g.attn2_smem = attn2_smem_bytes<KVT>(g.attn_hg, c.head_dim, g.attn_nbmax);
-		const bool want = !(getenv("CALM_B200_ATTN2") && atoi(getenv("CALM_B200_ATTN2")) == 0);
-		g.attn2 = want && attn2_shape_ok(g.attn_hg, g.attn_lpp, c.head_dim) && g.attn_nbmax <= ATTN2_MAXB && g.attn2_smem <= 200 * 1024;
+		g.attn2 = attn2_shape_ok(g.attn_hg, g.attn_lpp, c.head_dim) && g.attn_nbmax <= ATTN2_MAXB && g.attn2_smem <= 200 * 1024;
 		AttnArgs aa = {};
 		aa.head_dim = c.head_dim, aa.nsplit = g.attn_nsplit;
 		dispatch_attn<KVT>(aa, c.n_kv_heads * g.attn_qgroups, nullptr);
@@ -727,22 +637,16 @@ void make_plan() {
 	g.grid_up = imin(max_ctas(k_ffn_up<DBITS>, 256, g.smem_dim), cdiv(g.nact * c.hidden_dim, 8));
 	// TMA-ring kernels for the dense single-GPU stages whose rows are whole 1 KB / 2 KB chunks (ring.cuh)
 	g.ring_up_u = g.ring_wo_u = g.ring_down_u = 0;
-	{ // weights are read once per token: L2::evict_first on the ring's bulk copies
-		const int hint = getenv("CALM_B200_RING_HINT") ? atoi(getenv("CALM_B200_RING_HINT")) : 1;
-		CUDA_CHECK(cudaMemcpyToSymbol(d_ring_l2_hint, &hint, sizeof(int)));
-	}
-	if (const char* e = getenv("CALM_B200_RING")) sscanf(e, "%d,%d,%d,%d", &g.ring_up_ns, &g.ring_up_cps, &g.ring_res_ns, &g.ring_res_warps); // 0 slots: stage not ring-fed
-	const bool ring_ok = c.n_experts == 0; // MoE: the expert rows are known only after the router
-	const bool ring_up_on = ring_ok && g.ring_up_ns >= 2 && g.ring_up_ns <= RING_MAX_NS; // (row shards of w1 / w3 under tensor parallelism are fine)
-	const bool ring_res_on = ring_ok && (g.tp_world == 1 || g.tp_fused) /* the ring kernels carry the in-kernel exchange too */ && g.ring_res_ns >= 2 && g.ring_res_ns <= RING_MAX_NS && (g.ring_res_warps == 8 || g.ring_res_warps == 16); // (gf4 too)
+	const bool ring_up_on = c.n_experts == 0; // MoE: the expert rows are known only after the router (row shards of w1 / w3 under tensor parallelism are fine)
+	const bool ring_res_on = ring_up_on && (g.tp_world == 1 || g.tp_fused); // the ring kernels carry the in-kernel exchange too (gf4 too)
 	auto chunk_units = [](size_t rowbytes) { return rowbytes % 2048 == 0 ? 4 : (rowbytes % 1024 == 0 ? 2 : 0); };
 	if (ring_up_on) {
 		const int u = chunk_units((size_t)c.dim * DBITS / 8);
 		if (u) {
-			g.smem_up_ring = ring_smem_bytes<DBITS>(c.dim, u, g.ring_up_ns, 8);
+			g.smem_up_ring = ring_smem_bytes<DBITS>(c.dim, u, RING_UP_WARPS);
 			if (g.smem_up_ring <= 200 * 1024) {
 				g.ring_up_u = u;
-				g.grid_up_ring = imin(g.sms * imin(g.ring_up_cps, (int)(220 * 1024 / g.smem_up_ring)), c.hidden_dim);
+				g.grid_up_ring = imin(g.sms * imin(2, (int)(220 * 1024 / g.smem_up_ring)), c.hidden_dim); // two CTAs per SM where they fit
 				if (g.grid_up_ring < 1) g.grid_up_ring = 1;
 				FfnUpArgs fa = {};
 				ring_up_dispatch<DBITS>(fa, true);
@@ -753,12 +657,11 @@ void make_plan() {
 		auto plan_res = [&](int n, int& u_out, int& s_out, int& grid_out, size_t& smem_out) {
 			const size_t rowbytes = (size_t)n * DBITS / 8;
 			int u = chunk_units(rowbytes);
-			if (u == 4 && getenv("CALM_B200_RING_RES_U") && atoi(getenv("CALM_B200_RING_RES_U")) == 2) u = 2; // (experiments) 1 KB chunks
 			if (!u) return;
-			size_t smem = ring_smem_bytes<DBITS>(n, u, g.ring_res_ns, g.ring_res_warps);
-			if (smem > 220 * 1024 && u == 4) u = 2, smem = ring_smem_bytes<DBITS>(n, u, g.ring_res_ns, g.ring_res_warps); // long activation vectors (70B w2: 112 KB): 1 KB chunks
+			size_t smem = ring_smem_bytes<DBITS>(n, u, RING_RES_WARPS);
+			if (smem > 220 * 1024 && u == 4) u = 2, smem = ring_smem_bytes<DBITS>(n, u, RING_RES_WARPS); // long activation vectors (70B w2: 112 KB): 1 KB chunks
 			if (smem > 220 * 1024) return;
-			const int grid = imin(g.sms * imin(16 / g.ring_res_warps, (int)(224 * 1024 / smem)), c.dim / 2);
+			const int grid = imin(g.sms, c.dim / 2); // one CTA per SM
 			const int cpt = (int)(rowbytes / (u * 512));
 			if (g.tp_world > 1 && cdiv(c.dim / 2, grid) + 1 > RING_MAX_PAIRS) return; // the exchange keeps a CTA's rows in shared memory
 			const bool split = cdiv(c.dim / 2, grid) + 1 <= RING_MAX_PAIRS && cpt <= RING_MAX_SLICES; // K-slices of one chunk, folded in shared memory
@@ -840,7 +743,6 @@ void launch_token(int mode) {
 void set_params(int token, int pos, int step) {
 	g.cur_kv_len = pos >= g.cfg.seq_len ? g.cfg.seq_len : pos + 1;
 	g.cur_pos = pos;
-	same_carveout((const void*)k_set_params);
 	k_set_params<<<1, 1, 0, g.stream>>>(g.tp, token, pos, g.cfg.seq_len, step);
 	++g_launches;
 }
@@ -913,18 +815,12 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 	g.q_dim = q_dim, g.kv_dim = kv_dim, g.kv_mul = g.cfg.n_heads / g.cfg.n_kv_heads;
 	g.use_graph = !(getenv("CALM_B200_GRAPH") && atoi(getenv("CALM_B200_GRAPH")) == 0);
 	g.use_pdl = !(getenv("CALM_B200_PDL") && atoi(getenv("CALM_B200_PDL")) == 0);
-	g.carveout = getenv("CALM_B200_CARVEOUT") ? atoi(getenv("CALM_B200_CARVEOUT")) : -1;
 	g.debug = getenv("CALM_B200_DEBUG") && atoi(getenv("CALM_B200_DEBUG"));
 	if (g.debug) g.use_graph = false;
 	g.perf = (getenv("CALM_B200_PERF") && atoi(getenv("CALM_B200_PERF"))) || getenv("CUDA_INJECTION64_PATH");
 	if (getenv("CALM_B200_PERF") && atoi(getenv("CALM_B200_PERF"))) { // the reference driver only calls perf_cuda under a CUPTI injection (run.c:630): print at exit
 		static bool registered = false;
 		if (!registered) atexit(perf_cuda), registered = true;
-	}
-	if (const char* e = getenv("CALM_B200_PF")) { // kv,attn_wo,attn_up_MB,wo_up_MB,up_down_MB,down_qkv  (experiments; defaults in struct Engine)
-		int kv = 0, awo = 0, aup = 0, wup = 0, ud = 0, dq = 0;
-		sscanf(e, "%d,%d,%d,%d,%d,%d", &kv, &awo, &aup, &wup, &ud, &dq);
-		g.pf_kv = kv != 0, g.pf_attn_wo = awo != 0, g.pf_attn_up = (size_t)aup << 20, g.pf_wo_up = (size_t)wup << 20, g.pf_up_down = (size_t)ud << 20, g.pf_down_qkv = dq != 0;
 	}
 
 	CUDA_CHECK(cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking));
@@ -975,14 +871,13 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 	g.attn_lpp = 1;
 	while (g.attn_lpp * 8 < c.head_dim) g.attn_lpp *= 2;
 	int units = c.n_kv_heads * g.attn_qgroups;
-	const int split_mul = getenv("CALM_B200_ATTN_SPLIT_MUL") ? atoi(getenv("CALM_B200_ATTN_SPLIT_MUL")) : 1; // CTAs per SM (experiments)
-	int want = (split_mul > 1 ? split_mul : 1) * g.sms / units; // about one 256-thread CTA per SM
+	int want = g.sms / units; // about one 256-thread CTA per SM
 	int maxsplit = cdiv(c.seq_len, 64);                 // at least 64 positions per slice at full context
 	g.attn_nsplit = want < 1 ? 1 : (want > maxsplit ? maxsplit : want);
 	if (g.attn_nsplit > ATTN2_MAXB + 4) g.attn_nsplit = ATTN2_MAXB + 4; // k_attn2 keeps one (m, l) pair per slice in static shared memory
 	g.attn_partial = (float*)dev_alloc((size_t)units * g.attn_nsplit * g.attn_hg * (c.head_dim + 2) * sizeof(float));
 	{
-		const size_t cell_bytes = (size_t)units * (g.sms / units > g.attn_nsplit ? g.sms / units : g.attn_nsplit) * g.attn_hg * (c.head_dim + 2) * sizeof(unsigned long long);
+		const size_t cell_bytes = (size_t)units * g.attn_nsplit * g.attn_hg * (c.head_dim + 2) * sizeof(unsigned long long);
 		// (the attention grid must be co-resident for the cell fold: units * nsplit CTAs of <= 1/2 SM each)
 		g.attn_cells = (unsigned long long*)dev_alloc(cell_bytes);
 		CUDA_CHECK(cudaMemset(g.attn_cells, 0, cell_bytes));
@@ -992,12 +887,6 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 	g.attn_counter = (unsigned*)dev_alloc(units * sizeof(unsigned));
 	CUDA_CHECK(cudaMemset(g.attn_counter, 0, units * sizeof(unsigned)));
 
-	g.attn_nsplit_cap = g.attn_nsplit; // the partial buffer below is sized for this many slices
-	if (g.sms / units > g.attn_nsplit_cap) {
-		g.attn_nsplit_cap = g.sms / units;
-		CUDA_CHECK(cudaFree(g.attn_partial));
-		g.attn_partial = (float*)dev_alloc((size_t)units * g.attn_nsplit_cap * g.attn_hg * (c.head_dim + 2) * sizeof(float));
-	}
 	g.moe_sel = (MoeSel*)dev_alloc(sizeof(MoeSel));
 	CUDA_CHECK(cudaMemset(g.moe_sel, 0, sizeof(MoeSel)));
 	g.tp = (TokenParams*)dev_alloc(sizeof(TokenParams));
@@ -1007,6 +896,10 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 	case 16: make_plan_kv<16>(); break;
 	case 8: make_plan_kv<8>(); break;
 	default: make_plan_kv<4>(); break;
+	}
+	if (!getenv("CALM_B200_QUIET")) {
+		printf("# plan: attention %s, %d units x %d slices\n", g.attn2 ? "k_attn2" : "k_attn", units, g.attn_nsplit);
+		fflush(stdout);
 	}
 	g.cand_val = (float*)dev_alloc(g.ncand * sizeof(float));
 	g.cand_idx = (int*)dev_alloc(g.ncand * sizeof(int));
@@ -1279,30 +1172,23 @@ static void pf_reserve(int n) {
 static bool pf_supported() {
 	const Config& c = g.cfg;
 	return c.n_experts == 0 && g.tp_world == 1 && c.dim % PF_BM == 0 && g.q_dim % PF_BM == 0 && g.kv_dim % PF_BM == 0 && c.hidden_dim % PF_BM == 0 &&
-	       (c.head_dim == 64 || c.head_dim == 128) && !(getenv("CALM_B200_PREFILL") && atoi(getenv("CALM_B200_PREFILL")) == 0);
+	       (c.head_dim == 64 || c.head_dim == 128);
 }
 
 template <int MODE, int DBITS, typename KVT>
 static void pf_gemm(const CUtensorMap* tm, const PfGemmArgs& a, int rows, int n) {
 	static bool opted = false;
 	if (!opted) smem_optin(k_pf_gemm<MODE, DBITS, KVT>, pf_smem_bytes<MODE>()), opted = true;
-	same_carveout((const void*)k_pf_gemm<MODE, DBITS, KVT>);
-	cudaLaunchConfig_t cfg = {};
-	cfg.gridDim = dim3(rows / PF_BM, cdiv(n, PF_BN)), cfg.blockDim = dim3(PF_THREADS), cfg.dynamicSmemBytes = pf_smem_bytes<MODE>(), cfg.stream = g.stream;
-	cudaLaunchAttribute at[1];
-	at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-	at[0].val.programmaticStreamSerializationAllowed = g.use_pdl ? 1 : 0;
-	cfg.attrs = at, cfg.numAttrs = 1;
-	CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_pf_gemm<MODE, DBITS, KVT>, tm[0], tm[1], a));
+	launch_pdl(k_pf_gemm<MODE, DBITS, KVT>, dim3(rows / PF_BM, cdiv(n, PF_BN)), PF_THREADS, pf_smem_bytes<MODE>(), tm[0], tm[1], a);
 	++g_launches;
 }
 
 template <typename KVT, int HD>
 static void pf_attn(const PfAttnArgs& a, int n) {
 	const dim3 grid(cdiv(n, PFA_WARPS), g.cfg.n_kv_heads);
-	if (g.kv_mul % 4 == 0) launch_pdl_grid(k_pf_attn<KVT, HD, 4>, grid, PFA_WARPS * 32, a);
-	else if (g.kv_mul % 2 == 0) launch_pdl_grid(k_pf_attn<KVT, HD, 2>, grid, PFA_WARPS * 32, a);
-	else launch_pdl_grid(k_pf_attn<KVT, HD, 1>, grid, PFA_WARPS * 32, a);
+	if (g.kv_mul % 4 == 0) launch_pdl(k_pf_attn<KVT, HD, 4>, grid, PFA_WARPS * 32, 0, a);
+	else if (g.kv_mul % 2 == 0) launch_pdl(k_pf_attn<KVT, HD, 2>, grid, PFA_WARPS * 32, 0, a);
+	else launch_pdl(k_pf_attn<KVT, HD, 1>, grid, PFA_WARPS * 32, 0, a);
 	++g_launches;
 }
 

@@ -4,10 +4,11 @@
 // a warp requests one batch (8 x 16 B per lane), waits a DRAM round trip, consumes it, and only then requests the next --
 // so the bytes in flight per SM are duty-cycled, bounded by the register file, and nothing can be requested before the
 // dependency wait without costing a CTA of occupancy.  Here every warp owns a small ring of shared-memory slots that it
-// fills itself with cp.async.bulk (one elected lane, completion on the slot's mbarrier): requests run NS chunks ahead of
-// the arithmetic, continuously, across task boundaries, and the first NS chunks are requested BEFORE griddepcontrol.wait
-// (weights are immutable), i.e. while the previous kernel drains and the activation vector is staged.  There is no
-// producer warp and no CTA-wide hand-off: a warp waits only on its own mbarriers.
+// fills itself with cp.async.bulk (one elected lane, completion on the slot's mbarrier, L2::evict_first: every weight byte
+// is read once per token): requests run RING_NS chunks ahead of the arithmetic, continuously, across task boundaries, and
+// the first RING_NS chunks are requested BEFORE griddepcontrol.wait (weights are immutable), i.e. while the previous kernel
+// drains and the activation vector is staged.  There is no producer warp and no CTA-wide hand-off: a warp waits only on
+// its own mbarriers.  Slots per warp and warps per CTA are the best of the H100 sweep in profiles/README.md.
 //
 // Work split: one CTA owns a contiguous range of "tasks"; its warps take tasks from a shared-memory counter, so all warps
 // of an SM finish within one chunk of each other whatever the task count (the static row-pair stride of k_ffn_up costs a
@@ -23,36 +24,35 @@
 
 #include "stages.cuh"
 
-#define RING_MAX_WARPS 16 // warps per CTA: 8 (two CTAs per SM) or 16 (one CTA per SM when the activation vector is long: w2)
-#define RING_MAX_NS 4
+#define RING_NS 2         // slots per warp
+#define RING_UP_WARPS 8   // FFN up: two CTAs of 8 warps per SM
+#define RING_RES_WARPS 16 // wo / w2: one CTA of 16 warps per SM (the activation vector is long: w2)
 #define RING_MAX_PAIRS 48 // row pairs per CTA when K-slices are folded through shared memory
 #define RING_MAX_SLICES 32
 
-__device__ int d_ring_l2_hint = 1; // 1: weights are requested with L2::evict_first (read once per token); 0: default policy (experiments)
-
 struct RingCtl {
-	uint64_t bar[RING_MAX_WARPS][RING_MAX_NS];
-	int slot_task[RING_MAX_WARPS][RING_MAX_NS];
-	int slot_piece[RING_MAX_WARPS][RING_MAX_NS];
+	uint64_t bar[RING_RES_WARPS][RING_NS];
+	int slot_task[RING_RES_WARPS][RING_NS];
+	int slot_piece[RING_RES_WARPS][RING_NS];
 	int ctr; // next task of this CTA
 };
 
-// shared memory of a ring kernel: [32 floats block-reduce][activation vector][ring: warps x NS x 2 rows x CH bytes]
+// shared memory of a ring kernel: [32 floats block-reduce][activation vector][ring: warps x RING_NS x 2 rows x CH bytes]
 template <int DBITS>
-__host__ __device__ inline size_t ring_smem_bytes(int n, int u, int ns, int warps) {
+__host__ __device__ inline size_t ring_smem_bytes(int n, int u, int warps) {
 	size_t xs = ((size_t)(32 + xs_all_floats<DBITS>(n)) * sizeof(float) + 127) & ~(size_t)127;
-	return xs + (size_t)warps * ns * 2 * u * 512;
+	return xs + (size_t)warps * RING_NS * 2 * u * 512;
 }
 
 // The streaming loop of one warp.  rows(task, rp0, rp1, chunk0): byte pointers of the task's two rows and its first chunk
 // index inside the row; done(task, v0, v1): the two finished dot products (called by every lane, values valid in all).
 // issue_prologue() must be called (warp-uniformly) before consume_all(); in between the caller waits for the previous grid
 // and stages the activation vector.
-template <int DBITS, int U, int NS, typename RowsFn, typename DoneFn>
+template <int DBITS, int U, typename RowsFn, typename DoneFn>
 struct RingWarp {
 	static constexpr int CH = U * 512; // bytes per row and chunk
 	RingCtl* ctl;
-	unsigned char* ring; // this warp's NS slots
+	unsigned char* ring; // this warp's RING_NS slots
 	int warp, lane;
 	int t_hi, S; // end of the CTA's task range; chunks per task
 	uint64_t policy;
@@ -63,8 +63,8 @@ struct RingWarp {
 
 	__device__ __forceinline__ RingWarp(RingCtl* c, unsigned char* ring_base, int t_hi_, int S_, RowsFn r, DoneFn d)
 	    : ctl(c), warp(threadIdx.x >> 5), lane(threadIdx.x & 31), t_hi(t_hi_), S(S_), rows(r), done(d) {
-		ring = ring_base + (size_t)warp * NS * 2 * CH;
-		policy = d_ring_l2_hint ? l2_policy_evict_first() : 0;
+		ring = ring_base + (size_t)warp * RING_NS * 2 * CH;
+		policy = l2_policy_evict_first();
 		cur_piece = S; // forces a task grab
 	}
 
@@ -79,7 +79,7 @@ struct RingWarp {
 			}
 			cur_task = t, cur_piece = 0;
 		}
-		const int slot = issued % NS;
+		const int slot = issued % RING_NS;
 		if (lane == 0) {
 			const unsigned char *rp0, *rp1;
 			int chunk0;
@@ -88,20 +88,15 @@ struct RingWarp {
 			ctl->slot_task[warp][slot] = cur_task, ctl->slot_piece[warp][slot] = cur_piece;
 			uint64_t* bar = &ctl->bar[warp][slot];
 			mbar_expect_tx(bar, 2 * CH);
-			if (policy) {
-				tma_load_1d_hint(ring + (size_t)slot * 2 * CH, rp0 + off, CH, bar, policy);
-				tma_load_1d_hint(ring + (size_t)slot * 2 * CH + CH, rp1 + off, CH, bar, policy);
-			} else {
-				tma_load_1d(ring + (size_t)slot * 2 * CH, rp0 + off, CH, bar);
-				tma_load_1d(ring + (size_t)slot * 2 * CH + CH, rp1 + off, CH, bar);
-			}
+			tma_load_1d_hint(ring + (size_t)slot * 2 * CH, rp0 + off, CH, bar, policy);
+			tma_load_1d_hint(ring + (size_t)slot * 2 * CH + CH, rp1 + off, CH, bar, policy);
 		}
 		++issued, ++cur_piece;
 	}
 
 	__device__ __forceinline__ void issue_prologue() {
 #pragma unroll
-		for (int i = 0; i < NS; ++i)
+		for (int i = 0; i < RING_NS; ++i)
 			if (more) issue_one();
 		__syncwarp();
 	}
@@ -111,8 +106,8 @@ struct RingWarp {
 		constexpr int Q = WFmt<DBITS>::VW / 4;
 		float acc0 = 0.f, acc1 = 0.f;
 		while (consumed < issued) {
-			const int slot = consumed % NS;
-			mbar_wait(&ctl->bar[warp][slot], (consumed / NS) & 1);
+			const int slot = consumed % RING_NS;
+			mbar_wait(&ctl->bar[warp][slot], (consumed / RING_NS) & 1);
 			const int task = ctl->slot_task[warp][slot], piece = ctl->slot_piece[warp][slot];
 			int chunk0;
 			{
@@ -147,10 +142,9 @@ struct RingWarp {
 	}
 };
 
-template <int NS>
 __device__ __forceinline__ void ring_init(RingCtl* ctl, int t_lo) {
 	if (threadIdx.x == 0) ctl->ctr = t_lo;
-	if (threadIdx.x < (blockDim.x >> 5) * NS) mbar_init(&ctl->bar[threadIdx.x / NS][threadIdx.x % NS], 1);
+	if (threadIdx.x < (blockDim.x >> 5) * RING_NS) mbar_init(&ctl->bar[threadIdx.x / RING_NS][threadIdx.x % RING_NS], 1);
 	if (threadIdx.x == 0) mbar_init_fence();
 	__syncthreads();
 }
@@ -158,8 +152,8 @@ __device__ __forceinline__ void ring_init(RingCtl* ctl, int t_lo) {
 // ------------------------------------------------------------------------------------------------
 // FFN up: hb[i] = act(w1[i] . xn) * (w3[i] . xn)   (reference infer.c:437-450); task i = rows (w1[i], w3[i]), whole rows.
 
-template <int DBITS, int U, int NS>
-__global__ void __launch_bounds__(256, 2) k_ffn_up_ring(const FfnUpArgs a) {
+template <int DBITS, int U>
+__global__ void __launch_bounds__(RING_UP_WARPS * 32, 2) k_ffn_up_ring(const FfnUpArgs a) {
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	__shared__ RingCtl ctl;
 	float* red = reinterpret_cast<float*>(smem_raw);
@@ -169,7 +163,7 @@ __global__ void __launch_bounds__(256, 2) k_ffn_up_ring(const FfnUpArgs a) {
 	const int cpt = (int)(rowbytes / (U * 512));
 	const int t_lo = (int)(((long long)blockIdx.x * a.hidden) / gridDim.x), t_hi = (int)(((long long)(blockIdx.x + 1) * a.hidden) / gridDim.x);
 	pdl_launch_next();
-	ring_init<NS>(&ctl, t_lo);
+	ring_init(&ctl, t_lo);
 	float post = 1.f;
 	const unsigned char* w1 = reinterpret_cast<const unsigned char*>(a.w1);
 	const unsigned char* w3 = reinterpret_cast<const unsigned char*>(a.w3);
@@ -182,8 +176,8 @@ __global__ void __launch_bounds__(256, 2) k_ffn_up_ring(const FfnUpArgs a) {
 			a.hb[t] = (a.gelu ? act_gelu(u1) : act_silu(u1)) * u3;
 		}
 	};
-	RingWarp<DBITS, U, NS, decltype(rows), decltype(done)> rw(&ctl, ring, t_hi, cpt, rows, done);
-	rw.issue_prologue(); // the first NS chunks of every warp are in flight before the previous kernel has finished
+	RingWarp<DBITS, U, decltype(rows), decltype(done)> rw(&ctl, ring, t_hi, cpt, rows, done);
+	rw.issue_prologue(); // the first RING_NS chunks of every warp are in flight before the previous kernel has finished
 	pdl_wait_prev();
 	stamp_begin(a.stamp);
 	post = stage_vector<DBITS>(xs, red, a.x, a.dim, a.normw, a.eps, a.ln != 0, nullptr);
@@ -195,8 +189,8 @@ __global__ void __launch_bounds__(256, 2) k_ffn_up_ring(const FfnUpArgs a) {
 // y[row] += W[row] . xin  (wo, w2; dense).  Task = (row pair p, K-slice s of S chunks), t = p * nsl + s; with nsl > 1 the
 // slices of a pair land in part[][] and the last one to arrive adds them up in slice order.
 
-template <int DBITS, int U, int NS>
-__global__ void __launch_bounds__(512, 1) k_matres_ring(const MatResArgs a, const int S) {
+template <int DBITS, int U>
+__global__ void __launch_bounds__(RING_RES_WARPS * 32, 1) k_matres_ring(const MatResArgs a, const int S) {
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	__shared__ RingCtl ctl;
 	__shared__ float2 part[RING_MAX_PAIRS][RING_MAX_SLICES];
@@ -211,7 +205,7 @@ __global__ void __launch_bounds__(512, 1) k_matres_ring(const MatResArgs a, cons
 	const int p_lo = (int)(((long long)blockIdx.x * npairs) / gridDim.x), p_hi = (int)(((long long)(blockIdx.x + 1) * npairs) / gridDim.x);
 	pdl_launch_next();
 	if (threadIdx.x < RING_MAX_PAIRS) cnt[threadIdx.x] = 0;
-	ring_init<NS>(&ctl, p_lo * nsl);
+	ring_init(&ctl, p_lo * nsl);
 	const unsigned char* w = reinterpret_cast<const unsigned char*>(a.w);
 	auto rows = [&](int t, const unsigned char*& rp0, const unsigned char*& rp1, int& chunk0) {
 		const int p = t / nsl, s = t - p * nsl;
@@ -238,7 +232,7 @@ __global__ void __launch_bounds__(512, 1) k_matres_ring(const MatResArgs a, cons
 		cur.x += v0, cur.y += v1;
 		*dst = cur;
 	};
-	RingWarp<DBITS, U, NS, decltype(rows), decltype(done)> rw(&ctl, ring, p_hi * nsl, S, rows, done);
+	RingWarp<DBITS, U, decltype(rows), decltype(done)> rw(&ctl, ring, p_hi * nsl, S, rows, done);
 	rw.issue_prologue();
 	pdl_wait_prev();
 	stamp_begin(a.stamp);

@@ -243,7 +243,6 @@ struct EmbedArgs {
 	unsigned long long* stamp; // perf_cuda: {min start, max end} of this launch, or NULL
 	unsigned long long* stamp_reset; // perf_cuda: all slots of the token, re-armed here
 	int n_stamps;
-	Prefetch pf;
 	// sinks
 	KVT* key_cache;
 	const float* rope_freq;
@@ -252,9 +251,7 @@ struct EmbedArgs {
 
 template <int DBITS, typename KVT>
 __global__ void k_embed(const EmbedArgs<KVT> a) {
-	pdl_launch_next();
-	prefetch_ranges(a.pf); // layer 0's first weights: nothing else is streaming yet
-	pdl_wait_prev();
+	pdl_enter();
 	if (a.stamp_reset) { // grid-stride: (start, end) = (max, 0); every later kernel of the token waits for this grid
 		for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < a.n_stamps; j += gridDim.x * blockDim.x) a.stamp_reset[2 * j] = ~0ull, a.stamp_reset[2 * j + 1] = 0ull;
 	}
@@ -307,7 +304,6 @@ struct QkvArgs {
 	float eps, clip;
 	int ln;
 	unsigned long long* stamp;
-	Prefetch pf;
 };
 
 // Before waiting for the previous kernel a warp asks the L2 for its first row pair (cp.async.bulk.prefetch.L2: no registers;
@@ -347,12 +343,10 @@ __global__ void __launch_bounds__(QKV_THREADS, 3) k_qkv(const QkvArgs<KVT> a) {
 		rows_of(p0, rp, j, k);
 		l2_prefetch_row(rp[0], nvec * 16), l2_prefetch_row(rp[1], nvec * 16);
 	}
-	prefetch_ranges(a.pf);
 	pdl_wait_prev();
 	stamp_begin(a.stamp);
 	const float post = stage_vector<DBITS>(xs, red, a.x, a.dim, a.normw, a.eps, a.ln != 0, blockIdx.x == 0 ? a.xb_out : nullptr);
 	const int kv_pos = a.tp->kv_pos;
-	prefetch_kv(a.pf, a.tp->kv_len); // this layer's cache prefix, for the attention kernel that follows
 
 	for (int p = p0; p < npairs; p += gridDim.x * nwarps) {
 		const uint4* rp[2];
@@ -412,7 +406,6 @@ struct AttnArgs {
 	int* err;                           // mapped host word for the fold's watchdog
 	unsigned long long* dbg;            // perf: 16 timestamps of CTA 0 / extremes over CTAs (first layer only), or NULL
 	unsigned long long* stamp;
-	Prefetch pf;
 };
 
 template <typename KVT>
@@ -563,24 +556,21 @@ __device__ __forceinline__ void attn_tail(const AttnArgs& a, int HG, int unit, i
 	if (threadIdx.x == 0) a.counter[unit] = 0;
 }
 
-// One work item, executed by all warps of the calling CTA.  The warps form `hsets` equal sets (1 or 2);
-// every set walks all positions of the slice and serves HH of the unit's HG query heads (set s: heads
-// s*HH ...), which halves the per-thread state when a CTA has many warps but few registers.
-// P positions per lane group are in flight; PIPE requests the next P before consuming the current ones.
+// One work item, executed by all warps of the calling CTA.  Every warp walks its share of the slice's positions
+// for HH of the unit's HG query heads.  P positions per lane group are in flight, and the next P are requested
+// before the current ones are consumed.
 // LPPC > 0 (compile-time lanes per position, with HH * P == LPPC) selects the transposing score path: the
 // HH * P partial dot products of a step are reduced across the lane group so that every lane ends up with
 // ONE complete score (15 shuffles instead of 64 for 16 lanes), evaluates its two exponentials once, and
 // the probabilities are broadcast back for the value accumulation.
-// scratch: shared, >= max((nwarps / hsets) * HG * (hd + 2), 2 * nsplit * HG) floats.  flag: shared int.
-template <typename KVT, int HH, int P, bool PIPE, int LPPC = 0>
-__device__ __forceinline__ void attn_item(const AttnArgs& a, int HG, int hsets, int unit, int split, int kv_len, float* scratch, int* flag) {
+// scratch: shared, >= max(nwarps * HG * (hd + 2), 2 * nsplit * HG) floats.  flag: shared int.
+template <typename KVT, int HH, int P, int LPPC = 0>
+__device__ __forceinline__ void attn_item(const AttnArgs& a, int HG, int unit, int split, int kv_len, float* scratch, int* flag) {
 	typedef typename KvRaw<KVT>::type raw_t;
 	const int kvh = unit / a.qgroups;
 	const int hbase = kvh * a.kv_mul + (unit % a.qgroups) * HG; // first query head of this unit
-	const int lane = threadIdx.x & 31, nwarps = (blockDim.x >> 5) / hsets;
-	const int wset = (threadIdx.x >> 5) / nwarps, warp = (threadIdx.x >> 5) % nwarps;
-	const int h0 = wset * HH;                  // first head (within the unit) of this warp
-	const int nh = max(0, min(HH, HG - h0));   // heads this warp really has
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+	const int nh = min(HH, HG); // heads this warp really has
 	const int hd = a.head_dim, lpp = a.lpp;
 	const int G = 32 / lpp; // position groups per warp
 	const int grp = lane / lpp, li = lane % lpp;
@@ -599,11 +589,11 @@ __device__ __forceinline__ void attn_item(const AttnArgs& a, int HG, int hsets, 
 #pragma unroll
 		for (int d = 0; d < 8; ++d) {
 			acc[h][d] = 0.f;
-			qr[h][d] = (dact && h < nh) ? __ldcg(a.q + (size_t)(hbase + h0 + h) * hd + li * 8 + d) : 0.f;
+			qr[h][d] = (dact && h < nh) ? __ldcg(a.q + (size_t)(hbase + h) * hd + li * 8 + d) : 0.f;
 		}
 	}
 
-	const int stride = nwarps * G; // positions per step over all groups of a warp set
+	const int stride = nwarps * G; // positions per step over all groups of the CTA
 	auto fetch = [&](int tw, raw_t (&kr)[P], raw_t (&vr)[P]) {
 #pragma unroll
 		for (int i = 0; i < P; ++i) {
@@ -717,26 +707,18 @@ __device__ __forceinline__ void attn_item(const AttnArgs& a, int HG, int hsets, 
 	};
 
 	// software pipeline over steps of stride * P positions (warp-uniform trip count: the shuffles above are full-warp)
-	if (PIPE) {
-		raw_t ka[P], va[P], kb[P], vb[P];
-		const int step = stride * P;
-		int tw = t0 + warp * G;
-		if (tw < t1) fetch(tw, ka, va);
-		while (tw < t1) {
-			if (tw + step < t1) fetch(tw + step, kb, vb);
-			update(tw, ka, va);
-			tw += step;
-			if (tw >= t1) break;
-			if (tw + step < t1) fetch(tw + step, ka, va);
-			update(tw, kb, vb);
-			tw += step;
-		}
-	} else {
-		raw_t ka[P], va[P];
-		for (int tw = t0 + warp * G; tw < t1; tw += stride * P) {
-			fetch(tw, ka, va);
-			update(tw, ka, va);
-		}
+	raw_t ka[P], va[P], kb[P], vb[P];
+	const int step = stride * P;
+	int tw = t0 + warp * G;
+	if (tw < t1) fetch(tw, ka, va);
+	while (tw < t1) {
+		if (tw + step < t1) fetch(tw + step, kb, vb);
+		update(tw, ka, va);
+		tw += step;
+		if (tw >= t1) break;
+		if (tw + step < t1) fetch(tw + step, ka, va);
+		update(tw, kb, vb);
+		tw += step;
 	}
 
 	if constexpr (LPPC > 0) { // running max / sum live in the lanes that own the head: hand them to every lane of the group
@@ -747,15 +729,13 @@ __device__ __forceinline__ void attn_item(const AttnArgs& a, int HG, int hsets, 
 		}
 	}
 
-	attn_tail<HH>(a, HG, unit, split, hbase, h0, nh, warp, nwarps, m, l, acc, scratch, flag);
+	attn_tail<HH>(a, HG, unit, split, hbase, 0, nh, warp, nwarps, m, l, acc, scratch, flag);
 }
 
 #define ATTN_THREADS 256
 template <typename KVT, int HG>
-__global__ void __launch_bounds__(ATTN_THREADS) k_attn(const AttnArgs a) {
-	pdl_launch_next();
-	prefetch_ranges(a.pf); // wo and the head of w1 / w3: HBM is nearly idle while this kernel runs
-	pdl_wait_prev();
+__global__ void __launch_bounds__(ATTN_THREADS) k_attn(__grid_constant__ const AttnArgs a) {
+	pdl_enter();
 	stamp_begin(a.stamp);
 	extern __shared__ __align__(16) float smem[];
 	__shared__ int flag;
@@ -764,14 +744,14 @@ __global__ void __launch_bounds__(ATTN_THREADS) k_attn(const AttnArgs a) {
 	bool done = false;
 	if constexpr (HG == 2 || HG == 4 || HG == 8) {
 		if (a.lpp == 16 && HG >= 4) {
-			attn_item<KVT, HG, 16 / HG, true, 16>(a, HG, 1, unit, split, kv_len, smem, &flag);
+			attn_item<KVT, HG, 16 / HG, 16>(a, HG, unit, split, kv_len, smem, &flag);
 			done = true;
 		} else if (a.lpp == 8) {
-			attn_item<KVT, HG, 8 / HG, true, 8>(a, HG, 1, unit, split, kv_len, smem, &flag);
+			attn_item<KVT, HG, 8 / HG, 8>(a, HG, unit, split, kv_len, smem, &flag);
 			done = true;
 		}
 	}
-	if (!done) attn_item<KVT, HG, (HG > 4 ? 2 : 4), true>(a, HG, 1, unit, split, kv_len, smem, &flag);
+	if (!done) attn_item<KVT, HG, (HG > 4 ? 2 : 4)>(a, HG, unit, split, kv_len, smem, &flag);
 	stamp_end(a.stamp);
 }
 
@@ -907,9 +887,7 @@ struct MatResArgs {
 	int n, d, nact;
 	int accumulate;   // 1: y += ..., 0: y = ...
 	TpExchange tpx;   // world > 1: the partial is summed over the tensor-parallel ranks inside this kernel
-	const TokenParams* tp;
 	unsigned long long* stamp;
-	Prefetch pf;
 };
 
 template <int DBITS>
@@ -930,10 +908,8 @@ __global__ void __launch_bounds__(256, 2) k_matres(const MatResArgs a) {
 		const uint4* r0 = reinterpret_cast<const uint4*>(a.w) + (size_t)(2 * p0) * nvec;
 		l2_prefetch_row(r0, nvec * 16), l2_prefetch_row(r0 + nvec, nvec * 16);
 	}
-	prefetch_ranges(a.pf);
 	pdl_wait_prev();
 	stamp_begin(a.stamp);
-	prefetch_kv(a.pf, a.tp->kv_len); // w2: the NEXT layer's cache prefix (same token: same length)
 
 	for (int e = 0; e < a.nact; ++e) {
 		if (e > 0) __syncthreads();
@@ -978,7 +954,6 @@ __global__ void __launch_bounds__(256, 2) k_matres(const MatResArgs a) {
 
 struct FfnUpArgs {
 	unsigned long long* stamp;
-	Prefetch pf;
 	const float* x;
 	const float* normw; // NULL: stage `x` as is (norm_par: x = saved attention-norm output)
 	const void* gate;   // router (n_experts, dim) or NULL
@@ -993,7 +968,7 @@ struct FfnUpArgs {
 };
 
 template <int DBITS>
-__global__ void __launch_bounds__(256, 3) k_ffn_up(const FfnUpArgs a) {
+__global__ void __launch_bounds__(256, 3) k_ffn_up(__grid_constant__ const FfnUpArgs a) {
 	pdl_launch_next();
 	extern __shared__ __align__(16) float smem[];
 	__shared__ float glog[64];
@@ -1013,7 +988,6 @@ __global__ void __launch_bounds__(256, 3) k_ffn_up(const FfnUpArgs a) {
 	pdl_wait_prev();
 	stamp_begin(a.stamp);
 	const float post = stage_vector<DBITS>(xs, red, a.x, a.dim, a.normw, a.eps, a.ln != 0, nullptr);
-	prefetch_ranges(a.pf); // w2 (dense models): behind this kernel's own first requests
 
 	if (a.n_experts) {
 		for (int e = warp; e < a.n_experts; e += nwarps) {

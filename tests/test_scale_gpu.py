@@ -48,19 +48,35 @@ def fill_oracle_cache(model, n_pos, seed, kvbits):
         dst[:, :n_pos] = src.transpose(0, 2, 1, 3)
 
 
+# case: (spec, seq_len, positions, attention kernel prepare_cuda reports on its plan line).  At seq_len 4096 attn-l8 runs
+# k_attn2 (8 units x 16 slices on 132 SMs, 16 blocks of 16 positions per CTA) and tiny-hd256 runs k_attn (head_dim 256 has
+# no k_attn2 instantiation).  make_plan selects k_attn2 only while a CTA's slice is at most ATTN2_MAXB = 32 blocks and fits
+# its shared memory: at seq_len 16384 the slice is 1024 / 16 = 64 blocks on a 132-SM card (more on fewer SMs), so attn-l8
+# falls back to k_attn and its transposing score path (16 lanes per position, 4 query heads per kv head) for both caches.
+LONG_CONTEXT_CASES = {
+    "attn-l8": ("attn-l8", 4096, (63, 1023, 2047, 4095), "k_attn2"),
+    "tiny-hd256": ("tiny-hd256", 4096, (63, 1023, 2047, 4095), "k_attn"),
+    "attn-l8-16k": ("attn-l8", 16384, (5000, 9999, 16383), "k_attn"),  # kv_len 5001 is not a multiple of 16
+}
+
+
 @pytest.mark.parametrize("kvbits", [16, 8])
-@pytest.mark.parametrize("spec_name", ["attn-l8", "tiny-hd256"])
-def test_long_context_attention_vs_oracle(oracle_pkg, spec_name, kvbits):
-    """Llama-3-8B's attention geometry (and a 256-wide multi-query head) at context positions up to 4095, device vs
-    oracle on identical cache contents: the 16-slice merge, the transposing score path and the exponent accumulation
-    over thousands of positions, compared value for value."""
+@pytest.mark.parametrize("case", sorted(LONG_CONTEXT_CASES))
+def test_long_context_attention_vs_oracle(oracle_pkg, case, kvbits, capfd, monkeypatch):
+    """Device vs oracle on identical cache contents, compared value for value, over thousands of positions: the slice
+    merge and the exponent accumulation.  attn-l8 (Llama-3-8B's attention geometry) at seq_len 4096 runs k_attn2; at
+    seq_len 16384 its slices exceed k_attn2's shared memory and k_attn's transposing score path serves it; tiny-hd256
+    (a 256-wide multi-query head) runs k_attn's plain score path."""
+    spec_name, seq_len, positions, kernel = LONG_CONTEXT_CASES[case]
     spec = mg.SPECS[spec_name]
-    seq_len = 4096
+    monkeypatch.delenv("CALM_B200_QUIET", raising=False)  # the plan line names the attention kernel
     host = mg.HostModel(spec, seed=11, seq_len=seq_len, kvbits=kvbits)
     ck = oracle_pkg.Checker("port")
     tol = (TOL_SIGMA if kvbits == 16 else TOL8_SIGMA)
     with lib.DeviceModel(spec, host.tensors, seq_len=seq_len, kvbits=kvbits) as dm:
-        for pos in (63, 1023, 2047, 4095):
+        plan = [l for l in capfd.readouterr().out.splitlines() if l.startswith("# plan: attention ")]
+        assert plan and plan[-1].split()[3].rstrip(",") == kernel, plan
+        for pos in positions:
             ck.prepare(host)
             fill_oracle_cache(host, pos, seed=5, kvbits=kvbits)
             want = ck.forward(host, 17, pos)
@@ -69,7 +85,7 @@ def test_long_context_attention_vs_oracle(oracle_pkg, spec_name, kvbits):
             got = dm.forward(17, pos)
             sigma = float(want.std())
             err = float(np.abs(got - want).max())
-            print(f"{spec_name} kv{kvbits} pos {pos}: |cuda-oracle| {err:.2e} = {err / sigma:.1e} sigma")
+            print(f"{case} kv{kvbits} pos {pos}: |cuda-oracle| {err:.2e} = {err / sigma:.1e} sigma")
             assert err <= tol * sigma, (pos, err, sigma)
             srt = np.sort(want)
             if srt[-1] - srt[-2] > 2 * tol * sigma:
