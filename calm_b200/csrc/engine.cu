@@ -26,6 +26,17 @@ namespace {
 enum Stage { ST_EMBED, ST_QKV, ST_ATTN, ST_WO, ST_FFN_UP, ST_FFN_DOWN, ST_OUTPUT, ST_COUNT };
 const char* const kStageNames[ST_COUNT] = {"embed", "matmul_qkv", "attention", "matmul_attn", "matmul_ffn_up", "matmul_ffn_down", "output"};
 
+// a planned launch: the kernel chosen for a stage and its launch shape
+template <typename A>
+struct Launch {
+	void (*kernel)(A) = nullptr;
+	int grid = 0, block = 0;
+	size_t smem = 0;
+};
+struct ResLaunch : Launch<MatResArgs> {
+	int S = 1; // k_matres_ring: MatResArgs::S
+};
+
 struct Engine {
 	bool ready = false;
 	int device = -1;
@@ -58,17 +69,14 @@ struct Engine {
 
 	// attention launch shape
 	int attn_hg = 1, attn_qgroups = 1, attn_nsplit = 1, attn_lpp = 1;
-	// TMA-ring matvec kernels (ring.cuh): u = 512-byte units per row and chunk (0: not used)
-	int ring_up_u = 0, ring_wo_u = 0, ring_down_u = 0, ring_wo_s = 1, ring_down_s = 1;
-	int grid_up_ring = 0, grid_wo_ring = 0, grid_down_ring = 0;
-	size_t smem_up_ring = 0, smem_wo_ring = 0, smem_down_ring = 0;
-	bool attn2 = false; // k_attn2 (attn.cuh): KV slice requested into shared memory ahead of the dependency wait, tensor-core passes
 	int attn_nbmax = 0;
-	size_t attn2_smem = 0;
 
-	// launch plan (grid sizes / dynamic shared memory), fixed at prepare time
-	int grid_qkv = 0, grid_wo = 0, grid_up = 0, grid_down = 0, grid_out = 0;
-	size_t smem_dim = 0, smem_qdim = 0, smem_hidden = 0;
+	// launch plan, fixed at prepare time: the kernel that serves each shape-dependent stage, and its launch shape
+	Launch<AttnArgs> attn; // k_attn2 (attn.cuh) or k_attn
+	ResLaunch wo, down;    // k_matres_ring (ring.cuh) or k_matres
+	Launch<FfnUpArgs> up;  // k_ffn_up_ring or k_ffn_up
+	int grid_qkv = 0, grid_out = 0;
+	size_t smem_dim = 0;
 	int cur_kv_len = 0; // host copy, for the perf table only
 	int cur_pos = 0;
 
@@ -128,6 +136,12 @@ struct Prefill {
 	CUtensorMap tmN[2], tmA[2], tmH[2]; // (hi, lo) views of the three activation matrices the GEMMs read
 };
 Prefill pf;
+
+void pf_free() {
+	cudaFree(pf.X), cudaFree(pf.Q), cudaFree(pf.Nhi), cudaFree(pf.Nlo), cudaFree(pf.Ahi), cudaFree(pf.Alo), cudaFree(pf.Hhi), cudaFree(pf.Hlo), cudaFree(pf.rope), cudaFree(pf.tokens);
+	pf = Prefill();
+}
+
 int g_device_override = -1;
 uint64_t g_launches = 0;
 
@@ -152,15 +166,20 @@ void* dev_alloc(size_t bytes) {
 	return p;
 }
 
-// opt in to more than 48 KB of dynamic shared memory (once per kernel, with the LARGEST size any launch will use, outside stream capture)
+// let `kernel` take `smem` bytes of dynamic shared memory (outside stream capture).  The attribute only ever grows, so a
+// kernel launched at several sizes keeps the largest.
 template <typename F>
 void smem_optin(F kernel, size_t smem) {
 	if (smem > 227 * 1024) CALM_FATAL("kernel needs %zu bytes of shared memory per CTA (limit 227 KB)", smem);
-	if (smem > 48 * 1024) CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	cudaFuncAttributes fa;
+	CUDA_CHECK(cudaFuncGetAttributes(&fa, kernel));
+	if (smem > (size_t)fa.maxDynamicSharedSizeBytes) CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 }
 
+// CTAs of `kernel` resident on the device at once, each with `smem` bytes of dynamic shared memory (opted in here)
 template <typename F>
 int max_ctas(F kernel, int block, size_t smem) {
+	smem_optin(kernel, smem);
 	int per_sm = 0;
 	CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem));
 	if (per_sm < 1) CALM_FATAL("kernel does not fit on an SM (block %d, %zu bytes of shared memory)", block, smem);
@@ -284,7 +303,7 @@ void tp_fill(TpExchange& t, int idx) {
 }
 
 // Launch on the library's stream with programmatic stream serialization (PDL), so that consecutive kernels
-// of a token overlap their launch latency (the kernels order themselves with griddepcontrol.wait).
+// of a token overlap their launch latency (the kernels order themselves with griddepcontrol.wait).  Counts the launch.
 template <typename... KArgs, typename... Args>
 void launch_pdl(void (*kernel)(KArgs...), dim3 grid, int block, size_t smem, Args... args) {
 	cudaLaunchConfig_t cfg = {};
@@ -294,6 +313,35 @@ void launch_pdl(void (*kernel)(KArgs...), dim3 grid, int block, size_t smem, Arg
 	at[0].val.programmaticStreamSerializationAllowed = g.use_pdl ? 1 : 0;
 	cfg.attrs = at, cfg.numAttrs = 1;
 	CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, args...));
+	++g_launches;
+}
+
+template <typename A>
+void launch(const Launch<A>& p, const A& a) {
+	launch_pdl(p.kernel, p.grid, p.block, p.smem, a);
+}
+
+// planned at prepare time (outside stream capture): the launch's shared memory is opted in here
+template <typename A>
+Launch<A> plan(void (*kernel)(A), int grid, int block, size_t smem) {
+	smem_optin(kernel, smem);
+	return {kernel, grid, block, smem};
+}
+
+// the model's weight bits and KV cache element as template arguments: with_formats calls f(Formats<DBITS, KVT>())
+template <int DBITS, typename KVT>
+struct Formats {};
+
+template <typename F>
+void with_formats(F&& f) {
+	switch (g.w.dbits * 100 + g.kvbits) {
+	case 1616: return f(Formats<16, __half>());
+	case 1608: return f(Formats<16, uint8_t>());
+	case 816: return f(Formats<8, __half>());
+	case 808: return f(Formats<8, uint8_t>());
+	case 416: return f(Formats<4, __half>());
+	default: return f(Formats<4, uint8_t>());
+	}
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -346,82 +394,60 @@ size_t attn_smem(int hg, int head_dim, int nsplit) {
 	return smem2 > smem ? smem2 : smem;
 }
 
-// nl == NULL: only opt in to the shared-memory size (prepare time, outside stream capture; head_dim 256 with 8 query heads
-// per kv head needs 66 KB)
-template <typename KVT, int HG>
-void launch_attn(const AttnArgs& a, int nunits, int* nl) {
-	const size_t smem = attn_smem(HG, a.head_dim, a.nsplit);
-	if (!nl) {
-		smem_optin(k_attn<KVT, HG>, smem);
-		return;
-	}
-	launch_pdl(k_attn<KVT, HG>, nunits * a.nsplit, ATTN_THREADS, smem, a);
-	++*nl;
-}
-
-template <typename KVT, int HG, int HD>
-void launch_attn2(const AttnArgs& a, int nunits, int* nl) {
-	if (!nl) { // prepare time: opt-in, and the cell fold polls its peers: the whole grid must fit on the device at once
-		smem_optin(k_attn2<KVT, HG, HD>, g.attn2_smem);
-		int per_sm = 0;
-		CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_attn2<KVT, HG, HD>, ATTN_THREADS, g.attn2_smem));
-		if (per_sm * g.sms < nunits * a.nsplit) g.attn2 = false; // k_attn (global partials, last-CTA fold) has no such requirement
-		return;
-	}
-	launch_pdl(k_attn2<KVT, HG, HD>, nunits * a.nsplit, ATTN_THREADS, g.attn2_smem, a);
-	++*nl;
-}
-
 // shapes k_attn2 is instantiated for: head_dim 128 with 4 or 8 query heads per kv head, head_dim 64 with 2, 4 or 8
 bool attn2_shape_ok(int hg, int lpp, int head_dim) {
 	return head_dim == lpp * 8 && ((lpp == 16 && (hg == 4 || hg == 8)) || (lpp == 8 && (hg == 2 || hg == 4 || hg == 8)));
 }
 
+typedef void (*AttnKernel)(AttnArgs);
+
 template <typename KVT>
-void dispatch_attn(const AttnArgs& a, int nunits, int* nl) {
-	if (g.attn2) {
-		switch (g.attn_lpp * 100 + g.attn_hg) {
-		case 1604: launch_attn2<KVT, 4, 128>(a, nunits, nl); return;
-		case 1608: launch_attn2<KVT, 8, 128>(a, nunits, nl); return;
-		case 802: launch_attn2<KVT, 2, 64>(a, nunits, nl); return;
-		case 804: launch_attn2<KVT, 4, 64>(a, nunits, nl); return;
-		case 808: launch_attn2<KVT, 8, 64>(a, nunits, nl); return;
-		}
+AttnKernel attn2_kernel(int hg, int lpp) {
+	switch (lpp * 100 + hg) {
+	case 1604: return k_attn2<KVT, 4, 128>;
+	case 1608: return k_attn2<KVT, 8, 128>;
+	case 802: return k_attn2<KVT, 2, 64>;
+	case 804: return k_attn2<KVT, 4, 64>;
+	case 808: return k_attn2<KVT, 8, 64>;
 	}
-	switch (g.attn_hg) {
-	case 1: launch_attn<KVT, 1>(a, nunits, nl); break;
-	case 2: launch_attn<KVT, 2>(a, nunits, nl); break;
-	case 3: launch_attn<KVT, 3>(a, nunits, nl); break;
-	case 4: launch_attn<KVT, 4>(a, nunits, nl); break;
-	case 5: launch_attn<KVT, 5>(a, nunits, nl); break;
-	case 6: launch_attn<KVT, 6>(a, nunits, nl); break;
-	case 7: launch_attn<KVT, 7>(a, nunits, nl); break;
-	default: launch_attn<KVT, 8>(a, nunits, nl); break;
+	return nullptr;
+}
+
+template <typename KVT>
+AttnKernel attn_kernel(int hg) {
+	switch (hg) {
+	case 1: return k_attn<KVT, 1>;
+	case 2: return k_attn<KVT, 2>;
+	case 3: return k_attn<KVT, 3>;
+	case 4: return k_attn<KVT, 4>;
+	case 5: return k_attn<KVT, 5>;
+	case 6: return k_attn<KVT, 6>;
+	case 7: return k_attn<KVT, 7>;
+	default: return k_attn<KVT, 8>;
 	}
 }
 
-// ring kernels are instantiated for u in {2, 4} (1 KB / 2 KB per row and chunk)
-template <int DBITS>
-void ring_up_dispatch(const FfnUpArgs& a, bool attr_only) {
-	auto kernel = g.ring_up_u == 2 ? k_ffn_up_ring<DBITS, 2> : k_ffn_up_ring<DBITS, 4>;
-	if (attr_only) return smem_optin(kernel, g.smem_up_ring);
-	launch_pdl(kernel, g.grid_up_ring, RING_UP_WARPS * 32, g.smem_up_ring, a);
-}
-template <int DBITS>
-void ring_res_dispatch(const MatResArgs& a, int u, int S, int grid, size_t smem, bool attr_only) {
-	auto kernel = u == 2 ? k_matres_ring<DBITS, 2> : k_matres_ring<DBITS, 4>;
-	if (attr_only) return smem_optin(kernel, smem);
-	launch_pdl(kernel, grid, RING_RES_WARPS * 32, smem, a, S);
+// wo / w2: y += W . xin over this rank's share; under tensor parallelism the partials are summed over the ranks, inside the
+// kernel over peer memory or by an NCCL all-reduce after it.  idx: the exchange slot of this projection.
+void launch_res(const ResLaunch& p, MatResArgs& a, int idx) {
+	const int dim = g.cfg.dim;
+	a.S = p.S;
+	if (g.tp_fused) tp_fill(a.tpx, idx);
+	else if (g.tp_world > 1) a.y = g.xpart, a.accumulate = 0;
+	launch(p, a);
+	if (g.tp_world > 1 && !g.tp_fused) {
+		tp_allreduce(g.xpart, dim);
+		launch_pdl(k_addvec, cdiv(dim, 256), 256, 0, g.x, (const float*)g.xpart, dim);
+	}
 }
 
 // mode: 0 kv only, 1 logits -> host, 2 logits -> device + advance (greedy loop), 3 logits -> host + argmax, 4 logits -> device + min-p sample + advance
 template <int DBITS, typename KVT>
-int run_token(int mode) {
+void run_token(Formats<DBITS, KVT>, int mode) {
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const int dim = c.dim, hidden = c.hidden_dim, hd = c.head_dim;
 	const size_t wb = (size_t)DBITS; // bits per weight
-	int nl = 0;
 	g.n_stamps = 0;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * hd; // elements per layer
 
@@ -434,7 +460,6 @@ int run_token(int mode) {
 		a.n_layers = c.n_layers, a.n_kv_heads = c.n_kv_heads, a.head_dim = hd, a.seq_len = c.seq_len;
 		a.stamp = nullptr, a.stamp_reset = g.perf ? g.stamps : nullptr, a.n_stamps = MAX_STAMPS + 8; // + the 16 debug stamps
 		launch_pdl(k_embed<DBITS, KVT>, a.embed_blocks + 8, 256, 0, a);
-		++nl;
 	}
 
 	for (int l = 0; l < c.n_layers; ++l) {
@@ -448,7 +473,6 @@ int run_token(int mode) {
 			a.eps = c.norm_eps, a.clip = c.qkv_clip, a.ln = c.norm_ln;
 			a.stamp = t.slot;
 			launch_pdl(k_qkv<DBITS, KVT>, g.grid_qkv, QKV_THREADS, g.smem_dim, a);
-			++nl;
 		}
 		{
 			StageScope t(ST_ATTN, -1.0); // bytes depend on the position: accounted per token in launch_token()
@@ -462,23 +486,14 @@ int run_token(int mode) {
 			a.cells = g.attn_cells, a.epoch_stride = (unsigned)c.n_layers + 1, a.epoch_idx = (unsigned)l + 1, a.err = g.dev_err;
 			a.dbg = (g.perf && l == c.n_layers / 2) ? g.stamps + 2 * (size_t)MAX_STAMPS : nullptr;
 			a.stamp = t.slot;
-			dispatch_attn<KVT>(a, c.n_kv_heads * g.attn_qgroups, &nl);
+			launch(g.attn, a);
 		}
 		{
 			StageScope t(ST_WO, (double)dim * g.q_dim * wb / 8);
 			MatResArgs a = {};
 			a.xin = g.att, a.w = w.wo[l], a.y = g.x, a.sel = nullptr, a.n = g.q_dim, a.d = dim, a.nact = 1, a.accumulate = 1;
 			a.stamp = t.slot;
-			if (g.tp_fused) tp_fill(a.tpx, 2 * l); // partial over this rank's heads, summed over the ranks in the kernel
-			else if (g.tp_world > 1) a.y = g.xpart, a.accumulate = 0;
-			if (g.ring_wo_u) ring_res_dispatch<DBITS>(a, g.ring_wo_u, g.ring_wo_s, g.grid_wo_ring, g.smem_wo_ring, false);
-			else launch_pdl(k_matres<DBITS>, g.grid_wo, 256, g.smem_qdim, a);
-			++nl;
-			if (g.tp_world > 1 && !g.tp_fused) {
-				tp_allreduce(g.xpart, dim);
-				launch_pdl(k_addvec, cdiv(dim, 256), 256, 0, g.x, (const float*)g.xpart, dim);
-				++nl;
-			}
+			launch_res(g.wo, a, 2 * l); // partial over this rank's heads
 		}
 		{
 			StageScope t(ST_FFN_UP, (double)2 * g.nact * hidden * dim * wb / 8);
@@ -489,9 +504,7 @@ int run_token(int mode) {
 			a.eps = c.norm_eps, a.ln = c.norm_ln, a.gelu = c.act_gelu;
 			a.expert_stride = g.up_expert_stride;
 			a.stamp = t.slot;
-			if (g.ring_up_u) ring_up_dispatch<DBITS>(a, false);
-			else launch_pdl(k_ffn_up<DBITS>, g.grid_up, 256, g.smem_dim, a);
-			++nl;
+			launch(g.up, a);
 		}
 		{
 			StageScope t(ST_FFN_DOWN, (double)g.nact * hidden * dim * wb / 8);
@@ -499,16 +512,7 @@ int run_token(int mode) {
 			a.xin = g.hb, a.w = w.w2[l], a.y = g.x, a.sel = c.n_experts ? g.moe_sel : nullptr;
 			a.n = hidden, a.d = dim, a.nact = g.nact, a.accumulate = 1;
 			a.stamp = t.slot;
-			if (g.tp_fused) tp_fill(a.tpx, 2 * l + 1); // partial over this rank's FFN rows
-			else if (g.tp_world > 1) a.y = g.xpart, a.accumulate = 0;
-			if (g.ring_down_u) ring_res_dispatch<DBITS>(a, g.ring_down_u, g.ring_down_s, g.grid_down_ring, g.smem_down_ring, false);
-			else launch_pdl(k_matres<DBITS>, g.grid_down, 256, g.smem_hidden, a);
-			++nl;
-			if (g.tp_world > 1 && !g.tp_fused) {
-				tp_allreduce(g.xpart, dim);
-				launch_pdl(k_addvec, cdiv(dim, 256), 256, 0, g.x, (const float*)g.xpart, dim);
-				++nl;
-			}
+			launch_res(g.down, a, 2 * l + 1); // partial over this rank's FFN rows
 		}
 	}
 
@@ -535,14 +539,12 @@ int run_token(int mode) {
 			cand_val = (const float*)((char*)g.tp_area + g.tp_off_cval), cand_idx = (const int*)((char*)g.tp_area + g.tp_off_cidx);
 		}
 		launch_pdl(k_output<DBITS>, grid, 256, g.smem_dim, a);
-		++nl;
 		if (split) {
 			TpGatherArgs ga = {};
 			ga.world = g.tp_world, ga.rank = g.tp_rank, ga.tp = g.tp, ga.err = g.tp_err;
 			for (int p = 0; p < g.tp_world; ++p) ga.flags[p] = (unsigned*)((char*)g.tp_peer[p] + g.tp_off_flags);
 			ga.src = (const float*)((char*)g.tp_area + g.tp_off_logits), ga.dst = a.logits, ga.n = c.vocab_size;
 			launch_pdl(k_tp_gather, 32, 256, 0, ga);
-			++nl;
 		}
 		if (mode == 4) { // min-p sampling on the device (reference sampler.c:44-90), then the bookkeeping of k_advance
 			SampleArgs sa;
@@ -550,17 +552,11 @@ int run_token(int mode) {
 			sa.st = g.sample_state, sa.count = g.sample_count, sa.csum = g.sample_csum, sa.sidx = g.sample_idx, sa.sprob = g.sample_prob;
 			launch_pdl(k_sample_scan, g.sample_chunks, 256, 0, sa);
 			launch_pdl(k_sample_pick, 1, 256, 0, sa, g.sample_state, g.tp, g.out_tokens, g.last_token, 1);
-			nl += 2;
 		} else if (mode >= 2) {
 			launch_pdl(k_advance, 1, 256, 0, cand_val, cand_idx, ncand, g.tp, g.out_tokens, g.last_token, (int)(mode == 2), c.vocab_size);
-			++nl;
 		}
 	}
-	if (g.perf) {
-		launch_pdl(k_stamp_accum, 1, 256, 0, (const unsigned long long*)g.stamps, g.stamp_acc, g.n_stamps);
-		++nl;
-	}
-	return nl;
+	if (g.perf) launch_pdl(k_stamp_accum, 1, 256, 0, (const unsigned long long*)g.stamps, g.stamp_acc, g.n_stamps);
 }
 
 
@@ -606,81 +602,72 @@ void tp_shard_model() {
 	c.n_heads /= N, c.n_kv_heads /= N, c.hidden_dim = hl;
 }
 
-// Fix grid sizes and shared-memory opt-ins for this model (called once from prepare_cuda).
+// Choose the kernel and launch shape of every stage for this model and opt each kernel in to its shared memory (called once
+// from prepare_cuda).  Kernels are first touched here in the order the library has always used: k_matres, attention, k_qkv,
+// FFN up, the wo / w2 rings, k_output.  Under lazy module loading that order decides where their code is placed, and on an
+// H100 (700 W) other orders moved decode by 0.2-0.3 % (Llama-3-8B faster, Mixtral-8x7B slower).
 template <int DBITS, typename KVT>
-void make_plan() {
+void make_plan(Formats<DBITS, KVT>) {
 	const Config& c = g.cfg;
 	g.smem_dim = xs_bytes<DBITS>(c.dim);
-	g.smem_qdim = xs_bytes<DBITS>(g.q_dim);
-	g.smem_hidden = xs_bytes<DBITS>(c.hidden_dim);
-	size_t smem_res = g.smem_qdim > g.smem_hidden ? g.smem_qdim : g.smem_hidden;
-	if (smem_res > 227 * 1024 || g.smem_dim > 227 * 1024) CALM_FATAL("activation vector does not fit in shared memory (dim %d, hidden %d)", c.dim, c.hidden_dim);
-	smem_optin(k_qkv<DBITS, KVT>, g.smem_dim), smem_optin(k_ffn_up<DBITS>, g.smem_dim), smem_optin(k_output<DBITS>, g.smem_dim);
-	smem_optin(k_matres<DBITS>, smem_res); // ONE attribute per kernel: the larger of its two launch shapes (wo, w2)
-	{
-		// k_attn2 when the shape is instantiated and the CTA's share of the context fits in shared memory
-		g.attn_nbmax = cdiv(cdiv(c.seq_len, ATTN2_BP), g.attn_nsplit);
-		g.attn2_smem = attn2_smem_bytes<KVT>(g.attn_hg, c.head_dim, g.attn_nbmax);
-		g.attn2 = attn2_shape_ok(g.attn_hg, g.attn_lpp, c.head_dim) && g.attn_nbmax <= ATTN2_MAXB && g.attn2_smem <= 200 * 1024;
-		AttnArgs aa = {};
-		aa.head_dim = c.head_dim, aa.nsplit = g.attn_nsplit;
-		dispatch_attn<KVT>(aa, c.n_kv_heads * g.attn_qgroups, nullptr);
-	}
-	g.grid_qkv = balanced_grid(cdiv((g.q_dim + 2 * g.kv_dim) / 2, 8), max_ctas(k_qkv<DBITS, KVT>, QKV_THREADS, g.smem_dim));
-	g.grid_wo = balanced_grid(cdiv(c.dim / 2, 8), max_ctas(k_matres<DBITS>, 256, g.smem_qdim));
-	g.grid_down = balanced_grid(cdiv(c.dim / 2, 8), max_ctas(k_matres<DBITS>, 256, g.smem_hidden));
+	const size_t smem_qdim = xs_bytes<DBITS>(g.q_dim), smem_hidden = xs_bytes<DBITS>(c.hidden_dim);
+	if (smem_qdim > 227 * 1024 || smem_hidden > 227 * 1024 || g.smem_dim > 227 * 1024) CALM_FATAL("activation vector does not fit in shared memory (dim %d, hidden %d)", c.dim, c.hidden_dim);
+	const int grid_wo = balanced_grid(cdiv(c.dim / 2, 8), max_ctas(k_matres<DBITS>, 256, smem_qdim));
+	const int grid_down = balanced_grid(cdiv(c.dim / 2, 8), max_ctas(k_matres<DBITS>, 256, smem_hidden));
 	if (g.tp_fused) { // the in-kernel exchange needs co-resident grids (they are: balanced_grid stays under the cap) within its tables
-		for (int grid : {g.grid_wo, g.grid_down})
+		for (int grid : {grid_wo, grid_down})
 			if (cdiv(c.dim / 2, grid * 8) > TP_MAX_ITERS) CALM_FATAL("tensor parallelism: grid %d outside the exchange tables for dim %d", grid, c.dim);
 	}
-	// (the long FFN-up stage gets a full grid with uneven rounds rather than balanced_grid's even ones)
-	g.grid_up = imin(max_ctas(k_ffn_up<DBITS>, 256, g.smem_dim), cdiv(g.nact * c.hidden_dim, 8));
-	// TMA-ring kernels for the dense single-GPU stages whose rows are whole 1 KB / 2 KB chunks (ring.cuh)
-	g.ring_up_u = g.ring_wo_u = g.ring_down_u = 0;
+	{
+		// k_attn2 when the shape is instantiated, the CTA's share of the context fits in shared memory and the whole grid is
+		// resident at once (the cell fold polls its peers); otherwise k_attn (global partials, last-CTA fold)
+		const int units = c.n_kv_heads * g.attn_qgroups, grid = units * g.attn_nsplit;
+		g.attn_nbmax = cdiv(cdiv(c.seq_len, ATTN2_BP), g.attn_nsplit);
+		const size_t smem2 = attn2_smem_bytes<KVT>(g.attn_hg, c.head_dim, g.attn_nbmax);
+		AttnKernel k2 = nullptr;
+		if (attn2_shape_ok(g.attn_hg, g.attn_lpp, c.head_dim) && g.attn_nbmax <= ATTN2_MAXB && smem2 <= 200 * 1024) {
+			k2 = attn2_kernel<KVT>(g.attn_hg, g.attn_lpp);
+			if (max_ctas(k2, ATTN_THREADS, smem2) < grid) k2 = nullptr;
+		}
+		if (k2) g.attn = plan(k2, grid, ATTN_THREADS, smem2);
+		else g.attn = plan(attn_kernel<KVT>(g.attn_hg), grid, ATTN_THREADS, attn_smem(g.attn_hg, c.head_dim, g.attn_nsplit));
+		if (!getenv("CALM_B200_QUIET")) {
+			printf("# plan: attention %s, %d units x %d slices\n", k2 ? "k_attn2" : "k_attn", units, g.attn_nsplit);
+			fflush(stdout);
+		}
+	}
+	g.grid_qkv = balanced_grid(cdiv((g.q_dim + 2 * g.kv_dim) / 2, 8), max_ctas(k_qkv<DBITS, KVT>, QKV_THREADS, g.smem_dim));
+	// TMA-ring kernels for the dense stages whose rows are whole 1 KB / 2 KB chunks (ring.cuh)
 	const bool ring_up_on = c.n_experts == 0; // MoE: the expert rows are known only after the router (row shards of w1 / w3 under tensor parallelism are fine)
 	const bool ring_res_on = ring_up_on && (g.tp_world == 1 || g.tp_fused); // the ring kernels carry the in-kernel exchange too (gf4 too)
 	auto chunk_units = [](size_t rowbytes) { return rowbytes % 2048 == 0 ? 4 : (rowbytes % 1024 == 0 ? 2 : 0); };
-	if (ring_up_on) {
-		const int u = chunk_units((size_t)c.dim * DBITS / 8);
-		if (u) {
-			g.smem_up_ring = ring_smem_bytes<DBITS>(c.dim, u, RING_UP_WARPS);
-			if (g.smem_up_ring <= 200 * 1024) {
-				g.ring_up_u = u;
-				g.grid_up_ring = imin(g.sms * imin(2, (int)(220 * 1024 / g.smem_up_ring)), c.hidden_dim); // two CTAs per SM where they fit
-				if (g.grid_up_ring < 1) g.grid_up_ring = 1;
-				FfnUpArgs fa = {};
-				ring_up_dispatch<DBITS>(fa, true);
-			}
+	// FFN up: k_ffn_up_ring or k_ffn_up (the long FFN-up stage gets a full grid with uneven rounds rather than balanced_grid's
+	// even ones)
+	g.up = {k_ffn_up<DBITS>, imin(max_ctas(k_ffn_up<DBITS>, 256, g.smem_dim), cdiv(g.nact * c.hidden_dim, 8)), 256, g.smem_dim};
+	if (const int u = ring_up_on ? chunk_units((size_t)c.dim * DBITS / 8) : 0) {
+		const size_t smem = ring_smem_bytes<DBITS>(c.dim, u, RING_UP_WARPS);
+		if (smem <= 200 * 1024) {
+			const int grid = imin(g.sms * imin(2, (int)(220 * 1024 / smem)), c.hidden_dim); // two CTAs per SM where they fit
+			g.up = plan(u == 2 ? k_ffn_up_ring<DBITS, 2> : k_ffn_up_ring<DBITS, 4>, grid < 1 ? 1 : grid, RING_UP_WARPS * 32, smem);
 		}
 	}
-	if (ring_res_on) {
-		auto plan_res = [&](int n, int& u_out, int& s_out, int& grid_out, size_t& smem_out) {
-			const size_t rowbytes = (size_t)n * DBITS / 8;
-			int u = chunk_units(rowbytes);
-			if (!u) return;
-			size_t smem = ring_smem_bytes<DBITS>(n, u, RING_RES_WARPS);
-			if (smem > 220 * 1024 && u == 4) u = 2, smem = ring_smem_bytes<DBITS>(n, u, RING_RES_WARPS); // long activation vectors (70B w2: 112 KB): 1 KB chunks
-			if (smem > 220 * 1024) return;
-			const int grid = imin(g.sms, c.dim / 2); // one CTA per SM
-			const int cpt = (int)(rowbytes / (u * 512));
-			if (g.tp_world > 1 && cdiv(c.dim / 2, grid) + 1 > RING_MAX_PAIRS) return; // the exchange keeps a CTA's rows in shared memory
-			const bool split = cdiv(c.dim / 2, grid) + 1 <= RING_MAX_PAIRS && cpt <= RING_MAX_SLICES; // K-slices of one chunk, folded in shared memory
-			u_out = u, s_out = split ? 1 : cpt, grid_out = grid < 1 ? 1 : grid, smem_out = smem;
-			MatResArgs ma = {};
-			ring_res_dispatch<DBITS>(ma, u, s_out, grid_out, smem, true);
-		};
-		// ONE shared-memory attribute per kernel instantiation: wo and w2 may share one (same U): opt in to the larger first
-		int uw = 0, ud = 0, sw = 1, sd = 1, gw = 0, gd = 0;
-		size_t mw = 0, md = 0;
-		plan_res(g.q_dim, uw, sw, gw, mw);
-		plan_res(c.hidden_dim, ud, sd, gd, md);
-		if (uw && ud && uw == ud) { // same instantiation: its attribute must cover both launches
-			MatResArgs ma = {};
-			ring_res_dispatch<DBITS>(ma, uw, 1, 1, mw > md ? mw : md, true);
-		}
-		g.ring_wo_u = uw, g.ring_wo_s = sw, g.grid_wo_ring = gw, g.smem_wo_ring = mw;
-		g.ring_down_u = ud, g.ring_down_s = sd, g.grid_down_ring = gd, g.smem_down_ring = md;
-	}
+	// wo (n = q_dim) and w2 (n = hidden): k_matres_ring when the rows are whole chunks and the ring fits, else k_matres
+	auto plan_res = [&](int n, int grid_reg, size_t smem_reg) -> ResLaunch {
+		const ResLaunch reg = {{k_matres<DBITS>, grid_reg, 256, smem_reg}};
+		const size_t rowbytes = (size_t)n * DBITS / 8;
+		int u = ring_res_on ? chunk_units(rowbytes) : 0;
+		if (!u) return reg;
+		size_t smem = ring_smem_bytes<DBITS>(n, u, RING_RES_WARPS);
+		if (smem > 220 * 1024 && u == 4) u = 2, smem = ring_smem_bytes<DBITS>(n, u, RING_RES_WARPS); // long activation vectors (70B w2: 112 KB): 1 KB chunks
+		if (smem > 220 * 1024) return reg;
+		const int grid = imin(g.sms, c.dim / 2); // one CTA per SM
+		const int cpt = (int)(rowbytes / (u * 512));
+		if (g.tp_world > 1 && cdiv(c.dim / 2, grid) + 1 > RING_MAX_PAIRS) return reg; // the exchange keeps a CTA's rows in shared memory
+		const bool split = cdiv(c.dim / 2, grid) + 1 <= RING_MAX_PAIRS && cpt <= RING_MAX_SLICES; // K-slices of one chunk, folded in shared memory
+		return {plan(u == 2 ? k_matres_ring<DBITS, 2> : k_matres_ring<DBITS, 4>, grid < 1 ? 1 : grid, RING_RES_WARPS * 32, smem), split ? 1 : cpt};
+	};
+	g.wo = plan_res(g.q_dim, grid_wo, smem_qdim);
+	g.down = plan_res(c.hidden_dim, grid_down, smem_hidden);
 	g.out_row0 = 0, g.out_row1 = c.vocab_size;
 	if (g.tp_fused) { // vocabulary split: equal slices of whole 32-row CTA iterations (the last rank's may be short)
 		const int per = cdiv(cdiv(c.vocab_size, g.tp_world), 32) * 32;
@@ -693,38 +680,23 @@ void make_plan() {
 	g.ncand = g.grid_out;
 }
 
-template <int DBITS>
-void make_plan_kv() {
-	g.kvbits == 8 ? make_plan<DBITS, uint8_t>() : make_plan<DBITS, __half>();
-}
-
-template <int DBITS>
-int run_token_kv(int mode) {
-	return g.kvbits == 8 ? run_token<DBITS, uint8_t>(mode) : run_token<DBITS, __half>(mode);
-}
-
-int run_token_any(int mode) {
-	switch (g.w.dbits) {
-	case 16: return run_token_kv<16>(mode);
-	case 8: return run_token_kv<8>(mode);
-	default: return run_token_kv<4>(mode);
-	}
-}
-
-
 void launch_token(int mode) {
 	const int pv = g.perf ? 1 : 0; // the profiling variant is the same graph with stamp slots
+	auto run = [mode] { with_formats([mode](auto f) { run_token(f, mode); }); };
 	if (!g.use_graph) {
-		g_launches += run_token_any(mode);
+		run();
 		CUDA_CHECK(cudaGetLastError());
 	} else {
 		if (!g.graph[pv][mode]) {
+			const uint64_t n0 = g_launches;
 			cudaGraph_t graph;
 			CUDA_CHECK(cudaStreamBeginCapture(g.stream, cudaStreamCaptureModeThreadLocal));
-			g.graph_launches[pv][mode] = run_token_any(mode);
+			run();
 			CUDA_CHECK(cudaStreamEndCapture(g.stream, &graph));
 			CUDA_CHECK(cudaGraphInstantiate(&g.graph[pv][mode], graph, 0));
 			CUDA_CHECK(cudaGraphDestroy(graph));
+			g.graph_launches[pv][mode] = (int)(g_launches - n0);
+			g_launches = n0; // a captured launch counts when the graph runs
 		}
 		CUDA_CHECK(cudaGraphLaunch(g.graph[pv][mode], g.stream));
 		g_launches += g.graph_launches[pv][mode];
@@ -892,15 +864,7 @@ extern "C" void prepare_cuda(struct Transformer* transformer) {
 	g.tp = (TokenParams*)dev_alloc(sizeof(TokenParams));
 	CUDA_CHECK(cudaMemset(g.tp, 0, sizeof(TokenParams)));
 
-	switch (w.dbits) {
-	case 16: make_plan_kv<16>(); break;
-	case 8: make_plan_kv<8>(); break;
-	default: make_plan_kv<4>(); break;
-	}
-	if (!getenv("CALM_B200_QUIET")) {
-		printf("# plan: attention %s, %d units x %d slices\n", g.attn2 ? "k_attn2" : "k_attn", units, g.attn_nsplit);
-		fflush(stdout);
-	}
+	with_formats([](auto f) { make_plan(f); });
 	g.cand_val = (float*)dev_alloc(g.ncand * sizeof(float));
 	g.cand_idx = (int*)dev_alloc(g.ncand * sizeof(int));
 	g.out_tokens_cap = 1 << 16;
@@ -953,10 +917,7 @@ extern "C" void calm_b200_release(struct Transformer* transformer) {
 			if (g.graph[v][i]) CUDA_CHECK(cudaGraphExecDestroy(g.graph[v][i]));
 	cudaFree(g.stamps), cudaFree(g.stamp_acc), cudaFree(g.attn_cells);
 	if (g.dev_err) cudaFreeHost(g.dev_err);
-	if (pf.cap) {
-		cudaFree(pf.X), cudaFree(pf.Q), cudaFree(pf.Nhi), cudaFree(pf.Nlo), cudaFree(pf.Ahi), cudaFree(pf.Alo), cudaFree(pf.Hhi), cudaFree(pf.Hlo), cudaFree(pf.rope), cudaFree(pf.tokens);
-		pf = Prefill();
-	}
+	pf_free();
 	cudaFree(g.x), cudaFree(g.xb), cudaFree(g.q), cudaFree(g.att), cudaFree(g.hb), cudaFree(g.logits_dev);
 	cudaFreeHost(g.logits_host), cudaFreeHost(g.last_token);
 	cudaFree(g.kc), cudaFree(g.vc), cudaFree(g.rope_freq), cudaFree(g.rope_cs), cudaFree(g.attn_partial), cudaFree(g.attn_counter);
@@ -1148,7 +1109,7 @@ static void pf_reserve(int n) {
 	if (cap <= pf.cap) return;
 	if (pf.cap) {
 		CUDA_CHECK(cudaStreamSynchronize(g.stream));
-		cudaFree(pf.X), cudaFree(pf.Q), cudaFree(pf.Nhi), cudaFree(pf.Nlo), cudaFree(pf.Ahi), cudaFree(pf.Alo), cudaFree(pf.Hhi), cudaFree(pf.Hlo), cudaFree(pf.rope), cudaFree(pf.tokens);
+		pf_free();
 	}
 	pf.cap = cap;
 	auto zalloc = [&](size_t bytes) {
@@ -1177,10 +1138,8 @@ static bool pf_supported() {
 
 template <int MODE, int DBITS, typename KVT>
 static void pf_gemm(const CUtensorMap* tm, const PfGemmArgs& a, int rows, int n) {
-	static bool opted = false;
-	if (!opted) smem_optin(k_pf_gemm<MODE, DBITS, KVT>, pf_smem_bytes<MODE>()), opted = true;
+	smem_optin(k_pf_gemm<MODE, DBITS, KVT>, pf_smem_bytes<MODE>());
 	launch_pdl(k_pf_gemm<MODE, DBITS, KVT>, dim3(rows / PF_BM, cdiv(n, PF_BN)), PF_THREADS, pf_smem_bytes<MODE>(), tm[0], tm[1], a);
-	++g_launches;
 }
 
 template <typename KVT, int HD>
@@ -1189,20 +1148,17 @@ static void pf_attn(const PfAttnArgs& a, int n) {
 	if (g.kv_mul % 4 == 0) launch_pdl(k_pf_attn<KVT, HD, 4>, grid, PFA_WARPS * 32, 0, a);
 	else if (g.kv_mul % 2 == 0) launch_pdl(k_pf_attn<KVT, HD, 2>, grid, PFA_WARPS * 32, 0, a);
 	else launch_pdl(k_pf_attn<KVT, HD, 1>, grid, PFA_WARPS * 32, 0, a);
-	++g_launches;
 }
 
 template <int DBITS, typename KVT>
-static void pf_run(int n, int pos0) {
+static void pf_run(Formats<DBITS, KVT>, int n, int pos0) {
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
 	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
 	launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
-	g_launches += 2;
 	for (int l = 0; l < c.n_layers; ++l) {
 		launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_att_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
-		++g_launches;
 		PfGemmArgs a = {};
 		a.n_tokens = n;
 		a.w[0] = w.wq[l], a.w[1] = w.wk[l], a.w[2] = w.wv[l], a.K = c.dim;
@@ -1223,7 +1179,6 @@ static void pf_run(int n, int pos0) {
 
 		if (!c.norm_par) { // (parallel-norm models reuse the attention-norm output, reference infer.c:417-420)
 			launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_ffn_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
-			++g_launches;
 		}
 		PfGemmArgs u = {};
 		u.n_tokens = n, u.w[0] = w.w1[l], u.w[1] = w.w3[l], u.K = c.dim, u.Hhi = pf.Hhi, u.Hlo = pf.Hlo, u.hidden = c.hidden_dim, u.gelu = c.act_gelu;
@@ -1256,15 +1211,7 @@ extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* 
 		const int m = n - o < chunk_cap ? n - o : chunk_cap;
 		pf_reserve(m);
 		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		const int key = g.w.dbits * 100 + g.kvbits;
-		switch (key) {
-		case 1616: pf_run<16, __half>(m, pos0 + o); break;
-		case 1608: pf_run<16, uint8_t>(m, pos0 + o); break;
-		case 816: pf_run<8, __half>(m, pos0 + o); break;
-		case 808: pf_run<8, uint8_t>(m, pos0 + o); break;
-		case 416: pf_run<4, __half>(m, pos0 + o); break;
-		default: pf_run<4, uint8_t>(m, pos0 + o); break;
-		}
+		with_formats([&](auto f) { pf_run(f, m, pos0 + o); });
 		CUDA_CHECK(cudaStreamSynchronize(g.stream)); // `tokens` is the caller's memory (pageable): the copy above must have left it
 	}
 	CUDA_CHECK(cudaGetLastError());
@@ -1346,7 +1293,6 @@ static float matvec_impl(const void* w_device, const float* x_host, float* y_hos
 	CUDA_CHECK(cudaGetDeviceProperties(&prop, g.device));
 	g.sms = prop.multiProcessorCount;
 	size_t smem = xs_bytes<DBITS>(n);
-	smem_optin(k_matvec<DBITS>, smem);
 	int cap = max_ctas(k_matvec<DBITS>, 256, smem);
 	int grid = imin(cap, cdiv((d + 1) / 2, 8));
 	MatvecArgs a{x, w_device, y, n, d};

@@ -17,9 +17,10 @@
 // fold the slices of a pair in slice order (deterministic) through shared memory -- the last slice to finish does it.
 //
 // Arithmetic is dot_vec<> of common.cuh on the same vectors in the same per-lane order as warp_dot_rows, so results are
-// bit-identical to the register-fed kernels for whole rows.  Dense models on one GPU with row bytes a multiple of 512;
-// everything else (MoE expert offsets known only after the router, the in-kernel tensor-parallel exchange, odd shapes)
-// keeps k_ffn_up / k_matres.
+// bit-identical to the register-fed kernels for whole rows.  Rows must be whole 1 KB chunks.  The rings serve dense
+// models, with or without tensor parallelism: k_matres_ring carries the in-kernel exchange of stages.cuh TpExchange, and
+// only the NCCL all-reduce path keeps k_matres for wo / w2.  MoE layers (expert rows known only after the router) and
+// other row lengths keep k_ffn_up / k_matres.
 #pragma once
 
 #include "stages.cuh"
@@ -190,7 +191,7 @@ __global__ void __launch_bounds__(RING_UP_WARPS * 32, 2) k_ffn_up_ring(const Ffn
 // slices of a pair land in part[][] and the last one to arrive adds them up in slice order.
 
 template <int DBITS, int U>
-__global__ void __launch_bounds__(RING_RES_WARPS * 32, 1) k_matres_ring(const MatResArgs a, const int S) {
+__global__ void __launch_bounds__(RING_RES_WARPS * 32, 1) k_matres_ring(const MatResArgs a) {
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	__shared__ RingCtl ctl;
 	__shared__ float2 part[RING_MAX_PAIRS][RING_MAX_SLICES];
@@ -200,7 +201,7 @@ __global__ void __launch_bounds__(RING_RES_WARPS * 32, 1) k_matres_ring(const Ma
 	float* xs = red + 32;
 	unsigned char* ring = smem_raw + (((size_t)(32 + xs_all_floats<DBITS>(a.n)) * sizeof(float) + 127) & ~(size_t)127);
 	const size_t rowbytes = (size_t)a.n * DBITS / 8;
-	const int cpt = (int)(rowbytes / (U * 512)), nsl = cpt / S;
+	const int S = a.S, cpt = (int)(rowbytes / (U * 512)), nsl = cpt / S;
 	const int npairs = a.d / 2;
 	const int p_lo = (int)(((long long)blockIdx.x * npairs) / gridDim.x), p_hi = (int)(((long long)(blockIdx.x + 1) * npairs) / gridDim.x);
 	pdl_launch_next();

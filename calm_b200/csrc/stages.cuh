@@ -888,6 +888,7 @@ struct MatResArgs {
 	int accumulate;   // 1: y += ..., 0: y = ...
 	TpExchange tpx;   // world > 1: the partial is summed over the tensor-parallel ranks inside this kernel
 	unsigned long long* stamp;
+	int S;            // k_matres_ring: chunks per task, i.e. per K-slice of a row pair (k_matres reads whole rows)
 };
 
 template <int DBITS>
