@@ -668,6 +668,11 @@ void make_plan(Formats<DBITS, KVT>) {
 	};
 	g.wo = plan_res(g.q_dim, grid_wo, smem_qdim);
 	g.down = plan_res(c.hidden_dim, grid_down, smem_hidden);
+	if (!getenv("CALM_B200_QUIET")) {
+		auto res_name = [](const ResLaunch& r) { return r.kernel == k_matres<DBITS> ? "k_matres" : "k_matres_ring"; };
+		printf("# plan: matvec up %s, wo %s, down %s\n", g.up.kernel == k_ffn_up<DBITS> ? "k_ffn_up" : "k_ffn_up_ring", res_name(g.wo), res_name(g.down));
+		fflush(stdout);
+	}
 	g.out_row0 = 0, g.out_row1 = c.vocab_size;
 	if (g.tp_fused) { // vocabulary split: equal slices of whole 32-row CTA iterations (the last rank's may be short)
 		const int per = cdiv(cdiv(c.vocab_size, g.tp_world), 32) * 32;

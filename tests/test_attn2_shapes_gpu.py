@@ -34,12 +34,13 @@ def test_attn2_shapes_vs_oracle(oracle_pkg, shape, kvbits):
     ck = oracle_pkg.Checker("port")
     tol = TOL_SIGMA if kvbits == 16 else TOL8_SIGMA
     with lib.DeviceModel(spec, host.tensors, seq_len=seq_len, kvbits=kvbits) as dm:
-        for pos in (40, 1000, 2900, 4094):  # kv_len = pos + 1: none a multiple of 16
+        # kv_len = pos + 1: none a multiple of 16; pos 5094 is past seq_len (a rolled-over cache, this token in slot 1000)
+        for pos in (40, 1000, 2900, 4094, 5094):
             ck.prepare(host)
-            fill_oracle_cache(host, pos, seed=7, kvbits=kvbits)
+            fill_oracle_cache(host, min(pos, seq_len), seed=7, kvbits=kvbits)
             want = ck.forward(host, 19, pos)
             ck.release(host)
-            dm.fill_kv(pos, seed=7)
+            dm.fill_kv(min(pos, seq_len), seed=7)
             got = dm.forward(19, pos)
             sigma = float(want.std())
             err = float(np.abs(got - want).max())

@@ -53,11 +53,31 @@ def fill_oracle_cache(model, n_pos, seed, kvbits):
 # no k_attn2 instantiation).  make_plan selects k_attn2 only while a CTA's slice is at most ATTN2_MAXB = 32 blocks and fits
 # its shared memory: at seq_len 16384 the slice is 1024 / 16 = 64 blocks on a 132-SM card (more on fewer SMs), so attn-l8
 # falls back to k_attn and its transposing score path (16 lanes per position, 4 query heads per kv head) for both caches.
+# ("kv", slot) stands for the first position past seq_len whose token lands in cache slot `slot` (a rolled-over cache: slots
+# 0 and 1 hold the re-rotated sinks): slot 2 shares the sinks' block, 15 / 16 sit on a block edge, "last-slice" is in a
+# block the attention's last slice owns, -1 is slot seq_len - 1.  At seq_len 4009 the last 16-position block is a
+# partial bulk copy of 9 positions.
+ROLLED = (("kv", 2), ("kv", 15), ("kv", 16), ("kv", "last-slice"), ("kv", -1))
 LONG_CONTEXT_CASES = {
     "attn-l8": ("attn-l8", 4096, (63, 1023, 2047, 4095), "k_attn2"),
     "tiny-hd256": ("tiny-hd256", 4096, (63, 1023, 2047, 4095), "k_attn"),
     "attn-l8-16k": ("attn-l8", 16384, (5000, 9999, 16383), "k_attn"),  # kv_len 5001 is not a multiple of 16
+    "attn-l8-rolled": ("attn-l8", 4096, ROLLED, "k_attn2"),
+    "attn-l8-4009": ("attn-l8", 4009, (63, 2047, 4000, 4008), "k_attn2"),
+    "attn-l8-4009-rolled": ("attn-l8", 4009, ROLLED, "k_attn2"),
 }
+
+
+def rolled_position(p, seq_len, slices):
+    """A position of LONG_CONTEXT_CASES: an int as it stands, ("kv", slot) resolved for this seq_len and slice count."""
+    if isinstance(p, int):
+        return p
+    slot = p[1]
+    if slot == "last-slice":  # 16-position block b belongs to slice b % slices
+        slot = 16 * (slices * (-(-seq_len // 16) // (2 * slices)) + slices - 1) + 7
+    elif slot < 0:
+        slot += seq_len
+    return seq_len + slot - 2  # kv_pos = 2 + (pos - 2) % (seq_len - 2)
 
 
 @pytest.mark.parametrize("kvbits", [16, 8])
@@ -66,7 +86,8 @@ def test_long_context_attention_vs_oracle(oracle_pkg, case, kvbits, capfd, monke
     """Device vs oracle on identical cache contents, compared value for value, over thousands of positions: the slice
     merge and the exponent accumulation.  attn-l8 (Llama-3-8B's attention geometry) at seq_len 4096 runs k_attn2; at
     seq_len 16384 its slices exceed k_attn2's shared memory and k_attn's transposing score path serves it; tiny-hd256
-    (a 256-wide multi-query head) runs k_attn's plain score path."""
+    (a 256-wide multi-query head) runs k_attn's plain score path.  The rolled-over cases step k_attn2 past seq_len, where
+    it patches the sinks and this token's slot into its early copy of the cache."""
     spec_name, seq_len, positions, kernel = LONG_CONTEXT_CASES[case]
     spec = mg.SPECS[spec_name]
     monkeypatch.delenv("CALM_B200_QUIET", raising=False)  # the plan line names the attention kernel
@@ -76,16 +97,18 @@ def test_long_context_attention_vs_oracle(oracle_pkg, case, kvbits, capfd, monke
     with lib.DeviceModel(spec, host.tensors, seq_len=seq_len, kvbits=kvbits) as dm:
         plan = [l for l in capfd.readouterr().out.splitlines() if l.startswith("# plan: attention ")]
         assert plan and plan[-1].split()[3].rstrip(",") == kernel, plan
-        for pos in positions:
+        for pos in (rolled_position(p, seq_len, int(plan[-1].split()[-2])) for p in positions):
+            # past seq_len the cache is full: fill every slot on both sides, then one step writes slot kv_pos and re-rotates the sinks
             ck.prepare(host)
-            fill_oracle_cache(host, pos, seed=5, kvbits=kvbits)
+            fill_oracle_cache(host, min(pos, seq_len), seed=5, kvbits=kvbits)
             want = ck.forward(host, 17, pos)
             ck.release(host)
-            dm.fill_kv(pos, seed=5)
+            dm.fill_kv(min(pos, seq_len), seed=5)
             got = dm.forward(17, pos)
             sigma = float(want.std())
             err = float(np.abs(got - want).max())
-            print(f"{case} kv{kvbits} pos {pos}: |cuda-oracle| {err:.2e} = {err / sigma:.1e} sigma")
+            kv_pos = pos if pos < seq_len else 2 + (pos - 2) % (seq_len - 2)
+            print(f"{case} kv{kvbits} pos {pos} (slot {kv_pos}): |cuda-oracle| {err:.2e} = {err / sigma:.1e} sigma")
             assert err <= tol * sigma, (pos, err, sigma)
             srt = np.sort(want)
             if srt[-1] - srt[-2] > 2 * tol * sigma:
