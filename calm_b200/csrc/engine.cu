@@ -1273,6 +1273,56 @@ extern "C" void calm_b200_read_kv(struct Transformer* transformer, int layer, in
 	}
 }
 
+// (test aid) One engine buffer as floats, after the stream has drained; see include/calm_b200.h for the selectors.
+extern "C" int calm_b200_read_state(int which, int layer, float* out, int cap) {
+	if (!g.ready) CALM_FATAL("read_state before prepare_cuda");
+	const Config& c = g.cfg;
+	CUDA_CHECK(cudaStreamSynchronize(g.stream));
+	const float* f32 = nullptr;           // a float buffer, copied as it is
+	const __half *hi = nullptr, *lo = nullptr; // a prompt-pass activation pair, summed in float
+	size_t count = 0;
+	switch (which) {
+	case CALM_B200_STATE_X: f32 = g.x, count = c.dim; break;
+	case CALM_B200_STATE_XB: f32 = g.xb, count = c.dim; break;
+	case CALM_B200_STATE_Q: f32 = g.q, count = g.q_dim; break;
+	case CALM_B200_STATE_ATT: f32 = g.att, count = g.q_dim; break;
+	case CALM_B200_STATE_HB: f32 = g.hb, count = (size_t)g.nact * c.hidden_dim; break;
+	case CALM_B200_STATE_MOE_SEL: count = 2 * (size_t)g.nact; break;
+	case CALM_B200_STATE_KEYS:
+	case CALM_B200_STATE_VALUES:
+		if (layer < 0 || layer >= c.n_layers) CALM_FATAL("read_state: layer %d out of range", layer);
+		count = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
+		break;
+	case CALM_B200_STATE_PF_X: f32 = pf.X, count = (size_t)pf.cap * c.dim; break;
+	case CALM_B200_STATE_PF_Q: f32 = pf.Q, count = (size_t)pf.cap * g.q_dim; break;
+	case CALM_B200_STATE_PF_ATT: hi = pf.Ahi, lo = pf.Alo, count = (size_t)pf.cap * g.q_dim; break;
+	case CALM_B200_STATE_PF_HB: hi = pf.Hhi, lo = pf.Hlo, count = (size_t)pf.cap * c.hidden_dim; break;
+	default: CALM_FATAL("read_state: unknown selector %d", which);
+	}
+	if (count > 0x7fffffff) CALM_FATAL("read_state: %zu values do not fit the int the call returns", count);
+	if (!out || (size_t)cap < count || count == 0) return (int)count; // (no prompt pass yet: its matrices are empty)
+	if (f32) {
+		CUDA_CHECK(cudaMemcpy(out, f32, count * sizeof(float), cudaMemcpyDeviceToHost));
+	} else if (hi) {
+		std::vector<__half> h(count), l(count);
+		CUDA_CHECK(cudaMemcpy(h.data(), hi, count * sizeof(__half), cudaMemcpyDeviceToHost));
+		CUDA_CHECK(cudaMemcpy(l.data(), lo, count * sizeof(__half), cudaMemcpyDeviceToHost));
+		for (size_t i = 0; i < count; ++i) out[i] = __half2float(h[i]) + __half2float(l[i]);
+	} else if (which == CALM_B200_STATE_MOE_SEL) {
+		MoeSel sel;
+		CUDA_CHECK(cudaMemcpy(&sel, g.moe_sel, sizeof(sel), cudaMemcpyDeviceToHost));
+		for (int k = 0; k < g.nact; ++k) out[k] = (float)sel.expert[k], out[g.nact + k] = sel.weight[k];
+	} else { // one layer of the cache, [n_kv_heads][seq_len][head_dim]: halves, or e5m2 bytes (the high byte of a half)
+		const size_t es = g.kvbits / 8;
+		std::vector<unsigned char> raw(count * es);
+		const char* base = (const char*)(which == CALM_B200_STATE_KEYS ? g.kc : g.vc) + (size_t)layer * count * es;
+		CUDA_CHECK(cudaMemcpy(raw.data(), base, raw.size(), cudaMemcpyDeviceToHost));
+		for (size_t i = 0; i < count; ++i)
+			out[i] = es == 2 ? __half2float(((const __half*)raw.data())[i]) : __half2float(__ushort_as_half((unsigned short)(raw[i] << 8)));
+	}
+	return (int)count;
+}
+
 extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, uint64_t seed) {
 	(void)transformer;
 	const Config& c = g.cfg;

@@ -25,11 +25,14 @@ SYMBOLS = [
     "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_timer_start", "calm_b200_timer_stop",
-    "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_fill_kv", "calm_b200_matvec",
+    "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
     "calm_b200_tp_unique_id", "calm_b200_tp_init", "calm_b200_tp_world", "calm_b200_tp_mode",
     "calm_b200_decode_sample", "calm_b200_forward_sample", "calm_b200_read_device_logits", "calm_b200_sample_logits",
 ]
+
+# calm_b200_read_state selectors (include/calm_b200.h)
+STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11}
 
 _lib = None
 
@@ -59,6 +62,7 @@ def load() -> C.CDLL:
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
     L.calm_b200_launch_count.argtypes, L.calm_b200_launch_count.restype = [], C.c_uint64
     L.calm_b200_read_kv.argtypes, L.calm_b200_read_kv.restype = [T, C.c_int, C.c_int, _fptr, _fptr], None
+    L.calm_b200_read_state.argtypes, L.calm_b200_read_state.restype = [C.c_int, C.c_int, _fptr, C.c_int], C.c_int
     L.calm_b200_fill_kv.argtypes, L.calm_b200_fill_kv.restype = [T, C.c_int, C.c_uint64], None
     L.calm_b200_matvec.argtypes = [C.c_int, C.c_void_p, _fptr, _fptr, C.c_int, C.c_int, C.c_int, C.c_int]
     L.calm_b200_matvec.restype = C.c_float
@@ -172,6 +176,13 @@ class DeviceModel:
         v = np.zeros(self.spec.kv_dim, np.float32)
         self.lib.calm_b200_read_kv(C.byref(self.transformer), layer, kv_pos, k.ctypes.data_as(_fptr), v.ctypes.data_as(_fptr))
         return k, v
+
+    def read_state(self, which: str, layer: int = 0) -> np.ndarray:
+        """calm_b200_read_state: one engine buffer (a key of STATE) as a flat float32 array, for stage-level tests."""
+        n = self.lib.calm_b200_read_state(STATE[which], layer, None, 0)
+        out = np.zeros(n, np.float32)
+        assert self.lib.calm_b200_read_state(STATE[which], layer, out.ctypes.data_as(_fptr), n) == n
+        return out
 
     def fill_kv(self, n_pos: int, seed: int = 1) -> None:
         self.lib.calm_b200_fill_kv(C.byref(self.transformer), n_pos, seed)

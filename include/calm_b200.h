@@ -144,6 +144,27 @@ uint64_t calm_b200_launch_count(void);
  * (kv_dim values each, reference infer.c:378-381); for parity tests. */
 void calm_b200_read_kv(struct Transformer* transformer, int layer, int kv_pos, float* k_out, float* v_out);
 
+/* (test aid) Copy one of the engine's buffers to the host as floats, after waiting for the library's stream, so a test
+ * can check what each stage of the last token (or of the last prompt pass) wrote.  Returns the number of floats the
+ * buffer holds; nothing is copied when `out` is NULL or `cap` is smaller than that.  `layer` is read by the two cache
+ * selectors only.  With one layer nothing overwrites a stage's output before the token ends; with more, the
+ * activation buffers hold the last layer's values.  No kernel is launched and nothing on the token path changes.
+ *   X        float[dim]                   residual stream (after the last w2)
+ *   XB       float[dim]                   the attention norm's output that parallel-norm models keep for the FFN
+ *   Q        float[q_dim]                 rotated queries                          ATT  float[q_dim]  attention output
+ *   HB       float[n_active][hidden]      gated FFN hidden vector (one row per active expert; dense models: one row)
+ *   MOE_SEL  float[2 * n_active]          the router's experts (as floats), then their weights
+ *   KEYS, VALUES  float[n_kv_heads][seq_len][head_dim]   one layer of the cache, every slot, decoded from fp16 / e5m2
+ *   PF_X, PF_Q, PF_ATT, PF_HB   float[rows][dim | q_dim | q_dim | hidden]   the prompt pass's residual stream, rotated
+ *            queries, attention output and FFN hidden matrix (the last two kept as f16 hi + lo pairs, summed here in
+ *            float); rows = the pass's token tiles (a multiple of 128, at least n), of the last block of <= 2048 tokens */
+enum {
+	CALM_B200_STATE_X = 0, CALM_B200_STATE_XB = 1, CALM_B200_STATE_Q = 2, CALM_B200_STATE_ATT = 3, CALM_B200_STATE_HB = 4,
+	CALM_B200_STATE_MOE_SEL = 5, CALM_B200_STATE_KEYS = 6, CALM_B200_STATE_VALUES = 7,
+	CALM_B200_STATE_PF_X = 8, CALM_B200_STATE_PF_Q = 9, CALM_B200_STATE_PF_ATT = 10, CALM_B200_STATE_PF_HB = 11
+};
+int calm_b200_read_state(int which, int layer, float* out, int cap);
+
 /* Fill the KV cache positions [0, n_pos) of every layer with a deterministic
  * pseudo-random pattern (bench: decode at a late position without running the
  * whole prefix). */
