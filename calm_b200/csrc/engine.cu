@@ -134,11 +134,18 @@ struct Prefill {
 	float2* rope = nullptr;
 	int* tokens = nullptr;
 	CUtensorMap tmN[2], tmA[2], tmH[2]; // (hi, lo) views of the three activation matrices the GEMMs read
+	// scoring (calm_b200_score), allocated on its first call for `cap` rows: the classifier's per-tile records, the targets'
+	// logits, the targets and the log-probabilities
+	bool scoring = false;
+	float2* part = nullptr; // [cap][cdiv(vocab, PF_BM)]
+	float *tgt = nullptr, *logprob = nullptr;
+	int* targets = nullptr;
 };
 Prefill pf;
 
 void pf_free() {
 	cudaFree(pf.X), cudaFree(pf.Q), cudaFree(pf.Nhi), cudaFree(pf.Nlo), cudaFree(pf.Ahi), cudaFree(pf.Alo), cudaFree(pf.Hhi), cudaFree(pf.Hlo), cudaFree(pf.rope), cudaFree(pf.tokens);
+	cudaFree(pf.part), cudaFree(pf.tgt), cudaFree(pf.logprob), cudaFree(pf.targets);
 	pf = Prefill();
 }
 
@@ -1195,6 +1202,58 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0) {
 	}
 }
 
+// The scoring buffers for pf.cap rows (freed and re-made with the pass's own buffers when a longer block needs more rows)
+static void pf_score_reserve() {
+	if (pf.scoring) return;
+	const int nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	pf.part = (float2*)dev_alloc((size_t)pf.cap * nvt * sizeof(float2));
+	pf.tgt = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
+	pf.logprob = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
+	pf.targets = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
+	pf.scoring = true;
+}
+
+// After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records
+template <int DBITS, typename KVT>
+static void pf_score(Formats<DBITS, KVT>, int n) {
+	const Config& c = g.cfg;
+	const Weights& w = g.w;
+	const int nvt = cdiv(c.vocab_size, PF_BM);
+	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
+	PfGemmArgs a = {};
+	a.n_tokens = n, a.w[0] = w.wcls, a.K = c.dim;
+	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size;
+	pf_gemm<PF_CLS, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
+	launch_pdl(k_pf_logprob, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt);
+}
+
+// The batched pass over tokens[0 .. n) at positions pos0 .., in blocks of at most 2048 rows.  With `logprobs`, every block
+// is scored as well: logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]], so tokens[n] must exist.
+static void pf_pass(const int* tokens, int n, int pos0, float* logprobs) {
+	const int chunk_cap = 2048;
+	for (int o = 0; o < n; o += chunk_cap) {
+		const int m = n - o < chunk_cap ? n - o : chunk_cap;
+		pf_reserve(m);
+		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		if (logprobs) {
+			pf_score_reserve();
+			CUDA_CHECK(cudaMemcpyAsync(pf.targets, tokens + o + 1, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		}
+		with_formats([&](auto f) { pf_run(f, m, pos0 + o); });
+		if (logprobs) {
+			with_formats([&](auto f) { pf_score(f, m); });
+			CUDA_CHECK(cudaMemcpyAsync(logprobs + o, pf.logprob, (size_t)m * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+		}
+		CUDA_CHECK(cudaStreamSynchronize(g.stream)); // `tokens` is the caller's memory (pageable): the copy above must have left it
+	}
+	CUDA_CHECK(cudaGetLastError());
+}
+
+static void check_tokens(const int* tokens, int n) {
+	for (int i = 0; i < n; ++i)
+		if (tokens[i] < 0 || tokens[i] >= g.cfg.vocab_size) CALM_FATAL("token %d out of range", tokens[i]);
+}
+
 // Feed `n` prompt tokens at positions pos0 .. pos0 + n - 1: the KV cache afterwards is what n calls of
 // forward_cuda(token, pos, FF_UPDATE_KV_ONLY) leave (within the stated tolerance); no logits, no synchronisation.
 // Returns 1 when the tensor-core pass ran, 0 when the tokens were fed one by one (unsupported model shape, MoE, tensor
@@ -1202,8 +1261,7 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0) {
 extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* tokens, int n, int pos0) {
 	if (n <= 0) return 1;
 	check_call(transformer, tokens[0], pos0);
-	for (int i = 0; i < n; ++i)
-		if (tokens[i] < 0 || tokens[i] >= g.cfg.vocab_size) CALM_FATAL("token %d out of range", tokens[i]);
+	check_tokens(tokens, n);
 	if (!pf_supported() || pos0 + n > g.cfg.seq_len) {
 		for (int i = 0; i < n; ++i) {
 			set_params(tokens[i], pos0 + i, 0);
@@ -1211,15 +1269,34 @@ extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* 
 		}
 		return 0;
 	}
-	const int chunk_cap = 2048;
-	for (int o = 0; o < n; o += chunk_cap) {
-		const int m = n - o < chunk_cap ? n - o : chunk_cap;
-		pf_reserve(m);
-		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		with_formats([&](auto f) { pf_run(f, m, pos0 + o); });
-		CUDA_CHECK(cudaStreamSynchronize(g.stream)); // `tokens` is the caller's memory (pageable): the copy above must have left it
+	pf_pass(tokens, n, pos0, nullptr);
+	return 1;
+}
+
+// Score tokens[1 .. n) given what precedes each (the reference's study(), run.c:291-308): tokens[0 .. n - 1) go through
+// the prompt pass and logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]].  The cache is left as
+// forward_prefill_cuda(tokens, n - 1, pos0) leaves it.  Shapes the pass does not serve go one position at a time through
+// the decode path with a log-softmax in double on the host (returns 0).
+extern "C" int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs) {
+	if (n < 2) return 1;
+	check_call(transformer, tokens[0], pos0);
+	check_tokens(tokens, n);
+	const int rows = n - 1, vocab = g.cfg.vocab_size;
+	if (!pf_supported() || pos0 + rows > g.cfg.seq_len) {
+		for (int i = 0; i < rows; ++i) {
+			set_params(tokens[i], pos0 + i, 0);
+			launch_token(1);
+			sync_stream();
+			const float* l = g.logits_host;
+			double mx = l[0], s = 0.0;
+			for (int v = 1; v < vocab; ++v) mx = l[v] > mx ? l[v] : mx;
+			for (int v = 0; v < vocab; ++v) s += exp((double)l[v] - mx);
+			logprobs[i] = (float)((double)l[tokens[i + 1]] - mx - log(s));
+		}
+		CUDA_CHECK(cudaGetLastError());
+		return 0;
 	}
-	CUDA_CHECK(cudaGetLastError());
+	pf_pass(tokens, rows, pos0, logprobs);
 	return 1;
 }
 

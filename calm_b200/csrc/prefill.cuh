@@ -17,6 +17,11 @@
 //               softmax; reference infer.c:238-267), one warp per query token, K/V tiles staged in shared memory.
 //   k_pf_norm   RMSNorm / LayerNorm per token (reference infer.c:183-207) -> hi / lo f16 rows.
 //
+// Scoring (calm_b200_score, the reference's study(): run.c:291-308) adds the classifier over all rows of the block without
+// ever writing the [T][vocab] logits: the final norm (k_pf_norm), k_pf_gemm in PF_CLS mode, whose epilogue reduces each
+// token's 128 logits of the tile to one (max, sum exp(logit - max)) record and keeps the target's logit, and k_pf_logprob,
+// which merges a token's records in a fixed order into ln softmax(logits)[target].
+//
 // Parity contract (tests/test_prefill_gpu.py): after forward_prefill_cuda(tokens, n, pos0) the KV cache and the logits of
 // the following token equal those of n serial forward(FF_UPDATE_KV_ONLY) calls within the stated tolerances.
 #pragma once
@@ -29,7 +34,7 @@
 #define PF_BN 128 // tokens per tile       (two consumer warpgroups of 64: the M of the MMA)
 #define PF_BK 64  // k per stage: 64 f16 = 128 bytes = one swizzle atom
 #define PF_THREADS 384 // warpgroup 0: dequantising producers (thread 0 also issues the TMA); warpgroups 1, 2: MMA + epilogue
-enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3 };
+enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3, PF_CLS = 4 };
 
 // ---------------------------------------------------------------- wgmma / TMA wrappers
 __device__ __forceinline__ void wgmma_fence() { // accumulator registers written by ordinary instructions -> visible to wgmma
@@ -166,6 +171,11 @@ struct PfGemmArgs {
 	__half* Hhi;
 	__half* Hlo;
 	int hidden, gelu;
+	// CLS epilogue: w[0] = the classifier [vocab][K], one CTA column per 128 vocabulary rows
+	const int* targets; // [T] the token whose log-probability is wanted after each row
+	float2* part;       // [T][gridDim.x] (max, sum exp(logit - max)) of the token's logits in each vocabulary tile
+	float* tgt;         // [T] logit of the target
+	int vocab;
 };
 
 // 64 weights of one row (one k-stage) -> 8 swizzled 16-byte chunks of f16 in the weight tile
@@ -257,6 +267,8 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 			} else if constexpr (MODE == PF_UP) {
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)gr * rowbytes;
 				rowp[1] = reinterpret_cast<const unsigned char*>(a.w[1]) + (size_t)gr * rowbytes;
+			} else if constexpr (MODE == PF_CLS) { // the last vocabulary tile may be partial: its spare rows repeat the last row
+				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)min(gr, a.vocab - 1) * rowbytes;
 			} else {
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)gr * rowbytes;
 			}
@@ -317,6 +329,41 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 		// accumulator fragment of m64nN: register 4 j + 2 h + e holds token 16 w + lane / 4 + 8 h, weight row 8 j + 2 (lane % 4) + e
 		const int w4 = warp & 3;
 		const int tb = tok0 + c * 64 + w4 * 16 + (lane >> 2);
+		if constexpr (MODE == PF_CLS) {
+			// the quad of lanes 4 (lane / 4) .. + 3 holds all 128 logits of tokens tb and tb + 8: 32 per lane, then two shuffles.
+			// Every lane runs the shuffles; only the stores are masked to the block's tokens.
+			const int q = lane & 3;
+#pragma unroll
+			for (int h = 0; h < 2; ++h) {
+				const int t = tb + 8 * h;
+				float m = -FLT_MAX;
+#pragma unroll
+				for (int j = 0; j < PF_BM / 8; ++j)
+#pragma unroll
+					for (int e = 0; e < 2; ++e)
+						if (row0 + 8 * j + 2 * q + e < a.vocab) m = fmaxf(m, acc[0][4 * j + 2 * h + e]);
+				m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+				m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+				float s = 0.f;
+#pragma unroll
+				for (int j = 0; j < PF_BM / 8; ++j)
+#pragma unroll
+					for (int e = 0; e < 2; ++e)
+						if (row0 + 8 * j + 2 * q + e < a.vocab) s += expf(acc[0][4 * j + 2 * h + e] - m);
+				s += __shfl_xor_sync(0xffffffffu, s, 1);
+				s += __shfl_xor_sync(0xffffffffu, s, 2);
+				if (t < a.n_tokens) {
+					const int tr = a.targets[t] - row0; // the target's row in this tile, if it lies here
+#pragma unroll
+					for (int j = 0; j < PF_BM / 8; ++j)
+#pragma unroll
+						for (int e = 0; e < 2; ++e)
+							if (8 * j + 2 * q + e == tr) a.tgt[t] = acc[0][4 * j + 2 * h + e];
+					if (q == 0) a.part[(size_t)t * gridDim.x + blockIdx.x] = make_float2(m, s);
+				}
+			}
+			return;
+		}
 #pragma unroll
 		for (int j = 0; j < PF_BM / 8; ++j) {
 			const int gr = row0 + 8 * j + 2 * (lane & 3); // even: (gr, gr + 1) is a RoPE pair
@@ -357,6 +404,33 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 			}
 		}
 	}
+}
+
+// ---------------------------------------------------------------- scoring: log-probability of each row's target
+// One warp per token: merge the nvt (max, sum) records of the PF_CLS tiles, lane-strided and then by a butterfly, in an
+// order fixed by nvt alone (no atomics), so that repeated calls give the same bits.  logprob = tgt - M - ln S with
+// M = max m_v and S = sum s_v exp(m_v - M).
+__device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
+	const float mn = fmaxf(m, m2);
+	s = s * expf(m - mn) + s2 * expf(m2 - mn);
+	m = mn;
+}
+__global__ void __launch_bounds__(256) k_pf_logprob(const float2* part, const float* tgt, float* logprob, int n, int nvt) {
+	pdl_enter();
+	const int t = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+	if (t >= n) return;
+	const float2* p = part + (size_t)t * nvt;
+	float m = -FLT_MAX, s = 0.f;
+	for (int v = lane; v < nvt; v += 32) {
+		const float2 r = p[v];
+		lse_merge(m, s, r.x, r.y);
+	}
+#pragma unroll
+	for (int o = 16; o > 0; o >>= 1) { // lane 0's result: a fixed tree over the lanes
+		const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+		lse_merge(m, s, m2, s2);
+	}
+	if (lane == 0) logprob[t] = tgt[t] - m - logf(s);
 }
 
 // ---------------------------------------------------------------- causal attention of the block against the cache

@@ -22,7 +22,7 @@ _fptr = C.POINTER(C.c_float)
 
 # every symbol include/calm_b200.h declares
 SYMBOLS = [
-    "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda",
+    "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda", "calm_b200_score",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_fill_kv", "calm_b200_matvec",
@@ -51,6 +51,7 @@ def load() -> C.CDLL:
     L.forward_cuda.argtypes, L.forward_cuda.restype = [T, C.c_int, C.c_int, C.c_uint], _fptr
     L.perf_cuda.argtypes, L.perf_cuda.restype = [], None
     L.forward_prefill_cuda.argtypes, L.forward_prefill_cuda.restype = [T, C.POINTER(C.c_int), C.c_int, C.c_int], C.c_int
+    L.calm_b200_score.argtypes, L.calm_b200_score.restype = [T, C.POINTER(C.c_int), C.c_int, C.c_int, _fptr], C.c_int
     L.calm_b200_abi_version.argtypes, L.calm_b200_abi_version.restype = [], C.c_int
     L.calm_b200_set_device.argtypes, L.calm_b200_set_device.restype = [C.c_int], None
     L.calm_b200_free.argtypes, L.calm_b200_free.restype = [C.c_void_p], None
@@ -144,6 +145,14 @@ class DeviceModel:
         """forward_prefill_cuda: the batched prompt pass; returns 1 (tensor-core pass) or 0 (fed token by token)."""
         arr = np.ascontiguousarray(tokens, np.int32)
         return self.lib.forward_prefill_cuda(C.byref(self.transformer), arr.ctypes.data_as(C.POINTER(C.c_int)), len(arr), pos0)
+
+    def score(self, tokens, pos0: int = 0):
+        """calm_b200_score: (log-probabilities of tokens[1:] after what precedes each, as float32[n - 1], 1 when the
+        tensor-core pass served it or 0 when the decode path did)."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        out = np.zeros(max(len(arr) - 1, 0), np.float32)
+        served = self.lib.calm_b200_score(C.byref(self.transformer), arr.ctypes.data_as(C.POINTER(C.c_int)), len(arr), pos0, out.ctypes.data_as(_fptr))
+        return out, served
 
     def forward_raw(self, token: int, pos: int, flags: int = 0):
         return self.lib.forward_cuda(C.byref(self.transformer), token, pos, flags)

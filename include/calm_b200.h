@@ -95,7 +95,7 @@ int calm_b200_tp_mode(void);
 
 /* The prompt as ONE batched pass (the reference feeds prompt tokens one at a time through forward(.., FF_UPDATE_KV_ONLY),
  * run.c:206-209, README.md:80): n tokens at positions pos0 .. pos0+n-1 go through every layer together; the projections
- * are tensor-core GEMMs (tcgen05.mma, TMEM accumulators, weights dequantised on the fly, activations as an f16 hi + lo
+ * are tensor-core GEMMs (wgmma.mma_async, accumulators in registers, weights dequantised on the fly, activations as an f16 hi + lo
  * pair so inputs keep 22 bits), attention is causal over the block and the cache.  Afterwards the KV cache holds what n
  * serial KV-only calls would have left (within the stated tolerance); no logits, no synchronisation with the host beyond
  * reading `tokens`.  Returns 1 when the batched pass ran, 0 when the model shape is not served by it (MoE, tensor
@@ -103,6 +103,19 @@ int calm_b200_tp_mode(void);
  * tokens were fed one by one instead -- same result either way.  A host integrates it by replacing the prompt loop:
  * forward_prefill_cuda(t, prompt, n - 1, 0); logits = forward_cuda(t, prompt[n - 1], n - 1, 0);  (INTEGRATION.md). */
 int forward_prefill_cuda(struct Transformer* transformer, const int* tokens, int n, int pos0);
+
+/* Score a token sequence: what the reference's study() computes one forward() at a time (run.c:291-308).
+ * tokens[0 .. n-2] go through the batched prompt pass at positions pos0 .. pos0+n-2, and
+ *   logprobs[i] = ln softmax(logits after tokens[i] at pos0+i)[tokens[i+1]],   i in [0, n-1).
+ * The classifier runs over all n-1 rows on the tensor cores with the log-softmax fused into its epilogue, so the
+ * [n-1][vocab] logits are never written.  Afterwards the KV cache holds exactly what forward_prefill_cuda(t, tokens, n-1,
+ * pos0) leaves; the last token is only a target.  Every token, the target included, must be in the vocabulary.
+ * Returns 1 when the tensor-core pass ran.  Returns 0 when the positions went one by one through the decode path (the
+ * shapes forward_prefill_cuda does not serve, or pos0+n-1 > seq_len); both give the same values within the stated
+ * tolerance (DESIGN.md s.6).  n < 2: nothing to score, the cache is untouched, returns 1.  Under tensor parallelism every
+ * rank calls it with the same arguments, as with forward_cuda.  Perplexity over a text in chunks of m positions:
+ * chunk c is calm_b200_score(t, tokens + c, m + 1, 0, out + c)  (INTEGRATION.md). */
+int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs);
 
 /* forward + device-side greedy sample.  Returns argmax(logits) with the
  * reference's tie rule (lowest index, sampler.c:34-42).  The logits are still
