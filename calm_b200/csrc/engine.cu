@@ -1126,7 +1126,7 @@ static void pf_reserve(int n) {
 	pf.cap = cap;
 	auto zalloc = [&](size_t bytes) {
 		void* p = dev_alloc(bytes);
-		CUDA_CHECK(cudaMemset(p, 0, bytes)); // padding rows of a partial token tile stay zero
+		CUDA_CHECK(cudaMemset(p, 0, bytes)); // defined bytes for the first pass; later, padding rows of a partial token tile hold an earlier pass's values
 		return p;
 	};
 	pf.X = (float*)zalloc((size_t)cap * c.dim * sizeof(float));
@@ -1410,6 +1410,46 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 	else
 		k_fill_kv<__half><<<g.sms * 4, 256, 0, g.stream>>>((__half*)g.kc, (__half*)g.vc, lh, c.seq_len, c.head_dim, n_pos, seed);
 	++g_launches;
+	CUDA_CHECK(cudaStreamSynchronize(g.stream));
+}
+
+// (test aid) 0xFF bytes (NaN as f32, f16 and e5m2) into every buffer whose previous contents no later call may depend on,
+// and into the cache slots [kv_from_pos, seq_len) of every layer and kv head.  Only data is touched: TokenParams, the
+// attention's {value, epoch} cells and counter, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
+// counts, stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
+// as do the index buffers (cand_idx, sample_idx, out_tokens, pf.tokens, pf.targets): a stale index that is read is in range,
+// as after any earlier call, while 0xFFFFFFFF would send the read out of bounds.  DESIGN.md s.3 lists both groups.
+extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos) {
+	(void)transformer;
+	if (!g.ready) CALM_FATAL("poison_state before prepare_cuda");
+	if (kv_from_pos < 0) CALM_FATAL("poison_state: negative position");
+	const Config& c = g.cfg;
+	CUDA_CHECK(cudaStreamSynchronize(g.stream));
+	auto nan = [](void* p, size_t bytes) {
+		if (p) CUDA_CHECK(cudaMemsetAsync(p, 0xFF, bytes, g.stream));
+	};
+	nan(g.x, c.dim * sizeof(float)), nan(g.xb, c.dim * sizeof(float)), nan(g.xpart, c.dim * sizeof(float));
+	nan(g.q, g.q_dim * sizeof(float)), nan(g.att, g.q_dim * sizeof(float));
+	nan(g.hb, (size_t)g.nact * c.hidden_dim * sizeof(float));
+	nan(g.logits_dev, (size_t)c.vocab_size * sizeof(float));
+	nan(g.attn_partial, (size_t)c.n_kv_heads * g.attn_qgroups * g.attn_nsplit * g.attn_hg * (c.head_dim + 2) * sizeof(float));
+	nan(g.cand_val, g.ncand * sizeof(float));
+	nan(g.rope_cs, (size_t)(c.head_dim / 2) * sizeof(float2));
+	nan(g.sample_prob, (size_t)g.sample_chunks * SAMPLE_CHUNK * sizeof(float)), nan(g.sample_csum, g.sample_chunks * sizeof(float));
+	if (pf.cap) { // every row of the prompt pass's matrices, the padding rows of a partial token tile included
+		const size_t cap = pf.cap;
+		nan(pf.X, cap * c.dim * sizeof(float)), nan(pf.Q, cap * g.q_dim * sizeof(float));
+		nan(pf.Nhi, cap * c.dim * sizeof(__half)), nan(pf.Nlo, cap * c.dim * sizeof(__half));
+		nan(pf.Ahi, cap * g.q_dim * sizeof(__half)), nan(pf.Alo, cap * g.q_dim * sizeof(__half));
+		nan(pf.Hhi, cap * c.hidden_dim * sizeof(__half)), nan(pf.Hlo, cap * c.hidden_dim * sizeof(__half));
+		nan(pf.rope, cap * (c.head_dim / 2) * sizeof(float2));
+		if (pf.scoring) nan(pf.part, cap * cdiv(c.vocab_size, PF_BM) * sizeof(float2)), nan(pf.tgt, cap * sizeof(float)), nan(pf.logprob, cap * sizeof(float));
+	}
+	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
+		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;
+		for (void* cache : {g.kc, g.vc})
+			CUDA_CHECK(cudaMemset2DAsync((char*)cache + kv_from_pos * slot, pitch, 0xFF, width, (size_t)c.n_layers * c.n_kv_heads, g.stream));
+	}
 	CUDA_CHECK(cudaStreamSynchronize(g.stream));
 }
 

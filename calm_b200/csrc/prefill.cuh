@@ -123,7 +123,8 @@ __global__ void k_pf_rope(float2* rope, const float* freq, int n, int half_hd, i
 	rope[i] = make_float2(c, s);
 }
 
-// one CTA per token: norm (infer.c:183-207) then hi / lo split; rows beyond n (tile padding) are zeroed once at allocation
+// one CTA per token: norm (infer.c:183-207) then hi / lo split; rows beyond n (tile padding) are not written and hold whatever
+// an earlier, longer pass left: a GEMM's output column depends on its own token's row only, and every epilogue drops t >= n
 __global__ void __launch_bounds__(256) k_pf_norm(const float* X, const float* normw, __half* hi, __half* lo, int n, int dim, float eps, int ln) {
 	pdl_enter();
 	__shared__ float red[32];

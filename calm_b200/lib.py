@@ -25,7 +25,7 @@ SYMBOLS = [
     "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda", "calm_b200_score",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_timer_start", "calm_b200_timer_stop",
-    "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_fill_kv", "calm_b200_matvec",
+    "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
     "calm_b200_tp_unique_id", "calm_b200_tp_init", "calm_b200_tp_world", "calm_b200_tp_mode",
     "calm_b200_decode_sample", "calm_b200_forward_sample", "calm_b200_read_device_logits", "calm_b200_sample_logits",
@@ -64,6 +64,7 @@ def load() -> C.CDLL:
     L.calm_b200_launch_count.argtypes, L.calm_b200_launch_count.restype = [], C.c_uint64
     L.calm_b200_read_kv.argtypes, L.calm_b200_read_kv.restype = [T, C.c_int, C.c_int, _fptr, _fptr], None
     L.calm_b200_read_state.argtypes, L.calm_b200_read_state.restype = [C.c_int, C.c_int, _fptr, C.c_int], C.c_int
+    L.calm_b200_poison_state.argtypes, L.calm_b200_poison_state.restype = [T, C.c_int], None
     L.calm_b200_fill_kv.argtypes, L.calm_b200_fill_kv.restype = [T, C.c_int, C.c_uint64], None
     L.calm_b200_matvec.argtypes = [C.c_int, C.c_void_p, _fptr, _fptr, C.c_int, C.c_int, C.c_int, C.c_int]
     L.calm_b200_matvec.restype = C.c_float
@@ -172,6 +173,12 @@ class DeviceModel:
         self.lib.calm_b200_decode_sample(C.byref(self.transformer), token0, pos0, n, temperature, minp, C.byref(rng), out.ctypes.data_as(C.POINTER(C.c_int)))
         return out, int(rng.value)
 
+    def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
+        """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""
+        rng = C.c_ulonglong(rng_state)
+        tok = self.lib.calm_b200_forward_sample(C.byref(self.transformer), token, pos, temperature, minp, C.byref(rng))
+        return int(tok), int(rng.value)
+
     def device_logits(self) -> np.ndarray:
         out = np.zeros(self.vocab, np.float32)
         self.lib.calm_b200_read_device_logits(out.ctypes.data_as(_fptr))
@@ -192,6 +199,10 @@ class DeviceModel:
         out = np.zeros(n, np.float32)
         assert self.lib.calm_b200_read_state(STATE[which], layer, out.ctypes.data_as(_fptr), n) == n
         return out
+
+    def poison(self, kv_from_pos: int) -> None:
+        """calm_b200_poison_state: NaN bytes into every scratch buffer and the cache slots [kv_from_pos, seq_len)."""
+        self.lib.calm_b200_poison_state(C.byref(self.transformer), kv_from_pos)
 
     def fill_kv(self, n_pos: int, seed: int = 1) -> None:
         self.lib.calm_b200_fill_kv(C.byref(self.transformer), n_pos, seed)

@@ -178,6 +178,13 @@ enum {
 };
 int calm_b200_read_state(int which, int layer, float* out, int cap);
 
+/* (test aid) Overwrite with 0xFF bytes (NaN as f32, f16 and e5m2) every buffer whose previous contents must not influence
+ * any later call, and the KV-cache slots [kv_from_pos, seq_len) of every layer and kv head (kv_from_pos >= seq_len: none).
+ * Waits for the library's stream before and after.  Launches no kernel of the token path; changes no kernel.
+ * What steers control flow, a wait or an address (token parameters, the attention's fold cells and counter, the
+ * tensor-parallel exchange area, router and sampler state, index buffers, weights) is left alone: DESIGN.md s.3. */
+void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos);
+
 /* Fill the KV cache positions [0, n_pos) of every layer with a deterministic
  * pseudo-random pattern (bench: decode at a late position without running the
  * whole prefix). */
