@@ -12,6 +12,7 @@
 #include <math.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "stages.cuh"
@@ -133,6 +134,7 @@ struct Prefill {
 	__half *Nhi = nullptr, *Nlo = nullptr, *Ahi = nullptr, *Alo = nullptr, *Hhi = nullptr, *Hlo = nullptr;
 	float2* rope = nullptr;
 	int* tokens = nullptr;
+	int *rowpos = nullptr, *seg = nullptr; // packed blocks (calm_b200_score_batch): a row's RoPE position, its sequence's first row
 	CUtensorMap tmN[2], tmA[2], tmH[2]; // (hi, lo) views of the three activation matrices the GEMMs read
 	// scoring (calm_b200_score), allocated on its first call for `cap` rows: the classifier's per-tile records, the targets'
 	// logits, the targets and the log-probabilities
@@ -145,6 +147,7 @@ Prefill pf;
 
 void pf_free() {
 	cudaFree(pf.X), cudaFree(pf.Q), cudaFree(pf.Nhi), cudaFree(pf.Nlo), cudaFree(pf.Ahi), cudaFree(pf.Alo), cudaFree(pf.Hhi), cudaFree(pf.Hlo), cudaFree(pf.rope), cudaFree(pf.tokens);
+	cudaFree(pf.rowpos), cudaFree(pf.seg);
 	cudaFree(pf.part), cudaFree(pf.tgt), cudaFree(pf.logprob), cudaFree(pf.targets);
 	pf = Prefill();
 }
@@ -1136,6 +1139,7 @@ static void pf_reserve(int n) {
 	pf.Hhi = (__half*)zalloc((size_t)cap * c.hidden_dim * sizeof(__half)), pf.Hlo = (__half*)zalloc((size_t)cap * c.hidden_dim * sizeof(__half));
 	pf.rope = (float2*)zalloc((size_t)cap * (c.head_dim / 2) * sizeof(float2));
 	pf.tokens = (int*)zalloc((size_t)cap * sizeof(int));
+	pf.rowpos = (int*)zalloc((size_t)cap * sizeof(int)), pf.seg = (int*)zalloc((size_t)cap * sizeof(int));
 	pf_make_map(&pf.tmN[0], pf.Nhi, cap, c.dim), pf_make_map(&pf.tmN[1], pf.Nlo, cap, c.dim);
 	pf_make_map(&pf.tmA[0], pf.Ahi, cap, g.q_dim), pf_make_map(&pf.tmA[1], pf.Alo, cap, g.q_dim);
 	pf_make_map(&pf.tmH[0], pf.Hhi, cap, c.hidden_dim), pf_make_map(&pf.tmH[1], pf.Hlo, cap, c.hidden_dim);
@@ -1154,21 +1158,24 @@ static void pf_gemm(const CUtensorMap* tm, const PfGemmArgs& a, int rows, int n)
 	launch_pdl(k_pf_gemm<MODE, DBITS, KVT>, dim3(rows / PF_BM, cdiv(n, PF_BN)), PF_THREADS, pf_smem_bytes<MODE>(), tm[0], tm[1], a);
 }
 
-template <typename KVT, int HD>
+template <typename KVT, int HD, bool SEG>
 static void pf_attn(const PfAttnArgs& a, int n) {
 	const dim3 grid(cdiv(n, PFA_WARPS), g.cfg.n_kv_heads);
-	if (g.kv_mul % 4 == 0) launch_pdl(k_pf_attn<KVT, HD, 4>, grid, PFA_WARPS * 32, 0, a);
-	else if (g.kv_mul % 2 == 0) launch_pdl(k_pf_attn<KVT, HD, 2>, grid, PFA_WARPS * 32, 0, a);
-	else launch_pdl(k_pf_attn<KVT, HD, 1>, grid, PFA_WARPS * 32, 0, a);
+	if (g.kv_mul % 4 == 0) launch_pdl(k_pf_attn<KVT, HD, 4, SEG>, grid, PFA_WARPS * 32, 0, a);
+	else if (g.kv_mul % 2 == 0) launch_pdl(k_pf_attn<KVT, HD, 2, SEG>, grid, PFA_WARPS * 32, 0, a);
+	else launch_pdl(k_pf_attn<KVT, HD, 1, SEG>, grid, PFA_WARPS * 32, 0, a);
 }
 
+// The pass over the n rows in pf.tokens at cache slots pos0 + t.  packed: a block of independent sequences
+// (calm_b200_score_batch, pos0 = 0), with per-row RoPE positions in pf.rowpos and each row's sequence start in pf.seg.
 template <int DBITS, typename KVT>
-static void pf_run(Formats<DBITS, KVT>, int n, int pos0) {
+static void pf_run(Formats<DBITS, KVT>, int n, int pos0, bool packed = false) {
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
 	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
-	launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
+	if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
+	else launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
 	for (int l = 0; l < c.n_layers; ++l) {
 		launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_att_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
 		PfGemmArgs a = {};
@@ -1182,8 +1189,14 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0) {
 		PfAttnArgs aa = {};
 		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
 		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
-		if (c.head_dim == 128) pf_attn<KVT, 128>(aa, n);
-		else pf_attn<KVT, 64>(aa, n);
+		aa.seg = pf.seg;
+		if (packed) {
+			if (c.head_dim == 128) pf_attn<KVT, 128, true>(aa, n);
+			else pf_attn<KVT, 64, true>(aa, n);
+		} else {
+			if (c.head_dim == 128) pf_attn<KVT, 128, false>(aa, n);
+			else pf_attn<KVT, 64, false>(aa, n);
+		}
 
 		PfGemmArgs b = {};
 		b.n_tokens = n, b.w[0] = w.wo[l], b.K = g.q_dim, b.X = pf.X, b.dim = c.dim;
@@ -1298,6 +1311,76 @@ extern "C" int calm_b200_score(struct Transformer* transformer, const int* token
 	}
 	pf_pass(tokens, rows, pos0, logprobs);
 	return 1;
+}
+
+// One packed block of calm_b200_score_batch: sequence seqs[k] takes rows [s, s + R) with R = its rows rounded up to 8, RoPE
+// positions 0 .. R - 1 and cache slots s .. s + R - 1.  Its filler rows (after the live ones) repeat its last input token
+// and target its last token; causal attention keeps them out of every live row, and their results are dropped.
+static void pf_score_block(const int* tokens, const int* off, const int* len, const std::vector<int>& seqs, int rows, float* logprobs) {
+	std::vector<int> tok(rows), tgt(rows), pos(rows), seg(rows);
+	std::vector<float> lp(rows);
+	for (int k = 0, s = 0; k < (int)seqs.size(); ++k) {
+		const int* t = tokens + off[seqs[k]];
+		const int r = len[seqs[k]] - 1, R = cdiv(r, 8) * 8;
+		for (int j = 0; j < R; ++j) tok[s + j] = t[imin(j, r - 1)], tgt[s + j] = t[imin(j + 1, r)], pos[s + j] = j, seg[s + j] = s;
+		s += R;
+	}
+	pf_reserve(rows);
+	pf_score_reserve();
+	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.targets, tgt.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.seg, seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	with_formats([&](auto f) { pf_run(f, rows, 0, true); });
+	with_formats([&](auto f) { pf_score(f, rows); });
+	CUDA_CHECK(cudaMemcpyAsync(lp.data(), pf.logprob, (size_t)rows * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+	CUDA_CHECK(cudaStreamSynchronize(g.stream));
+	CUDA_CHECK(cudaGetLastError());
+	for (int k = 0, s = 0; k < (int)seqs.size(); ++k) {
+		const int r = len[seqs[k]] - 1;
+		memcpy(logprobs + off[seqs[k]], lp.data() + s, (size_t)r * sizeof(float));
+		s += cdiv(r, 8) * 8;
+	}
+}
+
+// Score nseq independent sequences from position 0 (include/calm_b200.h): next-fit packing in input order into blocks of
+// at most C = min(2048, seq_len rounded down to 8) rows, every sequence starting at a multiple of 8 rows so that a
+// k_pf_attn CTA never straddles two.  A sequence too long for a block is scored alone by calm_b200_score.
+extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
+	if (!g.ready) CALM_FATAL("score_batch before prepare_cuda");
+	if (n < 0 || nseq < 0) CALM_FATAL("score_batch: negative count (n %d, nseq %d)", n, nseq);
+	if (nseq == 0) return 1;
+	check_tokens(tokens, n);
+	std::vector<std::pair<long, long>> out; // [first, last + 1) of the logprobs each sequence writes
+	for (int i = 0; i < nseq; ++i) {
+		if (off[i] < 0 || len[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("score_batch: sequence %d (off %d, len %d) outside the %d tokens", i, off[i], len[i], n);
+		if (len[i] >= 2) out.push_back({off[i], (long)off[i] + len[i] - 1});
+	}
+	std::sort(out.begin(), out.end());
+	for (size_t k = 1; k < out.size(); ++k)
+		if (out[k].first < out[k - 1].second) CALM_FATAL("score_batch: output ranges [%ld, %ld) and [%ld, %ld) overlap", out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
+	int served = 1;
+	if (!pf_supported()) { // the shapes calm_b200_score serves on the decode path
+		for (int i = 0; i < nseq; ++i)
+			if (len[i] >= 2) calm_b200_score(transformer, tokens + off[i], len[i], 0, logprobs + off[i]);
+		return 0;
+	}
+	const int cap = imin(2048, g.cfg.seq_len / 8 * 8); // a row is its cache slot: no row may reach seq_len
+	std::vector<int> block, alone;
+	int rows = 0;
+	for (int i = 0; i < nseq; ++i) {
+		if (len[i] < 2) continue;
+		const int R = cdiv(len[i] - 1, 8) * 8;
+		if (R > cap) {
+			alone.push_back(i);
+			continue;
+		}
+		if (rows + R > cap) pf_score_block(tokens, off, len, block, rows, logprobs), block.clear(), rows = 0;
+		block.push_back(i), rows += R;
+	}
+	if (rows) pf_score_block(tokens, off, len, block, rows, logprobs);
+	for (int i : alone) served &= calm_b200_score(transformer, tokens + off[i], len[i], 0, logprobs + off[i]);
+	return served;
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -1417,7 +1500,8 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 // and into the cache slots [kv_from_pos, seq_len) of every layer and kv head.  Only data is touched: TokenParams, the
 // attention's {value, epoch} cells and counter, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
 // counts, stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
-// as do the index buffers (cand_idx, sample_idx, out_tokens, pf.tokens, pf.targets): a stale index that is read is in range,
+// as do the index buffers (cand_idx, sample_idx, out_tokens, pf.tokens, pf.targets, and pf.rowpos and pf.seg, read as a
+// RoPE position and as the first key slot of the packed attention's loop): a stale index that is read is in range,
 // as after any earlier call, while 0xFFFFFFFF would send the read out of bounds.  DESIGN.md s.3 lists both groups.
 extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos) {
 	(void)transformer;

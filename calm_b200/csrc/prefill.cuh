@@ -20,7 +20,9 @@
 // Scoring (calm_b200_score, the reference's study(): run.c:291-308) adds the classifier over all rows of the block without
 // ever writing the [T][vocab] logits: the final norm (k_pf_norm), k_pf_gemm in PF_CLS mode, whose epilogue reduces each
 // token's 128 logits of the tile to one (max, sum exp(logit - max)) record and keeps the target's logit, and k_pf_logprob,
-// which merges a token's records in a fixed order into ln softmax(logits)[target].
+// which merges a token's records in a fixed order into ln softmax(logits)[target].  calm_b200_score_batch packs several
+// independent sequences into one block: per-row RoPE positions (k_pf_rope_rows) and attention that starts each sequence's
+// key tiles at its own first row (k_pf_attn<.., SEG>); everything else works per row and is unchanged.
 //
 // Parity contract (tests/test_prefill_gpu.py): after forward_prefill_cuda(tokens, n, pos0) the KV cache and the logits of
 // the following token equal those of n serial forward(FF_UPDATE_KV_ONLY) calls within the stated tolerances.
@@ -120,6 +122,17 @@ __global__ void k_pf_rope(float2* rope, const float* freq, int n, int half_hd, i
 	if (i >= n * half_hd) return;
 	float s, c;
 	sincosf((float)(pos0 + i / half_hd) * freq[i % half_hd], &s, &c);
+	rope[i] = make_float2(c, s);
+}
+
+// rope[t][j] = (cos, sin)(rowpos[t] * freq[j]): the table of a packed block, whose rows restart at 0 with each sequence
+// (calm_b200_score_batch); for rowpos[t] = pos0 + t the same float arguments as k_pf_rope, so the same bits
+__global__ void k_pf_rope_rows(float2* rope, const float* freq, const int* rowpos, int n, int half_hd) {
+	pdl_enter();
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n * half_hd) return;
+	float s, c;
+	sincosf((float)rowpos[i / half_hd] * freq[i % half_hd], &s, &c);
 	rope[i] = make_float2(c, s);
 }
 
@@ -446,6 +459,7 @@ struct PfAttnArgs {
 	__half* Olo;
 	int n_tokens, pos0, seq_len, q_dim, kv_mul;
 	float inv_sqrt_hd;
+	const int* seg; // [T] (SEG variant) the first row of the row's sequence; read by no other variant
 };
 
 // DPL (2 or 4) consecutive cache elements -> floats with a single shared-memory load
@@ -473,8 +487,12 @@ __device__ __forceinline__ void pf_load_dims(const uint8_t* p, float (&o)[DPL]) 
 	}
 }
 
-// CTA = (kv head, 8 consecutive query tokens); warp = one token with all kv_mul query heads of the kv head (KM of them per pass)
-template <typename KVT, int HD, int KM>
+// CTA = (kv head, 8 consecutive query tokens); warp = one token with all kv_mul query heads of the kv head (KM of them per pass).
+// SEG: a packed block of independent sequences (calm_b200_score_batch, pos0 = 0, row t in cache slot t).  The host starts
+// every sequence at a multiple of 8 rows, so the CTA's rows share one segment starting at row s = seg[first row], and the key
+// tiles run from s: tile j of a sequence holds the same keys in the same order as tile j of the sequence scored alone from
+// position 0, and each warp's online softmax sees exactly the values of that lone pass.
+template <typename KVT, int HD, int KM, bool SEG = false>
 __global__ void __launch_bounds__(PFA_WARPS * 32) k_pf_attn(const PfAttnArgs a) {
 	pdl_enter();
 	constexpr int DPL = HD / 32;               // head dims owned by a lane in the value pass
@@ -487,6 +505,13 @@ __global__ void __launch_bounds__(PFA_WARPS * 32) k_pf_attn(const PfAttnArgs a) 
 	const bool live = t < a.n_tokens;
 	const int last = a.pos0 + min(a.n_tokens - 1, (int)blockIdx.x * PFA_WARPS + PFA_WARPS - 1); // last key position any warp of the CTA needs
 	const int mypos = a.pos0 + t;
+	int kfirst = 0; // first key slot of the CTA's rows
+	if constexpr (SEG) {
+		kfirst = a.seg[blockIdx.x * PFA_WARPS];
+		// a CTA straddling two sequences would attend across them: stop instead (no message: a format string would move the
+		// global-constant offsets every other kernel of the module is built with)
+		if (live && a.seg[t] != kfirst) __trap();
+	}
 	const KVT* kbase = reinterpret_cast<const KVT*>(a.kc) + (size_t)kvh * a.seq_len * HD;
 	const KVT* vbase = reinterpret_cast<const KVT*>(a.vc) + (size_t)kvh * a.seq_len * HD;
 	for (int hg = 0; hg < a.kv_mul; hg += KM) { // KM query heads per pass over the keys
@@ -499,7 +524,7 @@ __global__ void __launch_bounds__(PFA_WARPS * 32) k_pf_attn(const PfAttnArgs a) 
 #pragma unroll
 			for (int d = 0; d < DPL; ++d) acc[h][d] = 0.f;
 		}
-		for (int k0 = 0; k0 <= last; k0 += PFA_TILE) {
+		for (int k0 = kfirst; k0 <= last; k0 += PFA_TILE) {
 			__syncthreads(); // the previous tile is no longer being read
 			for (int i = threadIdx.x; i < PFA_TILE * HD * (int)sizeof(KVT) / 16; i += blockDim.x) {
 				const int row = i / (HD * (int)sizeof(KVT) / 16), c = i % (HD * (int)sizeof(KVT) / 16);

@@ -117,6 +117,19 @@ int forward_prefill_cuda(struct Transformer* transformer, const int* tokens, int
  * chunk c is calm_b200_score(t, tokens + c, m + 1, 0, out + c)  (INTEGRATION.md). */
 int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs);
 
+/* Score nseq independent sequences, each from position 0, packed into shared prompt-pass blocks.
+ * Sequence i is tokens[off[i] .. off[i] + len[i]) and writes
+ *   logprobs[off[i] + j] = ln softmax(logits after tokens[off[i] + j] at position j)[tokens[off[i] + j + 1]],  j in [0, len[i] - 1)
+ * -- exactly what calm_b200_score(t, tokens + off[i], len[i], 0, logprobs + off[i]) writes.  Sequences may share their
+ * boundary token (study()'s chunks: off = c * steps, len = steps + 1), but their output ranges must not overlap.
+ * Slots of logprobs no sequence writes are left untouched.  Returns 1 when every sequence went through the tensor-core
+ * pass, 0 when any went through the decode path.  The KV cache afterwards holds nothing a host can continue from.
+ * Every token of tokens[0 .. n) must be in the vocabulary, and 0 <= off[i], off[i] + len[i] <= n; a sequence with
+ * len[i] < 2 contributes nothing, nseq == 0 returns 1.  Many short sequences share one block of up to 2048 rows (DESIGN.md
+ * s.6), so they fill the GPU where one call per sequence would leave most of it idle. */
+int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len,
+                          int nseq, float* logprobs);
+
 /* forward + device-side greedy sample.  Returns argmax(logits) with the
  * reference's tie rule (lowest index, sampler.c:34-42).  The logits are still
  * written to state.logits. */
