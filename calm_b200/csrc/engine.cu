@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <map>
 #include <vector>
 
 #include "stages.cuh"
@@ -135,6 +136,7 @@ struct Prefill {
 	float2* rope = nullptr;
 	int* tokens = nullptr;
 	int *rowpos = nullptr, *seg = nullptr; // packed blocks (calm_b200_score_batch): a row's RoPE position, its sequence's first row
+	int2* ctx = nullptr; // packed blocks with contexts (calm_b200_score_context): a row's context, its first row and length
 	CUtensorMap tmN[2], tmA[2], tmH[2]; // (hi, lo) views of the three activation matrices the GEMMs read
 	// scoring (calm_b200_score), allocated on its first call for `cap` rows: the classifier's per-tile records, the targets'
 	// logits, the targets and the log-probabilities
@@ -147,7 +149,7 @@ Prefill pf;
 
 void pf_free() {
 	cudaFree(pf.X), cudaFree(pf.Q), cudaFree(pf.Nhi), cudaFree(pf.Nlo), cudaFree(pf.Ahi), cudaFree(pf.Alo), cudaFree(pf.Hhi), cudaFree(pf.Hlo), cudaFree(pf.rope), cudaFree(pf.tokens);
-	cudaFree(pf.rowpos), cudaFree(pf.seg);
+	cudaFree(pf.rowpos), cudaFree(pf.seg), cudaFree(pf.ctx);
 	cudaFree(pf.part), cudaFree(pf.tgt), cudaFree(pf.logprob), cudaFree(pf.targets);
 	pf = Prefill();
 }
@@ -1140,6 +1142,7 @@ static void pf_reserve(int n) {
 	pf.rope = (float2*)zalloc((size_t)cap * (c.head_dim / 2) * sizeof(float2));
 	pf.tokens = (int*)zalloc((size_t)cap * sizeof(int));
 	pf.rowpos = (int*)zalloc((size_t)cap * sizeof(int)), pf.seg = (int*)zalloc((size_t)cap * sizeof(int));
+	pf.ctx = (int2*)zalloc((size_t)cap * sizeof(int2));
 	pf_make_map(&pf.tmN[0], pf.Nhi, cap, c.dim), pf_make_map(&pf.tmN[1], pf.Nlo, cap, c.dim);
 	pf_make_map(&pf.tmA[0], pf.Ahi, cap, g.q_dim), pf_make_map(&pf.tmA[1], pf.Alo, cap, g.q_dim);
 	pf_make_map(&pf.tmH[0], pf.Hhi, cap, c.hidden_dim), pf_make_map(&pf.tmH[1], pf.Hlo, cap, c.hidden_dim);
@@ -1158,18 +1161,27 @@ static void pf_gemm(const CUtensorMap* tm, const PfGemmArgs& a, int rows, int n)
 	launch_pdl(k_pf_gemm<MODE, DBITS, KVT>, dim3(rows / PF_BM, cdiv(n, PF_BN)), PF_THREADS, pf_smem_bytes<MODE>(), tm[0], tm[1], a);
 }
 
-template <typename KVT, int HD, bool SEG>
+template <typename KVT, int HD, bool SEG, bool CTX = false>
 static void pf_attn(const PfAttnArgs& a, int n) {
 	const dim3 grid(cdiv(n, PFA_WARPS), g.cfg.n_kv_heads);
-	if (g.kv_mul % 4 == 0) launch_pdl(k_pf_attn<KVT, HD, 4, SEG>, grid, PFA_WARPS * 32, 0, a);
-	else if (g.kv_mul % 2 == 0) launch_pdl(k_pf_attn<KVT, HD, 2, SEG>, grid, PFA_WARPS * 32, 0, a);
-	else launch_pdl(k_pf_attn<KVT, HD, 1, SEG>, grid, PFA_WARPS * 32, 0, a);
+	if (g.kv_mul % 4 == 0) launch_pdl(k_pf_attn<KVT, HD, 4, SEG, CTX>, grid, PFA_WARPS * 32, 0, a);
+	else if (g.kv_mul % 2 == 0) launch_pdl(k_pf_attn<KVT, HD, 2, SEG, CTX>, grid, PFA_WARPS * 32, 0, a);
+	else launch_pdl(k_pf_attn<KVT, HD, 1, SEG, CTX>, grid, PFA_WARPS * 32, 0, a);
 }
 
-// The pass over the n rows in pf.tokens at cache slots pos0 + t.  packed: a block of independent sequences
-// (calm_b200_score_batch, pos0 = 0), with per-row RoPE positions in pf.rowpos and each row's sequence start in pf.seg.
+// What the rows of a prompt-pass block are
+enum PfRows {
+	PF_ONE,      // one sequence at cache slots pos0 + t
+	PF_PACKED,   // independent sequences (calm_b200_score_batch, pos0 = 0): per-row RoPE positions in pf.rowpos, each row's
+	             // sequence start in pf.seg
+	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block (calm_b200_score_context): each row's
+	             // context in pf.ctx
+};
+
+// The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says.
 template <int DBITS, typename KVT>
-static void pf_run(Formats<DBITS, KVT>, int n, int pos0, bool packed = false) {
+static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout = PF_ONE) {
+	const bool packed = layout != PF_ONE;
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
@@ -1189,8 +1201,11 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, bool packed = false) {
 		PfAttnArgs aa = {};
 		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
 		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
-		aa.seg = pf.seg;
-		if (packed) {
+		aa.seg = pf.seg, aa.ctx = pf.ctx;
+		if (layout == PF_CONTEXTS) {
+			if (c.head_dim == 128) pf_attn<KVT, 128, true, true>(aa, n);
+			else pf_attn<KVT, 64, true, true>(aa, n);
+		} else if (packed) {
 			if (c.head_dim == 128) pf_attn<KVT, 128, true>(aa, n);
 			else pf_attn<KVT, 64, true>(aa, n);
 		} else {
@@ -1331,7 +1346,7 @@ static void pf_score_block(const int* tokens, const int* off, const int* len, co
 	CUDA_CHECK(cudaMemcpyAsync(pf.targets, tgt.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.seg, seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	with_formats([&](auto f) { pf_run(f, rows, 0, true); });
+	with_formats([&](auto f) { pf_run(f, rows, 0, PF_PACKED); });
 	with_formats([&](auto f) { pf_score(f, rows); });
 	CUDA_CHECK(cudaMemcpyAsync(lp.data(), pf.logprob, (size_t)rows * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
 	CUDA_CHECK(cudaStreamSynchronize(g.stream));
@@ -1380,6 +1395,106 @@ extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int*
 	}
 	if (rows) pf_score_block(tokens, off, len, block, rows, logprobs);
 	for (int i : alone) served &= calm_b200_score(transformer, tokens + off[i], len[i], 0, logprobs + off[i]);
+	return served;
+}
+
+// A packed block of calm_b200_score_context being filled: per-row inputs, the sequences it scores with their first rows,
+// and the contexts it holds by (ctx_off, ctx_len) with their first rows.
+struct PfContextBlock {
+	std::vector<int> tok, tgt, pos, seg;
+	std::vector<int2> ctx;
+	std::vector<std::pair<int, int>> seqs;
+	std::map<std::pair<int, int>, int> placed;
+	int rows() const { return (int)tok.size(); }
+	// Rows for the r inputs t[0 .. r) at RoPE positions p0 .., continuing context cx, rounded up to a multiple of 8 with
+	// filler rows that repeat the last input; row j targets t[min(j + 1, tl)].  Returns the first row.
+	int add(const int* t, int r, int tl, int p0, int2 cx) {
+		const int s = rows();
+		for (int j = 0; j < cdiv(r, 8) * 8; ++j)
+			tok.push_back(t[imin(j, r - 1)]), tgt.push_back(t[imin(j + 1, tl)]), pos.push_back(p0 + j), seg.push_back(s), ctx.push_back(cx);
+		return s;
+	}
+};
+
+// Run a block and write its sequences' log-probabilities.  A block that holds no context runs the packed attention of
+// calm_b200_score_batch; only one with a context runs the context walk (k_pf_attn<.., SEG, CTX>).
+static void pf_score_context_block(PfContextBlock& b, const int* off, const int* len, float* logprobs) {
+	const int rows = b.rows();
+	const bool contexts = !b.placed.empty();
+	std::vector<float> lp(rows);
+	pf_reserve(rows);
+	pf_score_reserve();
+	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, b.tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.targets, b.tgt.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, b.pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.seg, b.seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	if (contexts) CUDA_CHECK(cudaMemcpyAsync(pf.ctx, b.ctx.data(), (size_t)rows * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
+	with_formats([&](auto f) { pf_run(f, rows, 0, contexts ? PF_CONTEXTS : PF_PACKED); });
+	with_formats([&](auto f) { pf_score(f, rows); });
+	CUDA_CHECK(cudaMemcpyAsync(lp.data(), pf.logprob, (size_t)rows * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+	CUDA_CHECK(cudaStreamSynchronize(g.stream));
+	CUDA_CHECK(cudaGetLastError());
+	for (const auto& [i, s] : b.seqs) memcpy(logprobs + off[i], lp.data() + s, (size_t)(len[i] - 1) * sizeof(float));
+	b = PfContextBlock();
+}
+
+// Score nseq sequences that continue contexts (include/calm_b200.h).  Next-fit packing in input order into blocks of at
+// most C = min(2048, seq_len rounded down to 8) rows: a context takes ceil8(ctx_len) rows at RoPE positions 0 ..; a
+// sequence takes ceil8(len - 1) rows at positions ctx_len .., after its context's rows in the same block.  Sequences with
+// the same (ctx_off, ctx_len) share one placement of the context per block; a sequence whose context is not yet in the
+// block brings it along.  A context and sequence too long for any block, together, are scored alone by calm_b200_score.
+extern "C" int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                       const int* off, const int* len, int nseq, float* logprobs) {
+	if (!g.ready) CALM_FATAL("score_context before prepare_cuda");
+	if (n < 0 || nseq < 0) CALM_FATAL("score_context: negative count (n %d, nseq %d)", n, nseq);
+	if (nseq == 0) return 1;
+	check_tokens(tokens, n);
+	std::vector<std::pair<long, long>> out; // [first, last + 1) of the logprobs each sequence writes
+	for (int i = 0; i < nseq; ++i) {
+		if (off[i] < 0 || len[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("score_context: sequence %d (off %d, len %d) outside the %d tokens", i, off[i], len[i], n);
+		if (ctx_off[i] < 0 || ctx_len[i] < 0 || (long)ctx_off[i] + ctx_len[i] > n)
+			CALM_FATAL("score_context: context of sequence %d (off %d, len %d) outside the %d tokens", i, ctx_off[i], ctx_len[i], n);
+		if (len[i] >= 2) out.push_back({off[i], (long)off[i] + len[i] - 1});
+	}
+	std::sort(out.begin(), out.end());
+	for (size_t k = 1; k < out.size(); ++k)
+		if (out[k].first < out[k - 1].second) CALM_FATAL("score_context: output ranges [%ld, %ld) and [%ld, %ld) overlap", out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
+	// calm_b200_score of ctx ++ sequence, by definition the result: for shapes the pass does not serve and units too big
+	auto alone = [&](int i) {
+		std::vector<int> cat(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
+		cat.insert(cat.end(), tokens + off[i], tokens + off[i] + len[i]);
+		std::vector<float> lp(cat.size() - 1);
+		const int served = calm_b200_score(transformer, cat.data(), (int)cat.size(), 0, lp.data());
+		memcpy(logprobs + off[i], lp.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(float));
+		return served;
+	};
+	if (!pf_supported()) {
+		for (int i = 0; i < nseq; ++i)
+			if (len[i] >= 2) alone(i);
+		return 0;
+	}
+	const int cap = imin(2048, g.cfg.seq_len / 8 * 8); // a row is its cache slot: no row may reach seq_len
+	PfContextBlock b;
+	std::vector<int> big;
+	for (int i = 0; i < nseq; ++i) {
+		if (len[i] < 2) continue;
+		const int R = cdiv(len[i] - 1, 8) * 8, Rc = cdiv(ctx_len[i], 8) * 8;
+		if (Rc + R > cap) {
+			big.push_back(i);
+			continue;
+		}
+		const std::pair<int, int> key(ctx_off[i], ctx_len[i]);
+		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_context_block(b, off, len, logprobs);
+		int c0 = 0;
+		if (ctx_len[i]) {
+			const auto it = b.placed.find(key);
+			c0 = it != b.placed.end() ? it->second : (b.placed[key] = b.add(tokens + ctx_off[i], ctx_len[i], ctx_len[i] - 1, 0, make_int2(0, 0)));
+		}
+		b.seqs.push_back({i, b.add(tokens + off[i], len[i] - 1, len[i] - 1, ctx_len[i], make_int2(c0, ctx_len[i]))});
+	}
+	if (b.rows()) pf_score_context_block(b, off, len, logprobs);
+	int served = 1;
+	for (int i : big) served &= alone(i);
 	return served;
 }
 
@@ -1500,8 +1615,8 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 // and into the cache slots [kv_from_pos, seq_len) of every layer and kv head.  Only data is touched: TokenParams, the
 // attention's {value, epoch} cells and counter, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
 // counts, stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
-// as do the index buffers (cand_idx, sample_idx, out_tokens, pf.tokens, pf.targets, and pf.rowpos and pf.seg, read as a
-// RoPE position and as the first key slot of the packed attention's loop): a stale index that is read is in range,
+// as do the index buffers (cand_idx, sample_idx, out_tokens, pf.tokens, pf.targets, and pf.rowpos, pf.seg and pf.ctx, read
+// as a RoPE position and as key slots of the packed attention's loop): a stale index that is read is in range,
 // as after any earlier call, while 0xFFFFFFFF would send the read out of bounds.  DESIGN.md s.3 lists both groups.
 extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos) {
 	(void)transformer;

@@ -23,6 +23,8 @@
 // which merges a token's records in a fixed order into ln softmax(logits)[target].  calm_b200_score_batch packs several
 // independent sequences into one block: per-row RoPE positions (k_pf_rope_rows) and attention that starts each sequence's
 // key tiles at its own first row (k_pf_attn<.., SEG>); everything else works per row and is unchanged.
+// calm_b200_score_context also packs contexts, once per block, and sequences that continue them: a sequence's rows attend
+// to its context's rows and then its own as one key sequence (k_pf_attn<.., SEG, CTX>).
 //
 // Parity contract (tests/test_prefill_gpu.py): after forward_prefill_cuda(tokens, n, pos0) the KV cache and the logits of
 // the following token equal those of n serial forward(FF_UPDATE_KV_ONLY) calls within the stated tolerances.
@@ -460,6 +462,7 @@ struct PfAttnArgs {
 	int n_tokens, pos0, seq_len, q_dim, kv_mul;
 	float inv_sqrt_hd;
 	const int* seg; // [T] (SEG variant) the first row of the row's sequence; read by no other variant
+	const int2* ctx; // [T] (CTX variant) the row's context: its first row and its length (0: none); read by no other variant
 };
 
 // DPL (2 or 4) consecutive cache elements -> floats with a single shared-memory load
@@ -492,8 +495,14 @@ __device__ __forceinline__ void pf_load_dims(const uint8_t* p, float (&o)[DPL]) 
 // every sequence at a multiple of 8 rows, so the CTA's rows share one segment starting at row s = seg[first row], and the key
 // tiles run from s: tile j of a sequence holds the same keys in the same order as tile j of the sequence scored alone from
 // position 0, and each warp's online softmax sees exactly the values of that lone pass.
-template <typename KVT, int HD, int KM, bool SEG = false>
+// CTX (with SEG): a packed block whose sequences continue shared contexts (calm_b200_score_context).  A CTA's rows start at
+// row s and continue the nc-row context at rows c0 .. c0 + nc - 1 (ctx[first row]).  The keys run over one virtual index v:
+// v < nc is row c0 + v, v >= nc is row s + v - nc; row t sees v <= nc + t - s.  A tile may straddle the two ranges, so each
+// tile row finds its own address.  Tile j then holds the keys of tile j of ctx ++ sequence scored alone from position 0,
+// with the same zero fill, visibility and value-loop bound, so every floating-point operation is that lone pass's.
+template <typename KVT, int HD, int KM, bool SEG = false, bool CTX = false>
 __global__ void __launch_bounds__(PFA_WARPS * 32) k_pf_attn(const PfAttnArgs a) {
+	static_assert(SEG || !CTX, "the context walk starts from a segmented block");
 	pdl_enter();
 	constexpr int DPL = HD / 32;               // head dims owned by a lane in the value pass
 	constexpr int KSTR = HD * sizeof(KVT) + 16; // padded key row: 16-byte reads of one row per lane are conflict-free per quarter warp
@@ -503,14 +512,18 @@ __global__ void __launch_bounds__(PFA_WARPS * 32) k_pf_attn(const PfAttnArgs a) 
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 	const int kvh = blockIdx.y, t = blockIdx.x * PFA_WARPS + warp;
 	const bool live = t < a.n_tokens;
-	const int last = a.pos0 + min(a.n_tokens - 1, (int)blockIdx.x * PFA_WARPS + PFA_WARPS - 1); // last key position any warp of the CTA needs
-	const int mypos = a.pos0 + t;
+	int last = a.pos0 + min(a.n_tokens - 1, (int)blockIdx.x * PFA_WARPS + PFA_WARPS - 1); // last key position any warp of the CTA needs
+	int mypos = a.pos0 + t;
 	int kfirst = 0; // first key slot of the CTA's rows
 	if constexpr (SEG) {
 		kfirst = a.seg[blockIdx.x * PFA_WARPS];
 		// a CTA straddling two sequences would attend across them: stop instead (no message: a format string would move the
 		// global-constant offsets every other kernel of the module is built with)
 		if (live && a.seg[t] != kfirst) __trap();
+		if constexpr (CTX) { // from here on, key positions are virtual indices
+			const int nc = a.ctx[blockIdx.x * PFA_WARPS].y;
+			last += nc - kfirst, mypos += nc - kfirst, kfirst = 0;
+		}
 	}
 	const KVT* kbase = reinterpret_cast<const KVT*>(a.kc) + (size_t)kvh * a.seq_len * HD;
 	const KVT* vbase = reinterpret_cast<const KVT*>(a.vc) + (size_t)kvh * a.seq_len * HD;
@@ -529,9 +542,14 @@ __global__ void __launch_bounds__(PFA_WARPS * 32) k_pf_attn(const PfAttnArgs a) 
 			for (int i = threadIdx.x; i < PFA_TILE * HD * (int)sizeof(KVT) / 16; i += blockDim.x) {
 				const int row = i / (HD * (int)sizeof(KVT) / 16), c = i % (HD * (int)sizeof(KVT) / 16);
 				const bool in = k0 + row <= last;
+				int slot = k0 + row;
+				if constexpr (CTX) { // (read per tile: held in registers through the score pass, they add spills)
+					const int2 cx = __ldg(a.ctx + blockIdx.x * PFA_WARPS);
+					slot = slot < cx.y ? cx.x + slot : __ldg(a.seg + blockIdx.x * PFA_WARPS) + slot - cx.y;
+				}
 				const uint4 z = make_uint4(0, 0, 0, 0);
-				*reinterpret_cast<uint4*>(ks + row * KSTR + c * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(kbase + (size_t)(k0 + row) * HD) + c) : z;
-				*reinterpret_cast<uint4*>(vs + row * HD * sizeof(KVT) + c * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(vbase + (size_t)(k0 + row) * HD) + c) : z;
+				*reinterpret_cast<uint4*>(ks + row * KSTR + c * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(kbase + (size_t)slot * HD) + c) : z;
+				*reinterpret_cast<uint4*>(vs + row * HD * sizeof(KVT) + c * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(vbase + (size_t)slot * HD) + c) : z;
 			}
 			__syncthreads();
 			if (!live || k0 > mypos) continue; // (warp-uniform) causal: nothing of this tile is visible to this token

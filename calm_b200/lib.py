@@ -22,7 +22,7 @@ _fptr = C.POINTER(C.c_float)
 
 # every symbol include/calm_b200.h declares
 SYMBOLS = [
-    "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda", "calm_b200_score", "calm_b200_score_batch",
+    "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda", "calm_b200_score", "calm_b200_score_batch", "calm_b200_score_context",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
@@ -55,6 +55,8 @@ def load() -> C.CDLL:
     _iptr = C.POINTER(C.c_int)
     L.calm_b200_score_batch.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, C.c_int, _fptr]
     L.calm_b200_score_batch.restype = C.c_int
+    L.calm_b200_score_context.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, _iptr, _iptr, C.c_int, _fptr]
+    L.calm_b200_score_context.restype = C.c_int
     L.calm_b200_abi_version.argtypes, L.calm_b200_abi_version.restype = [], C.c_int
     L.calm_b200_set_device.argtypes, L.calm_b200_set_device.restype = [C.c_int], None
     L.calm_b200_free.argtypes, L.calm_b200_free.restype = [C.c_void_p], None
@@ -173,6 +175,27 @@ class DeviceModel:
         ip = C.POINTER(C.c_int)
         served = self.lib.calm_b200_score_batch(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), o.ctypes.data_as(ip),
                                                 ln.ctypes.data_as(ip), len(o), out.ctypes.data_as(_fptr))
+        return out, served
+
+    def score_context(self, tokens, ctx_off, ctx_len, off, len_, out=None):
+        """calm_b200_score_context: sequences tokens[off[i] : off[i] + len_[i]], each continuing the context
+        tokens[ctx_off[i] : ctx_off[i] + ctx_len[i]], packed into shared prompt-pass blocks with each context computed once
+        per block.  Returns (float32[len(tokens)] with sequence i's log-probabilities at off[i] .. off[i] + len_[i] - 2, 1
+        when the tensor-core pass served every sequence or 0).  Slots no sequence writes keep what `out` held (NaN when no
+        `out` is given)."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        co = np.ascontiguousarray(ctx_off, np.int32)
+        cl = np.ascontiguousarray(ctx_len, np.int32)
+        o = np.ascontiguousarray(off, np.int32)
+        ln = np.ascontiguousarray(len_, np.int32)
+        assert co.shape == cl.shape == o.shape == ln.shape and o.ndim == 1
+        if out is None:
+            out = np.full(len(arr), np.nan, np.float32)
+        assert out.dtype == np.float32 and out.flags.c_contiguous and len(out) >= len(arr)
+        ip = C.POINTER(C.c_int)
+        served = self.lib.calm_b200_score_context(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), co.ctypes.data_as(ip),
+                                                  cl.ctypes.data_as(ip), o.ctypes.data_as(ip), ln.ctypes.data_as(ip), len(o),
+                                                  out.ctypes.data_as(_fptr))
         return out, served
 
     def forward_raw(self, token: int, pos: int, flags: int = 0):

@@ -130,6 +130,24 @@ int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, i
 int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len,
                           int nseq, float* logprobs);
 
+/* Score nseq sequences that each continue a context, packed into shared prompt-pass blocks with each context computed
+ * once per block.  Sequence i is tokens[off[i] .. off[i] + len[i]); it continues the context
+ * tokens[ctx_off[i] .. ctx_off[i] + ctx_len[i]) and writes
+ *   logprobs[off[i] + j] = ln softmax(logits after tokens[off[i] + j] at position ctx_len[i] + j)[tokens[off[i] + j + 1]],
+ *   j in [0, len[i] - 1)
+ * -- exactly what calm_b200_score(t, ctx_i ++ seq_i, ctx_len[i] + len[i], 0, tmp) writes at tmp[ctx_len[i] + j].  The
+ * first token of a sequence is an input only: for ln p(continuation | context), pass context[:-1] as the context and
+ * context[-1:] ++ continuation as the sequence (INTEGRATION.md).  ctx_len[i] == 0 means no context, as in
+ * calm_b200_score_batch.  Contexts are read only and may overlap anything; output ranges must not overlap, and slots of
+ * logprobs no sequence writes are left untouched.  Sequences with the same (ctx_off[i], ctx_len[i]) share one copy of the
+ * context's rows within a block; equal contents at different offsets are scored correctly but computed once per sequence.
+ * Returns 1 when every sequence went through the tensor-core pass, 0 when any went through the decode path.  The KV cache
+ * afterwards holds nothing a host can continue from.  Every token of tokens[0 .. n) must be in the vocabulary, and every
+ * context and sequence must lie inside them; a sequence with len[i] < 2 contributes nothing (its context is not placed),
+ * nseq == 0 returns 1.  A context with its sequence that does not fit one block of up to 2048 rows is scored alone by
+ * calm_b200_score (DESIGN.md s.6). */
+int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off, const int* len, int nseq, float* logprobs);
+
 /* forward + device-side greedy sample.  Returns argmax(logits) with the
  * reference's tie rule (lowest index, sampler.c:34-42).  The logits are still
  * written to state.logits. */
