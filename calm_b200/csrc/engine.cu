@@ -144,6 +144,10 @@ struct Prefill {
 	float2* part = nullptr; // [cap][cdiv(vocab, PF_BM)]
 	float *tgt = nullptr, *logprob = nullptr;
 	int* targets = nullptr;
+	// greedy scoring (calm_b200_score_greedy and its siblings), allocated on its first call for `cap` rows: each tile's
+	// argmax and the merged argmax of each row
+	int* gidx = nullptr; // [cap][cdiv(vocab, PF_BM)]
+	int* greedy = nullptr;
 };
 Prefill pf;
 
@@ -151,6 +155,7 @@ void pf_free() {
 	cudaFree(pf.X), cudaFree(pf.Q), cudaFree(pf.Nhi), cudaFree(pf.Nlo), cudaFree(pf.Ahi), cudaFree(pf.Alo), cudaFree(pf.Hhi), cudaFree(pf.Hlo), cudaFree(pf.rope), cudaFree(pf.tokens);
 	cudaFree(pf.rowpos), cudaFree(pf.seg), cudaFree(pf.ctx);
 	cudaFree(pf.part), cudaFree(pf.tgt), cudaFree(pf.logprob), cudaFree(pf.targets);
+	cudaFree(pf.gidx), cudaFree(pf.greedy);
 	pf = Prefill();
 }
 
@@ -1230,47 +1235,61 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout = PF_ONE)
 	}
 }
 
-// The scoring buffers for pf.cap rows (freed and re-made with the pass's own buffers when a longer block needs more rows)
-static void pf_score_reserve() {
-	if (pf.scoring) return;
+// The scoring buffers for pf.cap rows, and with `greedy` the argmax buffers, which the plain scoring calls never allocate
+// (freed and re-made with the pass's own buffers when a longer block needs more rows)
+static void pf_score_reserve(bool greedy) {
 	const int nvt = cdiv(g.cfg.vocab_size, PF_BM);
-	pf.part = (float2*)dev_alloc((size_t)pf.cap * nvt * sizeof(float2));
-	pf.tgt = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
-	pf.logprob = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
-	pf.targets = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
-	pf.scoring = true;
+	if (!pf.scoring) {
+		pf.part = (float2*)dev_alloc((size_t)pf.cap * nvt * sizeof(float2));
+		pf.tgt = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
+		pf.logprob = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
+		pf.targets = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
+		pf.scoring = true;
+	}
+	if (greedy && !pf.gidx) {
+		pf.gidx = (int*)dev_alloc((size_t)pf.cap * nvt * sizeof(int));
+		pf.greedy = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
+	}
 }
 
-// After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records
+// After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records;
+// with `greedy` the classifier and the merge also give each row's argmax in pf.greedy
 template <int DBITS, typename KVT>
-static void pf_score(Formats<DBITS, KVT>, int n) {
+static void pf_score(Formats<DBITS, KVT>, int n, bool greedy) {
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const int nvt = cdiv(c.vocab_size, PF_BM);
 	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
 	PfGemmArgs a = {};
 	a.n_tokens = n, a.w[0] = w.wcls, a.K = c.dim;
-	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size;
-	pf_gemm<PF_CLS, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-	launch_pdl(k_pf_logprob, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt);
+	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
+	if (greedy) {
+		pf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
+		launch_pdl(k_pf_logprob<true>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx, pf.greedy);
+	} else {
+		pf_gemm<PF_CLS, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
+		launch_pdl(k_pf_logprob<false>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)nullptr, (int*)nullptr);
+	}
 }
 
 // The batched pass over tokens[0 .. n) at positions pos0 .., in blocks of at most 2048 rows.  With `logprobs`, every block
-// is scored as well: logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]], so tokens[n] must exist.
-static void pf_pass(const int* tokens, int n, int pos0, float* logprobs) {
+// is scored as well: logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]], so tokens[n] must exist; with
+// `greedy` too, greedy[i] = the argmax of those logits.
+static void pf_pass(const int* tokens, int n, int pos0, float* logprobs, int* greedy = nullptr) {
 	const int chunk_cap = 2048;
 	for (int o = 0; o < n; o += chunk_cap) {
 		const int m = n - o < chunk_cap ? n - o : chunk_cap;
 		pf_reserve(m);
 		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 		if (logprobs) {
-			pf_score_reserve();
+			pf_score_reserve(greedy);
 			CUDA_CHECK(cudaMemcpyAsync(pf.targets, tokens + o + 1, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 		}
 		with_formats([&](auto f) { pf_run(f, m, pos0 + o); });
 		if (logprobs) {
-			with_formats([&](auto f) { pf_score(f, m); });
+			with_formats([&](auto f) { pf_score(f, m, greedy); });
 			CUDA_CHECK(cudaMemcpyAsync(logprobs + o, pf.logprob, (size_t)m * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+			if (greedy) CUDA_CHECK(cudaMemcpyAsync(greedy + o, pf.greedy, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 		}
 		CUDA_CHECK(cudaStreamSynchronize(g.stream)); // `tokens` is the caller's memory (pageable): the copy above must have left it
 	}
@@ -1305,7 +1324,8 @@ extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* 
 // the prompt pass and logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]].  The cache is left as
 // forward_prefill_cuda(tokens, n - 1, pos0) leaves it.  Shapes the pass does not serve go one position at a time through
 // the decode path with a log-softmax in double on the host (returns 0).
-extern "C" int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs) {
+// calm_b200_score, and with `greedy` calm_b200_score_greedy
+static int pf_score_one(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, int* greedy) {
 	if (n < 2) return 1;
 	check_call(transformer, tokens[0], pos0);
 	check_tokens(tokens, n);
@@ -1320,19 +1340,34 @@ extern "C" int calm_b200_score(struct Transformer* transformer, const int* token
 			for (int v = 1; v < vocab; ++v) mx = l[v] > mx ? l[v] : mx;
 			for (int v = 0; v < vocab; ++v) s += exp((double)l[v] - mx);
 			logprobs[i] = (float)((double)l[tokens[i + 1]] - mx - log(s));
+			if (greedy) { // first maximum (sampler.c:34-42), as calm_b200_forward_argmax
+				int best = 0;
+				for (int v = 1; v < vocab; ++v)
+					if (l[v] > l[best]) best = v;
+				greedy[i] = best;
+			}
 		}
 		CUDA_CHECK(cudaGetLastError());
 		return 0;
 	}
-	pf_pass(tokens, rows, pos0, logprobs);
+	pf_pass(tokens, rows, pos0, logprobs, greedy);
 	return 1;
+}
+
+extern "C" int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs) {
+	return pf_score_one(transformer, tokens, n, pos0, logprobs, nullptr);
+}
+
+extern "C" int calm_b200_score_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, int* greedy) {
+	if (!greedy) CALM_FATAL("score_greedy: greedy is NULL");
+	return pf_score_one(transformer, tokens, n, pos0, logprobs, greedy);
 }
 
 // One packed block of calm_b200_score_batch: sequence seqs[k] takes rows [s, s + R) with R = its rows rounded up to 8, RoPE
 // positions 0 .. R - 1 and cache slots s .. s + R - 1.  Its filler rows (after the live ones) repeat its last input token
 // and target its last token; causal attention keeps them out of every live row, and their results are dropped.
-static void pf_score_block(const int* tokens, const int* off, const int* len, const std::vector<int>& seqs, int rows, float* logprobs) {
-	std::vector<int> tok(rows), tgt(rows), pos(rows), seg(rows);
+static void pf_score_block(const int* tokens, const int* off, const int* len, const std::vector<int>& seqs, int rows, float* logprobs, int* greedy) {
+	std::vector<int> tok(rows), tgt(rows), pos(rows), seg(rows), gr(greedy ? rows : 0);
 	std::vector<float> lp(rows);
 	for (int k = 0, s = 0; k < (int)seqs.size(); ++k) {
 		const int* t = tokens + off[seqs[k]];
@@ -1341,19 +1376,21 @@ static void pf_score_block(const int* tokens, const int* off, const int* len, co
 		s += R;
 	}
 	pf_reserve(rows);
-	pf_score_reserve();
+	pf_score_reserve(greedy);
 	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.targets, tgt.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.seg, seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	with_formats([&](auto f) { pf_run(f, rows, 0, PF_PACKED); });
-	with_formats([&](auto f) { pf_score(f, rows); });
+	with_formats([&](auto f) { pf_score(f, rows, greedy); });
 	CUDA_CHECK(cudaMemcpyAsync(lp.data(), pf.logprob, (size_t)rows * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+	if (greedy) CUDA_CHECK(cudaMemcpyAsync(gr.data(), pf.greedy, (size_t)rows * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 	CUDA_CHECK(cudaStreamSynchronize(g.stream));
 	CUDA_CHECK(cudaGetLastError());
 	for (int k = 0, s = 0; k < (int)seqs.size(); ++k) {
 		const int r = len[seqs[k]] - 1;
 		memcpy(logprobs + off[seqs[k]], lp.data() + s, (size_t)r * sizeof(float));
+		if (greedy) memcpy(greedy + off[seqs[k]], gr.data() + s, (size_t)r * sizeof(int));
 		s += cdiv(r, 8) * 8;
 	}
 }
@@ -1361,7 +1398,8 @@ static void pf_score_block(const int* tokens, const int* off, const int* len, co
 // Score nseq independent sequences from position 0 (include/calm_b200.h): next-fit packing in input order into blocks of
 // at most C = min(2048, seq_len rounded down to 8) rows, every sequence starting at a multiple of 8 rows so that a
 // k_pf_attn CTA never straddles two.  A sequence too long for a block is scored alone by calm_b200_score.
-extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
+// With `greedy`, calm_b200_score_batch_greedy.
+static int pf_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
 	if (!g.ready) CALM_FATAL("score_batch before prepare_cuda");
 	if (n < 0 || nseq < 0) CALM_FATAL("score_batch: negative count (n %d, nseq %d)", n, nseq);
 	if (nseq == 0) return 1;
@@ -1375,27 +1413,39 @@ extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int*
 	for (size_t k = 1; k < out.size(); ++k)
 		if (out[k].first < out[k - 1].second) CALM_FATAL("score_batch: output ranges [%ld, %ld) and [%ld, %ld) overlap", out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
 	int served = 1;
+	// calm_b200_score(_greedy) of sequence i alone
+	auto alone = [&](int i) { return pf_score_one(transformer, tokens + off[i], len[i], 0, logprobs + off[i], greedy ? greedy + off[i] : nullptr); };
 	if (!pf_supported()) { // the shapes calm_b200_score serves on the decode path
 		for (int i = 0; i < nseq; ++i)
-			if (len[i] >= 2) calm_b200_score(transformer, tokens + off[i], len[i], 0, logprobs + off[i]);
+			if (len[i] >= 2) alone(i);
 		return 0;
 	}
 	const int cap = imin(2048, g.cfg.seq_len / 8 * 8); // a row is its cache slot: no row may reach seq_len
-	std::vector<int> block, alone;
+	std::vector<int> block, big;
 	int rows = 0;
 	for (int i = 0; i < nseq; ++i) {
 		if (len[i] < 2) continue;
 		const int R = cdiv(len[i] - 1, 8) * 8;
 		if (R > cap) {
-			alone.push_back(i);
+			big.push_back(i);
 			continue;
 		}
-		if (rows + R > cap) pf_score_block(tokens, off, len, block, rows, logprobs), block.clear(), rows = 0;
+		if (rows + R > cap) pf_score_block(tokens, off, len, block, rows, logprobs, greedy), block.clear(), rows = 0;
 		block.push_back(i), rows += R;
 	}
-	if (rows) pf_score_block(tokens, off, len, block, rows, logprobs);
-	for (int i : alone) served &= calm_b200_score(transformer, tokens + off[i], len[i], 0, logprobs + off[i]);
+	if (rows) pf_score_block(tokens, off, len, block, rows, logprobs, greedy);
+	for (int i : big) served &= alone(i);
 	return served;
+}
+
+extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
+	return pf_score_batch(transformer, tokens, n, off, len, nseq, logprobs, nullptr);
+}
+
+extern "C" int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
+                                            float* logprobs, int* greedy) {
+	if (!greedy) CALM_FATAL("score_batch_greedy: greedy is NULL");
+	return pf_score_batch(transformer, tokens, n, off, len, nseq, logprobs, greedy);
 }
 
 // A packed block of calm_b200_score_context being filled: per-row inputs, the sequences it scores with their first rows,
@@ -1418,23 +1468,28 @@ struct PfContextBlock {
 
 // Run a block and write its sequences' log-probabilities.  A block that holds no context runs the packed attention of
 // calm_b200_score_batch; only one with a context runs the context walk (k_pf_attn<.., SEG, CTX>).
-static void pf_score_context_block(PfContextBlock& b, const int* off, const int* len, float* logprobs) {
+static void pf_score_context_block(PfContextBlock& b, const int* off, const int* len, float* logprobs, int* greedy) {
 	const int rows = b.rows();
 	const bool contexts = !b.placed.empty();
 	std::vector<float> lp(rows);
+	std::vector<int> gr(greedy ? rows : 0);
 	pf_reserve(rows);
-	pf_score_reserve();
+	pf_score_reserve(greedy);
 	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, b.tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.targets, b.tgt.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, b.pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.seg, b.seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	if (contexts) CUDA_CHECK(cudaMemcpyAsync(pf.ctx, b.ctx.data(), (size_t)rows * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
 	with_formats([&](auto f) { pf_run(f, rows, 0, contexts ? PF_CONTEXTS : PF_PACKED); });
-	with_formats([&](auto f) { pf_score(f, rows); });
+	with_formats([&](auto f) { pf_score(f, rows, greedy); });
 	CUDA_CHECK(cudaMemcpyAsync(lp.data(), pf.logprob, (size_t)rows * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+	if (greedy) CUDA_CHECK(cudaMemcpyAsync(gr.data(), pf.greedy, (size_t)rows * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 	CUDA_CHECK(cudaStreamSynchronize(g.stream));
 	CUDA_CHECK(cudaGetLastError());
-	for (const auto& [i, s] : b.seqs) memcpy(logprobs + off[i], lp.data() + s, (size_t)(len[i] - 1) * sizeof(float));
+	for (const auto& [i, s] : b.seqs) {
+		memcpy(logprobs + off[i], lp.data() + s, (size_t)(len[i] - 1) * sizeof(float));
+		if (greedy) memcpy(greedy + off[i], gr.data() + s, (size_t)(len[i] - 1) * sizeof(int));
+	}
 	b = PfContextBlock();
 }
 
@@ -1443,8 +1498,9 @@ static void pf_score_context_block(PfContextBlock& b, const int* off, const int*
 // sequence takes ceil8(len - 1) rows at positions ctx_len .., after its context's rows in the same block.  Sequences with
 // the same (ctx_off, ctx_len) share one placement of the context per block; a sequence whose context is not yet in the
 // block brings it along.  A context and sequence too long for any block, together, are scored alone by calm_b200_score.
-extern "C" int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
-                                       const int* off, const int* len, int nseq, float* logprobs) {
+// With `greedy`, calm_b200_score_context_greedy.
+static int pf_score_contexts(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off, const int* len,
+                             int nseq, float* logprobs, int* greedy) {
 	if (!g.ready) CALM_FATAL("score_context before prepare_cuda");
 	if (n < 0 || nseq < 0) CALM_FATAL("score_context: negative count (n %d, nseq %d)", n, nseq);
 	if (nseq == 0) return 1;
@@ -1464,8 +1520,10 @@ extern "C" int calm_b200_score_context(struct Transformer* transformer, const in
 		std::vector<int> cat(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
 		cat.insert(cat.end(), tokens + off[i], tokens + off[i] + len[i]);
 		std::vector<float> lp(cat.size() - 1);
-		const int served = calm_b200_score(transformer, cat.data(), (int)cat.size(), 0, lp.data());
+		std::vector<int> gr(greedy ? cat.size() - 1 : 0);
+		const int served = pf_score_one(transformer, cat.data(), (int)cat.size(), 0, lp.data(), greedy ? gr.data() : nullptr);
 		memcpy(logprobs + off[i], lp.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(float));
+		if (greedy) memcpy(greedy + off[i], gr.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(int));
 		return served;
 	};
 	if (!pf_supported()) {
@@ -1484,7 +1542,7 @@ extern "C" int calm_b200_score_context(struct Transformer* transformer, const in
 			continue;
 		}
 		const std::pair<int, int> key(ctx_off[i], ctx_len[i]);
-		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_context_block(b, off, len, logprobs);
+		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_context_block(b, off, len, logprobs, greedy);
 		int c0 = 0;
 		if (ctx_len[i]) {
 			const auto it = b.placed.find(key);
@@ -1492,10 +1550,21 @@ extern "C" int calm_b200_score_context(struct Transformer* transformer, const in
 		}
 		b.seqs.push_back({i, b.add(tokens + off[i], len[i] - 1, len[i] - 1, ctx_len[i], make_int2(c0, ctx_len[i]))});
 	}
-	if (b.rows()) pf_score_context_block(b, off, len, logprobs);
+	if (b.rows()) pf_score_context_block(b, off, len, logprobs, greedy);
 	int served = 1;
 	for (int i : big) served &= alone(i);
 	return served;
+}
+
+extern "C" int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                       const int* off, const int* len, int nseq, float* logprobs) {
+	return pf_score_contexts(transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, nullptr);
+}
+
+extern "C" int calm_b200_score_context_greedy(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                              const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
+	if (!greedy) CALM_FATAL("score_context_greedy: greedy is NULL");
+	return pf_score_contexts(transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, greedy);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -1643,6 +1712,8 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		nan(pf.Hhi, cap * c.hidden_dim * sizeof(__half)), nan(pf.Hlo, cap * c.hidden_dim * sizeof(__half));
 		nan(pf.rope, cap * (c.head_dim / 2) * sizeof(float2));
 		if (pf.scoring) nan(pf.part, cap * cdiv(c.vocab_size, PF_BM) * sizeof(float2)), nan(pf.tgt, cap * sizeof(float)), nan(pf.logprob, cap * sizeof(float));
+		// the argmax records are vocabulary indices, but only ever compared and copied out, never used as an address
+		nan(pf.gidx, cap * cdiv(c.vocab_size, PF_BM) * sizeof(int)), nan(pf.greedy, cap * sizeof(int));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

@@ -24,7 +24,8 @@
 // independent sequences into one block: per-row RoPE positions (k_pf_rope_rows) and attention that starts each sequence's
 // key tiles at its own first row (k_pf_attn<.., SEG>); everything else works per row and is unchanged.
 // calm_b200_score_context also packs contexts, once per block, and sequences that continue them: a sequence's rows attend
-// to its context's rows and then its own as one key sequence (k_pf_attn<.., SEG, CTX>).
+// to its context's rows and then its own as one key sequence (k_pf_attn<.., SEG, CTX>).  The greedy scoring calls run
+// PF_CLS_GREEDY and k_pf_logprob<true>, which also give each row's argmax, with the same log-probability bits.
 //
 // Parity contract (tests/test_prefill_gpu.py): after forward_prefill_cuda(tokens, n, pos0) the KV cache and the logits of
 // the following token equal those of n serial forward(FF_UPDATE_KV_ONLY) calls within the stated tolerances.
@@ -38,7 +39,7 @@
 #define PF_BN 128 // tokens per tile       (two consumer warpgroups of 64: the M of the MMA)
 #define PF_BK 64  // k per stage: 64 f16 = 128 bytes = one swizzle atom
 #define PF_THREADS 384 // warpgroup 0: dequantising producers (thread 0 also issues the TMA); warpgroups 1, 2: MMA + epilogue
-enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3, PF_CLS = 4 };
+enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3, PF_CLS = 4, PF_CLS_GREEDY = 5 }; // PF_CLS_GREEDY: PF_CLS + each tile's argmax
 
 // ---------------------------------------------------------------- wgmma / TMA wrappers
 __device__ __forceinline__ void wgmma_fence() { // accumulator registers written by ordinary instructions -> visible to wgmma
@@ -192,6 +193,7 @@ struct PfGemmArgs {
 	float2* part;       // [T][gridDim.x] (max, sum exp(logit - max)) of the token's logits in each vocabulary tile
 	float* tgt;         // [T] logit of the target
 	int vocab;
+	int* gidx; // (PF_CLS_GREEDY) [T][gridDim.x] the lowest vocabulary index of the token's maximum logit in each tile
 };
 
 // 64 weights of one row (one k-stage) -> 8 swizzled 16-byte chunks of f16 in the weight tile
@@ -283,7 +285,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 			} else if constexpr (MODE == PF_UP) {
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)gr * rowbytes;
 				rowp[1] = reinterpret_cast<const unsigned char*>(a.w[1]) + (size_t)gr * rowbytes;
-			} else if constexpr (MODE == PF_CLS) { // the last vocabulary tile may be partial: its spare rows repeat the last row
+			} else if constexpr (MODE == PF_CLS || MODE == PF_CLS_GREEDY) { // the last vocabulary tile may be partial: its spare rows repeat the last row
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)min(gr, a.vocab - 1) * rowbytes;
 			} else {
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)gr * rowbytes;
@@ -345,21 +347,39 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 		// accumulator fragment of m64nN: register 4 j + 2 h + e holds token 16 w + lane / 4 + 8 h, weight row 8 j + 2 (lane % 4) + e
 		const int w4 = warp & 3;
 		const int tb = tok0 + c * 64 + w4 * 16 + (lane >> 2);
-		if constexpr (MODE == PF_CLS) {
+		if constexpr (MODE == PF_CLS || MODE == PF_CLS_GREEDY) {
 			// the quad of lanes 4 (lane / 4) .. + 3 holds all 128 logits of tokens tb and tb + 8: 32 per lane, then two shuffles.
 			// Every lane runs the shuffles; only the stores are masked to the block's tokens.
+			// PF_CLS_GREEDY also tracks gi, the vocabulary index of the first maximum: a lane's indices ascend with (j, e), so a
+			// strict > keeps the lowest, and the shuffles give a tie to the lower index.  m and s take the same operations in
+			// the same order as in PF_CLS, so the records are the same bits.
 			const int q = lane & 3;
 #pragma unroll
 			for (int h = 0; h < 2; ++h) {
 				const int t = tb + 8 * h;
 				float m = -FLT_MAX;
+				int gi = 0x7fffffff;
 #pragma unroll
 				for (int j = 0; j < PF_BM / 8; ++j)
 #pragma unroll
 					for (int e = 0; e < 2; ++e)
-						if (row0 + 8 * j + 2 * q + e < a.vocab) m = fmaxf(m, acc[0][4 * j + 2 * h + e]);
-				m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-				m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+						if (row0 + 8 * j + 2 * q + e < a.vocab) {
+							const float v = acc[0][4 * j + 2 * h + e];
+							if constexpr (MODE == PF_CLS_GREEDY) gi = v > m ? row0 + 8 * j + 2 * q + e : gi;
+							m = fmaxf(m, v);
+						}
+				if constexpr (MODE == PF_CLS_GREEDY) {
+#pragma unroll
+					for (int o = 1; o <= 2; o <<= 1) {
+						const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
+						const int i2 = __shfl_xor_sync(0xffffffffu, gi, o);
+						if (m2 > m || (m2 == m && i2 < gi)) gi = i2;
+						m = fmaxf(m, m2);
+					}
+				} else {
+					m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+					m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+				}
 				float s = 0.f;
 #pragma unroll
 				for (int j = 0; j < PF_BM / 8; ++j)
@@ -376,6 +396,8 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 						for (int e = 0; e < 2; ++e)
 							if (8 * j + 2 * q + e == tr) a.tgt[t] = acc[0][4 * j + 2 * h + e];
 					if (q == 0) a.part[(size_t)t * gridDim.x + blockIdx.x] = make_float2(m, s);
+					if constexpr (MODE == PF_CLS_GREEDY)
+						if (q == 0) a.gidx[(size_t)t * gridDim.x + blockIdx.x] = gi;
 				}
 			}
 			return;
@@ -426,27 +448,41 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 // One warp per token: merge the nvt (max, sum) records of the PF_CLS tiles, lane-strided and then by a butterfly, in an
 // order fixed by nvt alone (no atomics), so that repeated calls give the same bits.  logprob = tgt - M - ln S with
 // M = max m_v and S = sum s_v exp(m_v - M).
+// GREEDY (after PF_CLS_GREEDY) also merges the tiles' argmax records gidx into greedy[t], the lowest vocabulary index of
+// the maximum logit: lane-strided over ascending tiles a strict > keeps the first maximum, and in the butterfly an equal
+// value takes the lower index, so the result does not depend on the merge order.  The (M, S) merge is unchanged.
 __device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
 	const float mn = fmaxf(m, m2);
 	s = s * expf(m - mn) + s2 * expf(m2 - mn);
 	m = mn;
 }
-__global__ void __launch_bounds__(256) k_pf_logprob(const float2* part, const float* tgt, float* logprob, int n, int nvt) {
+template <bool GREEDY>
+__global__ void __launch_bounds__(256) k_pf_logprob(const float2* part, const float* tgt, float* logprob, int n, int nvt, const int* gidx, int* greedy) {
 	pdl_enter();
 	const int t = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
 	if (t >= n) return;
 	const float2* p = part + (size_t)t * nvt;
 	float m = -FLT_MAX, s = 0.f;
+	int gi = 0x7fffffff;
 	for (int v = lane; v < nvt; v += 32) {
 		const float2 r = p[v];
+		if constexpr (GREEDY)
+			if (r.x > m) gi = gidx[(size_t)t * nvt + v];
 		lse_merge(m, s, r.x, r.y);
 	}
 #pragma unroll
 	for (int o = 16; o > 0; o >>= 1) { // lane 0's result: a fixed tree over the lanes
 		const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+		if constexpr (GREEDY) {
+			const int i2 = __shfl_xor_sync(0xffffffffu, gi, o);
+			if (m2 > m || (m2 == m && i2 < gi)) gi = i2;
+		}
 		lse_merge(m, s, m2, s2);
 	}
-	if (lane == 0) logprob[t] = tgt[t] - m - logf(s);
+	if (lane == 0) {
+		logprob[t] = tgt[t] - m - logf(s);
+		if constexpr (GREEDY) greedy[t] = gi;
+	}
 }
 
 // ---------------------------------------------------------------- causal attention of the block against the cache

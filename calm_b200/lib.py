@@ -23,6 +23,7 @@ _fptr = C.POINTER(C.c_float)
 # every symbol include/calm_b200.h declares
 SYMBOLS = [
     "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda", "calm_b200_score", "calm_b200_score_batch", "calm_b200_score_context",
+    "calm_b200_score_greedy", "calm_b200_score_batch_greedy", "calm_b200_score_context_greedy",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
@@ -57,6 +58,12 @@ def load() -> C.CDLL:
     L.calm_b200_score_batch.restype = C.c_int
     L.calm_b200_score_context.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, _iptr, _iptr, C.c_int, _fptr]
     L.calm_b200_score_context.restype = C.c_int
+    L.calm_b200_score_greedy.argtypes = [T, _iptr, C.c_int, C.c_int, _fptr, _iptr]
+    L.calm_b200_score_greedy.restype = C.c_int
+    L.calm_b200_score_batch_greedy.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, C.c_int, _fptr, _iptr]
+    L.calm_b200_score_batch_greedy.restype = C.c_int
+    L.calm_b200_score_context_greedy.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, _iptr, _iptr, C.c_int, _fptr, _iptr]
+    L.calm_b200_score_context_greedy.restype = C.c_int
     L.calm_b200_abi_version.argtypes, L.calm_b200_abi_version.restype = [], C.c_int
     L.calm_b200_set_device.argtypes, L.calm_b200_set_device.restype = [C.c_int], None
     L.calm_b200_free.argtypes, L.calm_b200_free.restype = [C.c_void_p], None
@@ -197,6 +204,58 @@ class DeviceModel:
                                                   cl.ctypes.data_as(ip), o.ctypes.data_as(ip), ln.ctypes.data_as(ip), len(o),
                                                   out.ctypes.data_as(_fptr))
         return out, served
+
+    @staticmethod
+    def _greedy_out(n, out, greedy):
+        """The output arrays of a greedy scoring call over n tokens: NaN / -1 where none are given."""
+        if out is None:
+            out = np.full(n, np.nan, np.float32)
+        if greedy is None:
+            greedy = np.full(n, -1, np.int32)
+        assert out.dtype == np.float32 and out.flags.c_contiguous and len(out) >= n
+        assert greedy.dtype == np.int32 and greedy.flags.c_contiguous and len(greedy) >= n
+        return out, greedy
+
+    def score_greedy(self, tokens, pos0: int = 0):
+        """calm_b200_score_greedy: score()'s log-probabilities, bit for bit, and the argmax of the logits at each scored
+        position (lowest index on ties).  Returns (float32[n - 1], int32[n - 1], served)."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        out, greedy = self._greedy_out(max(len(arr) - 1, 0), None, None)
+        ip = C.POINTER(C.c_int)
+        served = self.lib.calm_b200_score_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), pos0, out.ctypes.data_as(_fptr),
+                                                 greedy.ctypes.data_as(ip))
+        return out, greedy, served
+
+    def score_batch_greedy(self, tokens, off, len_, out=None, greedy=None):
+        """calm_b200_score_batch_greedy: score_batch()'s log-probabilities, bit for bit, and the greedy token at the same
+        slots.  Returns (float32[len(tokens)], int32[len(tokens)], served); unwritten slots keep what `out` / `greedy` held
+        (NaN / -1 when not given)."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        o = np.ascontiguousarray(off, np.int32)
+        ln = np.ascontiguousarray(len_, np.int32)
+        assert o.shape == ln.shape and o.ndim == 1
+        out, greedy = self._greedy_out(len(arr), out, greedy)
+        ip = C.POINTER(C.c_int)
+        served = self.lib.calm_b200_score_batch_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), o.ctypes.data_as(ip),
+                                                       ln.ctypes.data_as(ip), len(o), out.ctypes.data_as(_fptr), greedy.ctypes.data_as(ip))
+        return out, greedy, served
+
+    def score_context_greedy(self, tokens, ctx_off, ctx_len, off, len_, out=None, greedy=None):
+        """calm_b200_score_context_greedy: score_context()'s log-probabilities, bit for bit, and the greedy token at the
+        same slots.  Returns (float32[len(tokens)], int32[len(tokens)], served); unwritten slots keep what `out` / `greedy`
+        held (NaN / -1 when not given)."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        co = np.ascontiguousarray(ctx_off, np.int32)
+        cl = np.ascontiguousarray(ctx_len, np.int32)
+        o = np.ascontiguousarray(off, np.int32)
+        ln = np.ascontiguousarray(len_, np.int32)
+        assert co.shape == cl.shape == o.shape == ln.shape and o.ndim == 1
+        out, greedy = self._greedy_out(len(arr), out, greedy)
+        ip = C.POINTER(C.c_int)
+        served = self.lib.calm_b200_score_context_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), co.ctypes.data_as(ip),
+                                                         cl.ctypes.data_as(ip), o.ctypes.data_as(ip), ln.ctypes.data_as(ip), len(o),
+                                                         out.ctypes.data_as(_fptr), greedy.ctypes.data_as(ip))
+        return out, greedy, served
 
     def forward_raw(self, token: int, pos: int, flags: int = 0):
         return self.lib.forward_cuda(C.byref(self.transformer), token, pos, flags)

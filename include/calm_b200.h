@@ -148,6 +148,21 @@ int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, in
  * calm_b200_score (DESIGN.md s.6). */
 int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off, const int* len, int nseq, float* logprobs);
 
+/* The three scoring calls above, each also returning the greedy token at every scored position.  Each takes its
+ * sibling's arguments plus `greedy` (not NULL), returns what the sibling returns and writes `logprobs` bit for bit as the
+ * sibling does.  greedy[i] is written at exactly the slots where logprobs[i] is, other slots are left untouched, and
+ *   greedy[i] = argmax over the vocabulary of the logits at the position logprobs[i] scores,
+ * ties going to the lowest index (the reference's sample_argmax, sampler.c:34-42, and calm_b200_forward_argmax).  On the
+ * tensor-core pass the logits are the fp32 classifier outputs the log-softmax is computed from, so the greedy token's
+ * logit is the maximum that log-softmax subtracts; on the decode path they are the logits forward_cuda returns.
+ * Uses: is_greedy of a loglikelihood request (every continuation token equals its position's greedy token), and
+ * verifying draft tokens on a live cache with calm_b200_score_greedy at pos0 > 0 (INTEGRATION.md). */
+int calm_b200_score_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, int* greedy);
+int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
+                                 float* logprobs, int* greedy);
+int calm_b200_score_context_greedy(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                   const int* off, const int* len, int nseq, float* logprobs, int* greedy);
+
 /* forward + device-side greedy sample.  Returns argmax(logits) with the
  * reference's tie rule (lowest index, sampler.c:34-42).  The logits are still
  * written to state.logits. */
