@@ -135,8 +135,8 @@ struct Prefill {
 	__half *Nhi = nullptr, *Nlo = nullptr, *Ahi = nullptr, *Alo = nullptr, *Hhi = nullptr, *Hlo = nullptr;
 	float2* rope = nullptr;
 	int* tokens = nullptr;
-	int *rowpos = nullptr, *seg = nullptr; // packed blocks (calm_b200_score_batch): a row's RoPE position, its sequence's first row
-	int2* ctx = nullptr; // packed blocks with contexts (calm_b200_score_context): a row's context, its first row and length
+	int *rowpos = nullptr, *seg = nullptr; // packed blocks (calm_b200_score_batch / _context): a row's RoPE position, its sequence's first row
+	int2* ctx = nullptr; // packed blocks that hold a context: a row's context, its first row and length
 	CUtensorMap tmN[2], tmA[2], tmH[2]; // (hi, lo) views of the three activation matrices the GEMMs read
 	// scoring (calm_b200_score), allocated on its first call for `cap` rows: the classifier's per-tile records, the targets'
 	// logits, the targets and the log-probabilities
@@ -1177,10 +1177,9 @@ static void pf_attn(const PfAttnArgs& a, int n) {
 // What the rows of a prompt-pass block are
 enum PfRows {
 	PF_ONE,      // one sequence at cache slots pos0 + t
-	PF_PACKED,   // independent sequences (calm_b200_score_batch, pos0 = 0): per-row RoPE positions in pf.rowpos, each row's
-	             // sequence start in pf.seg
-	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block (calm_b200_score_context): each row's
-	             // context in pf.ctx
+	PF_PACKED,   // a packed block of the scoring calls (pos0 = 0) that holds no context: per-row RoPE positions in pf.rowpos,
+	             // each row's sequence start in pf.seg
+	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block: each row's context in pf.ctx
 };
 
 // The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says.
@@ -1272,6 +1271,24 @@ static void pf_score(Formats<DBITS, KVT>, int n, bool greedy) {
 	}
 }
 
+// One block of the pass: the n rows the caller reserved (pf_reserve) and uploaded to pf.tokens (and, packed, to pf.rowpos,
+// pf.seg and pf.ctx) at cache slots pos0 + t, laid out as `layout` says.  With `logprobs`, the rows are scored against
+// targets[0 .. n) as well: logprobs[t] is row t's log-probability and, with `greedy`, greedy[t] its argmax.
+static void pf_block(int n, int pos0, PfRows layout, const int* targets, float* logprobs, int* greedy) {
+	if (logprobs) {
+		pf_score_reserve(greedy);
+		CUDA_CHECK(cudaMemcpyAsync(pf.targets, targets, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	}
+	with_formats([&](auto f) { pf_run(f, n, pos0, layout); });
+	if (logprobs) {
+		with_formats([&](auto f) { pf_score(f, n, greedy); });
+		CUDA_CHECK(cudaMemcpyAsync(logprobs, pf.logprob, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+		if (greedy) CUDA_CHECK(cudaMemcpyAsync(greedy, pf.greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+	}
+	CUDA_CHECK(cudaStreamSynchronize(g.stream)); // the uploads read the caller's memory (pageable): they must have left it
+	CUDA_CHECK(cudaGetLastError());
+}
+
 // The batched pass over tokens[0 .. n) at positions pos0 .., in blocks of at most 2048 rows.  With `logprobs`, every block
 // is scored as well: logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]], so tokens[n] must exist; with
 // `greedy` too, greedy[i] = the argmax of those logits.
@@ -1281,19 +1298,8 @@ static void pf_pass(const int* tokens, int n, int pos0, float* logprobs, int* gr
 		const int m = n - o < chunk_cap ? n - o : chunk_cap;
 		pf_reserve(m);
 		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		if (logprobs) {
-			pf_score_reserve(greedy);
-			CUDA_CHECK(cudaMemcpyAsync(pf.targets, tokens + o + 1, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		}
-		with_formats([&](auto f) { pf_run(f, m, pos0 + o); });
-		if (logprobs) {
-			with_formats([&](auto f) { pf_score(f, m, greedy); });
-			CUDA_CHECK(cudaMemcpyAsync(logprobs + o, pf.logprob, (size_t)m * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
-			if (greedy) CUDA_CHECK(cudaMemcpyAsync(greedy + o, pf.greedy, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-		}
-		CUDA_CHECK(cudaStreamSynchronize(g.stream)); // `tokens` is the caller's memory (pageable): the copy above must have left it
+		pf_block(m, pos0 + o, PF_ONE, tokens + o + 1, logprobs ? logprobs + o : nullptr, greedy ? greedy + o : nullptr);
 	}
-	CUDA_CHECK(cudaGetLastError());
 }
 
 static void check_tokens(const int* tokens, int n) {
@@ -1363,101 +1369,17 @@ extern "C" int calm_b200_score_greedy(struct Transformer* transformer, const int
 	return pf_score_one(transformer, tokens, n, pos0, logprobs, greedy);
 }
 
-// One packed block of calm_b200_score_batch: sequence seqs[k] takes rows [s, s + R) with R = its rows rounded up to 8, RoPE
-// positions 0 .. R - 1 and cache slots s .. s + R - 1.  Its filler rows (after the live ones) repeat its last input token
-// and target its last token; causal attention keeps them out of every live row, and their results are dropped.
-static void pf_score_block(const int* tokens, const int* off, const int* len, const std::vector<int>& seqs, int rows, float* logprobs, int* greedy) {
-	std::vector<int> tok(rows), tgt(rows), pos(rows), seg(rows), gr(greedy ? rows : 0);
-	std::vector<float> lp(rows);
-	for (int k = 0, s = 0; k < (int)seqs.size(); ++k) {
-		const int* t = tokens + off[seqs[k]];
-		const int r = len[seqs[k]] - 1, R = cdiv(r, 8) * 8;
-		for (int j = 0; j < R; ++j) tok[s + j] = t[imin(j, r - 1)], tgt[s + j] = t[imin(j + 1, r)], pos[s + j] = j, seg[s + j] = s;
-		s += R;
-	}
-	pf_reserve(rows);
-	pf_score_reserve(greedy);
-	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(pf.targets, tgt.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(pf.seg, seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	with_formats([&](auto f) { pf_run(f, rows, 0, PF_PACKED); });
-	with_formats([&](auto f) { pf_score(f, rows, greedy); });
-	CUDA_CHECK(cudaMemcpyAsync(lp.data(), pf.logprob, (size_t)rows * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
-	if (greedy) CUDA_CHECK(cudaMemcpyAsync(gr.data(), pf.greedy, (size_t)rows * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-	CUDA_CHECK(cudaStreamSynchronize(g.stream));
-	CUDA_CHECK(cudaGetLastError());
-	for (int k = 0, s = 0; k < (int)seqs.size(); ++k) {
-		const int r = len[seqs[k]] - 1;
-		memcpy(logprobs + off[seqs[k]], lp.data() + s, (size_t)r * sizeof(float));
-		if (greedy) memcpy(greedy + off[seqs[k]], gr.data() + s, (size_t)r * sizeof(int));
-		s += cdiv(r, 8) * 8;
-	}
-}
-
-// Score nseq independent sequences from position 0 (include/calm_b200.h): next-fit packing in input order into blocks of
-// at most C = min(2048, seq_len rounded down to 8) rows, every sequence starting at a multiple of 8 rows so that a
-// k_pf_attn CTA never straddles two.  A sequence too long for a block is scored alone by calm_b200_score.
-// With `greedy`, calm_b200_score_batch_greedy.
-static int pf_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
-	if (!g.ready) CALM_FATAL("score_batch before prepare_cuda");
-	if (n < 0 || nseq < 0) CALM_FATAL("score_batch: negative count (n %d, nseq %d)", n, nseq);
-	if (nseq == 0) return 1;
-	check_tokens(tokens, n);
-	std::vector<std::pair<long, long>> out; // [first, last + 1) of the logprobs each sequence writes
-	for (int i = 0; i < nseq; ++i) {
-		if (off[i] < 0 || len[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("score_batch: sequence %d (off %d, len %d) outside the %d tokens", i, off[i], len[i], n);
-		if (len[i] >= 2) out.push_back({off[i], (long)off[i] + len[i] - 1});
-	}
-	std::sort(out.begin(), out.end());
-	for (size_t k = 1; k < out.size(); ++k)
-		if (out[k].first < out[k - 1].second) CALM_FATAL("score_batch: output ranges [%ld, %ld) and [%ld, %ld) overlap", out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
-	int served = 1;
-	// calm_b200_score(_greedy) of sequence i alone
-	auto alone = [&](int i) { return pf_score_one(transformer, tokens + off[i], len[i], 0, logprobs + off[i], greedy ? greedy + off[i] : nullptr); };
-	if (!pf_supported()) { // the shapes calm_b200_score serves on the decode path
-		for (int i = 0; i < nseq; ++i)
-			if (len[i] >= 2) alone(i);
-		return 0;
-	}
-	const int cap = imin(2048, g.cfg.seq_len / 8 * 8); // a row is its cache slot: no row may reach seq_len
-	std::vector<int> block, big;
-	int rows = 0;
-	for (int i = 0; i < nseq; ++i) {
-		if (len[i] < 2) continue;
-		const int R = cdiv(len[i] - 1, 8) * 8;
-		if (R > cap) {
-			big.push_back(i);
-			continue;
-		}
-		if (rows + R > cap) pf_score_block(tokens, off, len, block, rows, logprobs, greedy), block.clear(), rows = 0;
-		block.push_back(i), rows += R;
-	}
-	if (rows) pf_score_block(tokens, off, len, block, rows, logprobs, greedy);
-	for (int i : big) served &= alone(i);
-	return served;
-}
-
-extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
-	return pf_score_batch(transformer, tokens, n, off, len, nseq, logprobs, nullptr);
-}
-
-extern "C" int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
-                                            float* logprobs, int* greedy) {
-	if (!greedy) CALM_FATAL("score_batch_greedy: greedy is NULL");
-	return pf_score_batch(transformer, tokens, n, off, len, nseq, logprobs, greedy);
-}
-
-// A packed block of calm_b200_score_context being filled: per-row inputs, the sequences it scores with their first rows,
-// and the contexts it holds by (ctx_off, ctx_len) with their first rows.
-struct PfContextBlock {
+// A packed block being filled: per-row inputs, the sequences it scores with their first rows, and the contexts it holds
+// by (ctx_off, ctx_len) with their first rows.  Row t of the block is cache slot t.
+struct PfPackedBlock {
 	std::vector<int> tok, tgt, pos, seg;
 	std::vector<int2> ctx;
 	std::vector<std::pair<int, int>> seqs;
 	std::map<std::pair<int, int>, int> placed;
 	int rows() const { return (int)tok.size(); }
 	// Rows for the r inputs t[0 .. r) at RoPE positions p0 .., continuing context cx, rounded up to a multiple of 8 with
-	// filler rows that repeat the last input; row j targets t[min(j + 1, tl)].  Returns the first row.
+	// filler rows that repeat the last input, so that a k_pf_attn CTA never straddles two sequences; row j targets
+	// t[min(j + 1, tl)].  Causal attention keeps filler rows out of every live row.  Returns the first row.
 	int add(const int* t, int r, int tl, int p0, int2 cx) {
 		const int s = rows();
 		for (int j = 0; j < cdiv(r, 8) * 8; ++j)
@@ -1466,55 +1388,50 @@ struct PfContextBlock {
 	}
 };
 
-// Run a block and write its sequences' log-probabilities.  A block that holds no context runs the packed attention of
-// calm_b200_score_batch; only one with a context runs the context walk (k_pf_attn<.., SEG, CTX>).
-static void pf_score_context_block(PfContextBlock& b, const int* off, const int* len, float* logprobs, int* greedy) {
+// Run a block and write its sequences' log-probabilities; the results of context and filler rows are dropped.  A block that
+// holds no context runs the packed attention (k_pf_attn<.., SEG>); only one with a context uploads pf.ctx and runs the
+// context walk (k_pf_attn<.., SEG, CTX>).
+static void pf_score_packed_block(PfPackedBlock& b, const int* off, const int* len, float* logprobs, int* greedy) {
 	const int rows = b.rows();
 	const bool contexts = !b.placed.empty();
 	std::vector<float> lp(rows);
 	std::vector<int> gr(greedy ? rows : 0);
 	pf_reserve(rows);
-	pf_score_reserve(greedy);
 	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, b.tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(pf.targets, b.tgt.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, b.pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.seg, b.seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	if (contexts) CUDA_CHECK(cudaMemcpyAsync(pf.ctx, b.ctx.data(), (size_t)rows * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
-	with_formats([&](auto f) { pf_run(f, rows, 0, contexts ? PF_CONTEXTS : PF_PACKED); });
-	with_formats([&](auto f) { pf_score(f, rows, greedy); });
-	CUDA_CHECK(cudaMemcpyAsync(lp.data(), pf.logprob, (size_t)rows * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
-	if (greedy) CUDA_CHECK(cudaMemcpyAsync(gr.data(), pf.greedy, (size_t)rows * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-	CUDA_CHECK(cudaStreamSynchronize(g.stream));
-	CUDA_CHECK(cudaGetLastError());
+	pf_block(rows, 0, contexts ? PF_CONTEXTS : PF_PACKED, b.tgt.data(), lp.data(), greedy ? gr.data() : nullptr);
 	for (const auto& [i, s] : b.seqs) {
 		memcpy(logprobs + off[i], lp.data() + s, (size_t)(len[i] - 1) * sizeof(float));
 		if (greedy) memcpy(greedy + off[i], gr.data() + s, (size_t)(len[i] - 1) * sizeof(int));
 	}
-	b = PfContextBlock();
+	b = PfPackedBlock();
 }
 
-// Score nseq sequences that continue contexts (include/calm_b200.h).  Next-fit packing in input order into blocks of at
-// most C = min(2048, seq_len rounded down to 8) rows: a context takes ceil8(ctx_len) rows at RoPE positions 0 ..; a
-// sequence takes ceil8(len - 1) rows at positions ctx_len .., after its context's rows in the same block.  Sequences with
-// the same (ctx_off, ctx_len) share one placement of the context per block; a sequence whose context is not yet in the
-// block brings it along.  A context and sequence too long for any block, together, are scored alone by calm_b200_score.
-// With `greedy`, calm_b200_score_context_greedy.
-static int pf_score_contexts(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off, const int* len,
-                             int nseq, float* logprobs, int* greedy) {
-	if (!g.ready) CALM_FATAL("score_context before prepare_cuda");
-	if (n < 0 || nseq < 0) CALM_FATAL("score_context: negative count (n %d, nseq %d)", n, nseq);
+// Score nseq sequences that continue contexts (include/calm_b200.h); `who` names the call in error messages.  Next-fit
+// packing in input order into blocks of at most C = min(2048, seq_len rounded down to 8) rows: a context takes
+// ceil8(ctx_len) rows at RoPE positions 0 ..; a sequence takes ceil8(len - 1) rows at positions ctx_len .., after its
+// context's rows in the same block.  Sequences with the same (ctx_off, ctx_len) share one placement of the context per
+// block; a sequence whose context is not yet in the block brings it along.  A context and sequence too long for any block,
+// together, are scored alone by calm_b200_score.  With every ctx_len 0 no block holds a context: calm_b200_score_batch.
+// With `greedy`, the greedy calls.
+static int pf_score_packed(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                           const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
+	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
+	if (n < 0 || nseq < 0) CALM_FATAL("%s: negative count (n %d, nseq %d)", who, n, nseq);
 	if (nseq == 0) return 1;
 	check_tokens(tokens, n);
 	std::vector<std::pair<long, long>> out; // [first, last + 1) of the logprobs each sequence writes
 	for (int i = 0; i < nseq; ++i) {
-		if (off[i] < 0 || len[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("score_context: sequence %d (off %d, len %d) outside the %d tokens", i, off[i], len[i], n);
+		if (off[i] < 0 || len[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("%s: sequence %d (off %d, len %d) outside the %d tokens", who, i, off[i], len[i], n);
 		if (ctx_off[i] < 0 || ctx_len[i] < 0 || (long)ctx_off[i] + ctx_len[i] > n)
-			CALM_FATAL("score_context: context of sequence %d (off %d, len %d) outside the %d tokens", i, ctx_off[i], ctx_len[i], n);
+			CALM_FATAL("%s: context of sequence %d (off %d, len %d) outside the %d tokens", who, i, ctx_off[i], ctx_len[i], n);
 		if (len[i] >= 2) out.push_back({off[i], (long)off[i] + len[i] - 1});
 	}
 	std::sort(out.begin(), out.end());
 	for (size_t k = 1; k < out.size(); ++k)
-		if (out[k].first < out[k - 1].second) CALM_FATAL("score_context: output ranges [%ld, %ld) and [%ld, %ld) overlap", out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
+		if (out[k].first < out[k - 1].second) CALM_FATAL("%s: output ranges [%ld, %ld) and [%ld, %ld) overlap", who, out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
 	// calm_b200_score of ctx ++ sequence, by definition the result: for shapes the pass does not serve and units too big
 	auto alone = [&](int i) {
 		std::vector<int> cat(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
@@ -1532,7 +1449,7 @@ static int pf_score_contexts(struct Transformer* transformer, const int* tokens,
 		return 0;
 	}
 	const int cap = imin(2048, g.cfg.seq_len / 8 * 8); // a row is its cache slot: no row may reach seq_len
-	PfContextBlock b;
+	PfPackedBlock b;
 	std::vector<int> big;
 	for (int i = 0; i < nseq; ++i) {
 		if (len[i] < 2) continue;
@@ -1542,7 +1459,7 @@ static int pf_score_contexts(struct Transformer* transformer, const int* tokens,
 			continue;
 		}
 		const std::pair<int, int> key(ctx_off[i], ctx_len[i]);
-		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_context_block(b, off, len, logprobs, greedy);
+		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_packed_block(b, off, len, logprobs, greedy);
 		int c0 = 0;
 		if (ctx_len[i]) {
 			const auto it = b.placed.find(key);
@@ -1550,21 +1467,33 @@ static int pf_score_contexts(struct Transformer* transformer, const int* tokens,
 		}
 		b.seqs.push_back({i, b.add(tokens + off[i], len[i] - 1, len[i] - 1, ctx_len[i], make_int2(c0, ctx_len[i]))});
 	}
-	if (b.rows()) pf_score_context_block(b, off, len, logprobs, greedy);
+	if (b.rows()) pf_score_packed_block(b, off, len, logprobs, greedy);
 	int served = 1;
 	for (int i : big) served &= alone(i);
 	return served;
 }
 
+extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
+	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
+	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, nullptr);
+}
+
+extern "C" int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
+                                            float* logprobs, int* greedy) {
+	if (!greedy) CALM_FATAL("score_batch_greedy: greedy is NULL");
+	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
+	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, greedy);
+}
+
 extern "C" int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
                                        const int* off, const int* len, int nseq, float* logprobs) {
-	return pf_score_contexts(transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, nullptr);
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, nullptr);
 }
 
 extern "C" int calm_b200_score_context_greedy(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
                                               const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
 	if (!greedy) CALM_FATAL("score_context_greedy: greedy is NULL");
-	return pf_score_contexts(transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, greedy);
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, greedy);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests

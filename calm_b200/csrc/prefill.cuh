@@ -20,10 +20,10 @@
 // Scoring (calm_b200_score, the reference's study(): run.c:291-308) adds the classifier over all rows of the block without
 // ever writing the [T][vocab] logits: the final norm (k_pf_norm), k_pf_gemm in PF_CLS mode, whose epilogue reduces each
 // token's 128 logits of the tile to one (max, sum exp(logit - max)) record and keeps the target's logit, and k_pf_logprob,
-// which merges a token's records in a fixed order into ln softmax(logits)[target].  calm_b200_score_batch packs several
-// independent sequences into one block: per-row RoPE positions (k_pf_rope_rows) and attention that starts each sequence's
-// key tiles at its own first row (k_pf_attn<.., SEG>); everything else works per row and is unchanged.
-// calm_b200_score_context also packs contexts, once per block, and sequences that continue them: a sequence's rows attend
+// which merges a token's records in a fixed order into ln softmax(logits)[target].  The packed scoring calls (score_batch,
+// score_context) put several sequences into one block: per-row RoPE positions (k_pf_rope_rows) and attention that starts
+// each sequence's key tiles at its own first row (k_pf_attn<.., SEG>); everything else works per row.  A packed block
+// may also hold contexts, once each, and sequences that continue them: a sequence's rows attend
 // to its context's rows and then its own as one key sequence (k_pf_attn<.., SEG, CTX>).  The greedy scoring calls run
 // PF_CLS_GREEDY and k_pf_logprob<true>, which also give each row's argmax, with the same log-probability bits.
 //
@@ -128,8 +128,8 @@ __global__ void k_pf_rope(float2* rope, const float* freq, int n, int half_hd, i
 	rope[i] = make_float2(c, s);
 }
 
-// rope[t][j] = (cos, sin)(rowpos[t] * freq[j]): the table of a packed block, whose rows restart at 0 with each sequence
-// (calm_b200_score_batch); for rowpos[t] = pos0 + t the same float arguments as k_pf_rope, so the same bits
+// rope[t][j] = (cos, sin)(rowpos[t] * freq[j]): the table of a packed block, whose positions restart with each context
+// and sequence it holds; for rowpos[t] = pos0 + t the same float arguments as k_pf_rope, so the same bits
 __global__ void k_pf_rope_rows(float2* rope, const float* freq, const int* rowpos, int n, int half_hd) {
 	pdl_enter();
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -527,11 +527,11 @@ __device__ __forceinline__ void pf_load_dims(const uint8_t* p, float (&o)[DPL]) 
 }
 
 // CTA = (kv head, 8 consecutive query tokens); warp = one token with all kv_mul query heads of the kv head (KM of them per pass).
-// SEG: a packed block of independent sequences (calm_b200_score_batch, pos0 = 0, row t in cache slot t).  The host starts
+// SEG: a packed block of the scoring calls (score_batch, score_context; pos0 = 0, row t in cache slot t).  The host starts
 // every sequence at a multiple of 8 rows, so the CTA's rows share one segment starting at row s = seg[first row], and the key
 // tiles run from s: tile j of a sequence holds the same keys in the same order as tile j of the sequence scored alone from
 // position 0, and each warp's online softmax sees exactly the values of that lone pass.
-// CTX (with SEG): a packed block whose sequences continue shared contexts (calm_b200_score_context).  A CTA's rows start at
+// CTX (with SEG): a packed block that also holds contexts its sequences continue.  A CTA's rows start at
 // row s and continue the nc-row context at rows c0 .. c0 + nc - 1 (ctx[first row]).  The keys run over one virtual index v:
 // v < nc is row c0 + v, v >= nc is row s + v - nc; row t sees v <= nc + t - s.  A tile may straddle the two ranges, so each
 // tile row finds its own address.  Tile j then holds the keys of tile j of ctx ++ sequence scored alone from position 0,

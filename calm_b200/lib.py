@@ -167,22 +167,33 @@ class DeviceModel:
         served = self.lib.calm_b200_score(C.byref(self.transformer), arr.ctypes.data_as(C.POINTER(C.c_int)), len(arr), pos0, out.ctypes.data_as(_fptr))
         return out, served
 
+    def _score_packed(self, fn, tokens, index, out, greedy=None, with_greedy=False):
+        """Call the packed scoring symbol `fn` over `tokens`.  `index` holds its per-sequence arrays in the C argument order
+        ((off, len) or (ctx_off, ctx_len, off, len)).  `out` defaults to NaN, and for a greedy symbol (`with_greedy`)
+        `greedy` to -1.  Returns (out, served), or (out, greedy, served) with `with_greedy`."""
+        ip = C.POINTER(C.c_int)
+        arr = np.ascontiguousarray(tokens, np.int32)
+        index = [np.ascontiguousarray(a, np.int32) for a in index]
+        assert index[0].ndim == 1 and all(a.shape == index[0].shape for a in index)
+        n = len(arr)
+        if out is None:
+            out = np.full(n, np.nan, np.float32)
+        assert out.dtype == np.float32 and out.flags.c_contiguous and len(out) >= n
+        outs = [out.ctypes.data_as(_fptr)]
+        if with_greedy:
+            if greedy is None:
+                greedy = np.full(n, -1, np.int32)
+            assert greedy.dtype == np.int32 and greedy.flags.c_contiguous and len(greedy) >= n
+            outs.append(greedy.ctypes.data_as(ip))
+        served = fn(C.byref(self.transformer), arr.ctypes.data_as(ip), n, *[a.ctypes.data_as(ip) for a in index], len(index[0]), *outs)
+        return (out, greedy, served) if with_greedy else (out, served)
+
     def score_batch(self, tokens, off, len_, out=None):
         """calm_b200_score_batch: independent sequences tokens[off[i] : off[i] + len_[i]], each scored from position 0 and
         packed into shared prompt-pass blocks.  Returns (float32[len(tokens)] with sequence i's log-probabilities at
         off[i] .. off[i] + len_[i] - 2, 1 when the tensor-core pass served every sequence or 0).  Slots no sequence writes
         keep what `out` held (NaN when no `out` is given)."""
-        arr = np.ascontiguousarray(tokens, np.int32)
-        o = np.ascontiguousarray(off, np.int32)
-        ln = np.ascontiguousarray(len_, np.int32)
-        assert o.shape == ln.shape and o.ndim == 1
-        if out is None:
-            out = np.full(len(arr), np.nan, np.float32)
-        assert out.dtype == np.float32 and out.flags.c_contiguous and len(out) >= len(arr)
-        ip = C.POINTER(C.c_int)
-        served = self.lib.calm_b200_score_batch(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), o.ctypes.data_as(ip),
-                                                ln.ctypes.data_as(ip), len(o), out.ctypes.data_as(_fptr))
-        return out, served
+        return self._score_packed(self.lib.calm_b200_score_batch, tokens, (off, len_), out)
 
     def score_context(self, tokens, ctx_off, ctx_len, off, len_, out=None):
         """calm_b200_score_context: sequences tokens[off[i] : off[i] + len_[i]], each continuing the context
@@ -190,37 +201,14 @@ class DeviceModel:
         per block.  Returns (float32[len(tokens)] with sequence i's log-probabilities at off[i] .. off[i] + len_[i] - 2, 1
         when the tensor-core pass served every sequence or 0).  Slots no sequence writes keep what `out` held (NaN when no
         `out` is given)."""
-        arr = np.ascontiguousarray(tokens, np.int32)
-        co = np.ascontiguousarray(ctx_off, np.int32)
-        cl = np.ascontiguousarray(ctx_len, np.int32)
-        o = np.ascontiguousarray(off, np.int32)
-        ln = np.ascontiguousarray(len_, np.int32)
-        assert co.shape == cl.shape == o.shape == ln.shape and o.ndim == 1
-        if out is None:
-            out = np.full(len(arr), np.nan, np.float32)
-        assert out.dtype == np.float32 and out.flags.c_contiguous and len(out) >= len(arr)
-        ip = C.POINTER(C.c_int)
-        served = self.lib.calm_b200_score_context(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), co.ctypes.data_as(ip),
-                                                  cl.ctypes.data_as(ip), o.ctypes.data_as(ip), ln.ctypes.data_as(ip), len(o),
-                                                  out.ctypes.data_as(_fptr))
-        return out, served
-
-    @staticmethod
-    def _greedy_out(n, out, greedy):
-        """The output arrays of a greedy scoring call over n tokens: NaN / -1 where none are given."""
-        if out is None:
-            out = np.full(n, np.nan, np.float32)
-        if greedy is None:
-            greedy = np.full(n, -1, np.int32)
-        assert out.dtype == np.float32 and out.flags.c_contiguous and len(out) >= n
-        assert greedy.dtype == np.int32 and greedy.flags.c_contiguous and len(greedy) >= n
-        return out, greedy
+        return self._score_packed(self.lib.calm_b200_score_context, tokens, (ctx_off, ctx_len, off, len_), out)
 
     def score_greedy(self, tokens, pos0: int = 0):
         """calm_b200_score_greedy: score()'s log-probabilities, bit for bit, and the argmax of the logits at each scored
         position (lowest index on ties).  Returns (float32[n - 1], int32[n - 1], served)."""
         arr = np.ascontiguousarray(tokens, np.int32)
-        out, greedy = self._greedy_out(max(len(arr) - 1, 0), None, None)
+        out = np.full(max(len(arr) - 1, 0), np.nan, np.float32)
+        greedy = np.full(len(out), -1, np.int32)
         ip = C.POINTER(C.c_int)
         served = self.lib.calm_b200_score_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), pos0, out.ctypes.data_as(_fptr),
                                                  greedy.ctypes.data_as(ip))
@@ -230,32 +218,13 @@ class DeviceModel:
         """calm_b200_score_batch_greedy: score_batch()'s log-probabilities, bit for bit, and the greedy token at the same
         slots.  Returns (float32[len(tokens)], int32[len(tokens)], served); unwritten slots keep what `out` / `greedy` held
         (NaN / -1 when not given)."""
-        arr = np.ascontiguousarray(tokens, np.int32)
-        o = np.ascontiguousarray(off, np.int32)
-        ln = np.ascontiguousarray(len_, np.int32)
-        assert o.shape == ln.shape and o.ndim == 1
-        out, greedy = self._greedy_out(len(arr), out, greedy)
-        ip = C.POINTER(C.c_int)
-        served = self.lib.calm_b200_score_batch_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), o.ctypes.data_as(ip),
-                                                       ln.ctypes.data_as(ip), len(o), out.ctypes.data_as(_fptr), greedy.ctypes.data_as(ip))
-        return out, greedy, served
+        return self._score_packed(self.lib.calm_b200_score_batch_greedy, tokens, (off, len_), out, greedy, with_greedy=True)
 
     def score_context_greedy(self, tokens, ctx_off, ctx_len, off, len_, out=None, greedy=None):
         """calm_b200_score_context_greedy: score_context()'s log-probabilities, bit for bit, and the greedy token at the
         same slots.  Returns (float32[len(tokens)], int32[len(tokens)], served); unwritten slots keep what `out` / `greedy`
         held (NaN / -1 when not given)."""
-        arr = np.ascontiguousarray(tokens, np.int32)
-        co = np.ascontiguousarray(ctx_off, np.int32)
-        cl = np.ascontiguousarray(ctx_len, np.int32)
-        o = np.ascontiguousarray(off, np.int32)
-        ln = np.ascontiguousarray(len_, np.int32)
-        assert co.shape == cl.shape == o.shape == ln.shape and o.ndim == 1
-        out, greedy = self._greedy_out(len(arr), out, greedy)
-        ip = C.POINTER(C.c_int)
-        served = self.lib.calm_b200_score_context_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), co.ctypes.data_as(ip),
-                                                         cl.ctypes.data_as(ip), o.ctypes.data_as(ip), ln.ctypes.data_as(ip), len(o),
-                                                         out.ctypes.data_as(_fptr), greedy.ctypes.data_as(ip))
-        return out, greedy, served
+        return self._score_packed(self.lib.calm_b200_score_context_greedy, tokens, (ctx_off, ctx_len, off, len_), out, greedy, with_greedy=True)
 
     def forward_raw(self, token: int, pos: int, flags: int = 0):
         return self.lib.forward_cuda(C.byref(self.transformer), token, pos, flags)

@@ -126,7 +126,8 @@ int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, i
  * pass, 0 when any went through the decode path.  The KV cache afterwards holds nothing a host can continue from.
  * Every token of tokens[0 .. n) must be in the vocabulary, and 0 <= off[i], off[i] + len[i] <= n; a sequence with
  * len[i] < 2 contributes nothing, nseq == 0 returns 1.  Many short sequences share one block of up to 2048 rows (DESIGN.md
- * s.6), so they fill the GPU where one call per sequence would leave most of it idle. */
+ * s.6), so they fill the GPU where one call per sequence would leave most of it idle.  It equals calm_b200_score_context
+ * with every ctx_len[i] == 0. */
 int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len,
                           int nseq, float* logprobs);
 

@@ -8,76 +8,40 @@ exact: each sequence's log-probabilities equal, bit for bit, what calm_b200_scor
   fill a block exactly, sequences too long for a block, a short seq_len and Llama-3-8B widths at vocabulary 128256.
 - Packing order does not matter; slots no sequence writes are left alone.
 - The decode-path fallback (MoE, head_dim 32, a sequence longer than seq_len) returns 0 with the lone call's values.
-- No result depends on what earlier calls left behind, and nothing after a batch depends on it either."""
+- No result depends on what earlier calls left behind, and nothing after a batch depends on it either.
+
+The call is calm_b200_score_context with every context empty; the helpers are test_score_context_gpu.py's, and a case
+here is its layout with ctx_off = ctx_len = 0."""
+import os
+import sys
 from dataclasses import replace
 
 import numpy as np
 import pytest
 import torch
 
-from calm_b200 import lib
-from calm_b200 import modelgen as mg
-from calm_b200.cstructs import FF_UPDATE_KV_ONLY
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from test_score_context_gpu import (SENTINEL, assert_independent_of_history, assert_nothing_after_depends_on_it,  # noqa: E402
+                                    assert_order_does_not_matter, check, fresh_results)
+
+from calm_b200 import lib  # noqa: E402
+from calm_b200 import modelgen as mg  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = np.float32(-12345.5)
-
 
 def pack(vocab, lens, seed):
-    """Random sequences of the given lengths, concatenated: (tokens, off, len)."""
+    """Random sequences of the given lengths, concatenated, with empty contexts: (tokens, ctx_off, ctx_len, off, len)."""
     rng = np.random.default_rng(seed)
     off = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.int32)
-    return rng.integers(0, vocab, int(sum(lens))).astype(np.int32), off, np.asarray(lens, np.int32)
+    zero = np.zeros(len(lens), np.int32)
+    return rng.integers(0, vocab, int(sum(lens))).astype(np.int32), zero, zero, off, np.asarray(lens, np.int32)
 
 
 def study_chunks(n_tokens, steps):
     """study()'s chunks of a text: chunk c scores positions c * steps .. and shares its last token with chunk c + 1."""
     off = np.arange(0, n_tokens - 1, steps, dtype=np.int32)
     return off, np.minimum(steps + 1, n_tokens - off).astype(np.int32)
-
-
-def lone(dm, tokens, off, lens):
-    """calm_b200_score of each sequence on its own from position 0: (list of log-probability arrays, all served)."""
-    want, served = [], 1
-    for o, n in zip(off, lens):
-        lp, s = dm.score(tokens[o:o + n], 0)
-        want.append(lp)
-        served &= s if n >= 2 else 1
-    return want, served
-
-
-def batch(dm, tokens, off, lens):
-    out = np.full(len(tokens), SENTINEL, np.float32)
-    got, served = dm.score_batch(tokens, off, lens, out)
-    assert got is out
-    return got, served
-
-
-def assert_matches(got, want, tokens, off, lens, label):
-    """Sequence by sequence bit for bit; every written value finite, every other slot still the sentinel."""
-    written = np.zeros(len(tokens), bool)
-    for i, (o, n) in enumerate(zip(off, lens)):
-        if n < 2:
-            continue
-        part = got[o:o + n - 1]
-        assert np.isfinite(part).all(), f"{label}: sequence {i} (len {n}) has a value that is not finite"
-        if not np.array_equal(part, want[i]):
-            j = int(np.argmax(part != want[i]))
-            raise AssertionError(f"{label}: sequence {i} (len {n}), position {j}: batch {part[j]!r} vs alone {want[i][j]!r} "
-                                 f"({int((part != want[i]).sum())} of {n - 1} positions differ)")
-        written[o:o + n - 1] = True
-    assert (got[~written] == SENTINEL).all(), f"{label}: a slot no sequence writes was changed"
-
-
-def check(spec, tensors, tokens, off, lens, label, seq_len=None, kvbits=16, served=1):
-    with lib.DeviceModel(spec, tensors, seq_len=seq_len, kvbits=kvbits) as dm:
-        want, s_lone = lone(dm, tokens, off, lens)
-    with lib.DeviceModel(spec, tensors, seq_len=seq_len, kvbits=kvbits) as dm:
-        got, s_batch = batch(dm, tokens, off, lens)
-    assert s_batch == served and s_lone == served, f"{label}: served {s_batch} (alone {s_lone}), expected {served}"
-    assert_matches(got, want, tokens, off, lens, label)
-    return got, want
 
 
 # pf-tiny at seq_len 512: capacity 512 rows.  Rows rounded up to 8: 8, 8, 16, 40, 136, 264 (one block of 472), then 512 (a
@@ -90,8 +54,7 @@ LENS = [2, 3, 9, 40, 129, 257, 513, 1, 257, 129, 40, 0]
 def test_packed_equals_alone(name, dtype, kvbits):
     spec = replace(mg.SPECS[name], dtype=dtype)
     tensors = mg.generate(spec, 11)
-    tokens, off, lens = pack(spec.vocab_size, LENS, 1)
-    check(spec, tensors, tokens, off, lens, f"{name}/{dtype}/kv{kvbits}", seq_len=512, kvbits=kvbits)
+    check(spec, tensors, pack(spec.vocab_size, LENS, 1), f"{name}/{dtype}/kv{kvbits}", seq_len=512, kvbits=kvbits, batch=True)
 
 
 def test_study_chunks_equal_the_per_chunk_loop():
@@ -102,7 +65,8 @@ def test_study_chunks_equal_the_per_chunk_loop():
     n = 3000
     tokens = np.asarray(mg.teacher_tokens(spec.vocab_size, n), np.int32)
     off, lens = study_chunks(n, 256)
-    got, want = check(spec, tensors, tokens, off, lens, "study chunks", seq_len=4096)
+    zero = np.zeros(len(off), np.int32)
+    got = check(spec, tensors, (tokens, zero, zero, off, lens), "study chunks", seq_len=4096, batch=True)
     with lib.DeviceModel(spec, tensors, seq_len=4096) as dm:
         loop = np.full(n, SENTINEL, np.float32)
         for c in range(0, n - 1, 256):
@@ -119,8 +83,7 @@ def test_study_chunks_equal_the_per_chunk_loop():
 def test_sequences_longer_than_a_block(seq_len, lens):
     spec = mg.SPECS["pf-tiny"]
     tensors = mg.generate(spec, 13)
-    tokens, off, lens = pack(spec.vocab_size, lens, 2)
-    check(spec, tensors, tokens, off, lens, f"seq_len {seq_len}", seq_len=seq_len)
+    check(spec, tensors, pack(spec.vocab_size, lens, 2), f"seq_len {seq_len}", seq_len=seq_len, batch=True)
 
 
 def test_llama3_8b_widths():
@@ -128,20 +91,13 @@ def test_llama3_8b_widths():
     spec = replace(mg.SPECS["llama3-8b-fp8"], n_layers=2)
     tensors = mg.generate(spec, 14, device="cuda")
     torch.cuda.synchronize()
-    tokens, off, lens = pack(spec.vocab_size, [129] * 16, 3)
-    check(spec, tensors, tokens, off, lens, "llama3-8b widths", seq_len=4096)
+    check(spec, tensors, pack(spec.vocab_size, [129] * 16, 3), "llama3-8b widths", seq_len=4096, batch=True)
 
 
 def test_packing_order_does_not_matter():
     spec = mg.SPECS["pf-tiny"]
     tensors = mg.generate(spec, 15)
-    tokens, off, lens = pack(spec.vocab_size, [7, 300, 2, 65, 129, 33, 400, 17, 256, 90], 4)
-    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-        base, served = batch(dm, tokens, off, lens)
-        assert served == 1
-        for order in (np.arange(len(off))[::-1], np.random.default_rng(5).permutation(len(off))):
-            got, served = batch(dm, tokens, off[order], lens[order])
-            assert served == 1 and np.array_equal(got, base), f"order {order.tolist()} changed the results"
+    assert_order_does_not_matter(spec, tensors, pack(spec.vocab_size, [7, 300, 2, 65, 129, 33, 400, 17, 256, 90], 4), batch=True)
 
 
 @pytest.mark.parametrize("name,seq_len,lens", [("tiny-moe", None, [20, 2, 33, 9]), ("tiny-fp8", None, [20, 2, 33, 9]),
@@ -151,8 +107,7 @@ def test_falls_back_to_the_decode_path(name, seq_len, lens):
     there.  Either way the call returns 0 and the lone calls' values."""
     spec = mg.SPECS[name]
     tensors = mg.generate(spec, 16)
-    tokens, off, lens = pack(spec.vocab_size, lens, 6)
-    check(spec, tensors, tokens, off, lens, name, seq_len=seq_len, served=0)
+    check(spec, tensors, pack(spec.vocab_size, lens, 6), name, seq_len=seq_len, served=0, batch=True)
 
 
 # ---- history independence
@@ -161,46 +116,13 @@ HIST_LENS = [40, 129, 2, 257, 9, 63]
 
 @pytest.fixture(scope="module")
 def hist():
-    spec = mg.SPECS["pf-tiny"]
-    tensors = mg.generate(spec, 17)
-    tokens, off, lens = pack(spec.vocab_size, HIST_LENS, 7)
-    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-        fresh, served = batch(dm, tokens, off, lens)
-    assert served == 1
-    return spec, tensors, tokens, off, lens, fresh
+    return fresh_results(17, lambda vocab: pack(vocab, HIST_LENS, 7), batch=True)
 
 
 @pytest.mark.parametrize("before", ["poison", "score", "prefill", "score+poison"])
 def test_batch_does_not_depend_on_history(hist, before):
-    spec, tensors, tokens, off, lens, fresh = hist
-    long = np.asarray(mg.teacher_tokens(spec.vocab_size, 500, start=3), np.int32)
-    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-        if "score" in before:
-            dm.score(long, 0)
-        if before == "prefill":
-            dm.prefill(long, 0)
-        if "poison" in before:
-            dm.poison(0)
-        got, served = batch(dm, tokens, off, lens)
-    assert served == 1
-    assert np.isfinite(got[got != SENTINEL]).all() and np.array_equal(got, fresh), f"after {before}: the batch changed"
+    assert_independent_of_history(hist, before, batch=True)
 
 
 def test_nothing_after_a_batch_depends_on_it(hist):
-    """forward_prefill_cuda and forward_cuda from position 0 after a batch equal the fresh engine's, bit for bit."""
-    spec, tensors, tokens, off, lens, _ = hist
-    prompt = np.asarray(mg.teacher_tokens(spec.vocab_size, 200, start=9), np.int32)
-    runs = []
-    for dirty in (False, True):
-        with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-            if dirty:
-                batch(dm, tokens, off, lens)
-            assert dm.prefill(prompt[:150], 0) == 1
-            after_pf = [dm.forward(int(prompt[p]), p) for p in range(150, 160)]
-            if dirty:
-                batch(dm, tokens, off, lens)
-            dm.forward(int(prompt[0]), 0, FF_UPDATE_KV_ONLY)
-            serial = [dm.forward(int(prompt[p]), p) for p in range(1, 12)]
-            runs.append(after_pf + serial)
-    for i, (a, b) in enumerate(zip(*runs)):
-        assert np.isfinite(a).all() and np.array_equal(a, b), f"logits {i} after a batch differ from the fresh engine's"
+    assert_nothing_after_depends_on_it(hist, batch=True)

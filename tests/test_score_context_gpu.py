@@ -9,9 +9,12 @@ the claim is exact: each sequence's log-probabilities equal, bit for bit, calm_b
   weight format, both caches, both head sizes, and Llama-3-8B widths at vocabulary 128256.
 - Contexts shared by adjacent and non-adjacent sequences, a shared group that spills into a second block, equal contents
   at two offsets; one placement per block shows in the launch count.
-- All contexts empty equals calm_b200_score_batch; input order does not matter; units too big for a block and the
-  decode-path shapes give the lone values.
-- No result depends on what earlier calls left behind, and nothing after a call depends on it either."""
+- All contexts empty equals calm_b200_score_batch, in values and in launches; input order does not matter; units too big
+  for a block and the decode-path shapes give the lone values.
+- No result depends on what earlier calls left behind, and nothing after a call depends on it either.
+
+calm_b200_score_batch is this call with every context empty, and test_score_batch_gpu.py checks it with the helpers
+defined here (`batch=True`), on cases whose contexts are all empty."""
 from dataclasses import replace
 
 import numpy as np
@@ -56,9 +59,11 @@ def lone(dm, tokens, co, cl, off, lens):
     return want, served
 
 
-def run(dm, tokens, co, cl, off, lens):
+def run(dm, tokens, co, cl, off, lens, batch=False):
+    """The context call, or with `batch` calm_b200_score_batch of the same sequences (co and cl unused), into an output
+    that holds the sentinel."""
     out = np.full(len(tokens), SENTINEL, np.float32)
-    got, served = dm.score_context(tokens, co, cl, off, lens, out)
+    got, served = dm.score_batch(tokens, off, lens, out) if batch else dm.score_context(tokens, co, cl, off, lens, out)
     assert got is out
     return got, served
 
@@ -79,15 +84,72 @@ def assert_matches(got, want, tokens, off, lens, label):
     assert (got[~written] == SENTINEL).all(), f"{label}: a slot no sequence writes was changed"
 
 
-def check(spec, tensors, case, label, seq_len=None, kvbits=16, served=1):
+def check(spec, tensors, case, label, seq_len=None, kvbits=16, served=1, batch=False):
     tokens, co, cl, off, lens = case
     with lib.DeviceModel(spec, tensors, seq_len=seq_len, kvbits=kvbits) as dm:
         want, s_lone = lone(dm, tokens, co, cl, off, lens)
     with lib.DeviceModel(spec, tensors, seq_len=seq_len, kvbits=kvbits) as dm:
-        got, s_ctx = run(dm, tokens, co, cl, off, lens)
-    assert s_ctx == served and s_lone == served, f"{label}: served {s_ctx} (alone {s_lone}), expected {served}"
+        got, s_packed = run(dm, tokens, co, cl, off, lens, batch)
+    assert s_packed == served and s_lone == served, f"{label}: served {s_packed} (alone {s_lone}), expected {served}"
     assert_matches(got, want, tokens, off, lens, label)
     return got
+
+
+def assert_order_does_not_matter(spec, tensors, case, batch=False):
+    tokens, co, cl, off, lens = case
+    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
+        base, served = run(dm, *case, batch)
+        assert served == 1
+        for order in (np.arange(len(off))[::-1], np.random.default_rng(5).permutation(len(off))):
+            got, served = run(dm, tokens, co[order], cl[order], off[order], lens[order], batch)
+            assert served == 1 and np.array_equal(got, base), f"order {order.tolist()} changed the results"
+
+
+# ---- history independence, from each call's module-scoped fixture
+def fresh_results(tensor_seed, make_case, batch=False):
+    """A pf-tiny model, a case and the call's results on a fresh engine at seq_len 512."""
+    spec = mg.SPECS["pf-tiny"]
+    tensors = mg.generate(spec, tensor_seed)
+    case = make_case(spec.vocab_size)
+    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
+        fresh, served = run(dm, *case, batch)
+    assert served == 1
+    return spec, tensors, case, fresh
+
+
+def assert_independent_of_history(hist, before, batch=False):
+    spec, tensors, case, fresh = hist
+    long = np.asarray(mg.teacher_tokens(spec.vocab_size, 500, start=3), np.int32)
+    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
+        if "score" in before:
+            dm.score(long, 0)
+        if before == "prefill":
+            dm.prefill(long, 0)
+        if "poison" in before:
+            dm.poison(0)
+        got, served = run(dm, *case, batch)
+    assert served == 1
+    assert np.isfinite(got[got != SENTINEL]).all() and np.array_equal(got, fresh), f"after {before}: the results changed"
+
+
+def assert_nothing_after_depends_on_it(hist, batch=False):
+    """forward_prefill_cuda and forward_cuda from position 0 after a call equal the fresh engine's, bit for bit."""
+    spec, tensors, case, _ = hist
+    prompt = np.asarray(mg.teacher_tokens(spec.vocab_size, 200, start=9), np.int32)
+    runs = []
+    for dirty in (False, True):
+        with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
+            if dirty:
+                run(dm, *case, batch)
+            assert dm.prefill(prompt[:150], 0) == 1
+            after_pf = [dm.forward(int(prompt[p]), p) for p in range(150, 160)]
+            if dirty:
+                run(dm, *case, batch)
+            dm.forward(int(prompt[0]), 0, FF_UPDATE_KV_ONLY)
+            serial = [dm.forward(int(prompt[p]), p) for p in range(1, 12)]
+            runs.append(after_pf + serial)
+    for i, (a, b) in enumerate(zip(*runs)):
+        assert np.isfinite(a).all() and np.array_equal(a, b), f"logits {i} after a call differ from the fresh engine's"
 
 
 # Boundaries inside a 32-key tile (1, 7, 8, 9, 31, 33, 100, 300), on a tile edge (32) and none (0); each context with every
@@ -151,8 +213,8 @@ def test_a_shared_context_is_computed_once_per_block():
 
 
 def test_all_contexts_empty_equals_score_batch():
-    """ctx_len 0 everywhere: the packing and the kernels of calm_b200_score_batch, on its LENS layout and on study()
-    chunks of a 3000-token text."""
+    """ctx_len 0 everywhere: calm_b200_score_batch's values and launches, on its LENS layout and on study() chunks of a
+    3000-token text."""
     spec = mg.SPECS["pf-tiny"]
     tensors = mg.generate(spec, 24)
     lens = np.asarray([2, 3, 9, 40, 129, 257, 513, 1, 257, 129, 40, 0], np.int32)
@@ -163,27 +225,27 @@ def test_all_contexts_empty_equals_score_batch():
     text = np.asarray(mg.teacher_tokens(spec.vocab_size, n), np.int32)
     study_off = np.arange(0, n - 1, 256, dtype=np.int32)
     study_len = np.minimum(257, n - study_off).astype(np.int32)
+    L = lib.load()
     for label, (tokens, off, ln), seq_len in (("LENS", (lens_tokens, lens_off, lens), 512), ("study", (text, study_off, study_len), 4096)):
         zero = np.zeros(len(off), np.int32)
         with lib.DeviceModel(spec, tensors, seq_len=seq_len) as dm:
             want = np.full(len(tokens), SENTINEL, np.float32)
+            n0 = L.calm_b200_launch_count()
             s_batch = dm.score_batch(tokens, off, ln, want)[1]
+            n_batch = L.calm_b200_launch_count() - n0
         with lib.DeviceModel(spec, tensors, seq_len=seq_len) as dm:
+            n0 = L.calm_b200_launch_count()
             got, s_ctx = run(dm, tokens, zero, zero, off, ln)
+            n_ctx = L.calm_b200_launch_count() - n0
         assert s_ctx == s_batch, f"{label}: served {s_ctx}, score_batch {s_batch}"
         assert np.isfinite(got[got != SENTINEL]).all() and np.array_equal(got, want), f"{label}: differs from calm_b200_score_batch"
+        assert n_ctx == n_batch, f"{label}: {n_ctx} launches, score_batch {n_batch}"
 
 
 def test_order_does_not_matter():
     spec = mg.SPECS["pf-tiny"]
     tensors = mg.generate(spec, 25)
-    tokens, co, cl, off, lens = layout(spec.vocab_size, [(100, [7, 40]), (0, [65]), (33, [2, 129, 17]), (300, [21, 21]), (9, [90])], 5)
-    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-        base, served = run(dm, tokens, co, cl, off, lens)
-        assert served == 1
-        for order in (np.arange(len(off))[::-1], np.random.default_rng(5).permutation(len(off))):
-            got, served = run(dm, tokens, co[order], cl[order], off[order], lens[order])
-            assert served == 1 and np.array_equal(got, base), f"order {order.tolist()} changed the results"
+    assert_order_does_not_matter(spec, tensors, layout(spec.vocab_size, [(100, [7, 40]), (0, [65]), (33, [2, 129, 17]), (300, [21, 21]), (9, [90])], 5))
 
 
 @pytest.mark.parametrize("seq_len,items,served", [
@@ -219,46 +281,13 @@ HIST_ITEMS = [(100, [40, 9]), (0, [129]), (33, [2, 65]), (7, [20])]
 
 @pytest.fixture(scope="module")
 def hist():
-    spec = mg.SPECS["pf-tiny"]
-    tensors = mg.generate(spec, 29)
-    case = layout(spec.vocab_size, HIST_ITEMS, 9)
-    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-        fresh, served = run(dm, *case)
-    assert served == 1
-    return spec, tensors, case, fresh
+    return fresh_results(29, lambda vocab: layout(vocab, HIST_ITEMS, 9))
 
 
 @pytest.mark.parametrize("before", ["poison", "score", "prefill", "score+poison"])
 def test_context_call_does_not_depend_on_history(hist, before):
-    spec, tensors, case, fresh = hist
-    long = np.asarray(mg.teacher_tokens(spec.vocab_size, 500, start=3), np.int32)
-    with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-        if "score" in before:
-            dm.score(long, 0)
-        if before == "prefill":
-            dm.prefill(long, 0)
-        if "poison" in before:
-            dm.poison(0)
-        got, served = run(dm, *case)
-    assert served == 1
-    assert np.isfinite(got[got != SENTINEL]).all() and np.array_equal(got, fresh), f"after {before}: the results changed"
+    assert_independent_of_history(hist, before)
 
 
 def test_nothing_after_a_context_call_depends_on_it(hist):
-    """forward_prefill_cuda and forward_cuda from position 0 after a call equal the fresh engine's, bit for bit."""
-    spec, tensors, case, _ = hist
-    prompt = np.asarray(mg.teacher_tokens(spec.vocab_size, 200, start=9), np.int32)
-    runs = []
-    for dirty in (False, True):
-        with lib.DeviceModel(spec, tensors, seq_len=512) as dm:
-            if dirty:
-                run(dm, *case)
-            assert dm.prefill(prompt[:150], 0) == 1
-            after_pf = [dm.forward(int(prompt[p]), p) for p in range(150, 160)]
-            if dirty:
-                run(dm, *case)
-            dm.forward(int(prompt[0]), 0, FF_UPDATE_KV_ONLY)
-            serial = [dm.forward(int(prompt[p]), p) for p in range(1, 12)]
-            runs.append(after_pf + serial)
-    for i, (a, b) in enumerate(zip(*runs)):
-        assert np.isfinite(a).all() and np.array_equal(a, b), f"logits {i} after a context call differ from the fresh engine's"
+    assert_nothing_after_depends_on_it(hist)

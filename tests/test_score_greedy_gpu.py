@@ -26,6 +26,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import stage_ref as sr  # noqa: E402
 from conftest import TOL_SIGMA  # noqa: E402
+from test_score_context_gpu import layout  # noqa: E402
 from test_score_gpu import STAGE, log_softmax_at  # noqa: E402
 from test_stages_gpu import make_model, pf_tol  # noqa: E402
 
@@ -156,21 +157,6 @@ def test_exact_ties_on_the_decode_path():
 
 
 # ---- 3. the packed calls equal the lone call
-def layout(vocab, items, seed):
-    """items: [(ctx_len, [sequence lengths])] -> (tokens, ctx_off, ctx_len, off, len), each context stored once."""
-    rng = np.random.default_rng(seed)
-    parts, co, cl, off, ln, at = [], [], [], [], [], 0
-    for c, lens in items:
-        parts.append(rng.integers(0, vocab, c))
-        c0, at = at, at + c
-        for n in lens:
-            parts.append(rng.integers(0, vocab, n))
-            co.append(c0), cl.append(c), off.append(at), ln.append(n)
-            at += n
-    i32 = lambda x: np.asarray(x, np.int32)  # noqa: E731
-    return i32(np.concatenate(parts)), i32(co), i32(cl), i32(off), i32(ln)
-
-
 def outputs(n):
     return np.full(n, SENTINEL_LP, np.float32), np.full(n, SENTINEL_G, np.int32)
 
