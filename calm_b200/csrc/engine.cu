@@ -128,6 +128,8 @@ struct Engine {
 
 Engine g;
 
+static_assert(PF_TOPK_MAX == CALM_B200_TOPK_MAX, "the tile lists hold the largest k a call accepts");
+
 // batched prompt pass (prefill.cuh): buffers for up to `cap` tokens, allocated on first use
 struct Prefill {
 	int cap = 0;
@@ -148,6 +150,12 @@ struct Prefill {
 	// argmax and the merged argmax of each row
 	int* gidx = nullptr; // [cap][cdiv(vocab, PF_BM)]
 	int* greedy = nullptr;
+	// top-k scoring (calm_b200_score_topk and its siblings), allocated on its first call for `cap` rows and the largest k:
+	// each tile's sorted top-k list, and each row's merged top-k ids and log-probabilities
+	float* topv = nullptr; // [cap][cdiv(vocab, PF_BM)][PF_TOPK_MAX]
+	int* topi = nullptr;
+	int* top_ids = nullptr; // [cap][PF_TOPK_MAX]
+	float* top_lp = nullptr;
 };
 Prefill pf;
 
@@ -156,6 +164,7 @@ void pf_free() {
 	cudaFree(pf.rowpos), cudaFree(pf.seg), cudaFree(pf.ctx);
 	cudaFree(pf.part), cudaFree(pf.tgt), cudaFree(pf.logprob), cudaFree(pf.targets);
 	cudaFree(pf.gidx), cudaFree(pf.greedy);
+	cudaFree(pf.topv), cudaFree(pf.topi), cudaFree(pf.top_ids), cudaFree(pf.top_lp);
 	pf = Prefill();
 }
 
@@ -1234,9 +1243,26 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout = PF_ONE)
 	}
 }
 
-// The scoring buffers for pf.cap rows, and with `greedy` the argmax buffers, which the plain scoring calls never allocate
-// (freed and re-made with the pass's own buffers when a longer block needs more rows)
-static void pf_score_reserve(bool greedy) {
+// What a scoring call returns besides the log-probabilities: with `greedy` the argmax of every scored position, with
+// k > 0 its k largest logits' indices and log-probabilities (top_ids / top_logprobs[i * k + r]).  Pointers are the
+// caller's, at the slot of logprobs[0].
+struct PfExtra {
+	int* greedy = nullptr;
+	int k = 0;
+	int* top_ids = nullptr;
+	float* top_logprobs = nullptr;
+	// the same outputs from slot `i` on
+	PfExtra at(size_t i) const {
+		PfExtra o = *this;
+		if (greedy) o.greedy += i;
+		if (k) o.top_ids += i * k, o.top_logprobs += i * k;
+		return o;
+	}
+};
+
+// The scoring buffers for pf.cap rows, with `greedy` the argmax buffers and with `topk` the top-k buffers, which the
+// plain scoring calls never allocate (freed and re-made with the pass's own buffers when a longer block needs more rows)
+static void pf_score_reserve(bool greedy, bool topk) {
 	const int nvt = cdiv(g.cfg.vocab_size, PF_BM);
 	if (!pf.scoring) {
 		pf.part = (float2*)dev_alloc((size_t)pf.cap * nvt * sizeof(float2));
@@ -1249,12 +1275,19 @@ static void pf_score_reserve(bool greedy) {
 		pf.gidx = (int*)dev_alloc((size_t)pf.cap * nvt * sizeof(int));
 		pf.greedy = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
 	}
+	if (topk && !pf.topv) { // sized for the largest k: at Llama-3-8B's vocabulary, 2048 rows take 328 MB of tile lists
+		pf.topv = (float*)dev_alloc((size_t)pf.cap * nvt * PF_TOPK_MAX * sizeof(float));
+		pf.topi = (int*)dev_alloc((size_t)pf.cap * nvt * PF_TOPK_MAX * sizeof(int));
+		pf.top_ids = (int*)dev_alloc((size_t)pf.cap * PF_TOPK_MAX * sizeof(int));
+		pf.top_lp = (float*)dev_alloc((size_t)pf.cap * PF_TOPK_MAX * sizeof(float));
+	}
 }
 
 // After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records;
-// with `greedy` the classifier and the merge also give each row's argmax in pf.greedy
+// with `greedy` the classifier and the merge also give each row's argmax in pf.greedy, with k > 0 its k largest logits'
+// indices and log-probabilities in pf.top_ids / pf.top_lp [n][k]
 template <int DBITS, typename KVT>
-static void pf_score(Formats<DBITS, KVT>, int n, bool greedy) {
+static void pf_score(Formats<DBITS, KVT>, int n, bool greedy, int k) {
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const int nvt = cdiv(c.vocab_size, PF_BM);
@@ -1262,28 +1295,41 @@ static void pf_score(Formats<DBITS, KVT>, int n, bool greedy) {
 	PfGemmArgs a = {};
 	a.n_tokens = n, a.w[0] = w.wcls, a.K = c.dim;
 	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
-	if (greedy) {
+	const float* nf = nullptr;
+	const int* ni = nullptr;
+	if (k) {
+		a.topv = pf.topv, a.topi = pf.topi, a.topk = k;
+		pf_gemm<PF_CLS_TOPK, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
+		launch_pdl(k_pf_logprob<false, true>, cdiv(n, 8), 256, (size_t)8 * nvt, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, ni,
+		           (int*)nullptr, (const float*)pf.topv, (const int*)pf.topi, k, pf.top_ids, pf.top_lp);
+	} else if (greedy) {
 		pf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-		launch_pdl(k_pf_logprob<true>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx, pf.greedy);
+		launch_pdl(k_pf_logprob<true>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx, pf.greedy,
+		           nf, ni, 0, (int*)nullptr, (float*)nullptr);
 	} else {
 		pf_gemm<PF_CLS, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-		launch_pdl(k_pf_logprob<false>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)nullptr, (int*)nullptr);
+		launch_pdl(k_pf_logprob<false>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, ni, (int*)nullptr, nf, ni, 0,
+		           (int*)nullptr, (float*)nullptr);
 	}
 }
 
 // One block of the pass: the n rows the caller reserved (pf_reserve) and uploaded to pf.tokens (and, packed, to pf.rowpos,
 // pf.seg and pf.ctx) at cache slots pos0 + t, laid out as `layout` says.  With `logprobs`, the rows are scored against
-// targets[0 .. n) as well: logprobs[t] is row t's log-probability and, with `greedy`, greedy[t] its argmax.
-static void pf_block(int n, int pos0, PfRows layout, const int* targets, float* logprobs, int* greedy) {
+// targets[0 .. n) as well: logprobs[t] is row t's log-probability, and `x` gets the extra outputs of row t at slot t.
+static void pf_block(int n, int pos0, PfRows layout, const int* targets, float* logprobs, const PfExtra& x) {
 	if (logprobs) {
-		pf_score_reserve(greedy);
+		pf_score_reserve(x.greedy, x.k > 0);
 		CUDA_CHECK(cudaMemcpyAsync(pf.targets, targets, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	}
 	with_formats([&](auto f) { pf_run(f, n, pos0, layout); });
 	if (logprobs) {
-		with_formats([&](auto f) { pf_score(f, n, greedy); });
+		with_formats([&](auto f) { pf_score(f, n, x.greedy, x.k); });
 		CUDA_CHECK(cudaMemcpyAsync(logprobs, pf.logprob, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
-		if (greedy) CUDA_CHECK(cudaMemcpyAsync(greedy, pf.greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+		if (x.greedy) CUDA_CHECK(cudaMemcpyAsync(x.greedy, pf.greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+		if (x.k) {
+			CUDA_CHECK(cudaMemcpyAsync(x.top_ids, pf.top_ids, (size_t)n * x.k * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+			CUDA_CHECK(cudaMemcpyAsync(x.top_logprobs, pf.top_lp, (size_t)n * x.k * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+		}
 	}
 	CUDA_CHECK(cudaStreamSynchronize(g.stream)); // the uploads read the caller's memory (pageable): they must have left it
 	CUDA_CHECK(cudaGetLastError());
@@ -1291,14 +1337,14 @@ static void pf_block(int n, int pos0, PfRows layout, const int* targets, float* 
 
 // The batched pass over tokens[0 .. n) at positions pos0 .., in blocks of at most 2048 rows.  With `logprobs`, every block
 // is scored as well: logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]], so tokens[n] must exist; with
-// `greedy` too, greedy[i] = the argmax of those logits.
-static void pf_pass(const int* tokens, int n, int pos0, float* logprobs, int* greedy = nullptr) {
+// `x`, the extra outputs of position i at its slot i.
+static void pf_pass(const int* tokens, int n, int pos0, float* logprobs, const PfExtra& x = PfExtra()) {
 	const int chunk_cap = 2048;
 	for (int o = 0; o < n; o += chunk_cap) {
 		const int m = n - o < chunk_cap ? n - o : chunk_cap;
 		pf_reserve(m);
 		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		pf_block(m, pos0 + o, PF_ONE, tokens + o + 1, logprobs ? logprobs + o : nullptr, greedy ? greedy + o : nullptr);
+		pf_block(m, pos0 + o, PF_ONE, tokens + o + 1, logprobs ? logprobs + o : nullptr, x.at(o));
 	}
 }
 
@@ -1330,8 +1376,8 @@ extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* 
 // the prompt pass and logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]].  The cache is left as
 // forward_prefill_cuda(tokens, n - 1, pos0) leaves it.  Shapes the pass does not serve go one position at a time through
 // the decode path with a log-softmax in double on the host (returns 0).
-// calm_b200_score, and with `greedy` calm_b200_score_greedy
-static int pf_score_one(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, int* greedy) {
+// calm_b200_score, and with the extra outputs `x` its greedy and top-k siblings
+static int pf_score_one(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, const PfExtra& x) {
 	if (n < 2) return 1;
 	check_call(transformer, tokens[0], pos0);
 	check_tokens(tokens, n);
@@ -1346,27 +1392,58 @@ static int pf_score_one(struct Transformer* transformer, const int* tokens, int 
 			for (int v = 1; v < vocab; ++v) mx = l[v] > mx ? l[v] : mx;
 			for (int v = 0; v < vocab; ++v) s += exp((double)l[v] - mx);
 			logprobs[i] = (float)((double)l[tokens[i + 1]] - mx - log(s));
-			if (greedy) { // first maximum (sampler.c:34-42), as calm_b200_forward_argmax
+			if (x.greedy) { // first maximum (sampler.c:34-42), as calm_b200_forward_argmax
 				int best = 0;
 				for (int v = 1; v < vocab; ++v)
 					if (l[v] > l[best]) best = v;
-				greedy[i] = best;
+				x.greedy[i] = best;
+			}
+			if (x.k) { // the k largest logits, equal logits by index ascending: the same order as the tensor-core pass
+				std::vector<int> idx(vocab);
+				for (int v = 0; v < vocab; ++v) idx[v] = v;
+				std::partial_sort(idx.begin(), idx.begin() + x.k, idx.end(), [l](int a, int b) { return l[a] > l[b] || (l[a] == l[b] && a < b); });
+				for (int r = 0; r < x.k; ++r) {
+					x.top_ids[(size_t)i * x.k + r] = idx[r];
+					x.top_logprobs[(size_t)i * x.k + r] = (float)((double)l[idx[r]] - mx - log(s));
+				}
 			}
 		}
 		CUDA_CHECK(cudaGetLastError());
 		return 0;
 	}
-	pf_pass(tokens, rows, pos0, logprobs, greedy);
+	pf_pass(tokens, rows, pos0, logprobs, x);
 	return 1;
 }
 
+static PfExtra greedy_out(int* greedy) {
+	PfExtra x;
+	x.greedy = greedy;
+	return x;
+}
+
+// The top-k outputs of `who`, checked before any device work
+static PfExtra topk_out(const char* who, int k, int* top_ids, float* top_logprobs) {
+	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
+	const int kmax = imin(CALM_B200_TOPK_MAX, g.cfg.vocab_size);
+	if (k < 1 || k > kmax) CALM_FATAL("%s: k %d outside [1, %d]", who, k, kmax);
+	if (!top_ids || !top_logprobs) CALM_FATAL("%s: top_ids or top_logprobs is NULL", who);
+	PfExtra x;
+	x.k = k, x.top_ids = top_ids, x.top_logprobs = top_logprobs;
+	return x;
+}
+
 extern "C" int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs) {
-	return pf_score_one(transformer, tokens, n, pos0, logprobs, nullptr);
+	return pf_score_one(transformer, tokens, n, pos0, logprobs, PfExtra());
 }
 
 extern "C" int calm_b200_score_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, int* greedy) {
 	if (!greedy) CALM_FATAL("score_greedy: greedy is NULL");
-	return pf_score_one(transformer, tokens, n, pos0, logprobs, greedy);
+	return pf_score_one(transformer, tokens, n, pos0, logprobs, greedy_out(greedy));
+}
+
+extern "C" int calm_b200_score_topk(struct Transformer* transformer, const int* tokens, int n, int pos0, int k, float* logprobs, int* top_ids,
+                                    float* top_logprobs) {
+	return pf_score_one(transformer, tokens, n, pos0, logprobs, topk_out("score_topk", k, top_ids, top_logprobs));
 }
 
 // A packed block being filled: per-row inputs, the sequences it scores with their first rows, and the contexts it holds
@@ -1391,20 +1468,26 @@ struct PfPackedBlock {
 // Run a block and write its sequences' log-probabilities; the results of context and filler rows are dropped.  A block that
 // holds no context runs the packed attention (k_pf_attn<.., SEG>); only one with a context uploads pf.ctx and runs the
 // context walk (k_pf_attn<.., SEG, CTX>).
-static void pf_score_packed_block(PfPackedBlock& b, const int* off, const int* len, float* logprobs, int* greedy) {
+static void pf_score_packed_block(PfPackedBlock& b, const int* off, const int* len, float* logprobs, const PfExtra& x) {
 	const int rows = b.rows();
 	const bool contexts = !b.placed.empty();
-	std::vector<float> lp(rows);
-	std::vector<int> gr(greedy ? rows : 0);
+	std::vector<float> lp(rows), tl((size_t)rows * x.k);
+	std::vector<int> gr(x.greedy ? rows : 0), ti((size_t)rows * x.k);
+	PfExtra bx = x; // the block's rows
+	bx.greedy = x.greedy ? gr.data() : nullptr, bx.top_ids = ti.data(), bx.top_logprobs = tl.data();
 	pf_reserve(rows);
 	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, b.tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, b.pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(pf.seg, b.seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	if (contexts) CUDA_CHECK(cudaMemcpyAsync(pf.ctx, b.ctx.data(), (size_t)rows * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
-	pf_block(rows, 0, contexts ? PF_CONTEXTS : PF_PACKED, b.tgt.data(), lp.data(), greedy ? gr.data() : nullptr);
+	pf_block(rows, 0, contexts ? PF_CONTEXTS : PF_PACKED, b.tgt.data(), lp.data(), bx);
 	for (const auto& [i, s] : b.seqs) {
 		memcpy(logprobs + off[i], lp.data() + s, (size_t)(len[i] - 1) * sizeof(float));
-		if (greedy) memcpy(greedy + off[i], gr.data() + s, (size_t)(len[i] - 1) * sizeof(int));
+		if (x.greedy) memcpy(x.greedy + off[i], gr.data() + s, (size_t)(len[i] - 1) * sizeof(int));
+		if (x.k) {
+			memcpy(x.top_ids + (size_t)off[i] * x.k, ti.data() + (size_t)s * x.k, (size_t)(len[i] - 1) * x.k * sizeof(int));
+			memcpy(x.top_logprobs + (size_t)off[i] * x.k, tl.data() + (size_t)s * x.k, (size_t)(len[i] - 1) * x.k * sizeof(float));
+		}
 	}
 	b = PfPackedBlock();
 }
@@ -1415,9 +1498,9 @@ static void pf_score_packed_block(PfPackedBlock& b, const int* off, const int* l
 // context's rows in the same block.  Sequences with the same (ctx_off, ctx_len) share one placement of the context per
 // block; a sequence whose context is not yet in the block brings it along.  A context and sequence too long for any block,
 // together, are scored alone by calm_b200_score.  With every ctx_len 0 no block holds a context: calm_b200_score_batch.
-// With `greedy`, the greedy calls.
+// With the extra outputs `x`, the greedy and top-k calls.
 static int pf_score_packed(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
-                           const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
+                           const int* off, const int* len, int nseq, float* logprobs, const PfExtra& x) {
 	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
 	if (n < 0 || nseq < 0) CALM_FATAL("%s: negative count (n %d, nseq %d)", who, n, nseq);
 	if (nseq == 0) return 1;
@@ -1436,11 +1519,18 @@ static int pf_score_packed(const char* who, struct Transformer* transformer, con
 	auto alone = [&](int i) {
 		std::vector<int> cat(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
 		cat.insert(cat.end(), tokens + off[i], tokens + off[i] + len[i]);
-		std::vector<float> lp(cat.size() - 1);
-		std::vector<int> gr(greedy ? cat.size() - 1 : 0);
-		const int served = pf_score_one(transformer, cat.data(), (int)cat.size(), 0, lp.data(), greedy ? gr.data() : nullptr);
+		const size_t m = cat.size() - 1;
+		std::vector<float> lp(m), tl(m * x.k);
+		std::vector<int> gr(x.greedy ? m : 0), ti(m * x.k);
+		PfExtra cx = x; // the rows of ctx ++ sequence
+		cx.greedy = x.greedy ? gr.data() : nullptr, cx.top_ids = ti.data(), cx.top_logprobs = tl.data();
+		const int served = pf_score_one(transformer, cat.data(), (int)cat.size(), 0, lp.data(), cx);
 		memcpy(logprobs + off[i], lp.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(float));
-		if (greedy) memcpy(greedy + off[i], gr.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(int));
+		if (x.greedy) memcpy(x.greedy + off[i], gr.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(int));
+		if (x.k) { // tmp[ctx_len + j] -> slot off[i] + j
+			memcpy(x.top_ids + (size_t)off[i] * x.k, ti.data() + (size_t)ctx_len[i] * x.k, (size_t)(len[i] - 1) * x.k * sizeof(int));
+			memcpy(x.top_logprobs + (size_t)off[i] * x.k, tl.data() + (size_t)ctx_len[i] * x.k, (size_t)(len[i] - 1) * x.k * sizeof(float));
+		}
 		return served;
 	};
 	if (!pf_supported()) {
@@ -1459,7 +1549,7 @@ static int pf_score_packed(const char* who, struct Transformer* transformer, con
 			continue;
 		}
 		const std::pair<int, int> key(ctx_off[i], ctx_len[i]);
-		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_packed_block(b, off, len, logprobs, greedy);
+		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_packed_block(b, off, len, logprobs, x);
 		int c0 = 0;
 		if (ctx_len[i]) {
 			const auto it = b.placed.find(key);
@@ -1467,7 +1557,7 @@ static int pf_score_packed(const char* who, struct Transformer* transformer, con
 		}
 		b.seqs.push_back({i, b.add(tokens + off[i], len[i] - 1, len[i] - 1, ctx_len[i], make_int2(c0, ctx_len[i]))});
 	}
-	if (b.rows()) pf_score_packed_block(b, off, len, logprobs, greedy);
+	if (b.rows()) pf_score_packed_block(b, off, len, logprobs, x);
 	int served = 1;
 	for (int i : big) served &= alone(i);
 	return served;
@@ -1475,25 +1565,38 @@ static int pf_score_packed(const char* who, struct Transformer* transformer, con
 
 extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
 	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
-	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, nullptr);
+	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, PfExtra());
 }
 
 extern "C" int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
                                             float* logprobs, int* greedy) {
 	if (!greedy) CALM_FATAL("score_batch_greedy: greedy is NULL");
 	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
-	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, greedy);
+	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, greedy_out(greedy));
+}
+
+extern "C" int calm_b200_score_batch_topk(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, int k,
+                                          float* logprobs, int* top_ids, float* top_logprobs) {
+	const PfExtra x = topk_out("score_batch_topk", k, top_ids, top_logprobs);
+	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
+	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, x);
 }
 
 extern "C" int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
                                        const int* off, const int* len, int nseq, float* logprobs) {
-	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, nullptr);
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, PfExtra());
 }
 
 extern "C" int calm_b200_score_context_greedy(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
                                               const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
 	if (!greedy) CALM_FATAL("score_context_greedy: greedy is NULL");
-	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, greedy);
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, greedy_out(greedy));
+}
+
+extern "C" int calm_b200_score_context_topk(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                            const int* off, const int* len, int nseq, int k, float* logprobs, int* top_ids, float* top_logprobs) {
+	const PfExtra x = topk_out("score_context_topk", k, top_ids, top_logprobs);
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, x);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -1643,6 +1746,9 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		if (pf.scoring) nan(pf.part, cap * cdiv(c.vocab_size, PF_BM) * sizeof(float2)), nan(pf.tgt, cap * sizeof(float)), nan(pf.logprob, cap * sizeof(float));
 		// the argmax records are vocabulary indices, but only ever compared and copied out, never used as an address
 		nan(pf.gidx, cap * cdiv(c.vocab_size, PF_BM) * sizeof(int)), nan(pf.greedy, cap * sizeof(int));
+		// so are the top-k records: ids only compared and copied out, values NaN like every other float
+		nan(pf.topv, cap * cdiv(c.vocab_size, PF_BM) * PF_TOPK_MAX * sizeof(float)), nan(pf.topi, cap * cdiv(c.vocab_size, PF_BM) * PF_TOPK_MAX * sizeof(int));
+		nan(pf.top_ids, cap * PF_TOPK_MAX * sizeof(int)), nan(pf.top_lp, cap * PF_TOPK_MAX * sizeof(float));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

@@ -25,7 +25,8 @@
 // each sequence's key tiles at its own first row (k_pf_attn<.., SEG>); everything else works per row.  A packed block
 // may also hold contexts, once each, and sequences that continue them: a sequence's rows attend
 // to its context's rows and then its own as one key sequence (k_pf_attn<.., SEG, CTX>).  The greedy scoring calls run
-// PF_CLS_GREEDY and k_pf_logprob<true>, which also give each row's argmax, with the same log-probability bits.
+// PF_CLS_GREEDY and k_pf_logprob<true>, which also give each row's argmax, with the same log-probability bits.  The top-k
+// scoring calls run PF_CLS_TOPK and k_pf_logprob<false, true>: each tile's k largest logits, merged into each row's k largest.
 //
 // Parity contract (tests/test_prefill_gpu.py): after forward_prefill_cuda(tokens, n, pos0) the KV cache and the logits of
 // the following token equal those of n serial forward(FF_UPDATE_KV_ONLY) calls within the stated tolerances.
@@ -39,7 +40,8 @@
 #define PF_BN 128 // tokens per tile       (two consumer warpgroups of 64: the M of the MMA)
 #define PF_BK 64  // k per stage: 64 f16 = 128 bytes = one swizzle atom
 #define PF_THREADS 384 // warpgroup 0: dequantising producers (thread 0 also issues the TMA); warpgroups 1, 2: MMA + epilogue
-enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3, PF_CLS = 4, PF_CLS_GREEDY = 5 }; // PF_CLS_GREEDY: PF_CLS + each tile's argmax
+enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3, PF_CLS = 4, PF_CLS_GREEDY = 5, PF_CLS_TOPK = 6 }; // PF_CLS_GREEDY: PF_CLS + each tile's argmax
+#define PF_TOPK_MAX 20 // PF_CLS_TOPK: PF_CLS + each tile's k <= PF_TOPK_MAX largest logits (CALM_B200_TOPK_MAX)
 
 // ---------------------------------------------------------------- wgmma / TMA wrappers
 __device__ __forceinline__ void wgmma_fence() { // accumulator registers written by ordinary instructions -> visible to wgmma
@@ -194,6 +196,11 @@ struct PfGemmArgs {
 	float* tgt;         // [T] logit of the target
 	int vocab;
 	int* gidx; // (PF_CLS_GREEDY) [T][gridDim.x] the lowest vocabulary index of the token's maximum logit in each tile
+	// (PF_CLS_TOPK) [T][gridDim.x][topk] the token's topk largest logits in each tile and their vocabulary indices, by logit
+	// descending and, on equal logits, index ascending; a tile with fewer than topk rows pads with (-INFINITY, INT_MAX)
+	float* topv;
+	int* topi;
+	int topk;
 };
 
 // 64 weights of one row (one k-stage) -> 8 swizzled 16-byte chunks of f16 in the weight tile
@@ -285,7 +292,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 			} else if constexpr (MODE == PF_UP) {
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)gr * rowbytes;
 				rowp[1] = reinterpret_cast<const unsigned char*>(a.w[1]) + (size_t)gr * rowbytes;
-			} else if constexpr (MODE == PF_CLS || MODE == PF_CLS_GREEDY) { // the last vocabulary tile may be partial: its spare rows repeat the last row
+			} else if constexpr (MODE == PF_CLS || MODE == PF_CLS_GREEDY || MODE == PF_CLS_TOPK) { // the last vocabulary tile may be partial: its spare rows repeat the last row
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)min(gr, a.vocab - 1) * rowbytes;
 			} else {
 				rowp[0] = reinterpret_cast<const unsigned char*>(a.w[0]) + (size_t)gr * rowbytes;
@@ -347,12 +354,16 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 		// accumulator fragment of m64nN: register 4 j + 2 h + e holds token 16 w + lane / 4 + 8 h, weight row 8 j + 2 (lane % 4) + e
 		const int w4 = warp & 3;
 		const int tb = tok0 + c * 64 + w4 * 16 + (lane >> 2);
-		if constexpr (MODE == PF_CLS || MODE == PF_CLS_GREEDY) {
+		if constexpr (MODE == PF_CLS || MODE == PF_CLS_GREEDY || MODE == PF_CLS_TOPK) {
 			// the quad of lanes 4 (lane / 4) .. + 3 holds all 128 logits of tokens tb and tb + 8: 32 per lane, then two shuffles.
 			// Every lane runs the shuffles; only the stores are masked to the block's tokens.
 			// PF_CLS_GREEDY also tracks gi, the vocabulary index of the first maximum: a lane's indices ascend with (j, e), so a
 			// strict > keeps the lowest, and the shuffles give a tie to the lower index.  m and s take the same operations in
 			// the same order as in PF_CLS, so the records are the same bits.
+			// PF_CLS_TOPK computes m and s exactly as PF_CLS and then selects the tile's topk largest logits, one per round: each
+			// lane offers its largest logit not yet taken (a strict > over ascending indices keeps the lowest index of equal
+			// values), the quad's shuffles keep the larger value or, on equal values, the lower index, and the lane that owns
+			// the winner marks it taken.
 			const int q = lane & 3;
 #pragma unroll
 			for (int h = 0; h < 2; ++h) {
@@ -398,6 +409,30 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 					if (q == 0) a.part[(size_t)t * gridDim.x + blockIdx.x] = make_float2(m, s);
 					if constexpr (MODE == PF_CLS_GREEDY)
 						if (q == 0) a.gidx[(size_t)t * gridDim.x + blockIdx.x] = gi;
+				}
+				if constexpr (MODE == PF_CLS_TOPK) {
+					const size_t rec = ((size_t)t * gridDim.x + blockIdx.x) * a.topk;
+					uint32_t taken = 0; // bit 2 j + e: this lane's logit of row 8 j + 2 q + e
+					for (int r = 0; r < a.topk; ++r) {
+						float bv = -INFINITY;
+						int bi = INT_MAX, bp = 0;
+#pragma unroll
+						for (int j = 0; j < PF_BM / 8; ++j)
+#pragma unroll
+							for (int e = 0; e < 2; ++e) {
+								const float v = acc[0][4 * j + 2 * h + e];
+								if (row0 + 8 * j + 2 * q + e < a.vocab && !((taken >> (2 * j + e)) & 1u) && v > bv) bv = v, bi = row0 + 8 * j + 2 * q + e, bp = 2 * j + e;
+							}
+						const int mine = bi;
+#pragma unroll
+						for (int o = 1; o <= 2; o <<= 1) {
+							const float v2 = __shfl_xor_sync(0xffffffffu, bv, o);
+							const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
+							if (v2 > bv || (v2 == bv && i2 < bi)) bv = v2, bi = i2;
+						}
+						if (bi == mine) taken |= 1u << bp; // (a lane with nothing left re-marks a taken or invalid bit)
+						if (q == 0 && t < a.n_tokens) a.topv[rec + r] = bv, a.topi[rec + r] = bi;
+					}
 				}
 			}
 			return;
@@ -451,13 +486,19 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 // GREEDY (after PF_CLS_GREEDY) also merges the tiles' argmax records gidx into greedy[t], the lowest vocabulary index of
 // the maximum logit: lane-strided over ascending tiles a strict > keeps the first maximum, and in the butterfly an equal
 // value takes the lower index, so the result does not depend on the merge order.  The (M, S) merge is unchanged.
+// TOPK (after PF_CLS_TOPK) also merges the tiles' sorted top-k lists topv / topi [n][nvt][k] into the row's k largest
+// logits: lane l owns tiles l, l + 32, .., with a head per tile in shared memory (how many of its entries are taken) and
+// its best head in registers; each round a butterfly picks the largest value, the lower index on equal values, and the
+// winning lane advances that tile and looks over its tiles again.  Indices are distinct, so the order of the merge does not
+// matter.  top_ids[t][r] is the index and top_logprobs[t][r] = logit - M - ln S, the expression of logprob[t].
 __device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
 	const float mn = fmaxf(m, m2);
 	s = s * expf(m - mn) + s2 * expf(m2 - mn);
 	m = mn;
 }
-template <bool GREEDY>
-__global__ void __launch_bounds__(256) k_pf_logprob(const float2* part, const float* tgt, float* logprob, int n, int nvt, const int* gidx, int* greedy) {
+template <bool GREEDY, bool TOPK = false>
+__global__ void __launch_bounds__(256) k_pf_logprob(const float2* part, const float* tgt, float* logprob, int n, int nvt, const int* gidx, int* greedy,
+                                                    const float* topv, const int* topi, int k, int* top_ids, float* top_logprobs) {
 	pdl_enter();
 	const int t = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
 	if (t >= n) return;
@@ -482,6 +523,42 @@ __global__ void __launch_bounds__(256) k_pf_logprob(const float2* part, const fl
 	if (lane == 0) {
 		logprob[t] = tgt[t] - m - logf(s);
 		if constexpr (GREEDY) greedy[t] = gi;
+	}
+	if constexpr (TOPK) {
+		extern __shared__ unsigned char pf_heads[]; // [8 warps][nvt]
+		unsigned char* head = pf_heads + (threadIdx.x >> 5) * nvt;
+		const float* tv = topv + (size_t)t * nvt * k;
+		const int* ti = topi + (size_t)t * nvt * k;
+		for (int v = lane; v < nvt; v += 32) head[v] = 0;
+		float bv;
+		int bi, bt;
+		auto best_head = [&]() {
+			bv = -INFINITY, bi = INT_MAX, bt = -1;
+			for (int v = lane; v < nvt; v += 32) {
+				const int h = head[v];
+				if (h < k) {
+					const float x = tv[(size_t)v * k + h];
+					const int i = ti[(size_t)v * k + h];
+					if (x > bv || (x == bv && i < bi)) bv = x, bi = i, bt = v;
+				}
+			}
+		};
+		best_head();
+		for (int r = 0; r < k; ++r) {
+			float wv = bv;
+			int wi = bi;
+#pragma unroll
+			for (int o = 16; o > 0; o >>= 1) {
+				const float v2 = __shfl_xor_sync(0xffffffffu, wv, o);
+				const int i2 = __shfl_xor_sync(0xffffffffu, wi, o);
+				if (v2 > wv || (v2 == wv && i2 < wi)) wv = v2, wi = i2;
+			}
+			if (lane == 0) top_ids[(size_t)t * k + r] = wi, top_logprobs[(size_t)t * k + r] = wv - m - logf(s);
+			if (wi == bi && bt >= 0) {
+				++head[bt];
+				best_head();
+			}
+		}
 	}
 }
 

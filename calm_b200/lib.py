@@ -24,6 +24,7 @@ _fptr = C.POINTER(C.c_float)
 SYMBOLS = [
     "upload_cuda", "prepare_cuda", "forward_cuda", "perf_cuda", "forward_prefill_cuda", "calm_b200_score", "calm_b200_score_batch", "calm_b200_score_context",
     "calm_b200_score_greedy", "calm_b200_score_batch_greedy", "calm_b200_score_context_greedy",
+    "calm_b200_score_topk", "calm_b200_score_batch_topk", "calm_b200_score_context_topk",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
@@ -31,6 +32,9 @@ SYMBOLS = [
     "calm_b200_tp_unique_id", "calm_b200_tp_init", "calm_b200_tp_world", "calm_b200_tp_mode",
     "calm_b200_decode_sample", "calm_b200_forward_sample", "calm_b200_read_device_logits", "calm_b200_sample_logits",
 ]
+
+# the largest k calm_b200_score_topk and its siblings accept (CALM_B200_TOPK_MAX)
+TOPK_MAX = 20
 
 # calm_b200_read_state selectors (include/calm_b200.h)
 STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11}
@@ -64,6 +68,12 @@ def load() -> C.CDLL:
     L.calm_b200_score_batch_greedy.restype = C.c_int
     L.calm_b200_score_context_greedy.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, _iptr, _iptr, C.c_int, _fptr, _iptr]
     L.calm_b200_score_context_greedy.restype = C.c_int
+    L.calm_b200_score_topk.argtypes = [T, _iptr, C.c_int, C.c_int, C.c_int, _fptr, _iptr, _fptr]
+    L.calm_b200_score_topk.restype = C.c_int
+    L.calm_b200_score_batch_topk.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, C.c_int, C.c_int, _fptr, _iptr, _fptr]
+    L.calm_b200_score_batch_topk.restype = C.c_int
+    L.calm_b200_score_context_topk.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, _iptr, _iptr, C.c_int, C.c_int, _fptr, _iptr, _fptr]
+    L.calm_b200_score_context_topk.restype = C.c_int
     L.calm_b200_abi_version.argtypes, L.calm_b200_abi_version.restype = [], C.c_int
     L.calm_b200_set_device.argtypes, L.calm_b200_set_device.restype = [C.c_int], None
     L.calm_b200_free.argtypes, L.calm_b200_free.restype = [C.c_void_p], None
@@ -167,10 +177,19 @@ class DeviceModel:
         served = self.lib.calm_b200_score(C.byref(self.transformer), arr.ctypes.data_as(C.POINTER(C.c_int)), len(arr), pos0, out.ctypes.data_as(_fptr))
         return out, served
 
-    def _score_packed(self, fn, tokens, index, out, greedy=None, with_greedy=False):
+    def _check_k(self, k):
+        """The binding's copy of the library's check on k, raised before the library would abort the process."""
+        kmax = min(TOPK_MAX, self.vocab)
+        if not isinstance(k, (int, np.integer)) or not 1 <= k <= kmax:
+            raise ValueError(f"k must be an integer in [1, {kmax}], got {k!r}")
+        return int(k)
+
+    def _score_packed(self, fn, tokens, index, out, greedy=None, with_greedy=False, k=None, top=None):
         """Call the packed scoring symbol `fn` over `tokens`.  `index` holds its per-sequence arrays in the C argument order
         ((off, len) or (ctx_off, ctx_len, off, len)).  `out` defaults to NaN, and for a greedy symbol (`with_greedy`)
-        `greedy` to -1.  Returns (out, served), or (out, greedy, served) with `with_greedy`."""
+        `greedy` to -1.  Returns (out, served), or (out, greedy, served) with `with_greedy`.  With `k`, a top-k symbol:
+        `top` = (top_ids int32[n, k], top_logprobs float32[n, k]) defaults to -1 / NaN, and the result is
+        (out, top_ids, top_logprobs, served)."""
         ip = C.POINTER(C.c_int)
         arr = np.ascontiguousarray(tokens, np.int32)
         index = [np.ascontiguousarray(a, np.int32) for a in index]
@@ -185,6 +204,14 @@ class DeviceModel:
                 greedy = np.full(n, -1, np.int32)
             assert greedy.dtype == np.int32 and greedy.flags.c_contiguous and len(greedy) >= n
             outs.append(greedy.ctypes.data_as(ip))
+        if k is not None:
+            k = self._check_k(k)
+            ids, tlp = top if top is not None else (np.full((n, k), -1, np.int32), np.full((n, k), np.nan, np.float32))
+            assert ids.dtype == np.int32 and tlp.dtype == np.float32 and ids.flags.c_contiguous and tlp.flags.c_contiguous
+            assert ids.shape[1:] == (k,) == tlp.shape[1:] and len(ids) >= n and len(tlp) >= n
+            served = fn(C.byref(self.transformer), arr.ctypes.data_as(ip), n, *[a.ctypes.data_as(ip) for a in index], len(index[0]), k, *outs,
+                        ids.ctypes.data_as(ip), tlp.ctypes.data_as(_fptr))
+            return out, ids, tlp, served
         served = fn(C.byref(self.transformer), arr.ctypes.data_as(ip), n, *[a.ctypes.data_as(ip) for a in index], len(index[0]), *outs)
         return (out, greedy, served) if with_greedy else (out, served)
 
@@ -225,6 +252,32 @@ class DeviceModel:
         same slots.  Returns (float32[len(tokens)], int32[len(tokens)], served); unwritten slots keep what `out` / `greedy`
         held (NaN / -1 when not given)."""
         return self._score_packed(self.lib.calm_b200_score_context_greedy, tokens, (ctx_off, ctx_len, off, len_), out, greedy, with_greedy=True)
+
+    def score_topk(self, tokens, k: int, pos0: int = 0):
+        """calm_b200_score_topk: score()'s log-probabilities, bit for bit, and at each scored position the k most likely
+        tokens (logit descending, lowest index on ties) with their log-probabilities.  Returns (float32[n - 1],
+        int32[n - 1, k], float32[n - 1, k], served).  Raises ValueError unless 1 <= k <= min(TOPK_MAX, vocab)."""
+        k = self._check_k(k)
+        arr = np.ascontiguousarray(tokens, np.int32)
+        out = np.full(max(len(arr) - 1, 0), np.nan, np.float32)
+        ids = np.full((len(out), k), -1, np.int32)
+        tlp = np.full((len(out), k), np.nan, np.float32)
+        ip = C.POINTER(C.c_int)
+        served = self.lib.calm_b200_score_topk(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), pos0, k, out.ctypes.data_as(_fptr),
+                                               ids.ctypes.data_as(ip), tlp.ctypes.data_as(_fptr))
+        return out, ids, tlp, served
+
+    def score_batch_topk(self, tokens, off, len_, k: int, out=None, top=None):
+        """calm_b200_score_batch_topk: score_batch()'s log-probabilities, bit for bit, and the top-k ids and
+        log-probabilities at the same slots.  Returns (float32[len(tokens)], int32[len(tokens), k], float32[len(tokens), k],
+        served); unwritten slots keep what `out` / `top` = (ids, logprobs) held (NaN / -1 / NaN when not given)."""
+        return self._score_packed(self.lib.calm_b200_score_batch_topk, tokens, (off, len_), out, k=k, top=top)
+
+    def score_context_topk(self, tokens, ctx_off, ctx_len, off, len_, k: int, out=None, top=None):
+        """calm_b200_score_context_topk: score_context()'s log-probabilities, bit for bit, and the top-k ids and
+        log-probabilities at the same slots.  Returns (float32[len(tokens)], int32[len(tokens), k], float32[len(tokens), k],
+        served); unwritten slots keep what `out` / `top` = (ids, logprobs) held (NaN / -1 / NaN when not given)."""
+        return self._score_packed(self.lib.calm_b200_score_context_topk, tokens, (ctx_off, ctx_len, off, len_), out, k=k, top=top)
 
     def forward_raw(self, token: int, pos: int, flags: int = 0):
         return self.lib.forward_cuda(C.byref(self.transformer), token, pos, flags)

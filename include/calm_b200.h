@@ -164,6 +164,26 @@ int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tok
 int calm_b200_score_context_greedy(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
                                    const int* off, const int* len, int nseq, float* logprobs, int* greedy);
 
+/* The three scoring calls above, each also returning the k most likely tokens at every scored position with their
+ * log-probabilities (an OpenAI-style completion's logprobs=k; INTEGRATION.md).  Each takes its sibling's arguments plus
+ * k, top_ids and top_logprobs, returns what the sibling returns and writes `logprobs` bit for bit as the sibling does.
+ * For every slot i where logprobs[i] is written it writes top_ids[i*k + r] and top_logprobs[i*k + r], r in [0, k); other
+ * slots are left untouched.  top_ids[i*k ..] are the k vocabulary indices with the largest logits at that position, by
+ * logit descending, equal logits lowest index first (the reference's sample_argmax rule, sampler.c:34-42), so
+ * top_ids[i*k] is what the _greedy sibling writes to greedy[i].  top_logprobs[i*k + r] = logit - M - ln S with the
+ * maximum M and sum S that give logprobs[i], evaluated the same way: where top_ids[i*k + r] is the target,
+ * top_logprobs[i*k + r] == logprobs[i] bit for bit, on the tensor-core pass and on the decode path alike.  The logits
+ * are those the greedy siblings describe.  1 <= k <= min(CALM_B200_TOPK_MAX, vocab_size) and both arrays not NULL, or
+ * the call aborts before any device work.  The first top-k call allocates the tile lists the merge reads:
+ * 2048 x ceil(vocab_size / 128) x CALM_B200_TOPK_MAX x 8 bytes (328 MB at a 128256-token vocabulary; DESIGN.md s.6). */
+#define CALM_B200_TOPK_MAX 20 /* the largest k a call accepts (the OpenAI API's top_logprobs limit) */
+int calm_b200_score_topk(struct Transformer* transformer, const int* tokens, int n, int pos0, int k, float* logprobs, int* top_ids,
+                         float* top_logprobs);
+int calm_b200_score_batch_topk(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, int k,
+                               float* logprobs, int* top_ids, float* top_logprobs);
+int calm_b200_score_context_topk(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                 const int* off, const int* len, int nseq, int k, float* logprobs, int* top_ids, float* top_logprobs);
+
 /* forward + device-side greedy sample.  Returns argmax(logits) with the
  * reference's tie rule (lowest index, sampler.c:34-42).  The logits are still
  * written to state.logits. */
