@@ -20,6 +20,7 @@
 #include "attn.cuh"
 #include "ring.cuh"
 #include "prefill.cuh"
+#include "verify.cuh"
 
 namespace {
 
@@ -156,6 +157,11 @@ struct Prefill {
 	int* topi = nullptr;
 	int* top_ids = nullptr; // [cap][PF_TOPK_MAX]
 	float* top_lp = nullptr;
+	// short blocks (calm_b200_verify_greedy), allocated on its first call: k_vf_gemm's partial sums, sized for the largest
+	// GEMM of the model, and its arrival counters, which are zero between launches
+	float* vacc = nullptr;
+	size_t vacc_floats = 0;
+	unsigned* vcnt = nullptr;
 };
 Prefill pf;
 
@@ -165,6 +171,7 @@ void pf_free() {
 	cudaFree(pf.part), cudaFree(pf.tgt), cudaFree(pf.logprob), cudaFree(pf.targets);
 	cudaFree(pf.gidx), cudaFree(pf.greedy);
 	cudaFree(pf.topv), cudaFree(pf.topi), cudaFree(pf.top_ids), cudaFree(pf.top_lp);
+	cudaFree(pf.vacc), cudaFree(pf.vcnt);
 	pf = Prefill();
 }
 
@@ -1599,6 +1606,166 @@ extern "C" int calm_b200_score_context_topk(struct Transformer* transformer, con
 	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, x);
 }
 
+// ---------------------------------------------------------------------------------------------
+// calm_b200_verify_greedy: a block of at most CALM_B200_VERIFY_MAX tokens (a decode token and its drafts) through the
+// prompt pass's per-row kernels and buffers, with the short-block GEMM of verify.cuh for the projections and the classifier.
+
+static_assert(VF_TOK == CALM_B200_VERIFY_MAX, "a short block is one token tile of k_vf_gemm");
+
+static int vf_slices(int K) {
+	return cdiv(K, VF_KS);
+}
+
+// k_vf_gemm's partial sums, for the largest (K-slices x rows) of the model's GEMMs, and its arrival counters (zeroed once)
+static void vf_reserve() {
+	if (pf.vacc) return;
+	const Config& c = g.cfg;
+	const size_t qkv = g.q_dim + 2 * g.kv_dim, cls = (size_t)imin(cdiv(c.vocab_size, PF_BM), VF_CLS_UNITS) * VF_ROWS;
+	const size_t rows = std::max({vf_slices(c.dim) * qkv, (size_t)vf_slices(g.q_dim) * c.dim, (size_t)vf_slices(c.dim) * 2 * c.hidden_dim,
+	                              (size_t)vf_slices(c.hidden_dim) * c.dim, vf_slices(c.dim) * cls});
+	const size_t units = std::max({qkv, (size_t)c.dim, (size_t)c.hidden_dim, cls}) / VF_ROWS;
+	pf.vacc_floats = rows * VF_TOK;
+	pf.vacc = (float*)dev_alloc(pf.vacc_floats * sizeof(float));
+	pf.vcnt = (unsigned*)dev_alloc(units * sizeof(unsigned));
+	CUDA_CHECK(cudaMemset(pf.vcnt, 0, units * sizeof(unsigned)));
+}
+
+// out = W . X^T over the rows of `a` for the n <= 16 rows of (hi, lo), in `units` row blocks of 128 (UP: of w1 and of w3
+// each); the classifier from vocabulary tile `tile0` on.  Every K-slice gets the same number of CTAs, as many as stay
+// resident together, each walking row blocks with the same stride.
+template <int MODE, int DBITS, typename KVT>
+static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int units, int tile0 = 0) {
+	static int cap = 0, sms = 0;
+	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT>, VF_THREADS, 0), sms = g.sms;
+	VfArgs v = {};
+	v.xhi = hi, v.xlo = lo, v.acc = pf.vacc, v.cnt = pf.vcnt;
+	v.nsl = vf_slices(a.K), v.units = units, v.rows = (MODE == PF_UP ? 2 : 1) * units * VF_ROWS;
+	v.tile0 = tile0, v.nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	const int tasks = (MODE == PF_UP ? 2 : 1) * units;
+	launch_pdl(k_vf_gemm<MODE, DBITS, KVT>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
+}
+
+// The block in pf.tokens at cache slots pos0 .. pos0 + n - 1: pf_run's kernel sequence for one sequence with k_vf_gemm
+// for the GEMMs, then the final norm, the classifier's tile records and their merge into pf.greedy
+template <int DBITS, typename KVT>
+static void vf_run(Formats<DBITS, KVT>, int n, int pos0) {
+	const Config& c = g.cfg;
+	const Weights& w = g.w;
+	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
+	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
+	launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
+	for (int l = 0; l < c.n_layers; ++l) {
+		launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_att_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
+		PfGemmArgs a = {};
+		a.n_tokens = n;
+		a.w[0] = w.wq[l], a.w[1] = w.wk[l], a.w[2] = w.wv[l], a.K = c.dim;
+		a.Q = pf.Q, a.q_dim = g.q_dim, a.kv_dim = g.kv_dim, a.head_dim = c.head_dim, a.seq_len = c.seq_len, a.pos0 = pos0;
+		a.bias = w.bqkv[l], a.clip = c.qkv_clip, a.rope = pf.rope;
+		a.kc = (KVT*)g.kc + l * kv_layer, a.vc = (KVT*)g.vc + l * kv_layer;
+		vf_gemm<PF_QKV, DBITS, KVT>(pf.Nhi, pf.Nlo, a, (g.q_dim + 2 * g.kv_dim) / VF_ROWS);
+		PfAttnArgs aa = {};
+		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
+		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
+		aa.seg = pf.seg, aa.ctx = pf.ctx;
+		if (c.head_dim == 128) pf_attn<KVT, 128, false>(aa, n);
+		else pf_attn<KVT, 64, false>(aa, n);
+		PfGemmArgs b = {};
+		b.n_tokens = n, b.w[0] = w.wo[l], b.K = g.q_dim, b.X = pf.X, b.dim = c.dim;
+		vf_gemm<PF_WO, DBITS, KVT>(pf.Ahi, pf.Alo, b, c.dim / VF_ROWS);
+		if (!c.norm_par) launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_ffn_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
+		PfGemmArgs u = {};
+		u.n_tokens = n, u.w[0] = w.w1[l], u.w[1] = w.w3[l], u.K = c.dim, u.Hhi = pf.Hhi, u.Hlo = pf.Hlo, u.hidden = c.hidden_dim, u.gelu = c.act_gelu;
+		vf_gemm<PF_UP, DBITS, KVT>(pf.Nhi, pf.Nlo, u, c.hidden_dim / VF_ROWS);
+		PfGemmArgs d = {};
+		d.n_tokens = n, d.w[0] = w.w2[l], d.K = c.hidden_dim, d.X = pf.X, d.dim = c.dim;
+		vf_gemm<PF_DOWN, DBITS, KVT>(pf.Hhi, pf.Hlo, d, c.dim / VF_ROWS);
+	}
+	const int nvt = cdiv(c.vocab_size, PF_BM);
+	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
+	PfGemmArgs a = {};
+	a.n_tokens = n, a.w[0] = w.wcls, a.K = c.dim;
+	a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
+	for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
+	launch_pdl(k_pf_logprob<true>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx, pf.greedy,
+	           (const float*)nullptr, (const int*)nullptr, 0, (int*)nullptr, (float*)nullptr);
+}
+
+extern "C" int calm_b200_verify_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, int* greedy) {
+	if (!g.ready) CALM_FATAL("verify_greedy before prepare_cuda");
+	if (n < 1 || n > CALM_B200_VERIFY_MAX) CALM_FATAL("verify_greedy: n %d outside [1, %d]", n, CALM_B200_VERIFY_MAX);
+	if (!tokens || !greedy) CALM_FATAL("verify_greedy: tokens or greedy is NULL");
+	check_call(transformer, tokens[0], pos0);
+	check_tokens(tokens, n);
+	if (!pf_supported() || pos0 + n > g.cfg.seq_len) {
+		for (int i = 0; i < n; ++i) greedy[i] = calm_b200_forward_argmax(transformer, tokens[i], pos0 + i);
+		return 0;
+	}
+	pf_reserve(n);
+	pf_score_reserve(true, false);
+	vf_reserve();
+	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	with_formats([&](auto f) { vf_run(f, n, pos0); });
+	CUDA_CHECK(cudaMemcpyAsync(greedy, pf.greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+	sync_stream();
+	CUDA_CHECK(cudaGetLastError());
+	return 1;
+}
+
+// The draft for `seq`: the key is its last gl tokens, for gl = 3, 2, 1 in turn, and the draft is the tokens that follow the
+// key's rightmost occurrence in the corpus among those some token follows, at most `cap` of them.  The corpus is `source`,
+// or with source == NULL `seq` itself, whose own final occurrence of the key is then passed over since nothing follows it.
+static int vf_lookup(const std::vector<int>& seq, const int* source, int n_source, int cap, int* draft) {
+	const int* corpus = source ? source : seq.data();
+	const int nc = source ? n_source : (int)seq.size();
+	for (int gl = 3; gl >= 1; --gl) {
+		if ((int)seq.size() < gl) continue;
+		const int* key = seq.data() + seq.size() - gl;
+		for (int i = nc - gl - 1; i >= 0; --i)
+			if (std::equal(key, key + gl, corpus + i)) {
+				const int d = imin(cap, nc - i - gl);
+				std::copy(corpus + i + gl, corpus + i + gl + d, draft);
+				return d;
+			}
+	}
+	return 0;
+}
+
+extern "C" int calm_b200_decode_lookup(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source, int n_source,
+                                       int max_draft, int* out_tokens) {
+	if (!g.ready) CALM_FATAL("decode_lookup before prepare_cuda");
+	if (!tokens || n < 1) CALM_FATAL("decode_lookup: needs at least one token (n = %d)", n);
+	if (n_tokens < 0 || (n_tokens > 0 && !out_tokens)) CALM_FATAL("decode_lookup: n_tokens %d or out_tokens NULL", n_tokens);
+	if (max_draft < 1 || max_draft > CALM_B200_VERIFY_MAX - 1) CALM_FATAL("decode_lookup: max_draft %d outside [1, %d]", max_draft, CALM_B200_VERIFY_MAX - 1);
+	if (source && n_source < 0) CALM_FATAL("decode_lookup: n_source %d", n_source);
+	check_call(transformer, tokens[n - 1], n - 1);
+	check_tokens(tokens, n);
+	if (source) check_tokens(source, n_source);
+	const bool served = pf_supported();
+	std::vector<int> seq(tokens, tokens + n);
+	seq.reserve(n + n_tokens);
+	int block[CALM_B200_VERIFY_MAX], greedy[CALM_B200_VERIFY_MAX];
+	int cur = tokens[n - 1], pos = n - 1, emitted = 0, steps = 0;
+	while (emitted < n_tokens) {
+		// drafts never run past the tokens still wanted or the end of the cache
+		const int cap = served ? imin(imin(max_draft, n_tokens - emitted - 1), g.cfg.seq_len - 1 - pos) : 0;
+		const int d = cap > 0 ? vf_lookup(seq, source, n_source, cap, block + 1) : 0;
+		++steps;
+		if (d == 0) { // no draft: one decode step
+			cur = calm_b200_forward_argmax(transformer, cur, pos++);
+			out_tokens[emitted++] = cur;
+			seq.push_back(cur);
+			continue;
+		}
+		block[0] = cur;
+		calm_b200_verify_greedy(transformer, block, d + 1, pos, greedy);
+		int acc = 0; // accepted drafts; greedy[acc] is the correction, or the bonus token after d accepted drafts
+		while (acc < d && block[1 + acc] == greedy[acc]) ++acc;
+		for (int i = 0; i <= acc; ++i) out_tokens[emitted++] = greedy[i], seq.push_back(greedy[i]);
+		cur = greedy[acc], pos += acc + 1;
+	}
+	return steps;
+}
+
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
 extern "C" void calm_b200_read_device_logits(float* out) {
 	CUDA_CHECK(cudaMemcpy(out, g.logits_dev, (size_t)g.cfg.vocab_size * sizeof(float), cudaMemcpyDeviceToHost));
@@ -1714,7 +1881,7 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 
 // (test aid) 0xFF bytes (NaN as f32, f16 and e5m2) into every buffer whose previous contents no later call may depend on,
 // and into the cache slots [kv_from_pos, seq_len) of every layer and kv head.  Only data is touched: TokenParams, the
-// attention's {value, epoch} cells and counter, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
+// attention's {value, epoch} cells and counter, k_vf_gemm's arrival counters, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
 // counts, stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
 // as do the index buffers (cand_idx, sample_idx, out_tokens, pf.tokens, pf.targets, and pf.rowpos, pf.seg and pf.ctx, read
 // as a RoPE position and as key slots of the packed attention's loop): a stale index that is read is in range,
@@ -1749,6 +1916,7 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		// so are the top-k records: ids only compared and copied out, values NaN like every other float
 		nan(pf.topv, cap * cdiv(c.vocab_size, PF_BM) * PF_TOPK_MAX * sizeof(float)), nan(pf.topi, cap * cdiv(c.vocab_size, PF_BM) * PF_TOPK_MAX * sizeof(int));
 		nan(pf.top_ids, cap * PF_TOPK_MAX * sizeof(int)), nan(pf.top_lp, cap * PF_TOPK_MAX * sizeof(float));
+		nan(pf.vacc, pf.vacc_floats * sizeof(float)); // (pf.vcnt, the short-block GEMM's arrival counters, steer control flow)
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

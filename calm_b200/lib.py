@@ -26,7 +26,7 @@ SYMBOLS = [
     "calm_b200_score_greedy", "calm_b200_score_batch_greedy", "calm_b200_score_context_greedy",
     "calm_b200_score_topk", "calm_b200_score_batch_topk", "calm_b200_score_context_topk",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
-    "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_timer_start", "calm_b200_timer_stop",
+    "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
     "calm_b200_tp_unique_id", "calm_b200_tp_init", "calm_b200_tp_world", "calm_b200_tp_mode",
@@ -35,6 +35,9 @@ SYMBOLS = [
 
 # the largest k calm_b200_score_topk and its siblings accept (CALM_B200_TOPK_MAX)
 TOPK_MAX = 20
+
+# the largest block calm_b200_verify_greedy takes (CALM_B200_VERIFY_MAX); decode_lookup drafts at most one fewer
+VERIFY_MAX = 16
 
 # calm_b200_read_state selectors (include/calm_b200.h)
 STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11}
@@ -80,6 +83,9 @@ def load() -> C.CDLL:
     L.calm_b200_release.argtypes, L.calm_b200_release.restype = [T], None
     L.calm_b200_forward_argmax.argtypes, L.calm_b200_forward_argmax.restype = [T, C.c_int, C.c_int], C.c_int
     L.calm_b200_decode_greedy.argtypes, L.calm_b200_decode_greedy.restype = [T, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)], None
+    L.calm_b200_verify_greedy.argtypes, L.calm_b200_verify_greedy.restype = [T, _iptr, C.c_int, C.c_int, _iptr], C.c_int
+    L.calm_b200_decode_lookup.argtypes = [T, _iptr, C.c_int, C.c_int, _iptr, C.c_int, C.c_int, _iptr]
+    L.calm_b200_decode_lookup.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -289,6 +295,38 @@ class DeviceModel:
         out = np.zeros(n, np.int32)
         self.lib.calm_b200_decode_greedy(C.byref(self.transformer), token0, pos0, n, out.ctypes.data_as(C.POINTER(C.c_int)))
         return out
+
+    def verify_greedy(self, tokens, pos0: int):
+        """calm_b200_verify_greedy: feed tokens (1 .. VERIFY_MAX of them) at pos0 .. and return (greedy int32[n], served):
+        greedy[i] is the argmax of the logits after tokens[i], served is 1 on the short-block path or 0 when n
+        forward_argmax calls gave them.  Raises ValueError for a bad length."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        if arr.ndim != 1 or not 1 <= len(arr) <= VERIFY_MAX:
+            raise ValueError(f"verify_greedy takes 1 to {VERIFY_MAX} tokens, got {arr.shape}")
+        greedy = np.full(len(arr), -1, np.int32)
+        ip = C.POINTER(C.c_int)
+        served = self.lib.calm_b200_verify_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), pos0, greedy.ctypes.data_as(ip))
+        return greedy, served
+
+    def decode_lookup(self, tokens, n_tokens: int, source=None, max_draft: int = 7):
+        """calm_b200_decode_lookup: greedy decoding with prompt-lookup drafts after `tokens` (the cache holds all but the
+        last).  The drafts come from `source`, or from tokens ++ emitted when it is None.  Returns (int32[n_tokens],
+        model steps run).  Raises ValueError for an empty `tokens`, a negative n_tokens or max_draft outside
+        [1, VERIFY_MAX - 1]."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        if arr.ndim != 1 or len(arr) < 1:
+            raise ValueError("decode_lookup needs at least one token")
+        if not isinstance(n_tokens, (int, np.integer)) or n_tokens < 0:
+            raise ValueError(f"n_tokens must be a non-negative integer, got {n_tokens!r}")
+        if not isinstance(max_draft, (int, np.integer)) or not 1 <= max_draft < VERIFY_MAX:
+            raise ValueError(f"max_draft must be an integer in [1, {VERIFY_MAX - 1}], got {max_draft!r}")
+        ip = C.POINTER(C.c_int)
+        out = np.full(int(n_tokens), -1, np.int32)
+        src = None if source is None else np.ascontiguousarray(source, np.int32)
+        steps = self.lib.calm_b200_decode_lookup(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), int(n_tokens),
+                                                 None if src is None else src.ctypes.data_as(ip), 0 if src is None else len(src), int(max_draft),
+                                                 out.ctypes.data_as(ip))
+        return out, steps
 
     def decode_sample(self, token0: int, pos0: int, n: int, temperature: float, minp: float, rng_state: int):
         """Device-resident temperature / min-p sampling; returns (tokens, new rng state)."""

@@ -195,6 +195,31 @@ int calm_b200_forward_argmax(struct Transformer* transformer, int token, int pos
  * This is what bench.py times as the in-HBM throughput. */
 void calm_b200_decode_greedy(struct Transformer* transformer, int token0, int pos0, int n_tokens, int* out_tokens);
 
+/* Verify draft tokens in one pass over the weights.  Feeds tokens[0 .. n) at positions pos0 .. pos0 + n - 1, writing
+ * their cache slots, and sets greedy[i] to the argmax of the logits after tokens[i], ties going to the lowest index (the
+ * rule of calm_b200_forward_argmax).  Slots past the prefix a caller accepts are scratch that later calls overwrite
+ * (INTEGRATION.md).  Returns 1 when the short-block path ran (DESIGN.md s.6: the prompt pass's per-row kernels with a
+ * GEMM that streams the weights over every SM).  Shapes the prompt pass does not serve (MoE, tensor parallelism, widths
+ * not multiples of 128, head_dim other than 64 / 128) and blocks past seq_len take n calm_b200_forward_argmax calls
+ * instead, with exactly their results, and return 0.  1 <= n <= CALM_B200_VERIFY_MAX and both arrays not NULL, or the
+ * call aborts before any device work. */
+#define CALM_B200_VERIFY_MAX 16
+int calm_b200_verify_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, int* greedy);
+
+/* Greedy decoding with prompt-lookup drafts.  tokens[0 .. n) is the sequence so far: the cache holds positions
+ * [0, n - 1) and tokens[n - 1] is fed at n - 1, as calm_b200_decode_greedy(t, tokens[n - 1], n - 1, n_tokens, out)
+ * feeds it.  Writes n_tokens greedy tokens to out_tokens and returns the model steps it ran (verify calls plus single
+ * decode steps).  Each step looks up the last 3, else 2, else 1 tokens of tokens ++ emitted in the corpus: source[0 ..
+ * n_source), or with source == NULL tokens ++ emitted itself (prompt lookup).  The rightmost occurrence that some token
+ * follows wins, and up to max_draft (1 .. CALM_B200_VERIFY_MAX - 1) of the tokens after it are the drafts, fewer at the
+ * corpus end, at seq_len and where fewer tokens are still wanted.  With drafts, one calm_b200_verify_greedy of the current
+ * token and the drafts accepts the longest prefix that matches and emits the greedy token after it; without, one decode
+ * step runs (calm_b200_forward_argmax), so a run that never matches emits calm_b200_decode_greedy's tokens.  Shapes the
+ * verify call does not serve take decode steps only.  Afterwards cache slots [0, n - 1 + n_tokens) are valid, as after
+ * calm_b200_decode_greedy; slots after them are scratch. */
+int calm_b200_decode_lookup(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source, int n_source,
+                            int max_draft, int* out_tokens);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
