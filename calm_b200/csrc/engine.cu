@@ -1190,426 +1190,6 @@ static void pf_attn(const PfAttnArgs& a, int n) {
 	else launch_pdl(k_pf_attn<KVT, HD, 1, SEG, CTX>, grid, PFA_WARPS * 32, 0, a);
 }
 
-// What the rows of a prompt-pass block are
-enum PfRows {
-	PF_ONE,      // one sequence at cache slots pos0 + t
-	PF_PACKED,   // a packed block of the scoring calls (pos0 = 0) that holds no context: per-row RoPE positions in pf.rowpos,
-	             // each row's sequence start in pf.seg
-	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block: each row's context in pf.ctx
-};
-
-// The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says.
-template <int DBITS, typename KVT>
-static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout = PF_ONE) {
-	const bool packed = layout != PF_ONE;
-	const Config& c = g.cfg;
-	const Weights& w = g.w;
-	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
-	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
-	if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
-	else launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
-	for (int l = 0; l < c.n_layers; ++l) {
-		launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_att_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
-		PfGemmArgs a = {};
-		a.n_tokens = n;
-		a.w[0] = w.wq[l], a.w[1] = w.wk[l], a.w[2] = w.wv[l], a.K = c.dim;
-		a.Q = pf.Q, a.q_dim = g.q_dim, a.kv_dim = g.kv_dim, a.head_dim = c.head_dim, a.seq_len = c.seq_len, a.pos0 = pos0;
-		a.bias = w.bqkv[l], a.clip = c.qkv_clip, a.rope = pf.rope;
-		a.kc = (KVT*)g.kc + l * kv_layer, a.vc = (KVT*)g.vc + l * kv_layer;
-		pf_gemm<PF_QKV, DBITS, KVT>(pf.tmN, a, g.q_dim + 2 * g.kv_dim, n);
-
-		PfAttnArgs aa = {};
-		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
-		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
-		aa.seg = pf.seg, aa.ctx = pf.ctx;
-		if (layout == PF_CONTEXTS) {
-			if (c.head_dim == 128) pf_attn<KVT, 128, true, true>(aa, n);
-			else pf_attn<KVT, 64, true, true>(aa, n);
-		} else if (packed) {
-			if (c.head_dim == 128) pf_attn<KVT, 128, true>(aa, n);
-			else pf_attn<KVT, 64, true>(aa, n);
-		} else {
-			if (c.head_dim == 128) pf_attn<KVT, 128, false>(aa, n);
-			else pf_attn<KVT, 64, false>(aa, n);
-		}
-
-		PfGemmArgs b = {};
-		b.n_tokens = n, b.w[0] = w.wo[l], b.K = g.q_dim, b.X = pf.X, b.dim = c.dim;
-		pf_gemm<PF_WO, DBITS, KVT>(pf.tmA, b, c.dim, n);
-
-		if (!c.norm_par) { // (parallel-norm models reuse the attention-norm output, reference infer.c:417-420)
-			launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_ffn_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
-		}
-		PfGemmArgs u = {};
-		u.n_tokens = n, u.w[0] = w.w1[l], u.w[1] = w.w3[l], u.K = c.dim, u.Hhi = pf.Hhi, u.Hlo = pf.Hlo, u.hidden = c.hidden_dim, u.gelu = c.act_gelu;
-		pf_gemm<PF_UP, DBITS, KVT>(pf.tmN, u, c.hidden_dim, n);
-
-		PfGemmArgs d = {};
-		d.n_tokens = n, d.w[0] = w.w2[l], d.K = c.hidden_dim, d.X = pf.X, d.dim = c.dim;
-		pf_gemm<PF_DOWN, DBITS, KVT>(pf.tmH, d, c.dim, n);
-	}
-}
-
-// What a scoring call returns besides the log-probabilities: with `greedy` the argmax of every scored position, with
-// k > 0 its k largest logits' indices and log-probabilities (top_ids / top_logprobs[i * k + r]).  Pointers are the
-// caller's, at the slot of logprobs[0].
-struct PfExtra {
-	int* greedy = nullptr;
-	int k = 0;
-	int* top_ids = nullptr;
-	float* top_logprobs = nullptr;
-	// the same outputs from slot `i` on
-	PfExtra at(size_t i) const {
-		PfExtra o = *this;
-		if (greedy) o.greedy += i;
-		if (k) o.top_ids += i * k, o.top_logprobs += i * k;
-		return o;
-	}
-};
-
-// The scoring buffers for pf.cap rows, with `greedy` the argmax buffers and with `topk` the top-k buffers, which the
-// plain scoring calls never allocate (freed and re-made with the pass's own buffers when a longer block needs more rows)
-static void pf_score_reserve(bool greedy, bool topk) {
-	const int nvt = cdiv(g.cfg.vocab_size, PF_BM);
-	if (!pf.scoring) {
-		pf.part = (float2*)dev_alloc((size_t)pf.cap * nvt * sizeof(float2));
-		pf.tgt = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
-		pf.logprob = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
-		pf.targets = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
-		pf.scoring = true;
-	}
-	if (greedy && !pf.gidx) {
-		pf.gidx = (int*)dev_alloc((size_t)pf.cap * nvt * sizeof(int));
-		pf.greedy = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
-	}
-	if (topk && !pf.topv) { // sized for the largest k: at Llama-3-8B's vocabulary, 2048 rows take 328 MB of tile lists
-		pf.topv = (float*)dev_alloc((size_t)pf.cap * nvt * PF_TOPK_MAX * sizeof(float));
-		pf.topi = (int*)dev_alloc((size_t)pf.cap * nvt * PF_TOPK_MAX * sizeof(int));
-		pf.top_ids = (int*)dev_alloc((size_t)pf.cap * PF_TOPK_MAX * sizeof(int));
-		pf.top_lp = (float*)dev_alloc((size_t)pf.cap * PF_TOPK_MAX * sizeof(float));
-	}
-}
-
-// After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records;
-// with `greedy` the classifier and the merge also give each row's argmax in pf.greedy, with k > 0 its k largest logits'
-// indices and log-probabilities in pf.top_ids / pf.top_lp [n][k]
-template <int DBITS, typename KVT>
-static void pf_score(Formats<DBITS, KVT>, int n, bool greedy, int k) {
-	const Config& c = g.cfg;
-	const Weights& w = g.w;
-	const int nvt = cdiv(c.vocab_size, PF_BM);
-	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
-	PfGemmArgs a = {};
-	a.n_tokens = n, a.w[0] = w.wcls, a.K = c.dim;
-	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
-	const float* nf = nullptr;
-	const int* ni = nullptr;
-	if (k) {
-		a.topv = pf.topv, a.topi = pf.topi, a.topk = k;
-		pf_gemm<PF_CLS_TOPK, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-		launch_pdl(k_pf_logprob<false, true>, cdiv(n, 8), 256, (size_t)8 * nvt, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, ni,
-		           (int*)nullptr, (const float*)pf.topv, (const int*)pf.topi, k, pf.top_ids, pf.top_lp);
-	} else if (greedy) {
-		pf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-		launch_pdl(k_pf_logprob<true>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx, pf.greedy,
-		           nf, ni, 0, (int*)nullptr, (float*)nullptr);
-	} else {
-		pf_gemm<PF_CLS, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-		launch_pdl(k_pf_logprob<false>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, ni, (int*)nullptr, nf, ni, 0,
-		           (int*)nullptr, (float*)nullptr);
-	}
-}
-
-// One block of the pass: the n rows the caller reserved (pf_reserve) and uploaded to pf.tokens (and, packed, to pf.rowpos,
-// pf.seg and pf.ctx) at cache slots pos0 + t, laid out as `layout` says.  With `logprobs`, the rows are scored against
-// targets[0 .. n) as well: logprobs[t] is row t's log-probability, and `x` gets the extra outputs of row t at slot t.
-static void pf_block(int n, int pos0, PfRows layout, const int* targets, float* logprobs, const PfExtra& x) {
-	if (logprobs) {
-		pf_score_reserve(x.greedy, x.k > 0);
-		CUDA_CHECK(cudaMemcpyAsync(pf.targets, targets, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	}
-	with_formats([&](auto f) { pf_run(f, n, pos0, layout); });
-	if (logprobs) {
-		with_formats([&](auto f) { pf_score(f, n, x.greedy, x.k); });
-		CUDA_CHECK(cudaMemcpyAsync(logprobs, pf.logprob, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
-		if (x.greedy) CUDA_CHECK(cudaMemcpyAsync(x.greedy, pf.greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-		if (x.k) {
-			CUDA_CHECK(cudaMemcpyAsync(x.top_ids, pf.top_ids, (size_t)n * x.k * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-			CUDA_CHECK(cudaMemcpyAsync(x.top_logprobs, pf.top_lp, (size_t)n * x.k * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
-		}
-	}
-	CUDA_CHECK(cudaStreamSynchronize(g.stream)); // the uploads read the caller's memory (pageable): they must have left it
-	CUDA_CHECK(cudaGetLastError());
-}
-
-// The batched pass over tokens[0 .. n) at positions pos0 .., in blocks of at most 2048 rows.  With `logprobs`, every block
-// is scored as well: logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]], so tokens[n] must exist; with
-// `x`, the extra outputs of position i at its slot i.
-static void pf_pass(const int* tokens, int n, int pos0, float* logprobs, const PfExtra& x = PfExtra()) {
-	const int chunk_cap = 2048;
-	for (int o = 0; o < n; o += chunk_cap) {
-		const int m = n - o < chunk_cap ? n - o : chunk_cap;
-		pf_reserve(m);
-		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		pf_block(m, pos0 + o, PF_ONE, tokens + o + 1, logprobs ? logprobs + o : nullptr, x.at(o));
-	}
-}
-
-static void check_tokens(const int* tokens, int n) {
-	for (int i = 0; i < n; ++i)
-		if (tokens[i] < 0 || tokens[i] >= g.cfg.vocab_size) CALM_FATAL("token %d out of range", tokens[i]);
-}
-
-// Feed `n` prompt tokens at positions pos0 .. pos0 + n - 1: the KV cache afterwards is what n calls of
-// forward_cuda(token, pos, FF_UPDATE_KV_ONLY) leave (within the stated tolerance); no logits, no synchronisation.
-// Returns 1 when the tensor-core pass ran, 0 when the tokens were fed one by one (unsupported model shape, MoE, tensor
-// parallelism, or a block that would roll the cache over).
-extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* tokens, int n, int pos0) {
-	if (n <= 0) return 1;
-	check_call(transformer, tokens[0], pos0);
-	check_tokens(tokens, n);
-	if (!pf_supported() || pos0 + n > g.cfg.seq_len) {
-		for (int i = 0; i < n; ++i) {
-			set_params(tokens[i], pos0 + i, 0);
-			launch_token(0);
-		}
-		return 0;
-	}
-	pf_pass(tokens, n, pos0, nullptr);
-	return 1;
-}
-
-// Score tokens[1 .. n) given what precedes each (the reference's study(), run.c:291-308): tokens[0 .. n - 1) go through
-// the prompt pass and logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]].  The cache is left as
-// forward_prefill_cuda(tokens, n - 1, pos0) leaves it.  Shapes the pass does not serve go one position at a time through
-// the decode path with a log-softmax in double on the host (returns 0).
-// calm_b200_score, and with the extra outputs `x` its greedy and top-k siblings
-static int pf_score_one(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, const PfExtra& x) {
-	if (n < 2) return 1;
-	check_call(transformer, tokens[0], pos0);
-	check_tokens(tokens, n);
-	const int rows = n - 1, vocab = g.cfg.vocab_size;
-	if (!pf_supported() || pos0 + rows > g.cfg.seq_len) {
-		for (int i = 0; i < rows; ++i) {
-			set_params(tokens[i], pos0 + i, 0);
-			launch_token(1);
-			sync_stream();
-			const float* l = g.logits_host;
-			double mx = l[0], s = 0.0;
-			for (int v = 1; v < vocab; ++v) mx = l[v] > mx ? l[v] : mx;
-			for (int v = 0; v < vocab; ++v) s += exp((double)l[v] - mx);
-			logprobs[i] = (float)((double)l[tokens[i + 1]] - mx - log(s));
-			if (x.greedy) { // first maximum (sampler.c:34-42), as calm_b200_forward_argmax
-				int best = 0;
-				for (int v = 1; v < vocab; ++v)
-					if (l[v] > l[best]) best = v;
-				x.greedy[i] = best;
-			}
-			if (x.k) { // the k largest logits, equal logits by index ascending: the same order as the tensor-core pass
-				std::vector<int> idx(vocab);
-				for (int v = 0; v < vocab; ++v) idx[v] = v;
-				std::partial_sort(idx.begin(), idx.begin() + x.k, idx.end(), [l](int a, int b) { return l[a] > l[b] || (l[a] == l[b] && a < b); });
-				for (int r = 0; r < x.k; ++r) {
-					x.top_ids[(size_t)i * x.k + r] = idx[r];
-					x.top_logprobs[(size_t)i * x.k + r] = (float)((double)l[idx[r]] - mx - log(s));
-				}
-			}
-		}
-		CUDA_CHECK(cudaGetLastError());
-		return 0;
-	}
-	pf_pass(tokens, rows, pos0, logprobs, x);
-	return 1;
-}
-
-static PfExtra greedy_out(int* greedy) {
-	PfExtra x;
-	x.greedy = greedy;
-	return x;
-}
-
-// The top-k outputs of `who`, checked before any device work
-static PfExtra topk_out(const char* who, int k, int* top_ids, float* top_logprobs) {
-	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
-	const int kmax = imin(CALM_B200_TOPK_MAX, g.cfg.vocab_size);
-	if (k < 1 || k > kmax) CALM_FATAL("%s: k %d outside [1, %d]", who, k, kmax);
-	if (!top_ids || !top_logprobs) CALM_FATAL("%s: top_ids or top_logprobs is NULL", who);
-	PfExtra x;
-	x.k = k, x.top_ids = top_ids, x.top_logprobs = top_logprobs;
-	return x;
-}
-
-extern "C" int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs) {
-	return pf_score_one(transformer, tokens, n, pos0, logprobs, PfExtra());
-}
-
-extern "C" int calm_b200_score_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, int* greedy) {
-	if (!greedy) CALM_FATAL("score_greedy: greedy is NULL");
-	return pf_score_one(transformer, tokens, n, pos0, logprobs, greedy_out(greedy));
-}
-
-extern "C" int calm_b200_score_topk(struct Transformer* transformer, const int* tokens, int n, int pos0, int k, float* logprobs, int* top_ids,
-                                    float* top_logprobs) {
-	return pf_score_one(transformer, tokens, n, pos0, logprobs, topk_out("score_topk", k, top_ids, top_logprobs));
-}
-
-// A packed block being filled: per-row inputs, the sequences it scores with their first rows, and the contexts it holds
-// by (ctx_off, ctx_len) with their first rows.  Row t of the block is cache slot t.
-struct PfPackedBlock {
-	std::vector<int> tok, tgt, pos, seg;
-	std::vector<int2> ctx;
-	std::vector<std::pair<int, int>> seqs;
-	std::map<std::pair<int, int>, int> placed;
-	int rows() const { return (int)tok.size(); }
-	// Rows for the r inputs t[0 .. r) at RoPE positions p0 .., continuing context cx, rounded up to a multiple of 8 with
-	// filler rows that repeat the last input, so that a k_pf_attn CTA never straddles two sequences; row j targets
-	// t[min(j + 1, tl)].  Causal attention keeps filler rows out of every live row.  Returns the first row.
-	int add(const int* t, int r, int tl, int p0, int2 cx) {
-		const int s = rows();
-		for (int j = 0; j < cdiv(r, 8) * 8; ++j)
-			tok.push_back(t[imin(j, r - 1)]), tgt.push_back(t[imin(j + 1, tl)]), pos.push_back(p0 + j), seg.push_back(s), ctx.push_back(cx);
-		return s;
-	}
-};
-
-// Run a block and write its sequences' log-probabilities; the results of context and filler rows are dropped.  A block that
-// holds no context runs the packed attention (k_pf_attn<.., SEG>); only one with a context uploads pf.ctx and runs the
-// context walk (k_pf_attn<.., SEG, CTX>).
-static void pf_score_packed_block(PfPackedBlock& b, const int* off, const int* len, float* logprobs, const PfExtra& x) {
-	const int rows = b.rows();
-	const bool contexts = !b.placed.empty();
-	std::vector<float> lp(rows), tl((size_t)rows * x.k);
-	std::vector<int> gr(x.greedy ? rows : 0), ti((size_t)rows * x.k);
-	PfExtra bx = x; // the block's rows
-	bx.greedy = x.greedy ? gr.data() : nullptr, bx.top_ids = ti.data(), bx.top_logprobs = tl.data();
-	pf_reserve(rows);
-	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, b.tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, b.pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(pf.seg, b.seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	if (contexts) CUDA_CHECK(cudaMemcpyAsync(pf.ctx, b.ctx.data(), (size_t)rows * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
-	pf_block(rows, 0, contexts ? PF_CONTEXTS : PF_PACKED, b.tgt.data(), lp.data(), bx);
-	for (const auto& [i, s] : b.seqs) {
-		memcpy(logprobs + off[i], lp.data() + s, (size_t)(len[i] - 1) * sizeof(float));
-		if (x.greedy) memcpy(x.greedy + off[i], gr.data() + s, (size_t)(len[i] - 1) * sizeof(int));
-		if (x.k) {
-			memcpy(x.top_ids + (size_t)off[i] * x.k, ti.data() + (size_t)s * x.k, (size_t)(len[i] - 1) * x.k * sizeof(int));
-			memcpy(x.top_logprobs + (size_t)off[i] * x.k, tl.data() + (size_t)s * x.k, (size_t)(len[i] - 1) * x.k * sizeof(float));
-		}
-	}
-	b = PfPackedBlock();
-}
-
-// Score nseq sequences that continue contexts (include/calm_b200.h); `who` names the call in error messages.  Next-fit
-// packing in input order into blocks of at most C = min(2048, seq_len rounded down to 8) rows: a context takes
-// ceil8(ctx_len) rows at RoPE positions 0 ..; a sequence takes ceil8(len - 1) rows at positions ctx_len .., after its
-// context's rows in the same block.  Sequences with the same (ctx_off, ctx_len) share one placement of the context per
-// block; a sequence whose context is not yet in the block brings it along.  A context and sequence too long for any block,
-// together, are scored alone by calm_b200_score.  With every ctx_len 0 no block holds a context: calm_b200_score_batch.
-// With the extra outputs `x`, the greedy and top-k calls.
-static int pf_score_packed(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
-                           const int* off, const int* len, int nseq, float* logprobs, const PfExtra& x) {
-	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
-	if (n < 0 || nseq < 0) CALM_FATAL("%s: negative count (n %d, nseq %d)", who, n, nseq);
-	if (nseq == 0) return 1;
-	check_tokens(tokens, n);
-	std::vector<std::pair<long, long>> out; // [first, last + 1) of the logprobs each sequence writes
-	for (int i = 0; i < nseq; ++i) {
-		if (off[i] < 0 || len[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("%s: sequence %d (off %d, len %d) outside the %d tokens", who, i, off[i], len[i], n);
-		if (ctx_off[i] < 0 || ctx_len[i] < 0 || (long)ctx_off[i] + ctx_len[i] > n)
-			CALM_FATAL("%s: context of sequence %d (off %d, len %d) outside the %d tokens", who, i, ctx_off[i], ctx_len[i], n);
-		if (len[i] >= 2) out.push_back({off[i], (long)off[i] + len[i] - 1});
-	}
-	std::sort(out.begin(), out.end());
-	for (size_t k = 1; k < out.size(); ++k)
-		if (out[k].first < out[k - 1].second) CALM_FATAL("%s: output ranges [%ld, %ld) and [%ld, %ld) overlap", who, out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
-	// calm_b200_score of ctx ++ sequence, by definition the result: for shapes the pass does not serve and units too big
-	auto alone = [&](int i) {
-		std::vector<int> cat(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
-		cat.insert(cat.end(), tokens + off[i], tokens + off[i] + len[i]);
-		const size_t m = cat.size() - 1;
-		std::vector<float> lp(m), tl(m * x.k);
-		std::vector<int> gr(x.greedy ? m : 0), ti(m * x.k);
-		PfExtra cx = x; // the rows of ctx ++ sequence
-		cx.greedy = x.greedy ? gr.data() : nullptr, cx.top_ids = ti.data(), cx.top_logprobs = tl.data();
-		const int served = pf_score_one(transformer, cat.data(), (int)cat.size(), 0, lp.data(), cx);
-		memcpy(logprobs + off[i], lp.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(float));
-		if (x.greedy) memcpy(x.greedy + off[i], gr.data() + ctx_len[i], (size_t)(len[i] - 1) * sizeof(int));
-		if (x.k) { // tmp[ctx_len + j] -> slot off[i] + j
-			memcpy(x.top_ids + (size_t)off[i] * x.k, ti.data() + (size_t)ctx_len[i] * x.k, (size_t)(len[i] - 1) * x.k * sizeof(int));
-			memcpy(x.top_logprobs + (size_t)off[i] * x.k, tl.data() + (size_t)ctx_len[i] * x.k, (size_t)(len[i] - 1) * x.k * sizeof(float));
-		}
-		return served;
-	};
-	if (!pf_supported()) {
-		for (int i = 0; i < nseq; ++i)
-			if (len[i] >= 2) alone(i);
-		return 0;
-	}
-	const int cap = imin(2048, g.cfg.seq_len / 8 * 8); // a row is its cache slot: no row may reach seq_len
-	PfPackedBlock b;
-	std::vector<int> big;
-	for (int i = 0; i < nseq; ++i) {
-		if (len[i] < 2) continue;
-		const int R = cdiv(len[i] - 1, 8) * 8, Rc = cdiv(ctx_len[i], 8) * 8;
-		if (Rc + R > cap) {
-			big.push_back(i);
-			continue;
-		}
-		const std::pair<int, int> key(ctx_off[i], ctx_len[i]);
-		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_packed_block(b, off, len, logprobs, x);
-		int c0 = 0;
-		if (ctx_len[i]) {
-			const auto it = b.placed.find(key);
-			c0 = it != b.placed.end() ? it->second : (b.placed[key] = b.add(tokens + ctx_off[i], ctx_len[i], ctx_len[i] - 1, 0, make_int2(0, 0)));
-		}
-		b.seqs.push_back({i, b.add(tokens + off[i], len[i] - 1, len[i] - 1, ctx_len[i], make_int2(c0, ctx_len[i]))});
-	}
-	if (b.rows()) pf_score_packed_block(b, off, len, logprobs, x);
-	int served = 1;
-	for (int i : big) served &= alone(i);
-	return served;
-}
-
-extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
-	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
-	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, PfExtra());
-}
-
-extern "C" int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
-                                            float* logprobs, int* greedy) {
-	if (!greedy) CALM_FATAL("score_batch_greedy: greedy is NULL");
-	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
-	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, greedy_out(greedy));
-}
-
-extern "C" int calm_b200_score_batch_topk(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, int k,
-                                          float* logprobs, int* top_ids, float* top_logprobs) {
-	const PfExtra x = topk_out("score_batch_topk", k, top_ids, top_logprobs);
-	const std::vector<int> empty(nseq > 0 ? nseq : 0); // every context empty
-	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, logprobs, x);
-}
-
-extern "C" int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
-                                       const int* off, const int* len, int nseq, float* logprobs) {
-	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, PfExtra());
-}
-
-extern "C" int calm_b200_score_context_greedy(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
-                                              const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
-	if (!greedy) CALM_FATAL("score_context_greedy: greedy is NULL");
-	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, greedy_out(greedy));
-}
-
-extern "C" int calm_b200_score_context_topk(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
-                                            const int* off, const int* len, int nseq, int k, float* logprobs, int* top_ids, float* top_logprobs) {
-	const PfExtra x = topk_out("score_context_topk", k, top_ids, top_logprobs);
-	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, logprobs, x);
-}
-
-// ---------------------------------------------------------------------------------------------
-// calm_b200_verify_greedy: a block of at most CALM_B200_VERIFY_MAX tokens (a decode token and its drafts) through the
-// prompt pass's per-row kernels and buffers, with the short-block GEMM of verify.cuh for the projections and the classifier.
-
 static_assert(VF_TOK == CALM_B200_VERIFY_MAX, "a short block is one token tile of k_vf_gemm");
 
 static int vf_slices(int K) {
@@ -1645,15 +1225,33 @@ static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int
 	launch_pdl(k_vf_gemm<MODE, DBITS, KVT>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
 }
 
-// The block in pf.tokens at cache slots pos0 .. pos0 + n - 1: pf_run's kernel sequence for one sequence with k_vf_gemm
-// for the GEMMs, then the final norm, the classifier's tile records and their merge into pf.greedy
+// What the rows of a prompt-pass block are
+enum PfRows {
+	PF_ONE,      // one sequence at cache slots pos0 + t
+	PF_SHORT,    // PF_ONE of at most VF_TOK rows (calm_b200_verify_greedy), whose GEMMs run on k_vf_gemm
+	PF_PACKED,   // a packed block of the scoring calls (pos0 = 0) that holds no context: per-row RoPE positions in pf.rowpos,
+	             // each row's sequence start in pf.seg
+	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block: each row's context in pf.ctx
+};
+
+// A layer GEMM of the pass over `rows` output rows of `a` (UP: of w1 and of w3 each), whose activations are the f16 pair
+// (hi, lo) behind the tensor maps tm: on k_vf_gemm for a short block, on k_pf_gemm for any other
+template <int MODE, int DBITS, typename KVT>
+static void pf_layer_gemm(PfRows layout, const CUtensorMap* tm, const __half* hi, const __half* lo, const PfGemmArgs& a, int rows) {
+	if (layout == PF_SHORT) vf_gemm<MODE, DBITS, KVT>(hi, lo, a, rows / VF_ROWS);
+	else pf_gemm<MODE, DBITS, KVT>(tm, a, rows, a.n_tokens);
+}
+
+// The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says.
 template <int DBITS, typename KVT>
-static void vf_run(Formats<DBITS, KVT>, int n, int pos0) {
+static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout) {
+	const bool packed = layout == PF_PACKED || layout == PF_CONTEXTS;
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
 	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
-	launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
+	if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
+	else launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
 	for (int l = 0; l < c.n_layers; ++l) {
 		launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_att_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
 		PfGemmArgs a = {};
@@ -1662,33 +1260,394 @@ static void vf_run(Formats<DBITS, KVT>, int n, int pos0) {
 		a.Q = pf.Q, a.q_dim = g.q_dim, a.kv_dim = g.kv_dim, a.head_dim = c.head_dim, a.seq_len = c.seq_len, a.pos0 = pos0;
 		a.bias = w.bqkv[l], a.clip = c.qkv_clip, a.rope = pf.rope;
 		a.kc = (KVT*)g.kc + l * kv_layer, a.vc = (KVT*)g.vc + l * kv_layer;
-		vf_gemm<PF_QKV, DBITS, KVT>(pf.Nhi, pf.Nlo, a, (g.q_dim + 2 * g.kv_dim) / VF_ROWS);
+		pf_layer_gemm<PF_QKV, DBITS, KVT>(layout, pf.tmN, pf.Nhi, pf.Nlo, a, g.q_dim + 2 * g.kv_dim);
+
 		PfAttnArgs aa = {};
 		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
 		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
 		aa.seg = pf.seg, aa.ctx = pf.ctx;
-		if (c.head_dim == 128) pf_attn<KVT, 128, false>(aa, n);
-		else pf_attn<KVT, 64, false>(aa, n);
+		if (layout == PF_CONTEXTS) {
+			if (c.head_dim == 128) pf_attn<KVT, 128, true, true>(aa, n);
+			else pf_attn<KVT, 64, true, true>(aa, n);
+		} else if (packed) {
+			if (c.head_dim == 128) pf_attn<KVT, 128, true>(aa, n);
+			else pf_attn<KVT, 64, true>(aa, n);
+		} else {
+			if (c.head_dim == 128) pf_attn<KVT, 128, false>(aa, n);
+			else pf_attn<KVT, 64, false>(aa, n);
+		}
+
 		PfGemmArgs b = {};
 		b.n_tokens = n, b.w[0] = w.wo[l], b.K = g.q_dim, b.X = pf.X, b.dim = c.dim;
-		vf_gemm<PF_WO, DBITS, KVT>(pf.Ahi, pf.Alo, b, c.dim / VF_ROWS);
-		if (!c.norm_par) launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_ffn_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
+		pf_layer_gemm<PF_WO, DBITS, KVT>(layout, pf.tmA, pf.Ahi, pf.Alo, b, c.dim);
+
+		if (!c.norm_par) { // (parallel-norm models reuse the attention-norm output, reference infer.c:417-420)
+			launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_ffn_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
+		}
 		PfGemmArgs u = {};
 		u.n_tokens = n, u.w[0] = w.w1[l], u.w[1] = w.w3[l], u.K = c.dim, u.Hhi = pf.Hhi, u.Hlo = pf.Hlo, u.hidden = c.hidden_dim, u.gelu = c.act_gelu;
-		vf_gemm<PF_UP, DBITS, KVT>(pf.Nhi, pf.Nlo, u, c.hidden_dim / VF_ROWS);
+		pf_layer_gemm<PF_UP, DBITS, KVT>(layout, pf.tmN, pf.Nhi, pf.Nlo, u, c.hidden_dim);
+
 		PfGemmArgs d = {};
 		d.n_tokens = n, d.w[0] = w.w2[l], d.K = c.hidden_dim, d.X = pf.X, d.dim = c.dim;
-		vf_gemm<PF_DOWN, DBITS, KVT>(pf.Hhi, pf.Hlo, d, c.dim / VF_ROWS);
+		pf_layer_gemm<PF_DOWN, DBITS, KVT>(layout, pf.tmH, pf.Hhi, pf.Hlo, d, c.dim);
 	}
+}
+
+// What a scoring call writes for each scored position: logprobs[i], with `greedy` its argmax, with k > 0 its k largest
+// logits' indices and log-probabilities (top_ids / top_logprobs[i * k + r]).  Pointers are at the slot of position 0.
+struct PfOut {
+	float* logprobs = nullptr;
+	int* greedy = nullptr;
+	int k = 0;
+	int* top_ids = nullptr;
+	float* top_logprobs = nullptr;
+	// the same outputs from slot `i` on
+	PfOut at(size_t i) const {
+		PfOut o = *this;
+		if (logprobs) o.logprobs += i;
+		if (greedy) o.greedy += i;
+		if (k) o.top_ids += i * k, o.top_logprobs += i * k;
+		return o;
+	}
+	// rows [s, s + m) of `src`, which holds the same outputs, to slots o .. o + m - 1: from the device on the stream, or
+	// from the host
+	void put(const PfOut& src, size_t s, size_t m, size_t o, bool from_device) const {
+		auto cp = [&](void* dst, const void* from, size_t bytes) {
+			if (from_device) CUDA_CHECK(cudaMemcpyAsync(dst, from, bytes, cudaMemcpyDeviceToHost, g.stream));
+			else memcpy(dst, from, bytes);
+		};
+		cp(logprobs + o, src.logprobs + s, m * sizeof(float));
+		if (greedy) cp(greedy + o, src.greedy + s, m * sizeof(int));
+		if (k) cp(top_ids + o * k, src.top_ids + s * k, m * k * sizeof(int)), cp(top_logprobs + o * k, src.top_logprobs + s * k, m * k * sizeof(float));
+	}
+};
+
+// Host rows for the outputs of `x`, where a block's or a lone pass's rows land before they go to the caller's slots
+struct PfRowBuf {
+	std::vector<float> lp, tl;
+	std::vector<int> gr, ti;
+	PfOut out; // x's outputs, in these rows
+	PfRowBuf(const PfOut& x, size_t rows) : lp(rows), tl(rows * x.k), gr(x.greedy ? rows : 0), ti(rows * x.k), out(x) {
+		out.logprobs = lp.data(), out.greedy = x.greedy ? gr.data() : nullptr, out.top_ids = ti.data(), out.top_logprobs = tl.data();
+	}
+	PfRowBuf(const PfRowBuf&) = delete;
+};
+
+// The scoring buffers for pf.cap rows, with `greedy` the argmax buffers and with `topk` the top-k buffers, which the
+// plain scoring calls never allocate (freed and re-made with the pass's own buffers when a longer block needs more rows)
+static void pf_score_reserve(bool greedy, bool topk) {
+	const int nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	if (!pf.scoring) {
+		pf.part = (float2*)dev_alloc((size_t)pf.cap * nvt * sizeof(float2));
+		pf.tgt = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
+		pf.logprob = (float*)dev_alloc((size_t)pf.cap * sizeof(float));
+		pf.targets = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
+		pf.scoring = true;
+	}
+	if (greedy && !pf.gidx) {
+		pf.gidx = (int*)dev_alloc((size_t)pf.cap * nvt * sizeof(int));
+		pf.greedy = (int*)dev_alloc((size_t)pf.cap * sizeof(int));
+	}
+	if (topk && !pf.topv) { // sized for the largest k: at Llama-3-8B's vocabulary, 2048 rows take 328 MB of tile lists
+		pf.topv = (float*)dev_alloc((size_t)pf.cap * nvt * PF_TOPK_MAX * sizeof(float));
+		pf.topi = (int*)dev_alloc((size_t)pf.cap * nvt * PF_TOPK_MAX * sizeof(int));
+		pf.top_ids = (int*)dev_alloc((size_t)pf.cap * PF_TOPK_MAX * sizeof(int));
+		pf.top_lp = (float*)dev_alloc((size_t)pf.cap * PF_TOPK_MAX * sizeof(float));
+	}
+}
+
+// After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records;
+// with `greedy` the classifier and the merge also give each row's argmax in pf.greedy, with k > 0 its k largest logits'
+// indices and log-probabilities in pf.top_ids / pf.top_lp [n][k].  A short block's greedy classifier runs on k_vf_gemm,
+// VF_CLS_UNITS vocabulary tiles per launch.
+template <int DBITS, typename KVT>
+static void pf_score(Formats<DBITS, KVT>, int n, PfRows layout, bool greedy, int k) {
+	const Config& c = g.cfg;
+	const Weights& w = g.w;
 	const int nvt = cdiv(c.vocab_size, PF_BM);
 	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
 	PfGemmArgs a = {};
 	a.n_tokens = n, a.w[0] = w.wcls, a.K = c.dim;
-	a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
-	for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
-	launch_pdl(k_pf_logprob<true>, cdiv(n, 8), 256, 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx, pf.greedy,
-	           (const float*)nullptr, (const int*)nullptr, 0, (int*)nullptr, (float*)nullptr);
+	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
+	if (k) {
+		a.topv = pf.topv, a.topi = pf.topi, a.topk = k;
+		pf_gemm<PF_CLS_TOPK, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
+	} else if (greedy && layout == PF_SHORT) {
+		for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
+	} else if (greedy) {
+		pf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
+	} else {
+		pf_gemm<PF_CLS, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
+	}
+	const auto merge = k ? k_pf_logprob<false, true> : greedy ? k_pf_logprob<true> : k_pf_logprob<false>;
+	launch_pdl(merge, cdiv(n, 8), 256, k ? (size_t)8 * nvt : 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx,
+	           pf.greedy, (const float*)pf.topv, (const int*)pf.topi, k, pf.top_ids, pf.top_lp);
 }
+
+// One block of the pass: the n rows the caller reserved (pf_reserve) and uploaded to pf.tokens (and, packed, to pf.rowpos,
+// pf.seg and pf.ctx) at cache slots pos0 + t, laid out as `layout` says.  With `x.logprobs`, the rows are scored against
+// targets[0 .. n) as well, and `x` gets the outputs of row t at slot t.
+static void pf_block(int n, int pos0, PfRows layout, const int* targets, const PfOut& x) {
+	if (x.logprobs) {
+		pf_score_reserve(x.greedy, x.k > 0);
+		CUDA_CHECK(cudaMemcpyAsync(pf.targets, targets, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	}
+	with_formats([&](auto f) { pf_run(f, n, pos0, layout); });
+	if (x.logprobs) {
+		with_formats([&](auto f) { pf_score(f, n, layout, x.greedy, x.k); });
+		PfOut dev = x;
+		dev.logprobs = pf.logprob, dev.greedy = pf.greedy, dev.top_ids = pf.top_ids, dev.top_logprobs = pf.top_lp;
+		x.put(dev, 0, n, 0, true);
+	}
+	CUDA_CHECK(cudaStreamSynchronize(g.stream)); // the uploads read the caller's memory (pageable): they must have left it
+	CUDA_CHECK(cudaGetLastError());
+}
+
+// The batched pass over tokens[0 .. n) at positions pos0 .., in blocks of at most 2048 rows.  With `x.logprobs`, every
+// block is scored as well: logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]], so tokens[n] must exist, and
+// `x` gets the outputs of position i at its slot i.
+static void pf_pass(const int* tokens, int n, int pos0, const PfOut& x = PfOut()) {
+	const int chunk_cap = 2048;
+	for (int o = 0; o < n; o += chunk_cap) {
+		const int m = n - o < chunk_cap ? n - o : chunk_cap;
+		pf_reserve(m);
+		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		pf_block(m, pos0 + o, PF_ONE, tokens + o + 1, x.at(o));
+	}
+}
+
+static void check_tokens(const int* tokens, int n) {
+	for (int i = 0; i < n; ++i)
+		if (tokens[i] < 0 || tokens[i] >= g.cfg.vocab_size) CALM_FATAL("token %d out of range", tokens[i]);
+}
+
+// Feed `n` prompt tokens at positions pos0 .. pos0 + n - 1: the KV cache afterwards is what n calls of
+// forward_cuda(token, pos, FF_UPDATE_KV_ONLY) leave (within the stated tolerance); no logits, no synchronisation.
+// Returns 1 when the tensor-core pass ran, 0 when the tokens were fed one by one (unsupported model shape, MoE, tensor
+// parallelism, or a block that would roll the cache over).
+extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* tokens, int n, int pos0) {
+	if (n <= 0) return 1;
+	check_call(transformer, tokens[0], pos0);
+	check_tokens(tokens, n);
+	if (!pf_supported() || pos0 + n > g.cfg.seq_len) {
+		for (int i = 0; i < n; ++i) {
+			set_params(tokens[i], pos0 + i, 0);
+			launch_token(0);
+		}
+		return 0;
+	}
+	pf_pass(tokens, n, pos0);
+	return 1;
+}
+
+// Score tokens[1 .. n) given what precedes each (the reference's study(), run.c:291-308): tokens[0 .. n - 1) go through
+// the prompt pass and logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]].  The cache is left as
+// forward_prefill_cuda(tokens, n - 1, pos0) leaves it.  Shapes the pass does not serve go one position at a time through
+// the decode path with a log-softmax in double on the host (returns 0).
+// calm_b200_score, and with the extra outputs of `x` its greedy and top-k siblings
+static int pf_score_one(struct Transformer* transformer, const int* tokens, int n, int pos0, const PfOut& x) {
+	if (n < 2) return 1;
+	check_call(transformer, tokens[0], pos0);
+	check_tokens(tokens, n);
+	const int rows = n - 1, vocab = g.cfg.vocab_size;
+	if (!pf_supported() || pos0 + rows > g.cfg.seq_len) {
+		for (int i = 0; i < rows; ++i) {
+			set_params(tokens[i], pos0 + i, 0);
+			launch_token(1);
+			sync_stream();
+			const float* l = g.logits_host;
+			double mx = l[0], s = 0.0;
+			for (int v = 1; v < vocab; ++v) mx = l[v] > mx ? l[v] : mx;
+			for (int v = 0; v < vocab; ++v) s += exp((double)l[v] - mx);
+			x.logprobs[i] = (float)((double)l[tokens[i + 1]] - mx - log(s));
+			if (x.greedy) { // first maximum (sampler.c:34-42), as calm_b200_forward_argmax
+				int best = 0;
+				for (int v = 1; v < vocab; ++v)
+					if (l[v] > l[best]) best = v;
+				x.greedy[i] = best;
+			}
+			if (x.k) { // the k largest logits, equal logits by index ascending: the same order as the tensor-core pass
+				std::vector<int> idx(vocab);
+				for (int v = 0; v < vocab; ++v) idx[v] = v;
+				std::partial_sort(idx.begin(), idx.begin() + x.k, idx.end(), [l](int a, int b) { return l[a] > l[b] || (l[a] == l[b] && a < b); });
+				for (int r = 0; r < x.k; ++r) {
+					x.top_ids[(size_t)i * x.k + r] = idx[r];
+					x.top_logprobs[(size_t)i * x.k + r] = (float)((double)l[idx[r]] - mx - log(s));
+				}
+			}
+		}
+		CUDA_CHECK(cudaGetLastError());
+		return 0;
+	}
+	pf_pass(tokens, rows, pos0, x);
+	return 1;
+}
+
+// The outputs of a greedy call `who`, checked before any device work
+static PfOut greedy_out(const char* who, float* logprobs, int* greedy) {
+	if (!greedy) CALM_FATAL("%s: greedy is NULL", who);
+	return PfOut{logprobs, greedy};
+}
+
+// The outputs of a top-k call `who`, checked before any device work
+static PfOut topk_out(const char* who, int k, float* logprobs, int* top_ids, float* top_logprobs) {
+	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
+	const int kmax = imin(CALM_B200_TOPK_MAX, g.cfg.vocab_size);
+	if (k < 1 || k > kmax) CALM_FATAL("%s: k %d outside [1, %d]", who, k, kmax);
+	if (!top_ids || !top_logprobs) CALM_FATAL("%s: top_ids or top_logprobs is NULL", who);
+	return PfOut{logprobs, nullptr, k, top_ids, top_logprobs};
+}
+
+extern "C" int calm_b200_score(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs) {
+	return pf_score_one(transformer, tokens, n, pos0, PfOut{logprobs});
+}
+
+extern "C" int calm_b200_score_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, float* logprobs, int* greedy) {
+	return pf_score_one(transformer, tokens, n, pos0, greedy_out("score_greedy", logprobs, greedy));
+}
+
+extern "C" int calm_b200_score_topk(struct Transformer* transformer, const int* tokens, int n, int pos0, int k, float* logprobs, int* top_ids,
+                                    float* top_logprobs) {
+	return pf_score_one(transformer, tokens, n, pos0, topk_out("score_topk", k, logprobs, top_ids, top_logprobs));
+}
+
+// A packed block being filled: per-row inputs, the sequences it scores with their first rows, and the contexts it holds
+// by (ctx_off, ctx_len) with their first rows.  Row t of the block is cache slot t.
+struct PfPackedBlock {
+	std::vector<int> tok, tgt, pos, seg;
+	std::vector<int2> ctx;
+	std::vector<std::pair<int, int>> seqs;
+	std::map<std::pair<int, int>, int> placed;
+	int rows() const { return (int)tok.size(); }
+	// Rows for the r inputs t[0 .. r) at RoPE positions p0 .., continuing context cx, rounded up to a multiple of 8 with
+	// filler rows that repeat the last input, so that a k_pf_attn CTA never straddles two sequences; row j targets
+	// t[min(j + 1, tl)].  Causal attention keeps filler rows out of every live row.  Returns the first row.
+	int add(const int* t, int r, int tl, int p0, int2 cx) {
+		const int s = rows();
+		for (int j = 0; j < cdiv(r, 8) * 8; ++j)
+			tok.push_back(t[imin(j, r - 1)]), tgt.push_back(t[imin(j + 1, tl)]), pos.push_back(p0 + j), seg.push_back(s), ctx.push_back(cx);
+		return s;
+	}
+};
+
+// Run a block and write its sequences' log-probabilities; the results of context and filler rows are dropped.  A block that
+// holds no context runs the packed attention (k_pf_attn<.., SEG>); only one with a context uploads pf.ctx and runs the
+// context walk (k_pf_attn<.., SEG, CTX>).
+static void pf_score_packed_block(PfPackedBlock& b, const int* off, const int* len, const PfOut& x) {
+	const int rows = b.rows();
+	const bool contexts = !b.placed.empty();
+	const PfRowBuf buf(x, rows);
+	pf_reserve(rows);
+	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, b.tok.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, b.pos.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.seg, b.seg.data(), (size_t)rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	if (contexts) CUDA_CHECK(cudaMemcpyAsync(pf.ctx, b.ctx.data(), (size_t)rows * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
+	pf_block(rows, 0, contexts ? PF_CONTEXTS : PF_PACKED, b.tgt.data(), buf.out);
+	for (const auto& [i, s] : b.seqs) x.put(buf.out, s, len[i] - 1, off[i], false);
+	b = PfPackedBlock();
+}
+
+// Score nseq sequences that continue contexts (include/calm_b200.h); `who` names the call in error messages.  Next-fit
+// packing in input order into blocks of at most C = min(2048, seq_len rounded down to 8) rows: a context takes
+// ceil8(ctx_len) rows at RoPE positions 0 ..; a sequence takes ceil8(len - 1) rows at positions ctx_len .., after its
+// context's rows in the same block.  Sequences with the same (ctx_off, ctx_len) share one placement of the context per
+// block; a sequence whose context is not yet in the block brings it along.  A context and sequence too long for any block,
+// together, are scored alone by calm_b200_score.  With every ctx_len 0 no block holds a context: calm_b200_score_batch.
+// With the extra outputs of `x`, the greedy and top-k calls.
+static int pf_score_packed(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                           const int* off, const int* len, int nseq, const PfOut& x) {
+	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
+	if (n < 0 || nseq < 0) CALM_FATAL("%s: negative count (n %d, nseq %d)", who, n, nseq);
+	if (nseq == 0) return 1;
+	check_tokens(tokens, n);
+	std::vector<std::pair<long, long>> out; // [first, last + 1) of the logprobs each sequence writes
+	for (int i = 0; i < nseq; ++i) {
+		if (off[i] < 0 || len[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("%s: sequence %d (off %d, len %d) outside the %d tokens", who, i, off[i], len[i], n);
+		if (ctx_off[i] < 0 || ctx_len[i] < 0 || (long)ctx_off[i] + ctx_len[i] > n)
+			CALM_FATAL("%s: context of sequence %d (off %d, len %d) outside the %d tokens", who, i, ctx_off[i], ctx_len[i], n);
+		if (len[i] >= 2) out.push_back({off[i], (long)off[i] + len[i] - 1});
+	}
+	std::sort(out.begin(), out.end());
+	for (size_t k = 1; k < out.size(); ++k)
+		if (out[k].first < out[k - 1].second) CALM_FATAL("%s: output ranges [%ld, %ld) and [%ld, %ld) overlap", who, out[k - 1].first, out[k - 1].second, out[k].first, out[k].second);
+	// calm_b200_score of ctx ++ sequence, by definition the result: for shapes the pass does not serve and units too big
+	auto alone = [&](int i) {
+		std::vector<int> cat(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
+		cat.insert(cat.end(), tokens + off[i], tokens + off[i] + len[i]);
+		const PfRowBuf buf(x, cat.size() - 1); // the rows of ctx ++ sequence
+		const int served = pf_score_one(transformer, cat.data(), (int)cat.size(), 0, buf.out);
+		x.put(buf.out, ctx_len[i], len[i] - 1, off[i], false);
+		return served;
+	};
+	if (!pf_supported()) {
+		for (int i = 0; i < nseq; ++i)
+			if (len[i] >= 2) alone(i);
+		return 0;
+	}
+	const int cap = imin(2048, g.cfg.seq_len / 8 * 8); // a row is its cache slot: no row may reach seq_len
+	PfPackedBlock b;
+	std::vector<int> big;
+	for (int i = 0; i < nseq; ++i) {
+		if (len[i] < 2) continue;
+		const int R = cdiv(len[i] - 1, 8) * 8, Rc = cdiv(ctx_len[i], 8) * 8;
+		if (Rc + R > cap) {
+			big.push_back(i);
+			continue;
+		}
+		const std::pair<int, int> key(ctx_off[i], ctx_len[i]);
+		if (b.rows() + (b.placed.count(key) ? 0 : Rc) + R > cap) pf_score_packed_block(b, off, len, x);
+		int c0 = 0;
+		if (ctx_len[i]) {
+			const auto it = b.placed.find(key);
+			c0 = it != b.placed.end() ? it->second : (b.placed[key] = b.add(tokens + ctx_off[i], ctx_len[i], ctx_len[i] - 1, 0, make_int2(0, 0)));
+		}
+		b.seqs.push_back({i, b.add(tokens + off[i], len[i] - 1, len[i] - 1, ctx_len[i], make_int2(c0, ctx_len[i]))});
+	}
+	if (b.rows()) pf_score_packed_block(b, off, len, x);
+	int served = 1;
+	for (int i : big) served &= alone(i);
+	return served;
+}
+
+// calm_b200_score_batch and its greedy and top-k siblings: the context calls with every context empty
+static int pf_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, const PfOut& x) {
+	const std::vector<int> empty(nseq > 0 ? nseq : 0);
+	return pf_score_packed("score_batch", transformer, tokens, n, empty.data(), empty.data(), off, len, nseq, x);
+}
+
+extern "C" int calm_b200_score_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, float* logprobs) {
+	return pf_score_batch(transformer, tokens, n, off, len, nseq, PfOut{logprobs});
+}
+
+extern "C" int calm_b200_score_batch_greedy(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
+                                            float* logprobs, int* greedy) {
+	return pf_score_batch(transformer, tokens, n, off, len, nseq, greedy_out("score_batch_greedy", logprobs, greedy));
+}
+
+extern "C" int calm_b200_score_batch_topk(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq, int k,
+                                          float* logprobs, int* top_ids, float* top_logprobs) {
+	return pf_score_batch(transformer, tokens, n, off, len, nseq, topk_out("score_batch_topk", k, logprobs, top_ids, top_logprobs));
+}
+
+extern "C" int calm_b200_score_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                       const int* off, const int* len, int nseq, float* logprobs) {
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, PfOut{logprobs});
+}
+
+extern "C" int calm_b200_score_context_greedy(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                              const int* off, const int* len, int nseq, float* logprobs, int* greedy) {
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, greedy_out("score_context_greedy", logprobs, greedy));
+}
+
+extern "C" int calm_b200_score_context_topk(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                            const int* off, const int* len, int nseq, int k, float* logprobs, int* top_ids, float* top_logprobs) {
+	return pf_score_packed("score_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nseq, topk_out("score_context_topk", k, logprobs, top_ids, top_logprobs));
+}
+
+// ---------------------------------------------------------------------------------------------
+// calm_b200_verify_greedy: a block of at most CALM_B200_VERIFY_MAX tokens (a decode token and its drafts) through the
+// prompt pass as a short block, whose projections and classifier run on the short-block GEMM of verify.cuh.
 
 extern "C" int calm_b200_verify_greedy(struct Transformer* transformer, const int* tokens, int n, int pos0, int* greedy) {
 	if (!g.ready) CALM_FATAL("verify_greedy before prepare_cuda");
@@ -1704,7 +1663,10 @@ extern "C" int calm_b200_verify_greedy(struct Transformer* transformer, const in
 	pf_score_reserve(true, false);
 	vf_reserve();
 	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	with_formats([&](auto f) { vf_run(f, n, pos0); });
+	with_formats([&](auto f) {
+		pf_run(f, n, pos0, PF_SHORT);
+		pf_score(f, n, PF_SHORT, true, 0);
+	});
 	CUDA_CHECK(cudaMemcpyAsync(greedy, pf.greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 	sync_stream();
 	CUDA_CHECK(cudaGetLastError());

@@ -27,6 +27,8 @@
 // to its context's rows and then its own as one key sequence (k_pf_attn<.., SEG, CTX>).  The greedy scoring calls run
 // PF_CLS_GREEDY and k_pf_logprob<true>, which also give each row's argmax, with the same log-probability bits.  The top-k
 // scoring calls run PF_CLS_TOPK and k_pf_logprob<false, true>: each tile's k largest logits, merged into each row's k largest.
+// The short-block GEMM of calm_b200_verify_greedy (k_vf_gemm, verify.cuh) dequantises through this file's weight
+// conversions (e5m2_word_h2, gf4_word_h2) and ends in its epilogue (pf_epilogue_pair for UP, WO and DOWN).
 //
 // Parity contract (tests/test_prefill_gpu.py): after forward_prefill_cuda(tokens, n, pos0) the KV cache and the logits of
 // the following token equal those of n serial forward(FF_UPDATE_KV_ONLY) calls within the stated tolerances.
@@ -210,6 +212,24 @@ __device__ __forceinline__ void pf_load_raw(const unsigned char* row, int kb, ui
 #pragma unroll
 	for (int i = 0; i < DBITS / 2; ++i) raw[i] = ldg_stream(p + i);
 }
+// The weight formats -> f16, exactly (the prompt pass and k_vf_gemm dequantise through these two)
+// four e5m2 weights -> two f16 pairs in weight order: an e5m2 byte is the high byte of the f16 (reference infer.c:28-35)
+__device__ __forceinline__ uint2 e5m2_word_h2(uint32_t w) {
+	return make_uint2(__byte_perm(w, 0, 0x1404), __byte_perm(w, 0, 0x3424));
+}
+// a gf4 word (scale byte + eight 3-bit codes) -> four f16 pairs in weight order: (q - 4) * s / -4 (reference
+// infer.c:37-40); at most 6 significant bits: exact in f16
+__device__ __forceinline__ uint4 gf4_word_h2(uint32_t w) {
+	const float sf = e5m2_to_float((uint8_t)(w & 0xff)) * -0.25f;
+	uint32_t h[4];
+#pragma unroll
+	for (int k = 0; k < 4; ++k) {
+		const float a0 = (float)((int)((w >> (8 + 6 * k)) & 7) - 4) * sf, a1 = (float)((int)((w >> (11 + 6 * k)) & 7) - 4) * sf;
+		h[k] = pack_h2(__float2half_rn(a0), __float2half_rn(a1));
+	}
+	return make_uint4(h[0], h[1], h[2], h[3]);
+}
+
 template <int DBITS>
 __device__ __forceinline__ void pf_store_a(unsigned char* tile, int r, const uint4 (&raw)[DBITS / 2]) {
 	unsigned char* rowp = tile + r * 128;
@@ -217,28 +237,19 @@ __device__ __forceinline__ void pf_store_a(unsigned char* tile, int r, const uin
 	if constexpr (DBITS == 16) {
 #pragma unroll
 		for (int c = 0; c < 8; ++c) put(c, raw[c]);
-	} else if constexpr (DBITS == 8) { // an e5m2 byte is the high byte of the f16 (reference infer.c:28-35)
+	} else if constexpr (DBITS == 8) {
 #pragma unroll
 		for (int i = 0; i < 4; ++i) {
-			const uint32_t w[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
-			put(2 * i, make_uint4(__byte_perm(w[0], 0, 0x1404), __byte_perm(w[0], 0, 0x3424), __byte_perm(w[1], 0, 0x1404), __byte_perm(w[1], 0, 0x3424)));
-			put(2 * i + 1, make_uint4(__byte_perm(w[2], 0, 0x1404), __byte_perm(w[2], 0, 0x3424), __byte_perm(w[3], 0, 0x1404), __byte_perm(w[3], 0, 0x3424)));
+			const uint2 h0 = e5m2_word_h2(raw[i].x), h1 = e5m2_word_h2(raw[i].y), h2 = e5m2_word_h2(raw[i].z), h3 = e5m2_word_h2(raw[i].w);
+			put(2 * i, make_uint4(h0.x, h0.y, h1.x, h1.y));
+			put(2 * i + 1, make_uint4(h2.x, h2.y, h3.x, h3.y));
 		}
-	} else { // gf4: (q - 4) * s / -4 (reference infer.c:37-40); at most 6 significant bits: exact in f16
+	} else {
 #pragma unroll
 		for (int i = 0; i < 2; ++i) {
 			const uint32_t w[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
 #pragma unroll
-			for (int j = 0; j < 4; ++j) {
-				const float sf = e5m2_to_float((uint8_t)(w[j] & 0xff)) * -0.25f;
-				uint32_t h[4];
-#pragma unroll
-				for (int k = 0; k < 4; ++k) {
-					const float a0 = (float)((int)((w[j] >> (8 + 6 * k)) & 7) - 4) * sf, a1 = (float)((int)((w[j] >> (11 + 6 * k)) & 7) - 4) * sf;
-					h[k] = pack_h2(__float2half_rn(a0), __float2half_rn(a1));
-				}
-				put(4 * i + j, make_uint4(h[0], h[1], h[2], h[3]));
-			}
+			for (int j = 0; j < 4; ++j) put(4 * i + j, gf4_word_h2(w[j]));
 		}
 	}
 }
@@ -254,6 +265,24 @@ __host__ __device__ constexpr size_t pf_stage_bytes() {
 template <int MODE>
 __host__ __device__ constexpr size_t pf_smem_bytes() {
 	return pf_stages<MODE>() * pf_stage_bytes<MODE>() + 1024; // + alignment slack
+}
+
+// The epilogue of UP, WO and DOWN for token t and the output rows (gr, gr + 1) (gr even) whose finished sums are x0, x1
+// (UP: of w1, with g0, g1 those of w3).  UP: act(w1 x) * (w3 x) as hi + lo; WO / DOWN: residual add.  (QKV's epilogue is
+// written out in each kernel: as a function it compiles to different instructions in k_pf_gemm.)
+template <int MODE>
+__device__ __forceinline__ void pf_epilogue_pair(const PfGemmArgs& a, int gr, int t, float x0, float x1, float g0, float g1) {
+	if constexpr (MODE == PF_UP) {
+		const float h0 = (a.gelu ? act_gelu(x0) : act_silu(x0)) * g0, h1 = (a.gelu ? act_gelu(x1) : act_silu(x1)) * g1;
+		__half hh0, hl0, hh1, hl1;
+		split_hl(h0, hh0, hl0), split_hl(h1, hh1, hl1);
+		*reinterpret_cast<uint32_t*>(a.Hhi + (size_t)t * a.hidden + gr) = pack_h2(hh0, hh1);
+		*reinterpret_cast<uint32_t*>(a.Hlo + (size_t)t * a.hidden + gr) = pack_h2(hl0, hl1);
+	} else {
+		float2* dst = reinterpret_cast<float2*>(a.X + (size_t)t * a.dim + gr);
+		const float2 o = *dst;
+		*dst = make_float2(o.x + x0, o.y + x1);
+	}
 }
 
 template <int MODE, int DBITS, typename KVT>
@@ -444,8 +473,8 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 			for (int h = 0; h < 2; ++h) {
 				const int t = tb + 8 * h;
 				if (t >= a.n_tokens) continue;
-				float x0 = acc[0][4 * j + 2 * h], x1 = acc[0][4 * j + 2 * h + 1];
 				if constexpr (MODE == PF_QKV) {
+					float x0 = acc[0][4 * j + 2 * h], x1 = acc[0][4 * j + 2 * h + 1];
 					const bool is_q = gr < a.q_dim, is_k = !is_q && gr < a.q_dim + a.kv_dim;
 					const int k = is_q ? gr : (is_k ? gr - a.q_dim : gr - a.q_dim - a.kv_dim);
 					const int d = k % a.head_dim, hh = k / a.head_dim;
@@ -462,17 +491,8 @@ __global__ void __launch_bounds__(PF_THREADS, 1) k_pf_gemm(const __grid_constant
 						KVT* dst = reinterpret_cast<KVT*>(is_k ? a.kc : a.vc) + ((size_t)hh * a.seq_len + a.pos0 + t) * a.head_dim + d;
 						kv_store(dst, x0), kv_store(dst + 1, x1);
 					}
-				} else if constexpr (MODE == PF_UP) {
-					const float g0 = acc[NA - 1][4 * j + 2 * h], g1 = acc[NA - 1][4 * j + 2 * h + 1];
-					const float h0 = (a.gelu ? act_gelu(x0) : act_silu(x0)) * g0, h1 = (a.gelu ? act_gelu(x1) : act_silu(x1)) * g1;
-					__half hh0, hl0, hh1, hl1;
-					split_hl(h0, hh0, hl0), split_hl(h1, hh1, hl1);
-					*reinterpret_cast<uint32_t*>(a.Hhi + (size_t)t * a.hidden + gr) = pack_h2(hh0, hh1);
-					*reinterpret_cast<uint32_t*>(a.Hlo + (size_t)t * a.hidden + gr) = pack_h2(hl0, hl1);
 				} else {
-					float2* dst = reinterpret_cast<float2*>(a.X + (size_t)t * a.dim + gr);
-					const float2 o = *dst;
-					*dst = make_float2(o.x + x0, o.y + x1);
+					pf_epilogue_pair<MODE>(a, gr, t, acc[0][4 * j + 2 * h], acc[0][4 * j + 2 * h + 1], acc[NA - 1][4 * j + 2 * h], acc[NA - 1][4 * j + 2 * h + 1]);
 				}
 			}
 		}

@@ -2,8 +2,8 @@
 // block of at most 16 tokens (a decode token and its drafts), streaming the weights over every SM as the decode does.
 //
 //   k_vf_gemm   out[rows][16 tokens] = W . X^T with mma.sync m16n8k16 (f16 in, fp32 accumulators): the weight rows are
-//               the M side, 16 per warp fragment, dequantised in registers with the prompt pass's exact fp16 / e5m2 /
-//               gf4 -> f16 conversions (pf_store_a); the tokens are the N side, two n8 tiles, and the activations enter
+//               the M side, 16 per warp fragment, dequantised in registers by the prompt pass's own fp16 / e5m2 /
+//               gf4 -> f16 conversions (e5m2_word_h2, gf4_word_h2, as pf_store_a); the tokens are the N side, two n8 tiles, and the activations enter
 //               as the pass's f16 hi + lo pair, two MMAs into one accumulator.  Inside a 64-wide k chunk, lane (g, t)
 //               owns k = 16 t .. 16 t + 15 of its rows g and g + 8 (one contiguous load per row) and the MMA's k slots
 //               are mapped onto those k in the same way for A and B, so every product still meets its own activation.
@@ -11,8 +11,8 @@
 //               slice sit in shared memory, and a CTA keeps its slice while it walks its row blocks.  Each task writes
 //               its fp32 partial sums; the CTA that completes a row block's last slice (an arrival counter, reset by
 //               that CTA) adds the slices in ascending order and runs the epilogue of k_pf_gemm on the completed sums:
-//               QKV bias / clip / RoPE / Q rows and KV append, residual add (WO, DOWN), act(w1 x) * (w3 x) split into
-//               hi + lo (UP), and for the classifier each 128-row vocabulary tile's (max, sum) and argmax records in the
+//               QKV bias / clip / RoPE / Q rows and KV append as k_pf_gemm writes it out, k_pf_gemm's pf_epilogue_pair
+//               for the residual add (WO, DOWN) and act(w1 x) * (w3 x) split into hi + lo (UP), and for the classifier each 128-row vocabulary tile's (max, sum) and argmax records in the
 //               layout PF_CLS_GREEDY writes, which the unchanged k_pf_logprob<true, false> merges.  Nothing is added
 //               with atomics and the fold order is fixed, so repeated calls give the same bits.
 #pragma once
@@ -65,24 +65,23 @@ __device__ __forceinline__ void vf_load(const unsigned char* row, int k0, uint32
 	}
 }
 
-// the same 16 weights as 8 f16 pairs in k order, converted exactly as pf_store_a converts them
+// the same 16 weights as 8 f16 pairs in k order, through pf_store_a's conversions
 template <int DBITS>
 __device__ __forceinline__ void vf_dequant(const uint32_t (&w)[VfFmt<DBITS>::WORDS], uint32_t (&h)[8]) {
 	if constexpr (DBITS == 16) {
 #pragma unroll
 		for (int i = 0; i < 8; ++i) h[i] = w[i];
-	} else if constexpr (DBITS == 8) { // an e5m2 byte is the high byte of the f16
+	} else if constexpr (DBITS == 8) {
 #pragma unroll
-		for (int i = 0; i < 4; ++i) h[2 * i] = __byte_perm(w[i], 0, 0x1404), h[2 * i + 1] = __byte_perm(w[i], 0, 0x3424);
-	} else { // gf4: (q - 4) * s / -4, 8 weights per word
+		for (int i = 0; i < 4; ++i) {
+			const uint2 p = e5m2_word_h2(w[i]);
+			h[2 * i] = p.x, h[2 * i + 1] = p.y;
+		}
+	} else {
 #pragma unroll
 		for (int j = 0; j < 2; ++j) {
-			const float sf = e5m2_to_float((uint8_t)(w[j] & 0xff)) * -0.25f;
-#pragma unroll
-			for (int k = 0; k < 4; ++k) {
-				const float a0 = (float)((int)((w[j] >> (8 + 6 * k)) & 7) - 4) * sf, a1 = (float)((int)((w[j] >> (11 + 6 * k)) & 7) - 4) * sf;
-				h[4 * j + k] = pack_h2(__float2half_rn(a0), __float2half_rn(a1));
-			}
+			const uint4 p = gf4_word_h2(w[j]);
+			h[4 * j] = p.x, h[4 * j + 1] = p.y, h[4 * j + 2] = p.z, h[4 * j + 3] = p.w;
 		}
 	}
 }
@@ -259,8 +258,8 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 			for (int j = 0; j < 4; ++j) {
 				const int t = 4 * tq + j;
 				if (t >= a.n_tokens) continue;
-				float x0 = x[0][j], x1 = x[1][j];
 				if constexpr (MODE == PF_QKV) {
+					float x0 = x[0][j], x1 = x[1][j];
 					const bool is_q = gr < a.q_dim, is_k = !is_q && gr < a.q_dim + a.kv_dim;
 					const int k = is_q ? gr : (is_k ? gr - a.q_dim : gr - a.q_dim - a.kv_dim);
 					const int d = k % a.head_dim, hh = k / a.head_dim;
@@ -277,17 +276,8 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 						KVT* dst = reinterpret_cast<KVT*>(is_k ? a.kc : a.vc) + ((size_t)hh * a.seq_len + a.pos0 + t) * a.head_dim + d;
 						kv_store(dst, x0), kv_store(dst + 1, x1);
 					}
-				} else if constexpr (MODE == PF_UP) {
-					const float g0 = gt[0][j], g1 = gt[1][j];
-					const float h0 = (a.gelu ? act_gelu(x0) : act_silu(x0)) * g0, h1 = (a.gelu ? act_gelu(x1) : act_silu(x1)) * g1;
-					__half hh0, hl0, hh1, hl1;
-					split_hl(h0, hh0, hl0), split_hl(h1, hh1, hl1);
-					*reinterpret_cast<uint32_t*>(a.Hhi + (size_t)t * a.hidden + gr) = pack_h2(hh0, hh1);
-					*reinterpret_cast<uint32_t*>(a.Hlo + (size_t)t * a.hidden + gr) = pack_h2(hl0, hl1);
 				} else {
-					float2* dst = reinterpret_cast<float2*>(a.X + (size_t)t * a.dim + gr);
-					const float2 o = *dst;
-					*dst = make_float2(o.x + x0, o.y + x1);
+					pf_epilogue_pair<MODE>(a, gr, t, x[0][j], x[1][j], gt[0][j], gt[1][j]);
 				}
 			}
 		}
