@@ -162,6 +162,17 @@ struct Prefill {
 	float* vacc = nullptr;
 	size_t vacc_floats = 0;
 	unsigned* vcnt = nullptr;
+	// sampled short blocks (calm_b200_verify_sample), allocated on its first call: the block's logit rows and each tile's
+	// maximum, and per row the sampler's survivor lists, chunk sums and counts, its SampleState and its token
+	float* vlogits = nullptr; // [VF_TOK][vocab]
+	float* vtmax = nullptr;   // [VF_TOK][cdiv(vocab, PF_BM)]
+	int* vsidx = nullptr;     // [VF_TOK][sample_chunks * SAMPLE_CHUNK]
+	float* vsprob = nullptr;
+	float* vcsum = nullptr;   // [VF_TOK][sample_chunks]
+	int* vcount = nullptr;
+	SampleState* vstate = nullptr; // [VF_TOK]
+	int* vsampled = nullptr;       // [VF_TOK]
+	int vrows = 0;                 // rows of the last sampled block (CALM_B200_STATE_PF_LOGITS)
 };
 Prefill pf;
 
@@ -172,6 +183,7 @@ void pf_free() {
 	cudaFree(pf.gidx), cudaFree(pf.greedy);
 	cudaFree(pf.topv), cudaFree(pf.topi), cudaFree(pf.top_ids), cudaFree(pf.top_lp);
 	cudaFree(pf.vacc), cudaFree(pf.vcnt);
+	cudaFree(pf.vlogits), cudaFree(pf.vtmax), cudaFree(pf.vsidx), cudaFree(pf.vsprob), cudaFree(pf.vcsum), cudaFree(pf.vcount), cudaFree(pf.vstate), cudaFree(pf.vsampled);
 	pf = Prefill();
 }
 
@@ -1060,6 +1072,15 @@ extern "C" int calm_b200_forward_sample(struct Transformer* transformer, int tok
 	return tok;
 }
 
+// The state step of the reference's xorshift* generator (sampler.c:7-13), which k_sample_pick takes once per draw: the
+// states of a run of draws do not depend on the logits, so the host can form them
+static unsigned long long xorshift_step(unsigned long long s) {
+	s ^= s >> 12;
+	s ^= s << 25;
+	s ^= s >> 27;
+	return s;
+}
+
 // The device sampler on its own: logits given by the host, any vocabulary size; returns the token and advances *rng_state.
 // Same kernels as the decode loop (k_sample_scan + k_sample_pick); device_us (optional) receives their mean duration.
 extern "C" int calm_b200_sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us) {
@@ -1221,6 +1242,7 @@ static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int
 	v.xhi = hi, v.xlo = lo, v.acc = pf.vacc, v.cnt = pf.vcnt;
 	v.nsl = vf_slices(a.K), v.units = units, v.rows = (MODE == PF_UP ? 2 : 1) * units * VF_ROWS;
 	v.tile0 = tile0, v.nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	v.logits = pf.vlogits, v.tmax = pf.vtmax;
 	const int tasks = (MODE == PF_UP ? 2 : 1) * units;
 	launch_pdl(k_vf_gemm<MODE, DBITS, KVT>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
 }
@@ -1360,9 +1382,10 @@ static void pf_score_reserve(bool greedy, bool topk) {
 // After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records;
 // with `greedy` the classifier and the merge also give each row's argmax in pf.greedy, with k > 0 its k largest logits'
 // indices and log-probabilities in pf.top_ids / pf.top_lp [n][k].  A short block's greedy classifier runs on k_vf_gemm,
-// VF_CLS_UNITS vocabulary tiles per launch.
+// VF_CLS_UNITS vocabulary tiles per launch; with `sample` (a short greedy block) it also writes the logit rows and tile
+// maxima that vf_sample_rows samples, and the merge is left out.
 template <int DBITS, typename KVT>
-static void pf_score(Formats<DBITS, KVT>, int n, PfRows layout, bool greedy, int k) {
+static void pf_score(Formats<DBITS, KVT>, int n, PfRows layout, bool greedy, int k, bool sample = false) {
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const int nvt = cdiv(c.vocab_size, PF_BM);
@@ -1374,7 +1397,11 @@ static void pf_score(Formats<DBITS, KVT>, int n, PfRows layout, bool greedy, int
 		a.topv = pf.topv, a.topi = pf.topi, a.topk = k;
 		pf_gemm<PF_CLS_TOPK, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
 	} else if (greedy && layout == PF_SHORT) {
-		for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
+		for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) {
+			if (sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
+			else vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
+		}
+		if (sample) return;
 	} else if (greedy) {
 		pf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
 	} else {
@@ -1673,6 +1700,75 @@ extern "C" int calm_b200_verify_greedy(struct Transformer* transformer, const in
 	return 1;
 }
 
+// ---------------------------------------------------------------------------------------------
+// calm_b200_verify_sample: the short block with the classifier in PF_CLS_SAMPLE, whose logit rows the unchanged device
+// sampler draws from, one row at a time.
+
+// the logit rows and tile maxima, and each row's sampler lists, sums, counts, state and token (pf.vlogits ..)
+static void vf_sample_reserve() {
+	if (pf.vlogits) return;
+	const size_t vocab = g.cfg.vocab_size, nvt = cdiv(g.cfg.vocab_size, PF_BM), nch = g.sample_chunks;
+	pf.vlogits = (float*)dev_alloc(VF_TOK * vocab * sizeof(float));
+	pf.vtmax = (float*)dev_alloc(VF_TOK * nvt * sizeof(float));
+	pf.vsidx = (int*)dev_alloc(VF_TOK * nch * SAMPLE_CHUNK * sizeof(int));
+	pf.vsprob = (float*)dev_alloc(VF_TOK * nch * SAMPLE_CHUNK * sizeof(float));
+	pf.vcsum = (float*)dev_alloc(VF_TOK * nch * sizeof(float));
+	pf.vcount = (int*)dev_alloc(VF_TOK * nch * sizeof(int));
+	pf.vstate = (SampleState*)dev_alloc(VF_TOK * sizeof(SampleState));
+	pf.vsampled = (int*)dev_alloc(VF_TOK * sizeof(int));
+}
+
+// The n rows of the last PF_CLS_SAMPLE classifier through the decode's sampler, side by side: row i is k_sample_scan +
+// k_sample_pick on its own lists and its own SampleState pf.vstate[i] (k_sample_scan_rows / k_sample_pick_rows), and its
+// token goes to pf.vsampled[i]
+static void vf_sample_rows(int n) {
+	const int vocab = g.cfg.vocab_size, nvt = cdiv(vocab, PF_BM), nch = g.sample_chunks;
+	SampleArgs sa;
+	sa.logits = pf.vlogits, sa.cand_val = pf.vtmax, sa.ncand = nvt, sa.vocab = vocab, sa.nchunks = nch;
+	sa.st = pf.vstate, sa.count = pf.vcount, sa.csum = pf.vcsum, sa.sidx = pf.vsidx, sa.sprob = pf.vsprob;
+	launch_pdl(k_sample_scan_rows, dim3(nch, n), 256, 0, sa);
+	launch_pdl(k_sample_pick_rows, n, 256, 0, sa, pf.vstate, pf.vsampled);
+}
+
+extern "C" int calm_b200_verify_sample(struct Transformer* transformer, const int* tokens, int n, int pos0, float temperature, float minp,
+                                       unsigned long long* rng_state, int* sampled) {
+	if (!g.ready) CALM_FATAL("verify_sample before prepare_cuda");
+	if (n < 1 || n > CALM_B200_VERIFY_MAX) CALM_FATAL("verify_sample: n %d outside [1, %d]", n, CALM_B200_VERIFY_MAX);
+	if (!tokens || !sampled || !rng_state) CALM_FATAL("verify_sample: tokens, rng_state or sampled is NULL");
+	if (temperature == 0.0f || minp >= 1.0f) return calm_b200_verify_greedy(transformer, tokens, n, pos0, sampled); // sample() is greedy there
+	check_call(transformer, tokens[0], pos0);
+	check_tokens(tokens, n);
+	int served = 0;
+	if (!pf_supported() || pos0 + n > g.cfg.seq_len) {
+		unsigned long long s = *rng_state; // a local copy: the caller's generator advances by the draws it keeps
+		for (int i = 0; i < n; ++i) sampled[i] = calm_b200_forward_sample(transformer, tokens[i], pos0 + i, temperature, minp, &s);
+	} else {
+		pf_reserve(n);
+		pf_score_reserve(true, false);
+		vf_reserve();
+		vf_sample_reserve();
+		SampleState st[CALM_B200_VERIFY_MAX]; // row i draws the (i + 1)-th coin: the caller's state advanced i times
+		unsigned long long s = *rng_state;
+		for (int i = 0; i < n; ++i) st[i].rng = s, st[i].temperature = temperature, st[i].cut_delta = logf(minp) * temperature, s = xorshift_step(s);
+		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tokens, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		CUDA_CHECK(cudaMemcpyAsync(pf.vstate, st, (size_t)n * sizeof(SampleState), cudaMemcpyHostToDevice, g.stream));
+		with_formats([&](auto f) {
+			pf_run(f, n, pos0, PF_SHORT);
+			pf_score(f, n, PF_SHORT, true, 0, true);
+		});
+		vf_sample_rows(n);
+		CUDA_CHECK(cudaMemcpyAsync(sampled, pf.vsampled, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+		sync_stream();
+		CUDA_CHECK(cudaGetLastError());
+		pf.vrows = n;
+		served = 1;
+	}
+	int acc = 0; // accepted drafts: the caller emits sampled[0 .. acc], one draw each
+	while (acc < n - 1 && sampled[acc] == tokens[acc + 1]) ++acc;
+	for (int i = 0; i <= acc; ++i) *rng_state = xorshift_step(*rng_state);
+	return served;
+}
+
 // The draft for `seq`: the key is its last gl tokens, for gl = 3, 2, 1 in turn, and the draft is the tokens that follow the
 // key's rightmost occurrence in the corpus among those some token follows, at most `cap` of them.  The corpus is `source`,
 // or with source == NULL `seq` itself, whose own final occurrence of the key is then passed over since nothing follows it.
@@ -1692,13 +1788,22 @@ static int vf_lookup(const std::vector<int>& seq, const int* source, int n_sourc
 	return 0;
 }
 
-extern "C" int calm_b200_decode_lookup(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source, int n_source,
-                                       int max_draft, int* out_tokens) {
-	if (!g.ready) CALM_FATAL("decode_lookup before prepare_cuda");
-	if (!tokens || n < 1) CALM_FATAL("decode_lookup: needs at least one token (n = %d)", n);
-	if (n_tokens < 0 || (n_tokens > 0 && !out_tokens)) CALM_FATAL("decode_lookup: n_tokens %d or out_tokens NULL", n_tokens);
-	if (max_draft < 1 || max_draft > CALM_B200_VERIFY_MAX - 1) CALM_FATAL("decode_lookup: max_draft %d outside [1, %d]", max_draft, CALM_B200_VERIFY_MAX - 1);
-	if (source && n_source < 0) CALM_FATAL("decode_lookup: n_source %d", n_source);
+// The argument checks of the lookup calls (`who`), before any device work
+static void lookup_checks(const char* who, const int* tokens, int n, int n_tokens, const int* source, int n_source, int max_draft, const int* out_tokens) {
+	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
+	if (!tokens || n < 1) CALM_FATAL("%s: needs at least one token (n = %d)", who, n);
+	if (n_tokens < 0 || (n_tokens > 0 && !out_tokens)) CALM_FATAL("%s: n_tokens %d or out_tokens NULL", who, n_tokens);
+	if (max_draft < 1 || max_draft > CALM_B200_VERIFY_MAX - 1) CALM_FATAL("%s: max_draft %d outside [1, %d]", who, max_draft, CALM_B200_VERIFY_MAX - 1);
+	if (source && n_source < 0) CALM_FATAL("%s: n_source %d", who, n_source);
+}
+
+// The loop of calm_b200_decode_lookup and calm_b200_decode_lookup_sample, after lookup_checks: step(cur, pos) is one
+// decode step, which returns the token after `cur`; verify(block, m, pos, out) feeds block[0 .. m) at pos .. and writes
+// the token after each to out[0 .. m).  The longest prefix of drafts that out confirms is accepted, and the token after it
+// is emitted too.
+template <typename Step, typename Verify>
+static int lookup_loop(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source, int n_source, int max_draft,
+                       int* out_tokens, Step step, Verify verify) {
 	check_call(transformer, tokens[n - 1], n - 1);
 	check_tokens(tokens, n);
 	if (source) check_tokens(source, n_source);
@@ -1713,19 +1818,40 @@ extern "C" int calm_b200_decode_lookup(struct Transformer* transformer, const in
 		const int d = cap > 0 ? vf_lookup(seq, source, n_source, cap, block + 1) : 0;
 		++steps;
 		if (d == 0) { // no draft: one decode step
-			cur = calm_b200_forward_argmax(transformer, cur, pos++);
+			cur = step(cur, pos++);
 			out_tokens[emitted++] = cur;
 			seq.push_back(cur);
 			continue;
 		}
 		block[0] = cur;
-		calm_b200_verify_greedy(transformer, block, d + 1, pos, greedy);
+		verify(block, d + 1, pos, greedy);
 		int acc = 0; // accepted drafts; greedy[acc] is the correction, or the bonus token after d accepted drafts
 		while (acc < d && block[1 + acc] == greedy[acc]) ++acc;
 		for (int i = 0; i <= acc; ++i) out_tokens[emitted++] = greedy[i], seq.push_back(greedy[i]);
 		cur = greedy[acc], pos += acc + 1;
 	}
 	return steps;
+}
+
+extern "C" int calm_b200_decode_lookup(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source, int n_source,
+                                       int max_draft, int* out_tokens) {
+	lookup_checks("decode_lookup", tokens, n, n_tokens, source, n_source, max_draft, out_tokens);
+	return lookup_loop(
+	    transformer, tokens, n, n_tokens, source, n_source, max_draft, out_tokens, [&](int cur, int pos) { return calm_b200_forward_argmax(transformer, cur, pos); },
+	    [&](const int* block, int m, int pos, int* out) { calm_b200_verify_greedy(transformer, block, m, pos, out); });
+}
+
+// decode_lookup's loop with sampled tokens: a step is calm_b200_forward_sample, a verification calm_b200_verify_sample, and
+// both advance the caller's generator by the tokens they emit
+extern "C" int calm_b200_decode_lookup_sample(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source, int n_source,
+                                              int max_draft, float temperature, float minp, unsigned long long* rng_state, int* out_tokens) {
+	lookup_checks("decode_lookup_sample", tokens, n, n_tokens, source, n_source, max_draft, out_tokens);
+	if (!rng_state) CALM_FATAL("decode_lookup_sample: rng_state is NULL");
+	if (temperature == 0.0f || minp >= 1.0f) return calm_b200_decode_lookup(transformer, tokens, n, n_tokens, source, n_source, max_draft, out_tokens);
+	return lookup_loop(
+	    transformer, tokens, n, n_tokens, source, n_source, max_draft, out_tokens,
+	    [&](int cur, int pos) { return calm_b200_forward_sample(transformer, cur, pos, temperature, minp, rng_state); },
+	    [&](const int* block, int m, int pos, int* out) { calm_b200_verify_sample(transformer, block, m, pos, temperature, minp, rng_state, out); });
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -1802,6 +1928,7 @@ extern "C" int calm_b200_read_state(int which, int layer, float* out, int cap) {
 	case CALM_B200_STATE_PF_Q: f32 = pf.Q, count = (size_t)pf.cap * g.q_dim; break;
 	case CALM_B200_STATE_PF_ATT: hi = pf.Ahi, lo = pf.Alo, count = (size_t)pf.cap * g.q_dim; break;
 	case CALM_B200_STATE_PF_HB: hi = pf.Hhi, lo = pf.Hlo, count = (size_t)pf.cap * c.hidden_dim; break;
+	case CALM_B200_STATE_PF_LOGITS: f32 = pf.vlogits, count = (size_t)pf.vrows * c.vocab_size; break;
 	default: CALM_FATAL("read_state: unknown selector %d", which);
 	}
 	if (count > 0x7fffffff) CALM_FATAL("read_state: %zu values do not fit the int the call returns", count);
@@ -1844,8 +1971,8 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 // (test aid) 0xFF bytes (NaN as f32, f16 and e5m2) into every buffer whose previous contents no later call may depend on,
 // and into the cache slots [kv_from_pos, seq_len) of every layer and kv head.  Only data is touched: TokenParams, the
 // attention's {value, epoch} cells and counter, k_vf_gemm's arrival counters, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
-// counts, stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
-// as do the index buffers (cand_idx, sample_idx, out_tokens, pf.tokens, pf.targets, and pf.rowpos, pf.seg and pf.ctx, read
+// counts (the decode's and the sampled short block's), stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
+// as do the index buffers (cand_idx, sample_idx, pf.vsidx, out_tokens, pf.tokens, pf.targets, and pf.rowpos, pf.seg and pf.ctx, read
 // as a RoPE position and as key slots of the packed attention's loop): a stale index that is read is in range,
 // as after any earlier call, while 0xFFFFFFFF would send the read out of bounds.  DESIGN.md s.3 lists both groups.
 extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos) {
@@ -1879,6 +2006,11 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		nan(pf.topv, cap * cdiv(c.vocab_size, PF_BM) * PF_TOPK_MAX * sizeof(float)), nan(pf.topi, cap * cdiv(c.vocab_size, PF_BM) * PF_TOPK_MAX * sizeof(int));
 		nan(pf.top_ids, cap * PF_TOPK_MAX * sizeof(int)), nan(pf.top_lp, cap * PF_TOPK_MAX * sizeof(float));
 		nan(pf.vacc, pf.vacc_floats * sizeof(float)); // (pf.vcnt, the short-block GEMM's arrival counters, steer control flow)
+		// the sampled block's logit rows, tile maxima, survivor probabilities and chunk sums, and its tokens (only copied out);
+		// its survivor counts and SampleStates steer the sampler like sample_count / sample_state, and pf.vsidx is an index buffer
+		const size_t nch = g.sample_chunks;
+		nan(pf.vlogits, VF_TOK * (size_t)c.vocab_size * sizeof(float)), nan(pf.vtmax, VF_TOK * (size_t)cdiv(c.vocab_size, PF_BM) * sizeof(float));
+		nan(pf.vsprob, VF_TOK * nch * SAMPLE_CHUNK * sizeof(float)), nan(pf.vcsum, VF_TOK * nch * sizeof(float)), nan(pf.vsampled, VF_TOK * sizeof(int));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

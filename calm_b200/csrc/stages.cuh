@@ -1255,8 +1255,8 @@ struct SampleArgs {
 	float* sprob;
 };
 
-__global__ void __launch_bounds__(256) k_sample_scan(const SampleArgs a) {
-	pdl_enter();
+// one chunk of the vocabulary: its survivors, in index order, and their sequential sum
+__device__ __forceinline__ void sample_scan(const SampleArgs& a, const unsigned chunk) {
 	__shared__ float red[8];
 	__shared__ int wcount[8];
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1270,7 +1270,7 @@ __global__ void __launch_bounds__(256) k_sample_scan(const SampleArgs a) {
 	const float temp = a.st->temperature, cutoff = mx + a.st->cut_delta;
 
 	// 4 consecutive entries per thread, so that thread order is index order
-	const int base = blockIdx.x * SAMPLE_CHUNK + tid * 4;
+	const int base = chunk * SAMPLE_CHUNK + tid * 4;
 	float p[4];
 	int keep = 0;
 #pragma unroll
@@ -1289,8 +1289,8 @@ __global__ void __launch_bounds__(256) k_sample_scan(const SampleArgs a) {
 	__syncthreads();
 	int off = incl - keep;
 	for (int w = 0; w < warp; ++w) off += wcount[w];
-	int* li = a.sidx + (size_t)blockIdx.x * SAMPLE_CHUNK;
-	float* lp = a.sprob + (size_t)blockIdx.x * SAMPLE_CHUNK;
+	int* li = a.sidx + (size_t)chunk * SAMPLE_CHUNK;
+	float* lp = a.sprob + (size_t)chunk * SAMPLE_CHUNK;
 #pragma unroll
 	for (int k = 0; k < 4; ++k)
 		if (p[k] >= 0.f) li[off] = base + k, lp[off] = p[k], ++off;
@@ -1300,8 +1300,13 @@ __global__ void __launch_bounds__(256) k_sample_scan(const SampleArgs a) {
 		for (int w = 0; w < 8; ++w) n += wcount[w];
 		float sum = 0.f;
 		for (int j = 0; j < n; ++j) sum += lp[j];
-		a.count[blockIdx.x] = n, a.csum[blockIdx.x] = sum;
+		a.count[chunk] = n, a.csum[chunk] = sum;
 	}
+}
+
+__global__ void __launch_bounds__(256) k_sample_scan(const SampleArgs a) {
+	pdl_enter();
+	sample_scan(a, blockIdx.x);
 }
 
 __device__ __forceinline__ unsigned xorshift_u32(unsigned long long& s) { // reference sampler.c:7-13
@@ -1316,8 +1321,7 @@ __device__ __forceinline__ unsigned xorshift_u32(unsigned long long& s) { // ref
 // then performs exactly the reference's left-to-right float additions on them (4 cycles each instead of a global-memory
 // round trip); with more survivors the per-chunk sums of k_sample_scan are walked and only the chunk holding the coin is
 // expanded.
-__global__ void __launch_bounds__(256) k_sample_pick(const SampleArgs a, SampleState* st, TokenParams* tp, int* out_tokens, int* last_token, int advance) {
-	pdl_enter();
+__device__ __forceinline__ void sample_pick(const SampleArgs a, SampleState* st, TokenParams* tp, int* out_tokens, int* last_token, int advance) {
 	__shared__ float sp[SAMPLE_EXACT];
 	__shared__ int si[SAMPLE_EXACT];
 	__shared__ int coff[256]; // exclusive prefix of the chunk counts (nchunks <= 256: vocabularies up to 262144)
@@ -1398,6 +1402,34 @@ __global__ void __launch_bounds__(256) k_sample_pick(const SampleArgs a, SampleS
 		tp->kv_len = pos >= seq_len ? seq_len : pos + 1;
 		tp->step += 1;
 	}
+}
+
+__global__ void __launch_bounds__(256) k_sample_pick(const SampleArgs a, SampleState* st, TokenParams* tp, int* out_tokens, int* last_token, int advance) {
+	pdl_enter();
+	sample_pick(a, st, tp, out_tokens, last_token, advance);
+}
+
+// n rows sampled side by side (calm_b200_verify_sample): row r is `a` with every array advanced by r rows -- logits by
+// `vocab`, cand_val by `ncand`, the state by one, the counts and sums by `nchunks` and the lists by nchunks * SAMPLE_CHUNK
+// -- and its token goes to tokens[r].  k_sample_scan_rows runs chunk blockIdx.x of row blockIdx.y, k_sample_pick_rows row
+// blockIdx.x; each row is exactly k_sample_scan + k_sample_pick on that row.
+__device__ __forceinline__ SampleArgs sample_row(const SampleArgs& a, int r) {
+	SampleArgs b = a;
+	b.logits += (size_t)r * a.vocab, b.cand_val += (size_t)r * a.ncand, b.st += r;
+	b.count += (size_t)r * a.nchunks, b.csum += (size_t)r * a.nchunks;
+	b.sidx += (size_t)r * a.nchunks * SAMPLE_CHUNK, b.sprob += (size_t)r * a.nchunks * SAMPLE_CHUNK;
+	return b;
+}
+
+__global__ void __launch_bounds__(256) k_sample_scan_rows(const SampleArgs a) {
+	pdl_enter();
+	sample_scan(sample_row(a, blockIdx.y), blockIdx.x);
+}
+
+__global__ void __launch_bounds__(256) k_sample_pick_rows(const SampleArgs a, SampleState* st, int* tokens) {
+	pdl_enter();
+	const int r = blockIdx.x;
+	sample_pick(sample_row(a, r), st + r, nullptr, nullptr, tokens + r, 0);
 }
 
 // per-chunk maxima of a logits vector (stand-alone sampler entry point: what k_output's candidates are in a token)

@@ -1,4 +1,4 @@
-// verify.cuh -- the short-block GEMM of calm_b200_verify_greedy: the five projections of a layer and the classifier for a
+// verify.cuh -- the short-block GEMM of calm_b200_verify_greedy / _sample: the five projections of a layer and the classifier for a
 // block of at most 16 tokens (a decode token and its drafts), streaming the weights over every SM as the decode does.
 //
 //   k_vf_gemm   out[rows][16 tokens] = W . X^T with mma.sync m16n8k16 (f16 in, fp32 accumulators): the weight rows are
@@ -15,6 +15,9 @@
 //               for the residual add (WO, DOWN) and act(w1 x) * (w3 x) split into hi + lo (UP), and for the classifier each 128-row vocabulary tile's (max, sum) and argmax records in the
 //               layout PF_CLS_GREEDY writes, which the unchanged k_pf_logprob<true, false> merges.  Nothing is added
 //               with atomics and the fold order is fixed, so repeated calls give the same bits.
+//               PF_CLS_SAMPLE (calm_b200_verify_sample) is PF_CLS_GREEDY that also stores the fold's logits of every
+//               token row, and each tile's maximum, which k_sample_scan_rows / k_sample_pick_rows (stages.cuh) sample,
+//               all rows side by side: the same accumulator values the argmax records come from.
 #pragma once
 
 #include "prefill.cuh"
@@ -35,6 +38,8 @@ struct VfArgs {
 	int units;         // row blocks; UP: hidden / 128, whose w1 and w3 rows are tasks of their own
 	int rows;          // rows of the partial-sum layout (UP: 2 * hidden)
 	int tile0, nvt;    // CLS: the first vocabulary tile of this launch, and the tiles of the vocabulary
+	float* logits;     // PF_CLS_SAMPLE: [n_tokens][vocab] the logit rows
+	float* tmax;       // PF_CLS_SAMPLE: [n_tokens][nvt] each tile's maximum logit (the sampler's cand_val)
 };
 
 template <int DBITS>
@@ -89,7 +94,7 @@ __device__ __forceinline__ void vf_dequant(const uint32_t (&w)[VfFmt<DBITS>::WOR
 template <int MODE, int DBITS, typename KVT>
 __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, const VfArgs v) {
 	constexpr int W = VfFmt<DBITS>::WORDS, U = VfFmt<DBITS>::U;
-	constexpr bool CLS = MODE == PF_CLS_GREEDY;
+	constexpr bool CLS = MODE == PF_CLS_GREEDY || MODE == PF_CLS_SAMPLE;
 	__shared__ __align__(16) __half xs[2][VF_TOK][VF_XSTR];
 	__shared__ unsigned last_s;
 	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
@@ -249,6 +254,16 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 					a.part[(size_t)t * v.nvt + tile] = make_float2(m, sum);
 					a.gidx[(size_t)t * v.nvt + tile] = gi;
 					if (tile == 0) a.tgt[t] = lg[t][0]; // (the target is token 0: k_pf_logprob needs one, the caller reads only the argmax)
+				}
+				if constexpr (MODE == PF_CLS_SAMPLE) { // the same values out: the tile's logits, coalesced, and its maximum
+					if (t < a.n_tokens) {
+#pragma unroll
+						for (int i = 0; i < 4; ++i) {
+							const int r = lane + 32 * i;
+							if (rbase + r < a.vocab) v.logits[(size_t)t * a.vocab + rbase + r] = lg[t][r];
+						}
+						if (lane == 0) v.tmax[(size_t)t * v.nvt + tile] = m;
+					}
 				}
 			}
 			__syncthreads(); // lg is rewritten by this CTA's next fold only after this

@@ -26,7 +26,8 @@ SYMBOLS = [
     "calm_b200_score_greedy", "calm_b200_score_batch_greedy", "calm_b200_score_context_greedy",
     "calm_b200_score_topk", "calm_b200_score_batch_topk", "calm_b200_score_context_topk",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
-    "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_timer_start", "calm_b200_timer_stop",
+    "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
+    "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
     "calm_b200_tp_unique_id", "calm_b200_tp_init", "calm_b200_tp_world", "calm_b200_tp_mode",
@@ -40,7 +41,7 @@ TOPK_MAX = 20
 VERIFY_MAX = 16
 
 # calm_b200_read_state selectors (include/calm_b200.h)
-STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11}
+STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11, "pf_logits": 12}
 
 _lib = None
 
@@ -86,6 +87,11 @@ def load() -> C.CDLL:
     L.calm_b200_verify_greedy.argtypes, L.calm_b200_verify_greedy.restype = [T, _iptr, C.c_int, C.c_int, _iptr], C.c_int
     L.calm_b200_decode_lookup.argtypes = [T, _iptr, C.c_int, C.c_int, _iptr, C.c_int, C.c_int, _iptr]
     L.calm_b200_decode_lookup.restype = C.c_int
+    _u64p = C.POINTER(C.c_ulonglong)
+    L.calm_b200_verify_sample.argtypes = [T, _iptr, C.c_int, C.c_int, C.c_float, C.c_float, _u64p, _iptr]
+    L.calm_b200_verify_sample.restype = C.c_int
+    L.calm_b200_decode_lookup_sample.argtypes = [T, _iptr, C.c_int, C.c_int, _iptr, C.c_int, C.c_int, C.c_float, C.c_float, _u64p, _iptr]
+    L.calm_b200_decode_lookup_sample.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -121,6 +127,12 @@ def tp_unique_id() -> bytes:
     buf = C.create_string_buffer(128)
     load().calm_b200_tp_unique_id(buf)
     return buf.raw
+
+
+def _check_rng(rng_state):
+    """A generator state the C calls can take (a NULL state would abort the process)."""
+    if not isinstance(rng_state, (int, np.integer)) or not 0 <= rng_state < 1 << 64:
+        raise ValueError(f"rng_state must be an unsigned 64-bit integer, got {rng_state!r}")
 
 
 class DeviceModel:
@@ -296,37 +308,82 @@ class DeviceModel:
         self.lib.calm_b200_decode_greedy(C.byref(self.transformer), token0, pos0, n, out.ctypes.data_as(C.POINTER(C.c_int)))
         return out
 
+    @staticmethod
+    def _verify_block(tokens, who):
+        """The verify calls' tokens as int32, or ValueError for a bad length."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        if arr.ndim != 1 or not 1 <= len(arr) <= VERIFY_MAX:
+            raise ValueError(f"{who} takes 1 to {VERIFY_MAX} tokens, got {arr.shape}")
+        return arr
+
     def verify_greedy(self, tokens, pos0: int):
         """calm_b200_verify_greedy: feed tokens (1 .. VERIFY_MAX of them) at pos0 .. and return (greedy int32[n], served):
         greedy[i] is the argmax of the logits after tokens[i], served is 1 on the short-block path or 0 when n
         forward_argmax calls gave them.  Raises ValueError for a bad length."""
-        arr = np.ascontiguousarray(tokens, np.int32)
-        if arr.ndim != 1 or not 1 <= len(arr) <= VERIFY_MAX:
-            raise ValueError(f"verify_greedy takes 1 to {VERIFY_MAX} tokens, got {arr.shape}")
+        arr = self._verify_block(tokens, "verify_greedy")
         greedy = np.full(len(arr), -1, np.int32)
         ip = C.POINTER(C.c_int)
         served = self.lib.calm_b200_verify_greedy(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), pos0, greedy.ctypes.data_as(ip))
         return greedy, served
+
+    def verify_sample(self, tokens, pos0: int, temperature: float, minp: float, rng_state: int):
+        """calm_b200_verify_sample: feed tokens (1 .. VERIFY_MAX of them) at pos0 .. and return (sampled int32[n], new rng
+        state, served): sampled[i] is the reference sampler's draw on the logits after tokens[i] with the (i + 1)-th coin of
+        rng_state, and the new state is rng_state advanced by the draws the caller emits (the accepted drafts plus one).
+        served is 1 on the short-block path or 0 when forward_sample calls gave them.  Raises ValueError for a bad length or
+        rng_state."""
+        if tokens is None:
+            raise ValueError("verify_sample needs tokens")
+        arr = self._verify_block(tokens, "verify_sample")
+        _check_rng(rng_state)
+        sampled = np.full(len(arr), -1, np.int32)
+        ip = C.POINTER(C.c_int)
+        rng = C.c_ulonglong(rng_state)
+        served = self.lib.calm_b200_verify_sample(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), pos0, temperature, minp, C.byref(rng),
+                                                  sampled.ctypes.data_as(ip))
+        return sampled, int(rng.value), served
+
+    @staticmethod
+    def _lookup_args(tokens, n_tokens, source, max_draft, who):
+        """The lookup calls' (tokens, out, source) arrays, or ValueError for an empty `tokens`, a negative n_tokens or
+        max_draft outside [1, VERIFY_MAX - 1]."""
+        arr = np.ascontiguousarray(tokens, np.int32)
+        if arr.ndim != 1 or len(arr) < 1:
+            raise ValueError(f"{who} needs at least one token")
+        if not isinstance(n_tokens, (int, np.integer)) or n_tokens < 0:
+            raise ValueError(f"n_tokens must be a non-negative integer, got {n_tokens!r}")
+        if not isinstance(max_draft, (int, np.integer)) or not 1 <= max_draft < VERIFY_MAX:
+            raise ValueError(f"max_draft must be an integer in [1, {VERIFY_MAX - 1}], got {max_draft!r}")
+        src = None if source is None else np.ascontiguousarray(source, np.int32)
+        return arr, np.full(int(n_tokens), -1, np.int32), src
 
     def decode_lookup(self, tokens, n_tokens: int, source=None, max_draft: int = 7):
         """calm_b200_decode_lookup: greedy decoding with prompt-lookup drafts after `tokens` (the cache holds all but the
         last).  The drafts come from `source`, or from tokens ++ emitted when it is None.  Returns (int32[n_tokens],
         model steps run).  Raises ValueError for an empty `tokens`, a negative n_tokens or max_draft outside
         [1, VERIFY_MAX - 1]."""
-        arr = np.ascontiguousarray(tokens, np.int32)
-        if arr.ndim != 1 or len(arr) < 1:
-            raise ValueError("decode_lookup needs at least one token")
-        if not isinstance(n_tokens, (int, np.integer)) or n_tokens < 0:
-            raise ValueError(f"n_tokens must be a non-negative integer, got {n_tokens!r}")
-        if not isinstance(max_draft, (int, np.integer)) or not 1 <= max_draft < VERIFY_MAX:
-            raise ValueError(f"max_draft must be an integer in [1, {VERIFY_MAX - 1}], got {max_draft!r}")
+        arr, out, src = self._lookup_args(tokens, n_tokens, source, max_draft, "decode_lookup")
         ip = C.POINTER(C.c_int)
-        out = np.full(int(n_tokens), -1, np.int32)
-        src = None if source is None else np.ascontiguousarray(source, np.int32)
         steps = self.lib.calm_b200_decode_lookup(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), int(n_tokens),
                                                  None if src is None else src.ctypes.data_as(ip), 0 if src is None else len(src), int(max_draft),
                                                  out.ctypes.data_as(ip))
         return out, steps
+
+    def decode_lookup_sample(self, tokens, n_tokens: int, temperature: float, minp: float, rng_state: int, source=None, max_draft: int = 7):
+        """calm_b200_decode_lookup_sample: decode_lookup's loop with temperature / min-p sampling, each draft accepted
+        exactly when the sampled token equals it.  Returns (int32[n_tokens], model steps run, new rng state); the state is
+        where decode_sample of the same tokens leaves it.  Raises ValueError where decode_lookup does, and for a bad
+        rng_state."""
+        if tokens is None:
+            raise ValueError("decode_lookup_sample needs at least one token")
+        arr, out, src = self._lookup_args(tokens, n_tokens, source, max_draft, "decode_lookup_sample")
+        _check_rng(rng_state)
+        ip = C.POINTER(C.c_int)
+        rng = C.c_ulonglong(rng_state)
+        steps = self.lib.calm_b200_decode_lookup_sample(C.byref(self.transformer), arr.ctypes.data_as(ip), len(arr), int(n_tokens),
+                                                        None if src is None else src.ctypes.data_as(ip), 0 if src is None else len(src), int(max_draft),
+                                                        temperature, minp, C.byref(rng), out.ctypes.data_as(ip))
+        return out, steps, int(rng.value)
 
     def decode_sample(self, token0: int, pos0: int, n: int, temperature: float, minp: float, rng_state: int):
         """Device-resident temperature / min-p sampling; returns (tokens, new rng state)."""

@@ -220,6 +220,30 @@ int calm_b200_verify_greedy(struct Transformer* transformer, const int* tokens, 
 int calm_b200_decode_lookup(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source, int n_source,
                             int max_draft, int* out_tokens);
 
+/* Verify draft tokens by sampling (speculative sampling for deterministic drafts, DESIGN.md s.6).  Feeds tokens[0 .. n)
+ * at pos0 .. pos0 + n - 1 and writes their cache slots, as calm_b200_verify_greedy does, and sets sampled[i] to the
+ * reference's sample() (sampler.c:80-90) of the logits after tokens[i], drawn with the (i + 1)-th coin of *rng_state's
+ * xorshift* generator (the coin calm_b200_decode_sample would use there).  With a accepted drafts -- the longest prefix
+ * with sampled[i] == tokens[i + 1], i < n - 1 -- the caller emits sampled[0 .. a], and *rng_state is left advanced by
+ * a + 1 draws, as a + 1 calls of calm_b200_forward_sample leave it.  Accepting a draft exactly when the target's own
+ * sample equals it gives the target's distribution.  Returns 1 on the short-block path.  temperature == 0 or minp >= 1
+ * is calm_b200_verify_greedy and leaves the generator alone, as sample() does.  The shapes and blocks verify_greedy does
+ * not serve run n calm_b200_forward_sample calls on a copy of the state instead, with exactly their tokens, and return 0.
+ * 1 <= n <= CALM_B200_VERIFY_MAX and no array NULL, or the call aborts before any device work.  The first call allocates
+ * the logit rows and per-row sampler lists: 16 x vocab_size x 4 bytes and 16 x ceil(vocab_size / 1024) x 8 KB (8.2 MB
+ * and 16.5 MB at a 128256-token vocabulary). */
+int calm_b200_verify_sample(struct Transformer* transformer, const int* tokens, int n, int pos0, float temperature, float minp,
+                            unsigned long long* rng_state, int* sampled);
+
+/* calm_b200_decode_lookup's loop, draft rule, caps and end-of-cache handling with sampled tokens: a step with drafts is
+ * one calm_b200_verify_sample, a step without is one calm_b200_forward_sample.  Writes n_tokens tokens, returns the model
+ * steps, and leaves *rng_state where calm_b200_decode_sample of the same tokens leaves it: a run that never finds a
+ * draft is calm_b200_decode_sample, bit for bit.  temperature == 0 or minp >= 1 is calm_b200_decode_lookup, and
+ * rng_state must not be NULL. */
+int calm_b200_decode_lookup_sample(struct Transformer* transformer, const int* tokens, int n, int n_tokens, const int* source,
+                                   int n_source, int max_draft, float temperature, float minp, unsigned long long* rng_state,
+                                   int* out_tokens);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
@@ -262,11 +286,14 @@ void calm_b200_read_kv(struct Transformer* transformer, int layer, int kv_pos, f
  *   KEYS, VALUES  float[n_kv_heads][seq_len][head_dim]   one layer of the cache, every slot, decoded from fp16 / e5m2
  *   PF_X, PF_Q, PF_ATT, PF_HB   float[rows][dim | q_dim | q_dim | hidden]   the prompt pass's residual stream, rotated
  *            queries, attention output and FFN hidden matrix (the last two kept as f16 hi + lo pairs, summed here in
- *            float); rows = the pass's token tiles (a multiple of 128, at least n), of the last block of <= 2048 tokens */
+ *            float); rows = the pass's token tiles (a multiple of 128, at least n), of the last block of <= 2048 tokens
+ *   PF_LOGITS  float[n][vocab]          the logit rows of the last calm_b200_verify_sample block that took the short-block
+ *            path (n of its tokens), the values its sampler drew from */
 enum {
 	CALM_B200_STATE_X = 0, CALM_B200_STATE_XB = 1, CALM_B200_STATE_Q = 2, CALM_B200_STATE_ATT = 3, CALM_B200_STATE_HB = 4,
 	CALM_B200_STATE_MOE_SEL = 5, CALM_B200_STATE_KEYS = 6, CALM_B200_STATE_VALUES = 7,
-	CALM_B200_STATE_PF_X = 8, CALM_B200_STATE_PF_Q = 9, CALM_B200_STATE_PF_ATT = 10, CALM_B200_STATE_PF_HB = 11
+	CALM_B200_STATE_PF_X = 8, CALM_B200_STATE_PF_Q = 9, CALM_B200_STATE_PF_ATT = 10, CALM_B200_STATE_PF_HB = 11,
+	CALM_B200_STATE_PF_LOGITS = 12
 };
 int calm_b200_read_state(int which, int layer, float* out, int cap);
 
