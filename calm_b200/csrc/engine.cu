@@ -21,6 +21,7 @@
 #include "ring.cuh"
 #include "prefill.cuh"
 #include "verify.cuh"
+#include "sample_n.cuh"
 
 namespace {
 
@@ -173,6 +174,12 @@ struct Prefill {
 	SampleState* vstate = nullptr; // [VF_TOK]
 	int* vsampled = nullptr;       // [VF_TOK]
 	int vrows = 0;                 // rows of the last sampled block (CALM_B200_STATE_PF_LOGITS)
+	// n samples of one prompt (calm_b200_decode_sample_n), allocated on its first call: the attention's chunk partials
+	// (regrown when a call needs more chunks), the RoPE position of every row of the call and the tokens of every step
+	float* snpart = nullptr; // [VF_TOK][n_heads][snchunks][head_dim + 2]
+	int snchunks = 0;
+	int* snpos = nullptr;    // [seq_len]: step j's rows at [j * nseq, (j + 1) * nseq)
+	int* sntok = nullptr;    // [seq_len]: step j's tokens at [j * nseq, (j + 1) * nseq)
 };
 Prefill pf;
 
@@ -184,6 +191,7 @@ void pf_free() {
 	cudaFree(pf.topv), cudaFree(pf.topi), cudaFree(pf.top_ids), cudaFree(pf.top_lp);
 	cudaFree(pf.vacc), cudaFree(pf.vcnt);
 	cudaFree(pf.vlogits), cudaFree(pf.vtmax), cudaFree(pf.vsidx), cudaFree(pf.vsprob), cudaFree(pf.vcsum), cudaFree(pf.vcount), cudaFree(pf.vstate), cudaFree(pf.vsampled);
+	cudaFree(pf.snpart), cudaFree(pf.snpos), cudaFree(pf.sntok);
 	pf = Prefill();
 }
 
@@ -1251,6 +1259,8 @@ static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int
 enum PfRows {
 	PF_ONE,      // one sequence at cache slots pos0 + t
 	PF_SHORT,    // PF_ONE of at most VF_TOK rows (calm_b200_verify_greedy), whose GEMMs run on k_vf_gemm
+	PF_SAMPLES,  // a step of calm_b200_decode_sample_n (PfSampleStep): PF_SHORT's GEMMs, per-row RoPE positions from
+	             // pf.snpos and the shared-prompt attention of sample_n.cuh
 	PF_PACKED,   // a packed block of the scoring calls (pos0 = 0) that holds no context: per-row RoPE positions in pf.rowpos,
 	             // each row's sequence start in pf.seg
 	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block: each row's context in pf.ctx
@@ -1260,19 +1270,42 @@ enum PfRows {
 // (hi, lo) behind the tensor maps tm: on k_vf_gemm for a short block, on k_pf_gemm for any other
 template <int MODE, int DBITS, typename KVT>
 static void pf_layer_gemm(PfRows layout, const CUtensorMap* tm, const __half* hi, const __half* lo, const PfGemmArgs& a, int rows) {
-	if (layout == PF_SHORT) vf_gemm<MODE, DBITS, KVT>(hi, lo, a, rows / VF_ROWS);
+	if (layout == PF_SHORT || layout == PF_SAMPLES) vf_gemm<MODE, DBITS, KVT>(hi, lo, a, rows / VF_ROWS);
 	else pf_gemm<MODE, DBITS, KVT>(tm, a, rows, a.n_tokens);
 }
 
-// The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says.
+// A step of calm_b200_decode_sample_n: its n = nseq rows are the sequences, all at RoPE position pos0 + step, row b in
+// cache slot pos0 + step * nseq + b; the prompt is in slots [0, pos0)
+struct PfSampleStep {
+	int pos0, step, nseq;
+};
+
+// The shared-prompt attention of a PF_SAMPLES step (sample_n.cuh): chunk partials, then their fold into pf.Ahi / pf.Alo
+template <typename KVT, int HD>
+static void sn_attn(const SnAttnArgs& a) {
+	const int nkeys = a.pos0 + a.step + 1, npre = a.pos0 / SN_CHUNK, nsuf = cdiv(nkeys, SN_CHUNK) - npre;
+	const dim3 grid(npre + a.nseq * nsuf, g.cfg.n_kv_heads);
+	auto run = [&](auto kernel, size_t smem) {
+		smem_optin(kernel, smem);
+		launch_pdl(kernel, grid, SN_WARPS * 32, smem, a);
+	};
+	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4>, sn_smem_bytes<KVT, HD, 4>());
+	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2>, sn_smem_bytes<KVT, HD, 2>());
+	else run(k_sn_attn<KVT, HD, 1>, sn_smem_bytes<KVT, HD, 1>());
+	launch_pdl(k_sn_fold<HD>, dim3(cdiv(g.cfg.n_heads, SN_WARPS), a.nseq), SN_WARPS * 32, 0, a);
+}
+
+// The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says (PF_SAMPLES: the step `ss`,
+// whose slot base pos0 is ss->pos0 + ss->step * n).
 template <int DBITS, typename KVT>
-static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout) {
+static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const PfSampleStep* ss = nullptr) {
 	const bool packed = layout == PF_PACKED || layout == PF_CONTEXTS;
 	const Config& c = g.cfg;
 	const Weights& w = g.w;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
 	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
-	if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
+	if (layout == PF_SAMPLES) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.snpos + (size_t)ss->step * n, n, c.head_dim / 2);
+	else if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
 	else launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
 	for (int l = 0; l < c.n_layers; ++l) {
 		launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)w.rms_att_weight[l], pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
@@ -1288,7 +1321,14 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout) {
 		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
 		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
 		aa.seg = pf.seg, aa.ctx = pf.ctx;
-		if (layout == PF_CONTEXTS) {
+		if (layout == PF_SAMPLES) {
+			SnAttnArgs sa = {};
+			sa.Q = pf.Q, sa.kc = a.kc, sa.vc = a.vc, sa.part = pf.snpart, sa.Ohi = pf.Ahi, sa.Olo = pf.Alo;
+			sa.pos0 = ss->pos0, sa.step = ss->step, sa.nseq = ss->nseq, sa.seq_len = c.seq_len, sa.q_dim = g.q_dim, sa.kv_mul = g.kv_mul;
+			sa.n_heads = c.n_heads, sa.nchmax = pf.snchunks, sa.inv_sqrt_hd = aa.inv_sqrt_hd;
+			if (c.head_dim == 128) sn_attn<KVT, 128>(sa);
+			else sn_attn<KVT, 64>(sa);
+		} else if (layout == PF_CONTEXTS) {
 			if (c.head_dim == 128) pf_attn<KVT, 128, true, true>(aa, n);
 			else pf_attn<KVT, 64, true, true>(aa, n);
 		} else if (packed) {
@@ -1396,7 +1436,7 @@ static void pf_score(Formats<DBITS, KVT>, int n, PfRows layout, bool greedy, int
 	if (k) {
 		a.topv = pf.topv, a.topi = pf.topi, a.topk = k;
 		pf_gemm<PF_CLS_TOPK, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-	} else if (greedy && layout == PF_SHORT) {
+	} else if (greedy && (layout == PF_SHORT || layout == PF_SAMPLES)) {
 		for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) {
 			if (sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
 			else vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
@@ -1720,14 +1760,14 @@ static void vf_sample_reserve() {
 
 // The n rows of the last PF_CLS_SAMPLE classifier through the decode's sampler, side by side: row i is k_sample_scan +
 // k_sample_pick on its own lists and its own SampleState pf.vstate[i] (k_sample_scan_rows / k_sample_pick_rows), and its
-// token goes to pf.vsampled[i]
-static void vf_sample_rows(int n) {
+// token goes to out[i] (default pf.vsampled[i])
+static void vf_sample_rows(int n, int* out = nullptr) {
 	const int vocab = g.cfg.vocab_size, nvt = cdiv(vocab, PF_BM), nch = g.sample_chunks;
 	SampleArgs sa;
 	sa.logits = pf.vlogits, sa.cand_val = pf.vtmax, sa.ncand = nvt, sa.vocab = vocab, sa.nchunks = nch;
 	sa.st = pf.vstate, sa.count = pf.vcount, sa.csum = pf.vcsum, sa.sidx = pf.vsidx, sa.sprob = pf.vsprob;
 	launch_pdl(k_sample_scan_rows, dim3(nch, n), 256, 0, sa);
-	launch_pdl(k_sample_pick_rows, n, 256, 0, sa, pf.vstate, pf.vsampled);
+	launch_pdl(k_sample_pick_rows, n, 256, 0, sa, pf.vstate, out ? out : pf.vsampled);
 }
 
 extern "C" int calm_b200_verify_sample(struct Transformer* transformer, const int* tokens, int n, int pos0, float temperature, float minp,
@@ -1852,6 +1892,81 @@ extern "C" int calm_b200_decode_lookup_sample(struct Transformer* transformer, c
 	    transformer, tokens, n, n_tokens, source, n_source, max_draft, out_tokens,
 	    [&](int cur, int pos) { return calm_b200_forward_sample(transformer, cur, pos, temperature, minp, rng_state); },
 	    [&](const int* block, int m, int pos, int* out) { calm_b200_verify_sample(transformer, block, m, pos, temperature, minp, rng_state, out); });
+}
+
+// ---------------------------------------------------------------------------------------------
+// calm_b200_decode_sample_n: nseq continuations of one prompt, one short block per step whose rows are the sequences
+// (PF_SAMPLES), with the prompt's keys read once per step for all of them (sample_n.cuh).
+
+static_assert(CALM_B200_SAMPLE_N_MAX == VF_TOK, "the sequences of a step are one token tile of k_vf_gemm");
+
+// the chunk partials for `chunks` chunks per query (kept when large enough), the positions and the step tokens
+static void sn_reserve(int chunks) {
+	const Config& c = g.cfg;
+	if (!pf.snpos) {
+		pf.snpos = (int*)dev_alloc((size_t)c.seq_len * sizeof(int));
+		pf.sntok = (int*)dev_alloc((size_t)c.seq_len * sizeof(int));
+	}
+	if (chunks <= pf.snchunks) return;
+	if (pf.snpart) {
+		CUDA_CHECK(cudaStreamSynchronize(g.stream));
+		cudaFree(pf.snpart);
+	}
+	pf.snchunks = chunks;
+	pf.snpart = (float*)dev_alloc((size_t)VF_TOK * c.n_heads * chunks * (c.head_dim + 2) * sizeof(float));
+}
+
+extern "C" int calm_b200_decode_sample_n(struct Transformer* transformer, int token0, int pos0, int n_tokens, int nseq, float temperature, float minp,
+                                         unsigned long long* rng_states, int* out_tokens) {
+	if (!g.ready) CALM_FATAL("decode_sample_n before prepare_cuda");
+	if (nseq < 1 || nseq > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("decode_sample_n: nseq %d outside [1, %d]", nseq, CALM_B200_SAMPLE_N_MAX);
+	if (n_tokens < 0) CALM_FATAL("decode_sample_n: negative n_tokens %d", n_tokens);
+	if (n_tokens > 0 && (!rng_states || !out_tokens)) CALM_FATAL("decode_sample_n: rng_states or out_tokens is NULL");
+	check_call(transformer, token0, pos0);
+	if (n_tokens == 0) return 1;
+	if (!pf_supported() || (long long)pos0 + (long long)nseq * n_tokens > g.cfg.seq_len) {
+		for (int b = 0; b < nseq; ++b) calm_b200_decode_sample(transformer, token0, pos0, n_tokens, temperature, minp, &rng_states[b], out_tokens + (size_t)b * n_tokens);
+		return 0;
+	}
+	const bool greedy = temperature == 0.0f || minp >= 1.0f; // sample() is greedy there and leaves the generator alone
+	pf_reserve(nseq);
+	pf_score_reserve(true, false);
+	vf_reserve();
+	vf_sample_reserve();
+	sn_reserve(cdiv(pos0 + n_tokens, SN_CHUNK));
+	const size_t rows = (size_t)n_tokens * nseq;
+	std::vector<int> pos(rows), tok(nseq, token0);
+	for (size_t r = 0; r < rows; ++r) pos[r] = pos0 + (int)(r / nseq);
+	CUDA_CHECK(cudaMemcpyAsync(pf.snpos, pos.data(), rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tok.data(), nseq * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	SampleState st[CALM_B200_SAMPLE_N_MAX];
+	if (!greedy) {
+		for (int b = 0; b < nseq; ++b) st[b].rng = rng_states[b], st[b].temperature = temperature, st[b].cut_delta = logf(minp) * temperature;
+		CUDA_CHECK(cudaMemcpyAsync(pf.vstate, st, nseq * sizeof(SampleState), cudaMemcpyHostToDevice, g.stream));
+	}
+	for (int j = 0; j < n_tokens; ++j) {
+		const PfSampleStep ss = {pos0, j, nseq};
+		int* out = pf.sntok + (size_t)j * nseq;
+		with_formats([&](auto f) {
+			pf_run(f, nseq, pos0 + j * nseq, PF_SAMPLES, &ss);
+			pf_score(f, nseq, PF_SAMPLES, true, 0, !greedy);
+		});
+		if (greedy) CUDA_CHECK(cudaMemcpyAsync(out, pf.greedy, nseq * sizeof(int), cudaMemcpyDeviceToDevice, g.stream));
+		else vf_sample_rows(nseq, out);
+		if (j + 1 < n_tokens) CUDA_CHECK(cudaMemcpyAsync(pf.tokens, out, nseq * sizeof(int), cudaMemcpyDeviceToDevice, g.stream));
+	}
+	std::vector<int> all(rows);
+	CUDA_CHECK(cudaMemcpyAsync(all.data(), pf.sntok, rows * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+	if (!greedy) CUDA_CHECK(cudaMemcpyAsync(st, pf.vstate, nseq * sizeof(SampleState), cudaMemcpyDeviceToHost, g.stream));
+	sync_stream();
+	CUDA_CHECK(cudaGetLastError());
+	for (int b = 0; b < nseq; ++b)
+		for (int i = 0; i < n_tokens; ++i) out_tokens[(size_t)b * n_tokens + i] = all[(size_t)i * nseq + b];
+	if (!greedy) {
+		for (int b = 0; b < nseq; ++b) rng_states[b] = st[b].rng;
+		pf.vrows = nseq;
+	}
+	return 1;
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -2011,6 +2126,9 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		const size_t nch = g.sample_chunks;
 		nan(pf.vlogits, VF_TOK * (size_t)c.vocab_size * sizeof(float)), nan(pf.vtmax, VF_TOK * (size_t)cdiv(c.vocab_size, PF_BM) * sizeof(float));
 		nan(pf.vsprob, VF_TOK * nch * SAMPLE_CHUNK * sizeof(float)), nan(pf.vcsum, VF_TOK * nch * sizeof(float)), nan(pf.vsampled, VF_TOK * sizeof(int));
+		// decode_sample_n's chunk partials and step tokens, which every call writes before it reads them (its positions,
+		// read as RoPE positions, are an index buffer)
+		nan(pf.snpart, (size_t)VF_TOK * c.n_heads * pf.snchunks * (c.head_dim + 2) * sizeof(float)), nan(pf.sntok, (size_t)c.seq_len * sizeof(int));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

@@ -1,0 +1,185 @@
+// sample_n.cuh -- the attention of calm_b200_decode_sample_n: nseq sequences that continue one shared prompt, one token
+// each per step, through the short-block pass (verify.cuh's k_vf_gemm for the projections and the classifier).
+//
+// Cache layout.  The prompt is in slots [0, pos0).  At step j every row b (one per sequence) is at RoPE position pos0 + j
+// and writes slot pos0 + j * nseq + b, so a step is an ordinary short block at slot base pos0 + j * nseq and the QKV
+// epilogue appends its keys unchanged.  Row b's keys at step j, in order, are the prompt's slots 0 .. pos0 - 1 and then
+// its own slots pos0 + i * nseq + b for i = 0 .. j: its virtual key index v = 0 .. pos0 + j.
+//
+//   k_sn_attn   split-KV, multi-query attention over fixed chunks of SN_CHUNK virtual keys.  A chunk wholly inside the
+//               prompt holds the same keys for every row, so one CTA per (kv head, chunk) stages its K and V tiles in
+//               shared memory once and computes a partial (m, l, acc[HD]) for every row and query head of the kv head.
+//               A chunk that reaches past the prompt is computed per row, over that row's own virtual keys.  fp32 math
+//               on the fp16 / e5m2 cache entries, as k_pf_attn.  A warp takes KM query heads of one row at a time; its
+//               lanes own the chunk's keys lane + 32 i for the scores and head dims for the values.
+//   k_sn_fold   one warp per (row, query head): the row's chunk partials folded in ascending chunk order against their
+//               common maximum, written as the f16 hi + lo pair that wo's k_vf_gemm reads.
+//
+// A row's output depends on its query, its keys and the chunking only, never on how many rows run beside it: which chunks
+// are shared depends on pos0 and j alone, a query's arithmetic does not depend on the warp that runs it, and nothing is
+// added with atomics.
+#pragma once
+
+#include "prefill.cuh"
+
+#define SN_CHUNK 128 // virtual keys per chunk: four per lane in the score pass
+#define SN_WARPS 8
+
+struct SnAttnArgs {
+	const float* Q;  // [nseq][q_dim] the step's rotated queries
+	const void* kc;  // this layer
+	const void* vc;
+	float* part;     // [nseq][n_heads][nchmax][HD + 2] per chunk: m, l, acc[HD]
+	__half* Ohi;     // [nseq][q_dim]
+	__half* Olo;
+	int pos0, step, nseq, seq_len, q_dim, kv_mul, n_heads, nchmax;
+	float inv_sqrt_hd;
+};
+
+// dynamic shared memory of k_sn_attn: the K tile (padded rows), the V tile, each warp's KM queries
+template <typename KVT, int HD, int KM>
+constexpr size_t sn_smem_bytes() {
+	return (size_t)SN_CHUNK * (HD * sizeof(KVT) + 16) + (size_t)SN_CHUNK * HD * sizeof(KVT) + (size_t)SN_WARPS * KM * HD * sizeof(float);
+}
+
+// grid (prompt chunks + nseq x suffix chunks, kv heads): CTA x < pos0 / SN_CHUNK is prompt chunk x for every row, the
+// others are suffix chunk x' % nsuf of row x' / nsuf (x' = x - prompt chunks)
+template <typename KVT, int HD, int KM>
+__global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
+	pdl_enter();
+	constexpr int DPL = HD / 32, KPL = SN_CHUNK / 32;
+	constexpr int VSTR = HD * sizeof(KVT), KSTR = VSTR + 16; // padded key row, as k_pf_attn's
+	extern __shared__ __align__(16) unsigned char sn_smem[];
+	unsigned char* ks = sn_smem;
+	unsigned char* vs = ks + SN_CHUNK * KSTR;
+	float* qs = reinterpret_cast<float*>(vs + SN_CHUNK * VSTR) + (threadIdx.x >> 5) * KM * HD;
+	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, kvh = blockIdx.y;
+	const int nkeys = a.pos0 + a.step + 1, npre = a.pos0 / SN_CHUNK, nsuf = (nkeys + SN_CHUNK - 1) / SN_CHUNK - npre;
+	int c = blockIdx.x, b0 = 0, nrows = a.nseq;
+	if (c >= npre) {
+		const int x = c - npre;
+		b0 = x / nsuf, c = npre + x % nsuf, nrows = 1;
+	}
+	const int v0 = c * SN_CHUNK, nk = min(SN_CHUNK, nkeys - v0);
+	const KVT* kbase = reinterpret_cast<const KVT*>(a.kc) + (size_t)kvh * a.seq_len * HD;
+	const KVT* vbase = reinterpret_cast<const KVT*>(a.vc) + (size_t)kvh * a.seq_len * HD;
+	for (int i = threadIdx.x; i < SN_CHUNK * (VSTR / 16); i += blockDim.x) {
+		const int row = i / (VSTR / 16), cc = i % (VSTR / 16), v = v0 + row;
+		const bool in = row < nk;
+		const int slot = v < a.pos0 ? v : a.pos0 + (v - a.pos0) * a.nseq + b0;
+		const uint4 z = make_uint4(0, 0, 0, 0);
+		*reinterpret_cast<uint4*>(ks + row * KSTR + cc * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(kbase + (size_t)slot * HD) + cc) : z;
+		*reinterpret_cast<uint4*>(vs + row * VSTR + cc * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(vbase + (size_t)slot * HD) + cc) : z;
+	}
+	__syncthreads();
+
+	const int groups = nrows * a.kv_mul / KM;
+	for (int gq = warp; gq < groups; gq += SN_WARPS) {
+		const int b = b0 + gq * KM / a.kv_mul, h0 = kvh * a.kv_mul + gq * KM % a.kv_mul;
+		__syncwarp(); // the previous group's queries are no longer being read
+		for (int i = lane; i < KM * HD; i += 32) qs[i] = a.Q[(size_t)b * a.q_dim + (size_t)h0 * HD + i];
+		__syncwarp();
+		// scores of keys lane + 32 i against the KM heads
+		float sc[KM][KPL];
+#pragma unroll
+		for (int h = 0; h < KM; ++h)
+#pragma unroll
+			for (int i = 0; i < KPL; ++i) sc[h][i] = 0.f;
+#pragma unroll 2
+		for (int c8 = 0; c8 < HD / 8; ++c8) {
+			float4 q[KM][2];
+#pragma unroll
+			for (int h = 0; h < KM; ++h) q[h][0] = *reinterpret_cast<const float4*>(qs + h * HD + c8 * 8), q[h][1] = *reinterpret_cast<const float4*>(qs + h * HD + c8 * 8 + 4);
+#pragma unroll
+			for (int i = 0; i < KPL; ++i) {
+				float kf[8];
+				kv_load8(reinterpret_cast<const KVT*>(ks + (lane + 32 * i) * KSTR) + c8 * 8, kf);
+#pragma unroll
+				for (int h = 0; h < KM; ++h) {
+					float s = sc[h][i];
+					s = fmaf(q[h][0].x, kf[0], s), s = fmaf(q[h][0].y, kf[1], s), s = fmaf(q[h][0].z, kf[2], s), s = fmaf(q[h][0].w, kf[3], s);
+					s = fmaf(q[h][1].x, kf[4], s), s = fmaf(q[h][1].y, kf[5], s), s = fmaf(q[h][1].z, kf[6], s), s = fmaf(q[h][1].w, kf[7], s);
+					sc[h][i] = s;
+				}
+			}
+		}
+		// the chunk's softmax numerators against its own maximum, and their sum
+		float m[KM], l[KM];
+#pragma unroll
+		for (int h = 0; h < KM; ++h) {
+			float mx = -FLT_MAX;
+#pragma unroll
+			for (int i = 0; i < KPL; ++i) {
+				sc[h][i] = lane + 32 * i < nk ? sc[h][i] * a.inv_sqrt_hd : -FLT_MAX;
+				mx = fmaxf(mx, sc[h][i]);
+			}
+			mx = warp_max(mx);
+			float s = 0.f;
+#pragma unroll
+			for (int i = 0; i < KPL; ++i) {
+				sc[h][i] = lane + 32 * i < nk ? expf(sc[h][i] - mx) : 0.f;
+				s += sc[h][i];
+			}
+			m[h] = mx, l[h] = warp_sum(s);
+		}
+		// values: lane owns head dims [lane * DPL, lane * DPL + DPL), keys in ascending order
+		float acc[KM][DPL];
+#pragma unroll
+		for (int h = 0; h < KM; ++h)
+#pragma unroll
+			for (int d = 0; d < DPL; ++d) acc[h][d] = 0.f;
+#pragma unroll
+		for (int i = 0; i < KPL; ++i) {
+			const int jn = min(32, nk - 32 * i);
+			for (int j = 0; j < jn; ++j) {
+				float vf[DPL];
+				pf_load_dims<DPL>(reinterpret_cast<const KVT*>(vs + (32 * i + j) * VSTR) + lane * DPL, vf);
+#pragma unroll
+				for (int h = 0; h < KM; ++h) {
+					const float pj = __shfl_sync(0xffffffffu, sc[h][i], j);
+#pragma unroll
+					for (int d = 0; d < DPL; ++d) acc[h][d] = fmaf(pj, vf[d], acc[h][d]);
+				}
+			}
+		}
+#pragma unroll
+		for (int h = 0; h < KM; ++h) {
+			float* o = a.part + (((size_t)b * a.n_heads + h0 + h) * a.nchmax + c) * (HD + 2);
+			if (lane == 0) o[0] = m[h], o[1] = l[h];
+#pragma unroll
+			for (int d = 0; d < DPL; ++d) o[2 + lane * DPL + d] = acc[h][d];
+		}
+	}
+}
+
+// grid (cdiv(n_heads, SN_WARPS), nseq): warp = query head, lane = head dims [lane * DPL, lane * DPL + DPL)
+template <int HD>
+__global__ void __launch_bounds__(SN_WARPS * 32) k_sn_fold(const SnAttnArgs a) {
+	pdl_enter();
+	constexpr int DPL = HD / 32;
+	const int lane = threadIdx.x & 31, h = blockIdx.x * SN_WARPS + (threadIdx.x >> 5), b = blockIdx.y;
+	if (h >= a.n_heads) return;
+	const int nch = (a.pos0 + a.step + SN_CHUNK) / SN_CHUNK;
+	const float* p = a.part + ((size_t)b * a.n_heads + h) * a.nchmax * (HD + 2);
+	float mx = -FLT_MAX;
+	for (int c = lane; c < nch; c += 32) mx = fmaxf(mx, __ldcg(p + (size_t)c * (HD + 2)));
+	mx = warp_max(mx);
+	float l = 0.f, acc[DPL];
+#pragma unroll
+	for (int d = 0; d < DPL; ++d) acc[d] = 0.f;
+	for (int c = 0; c < nch; ++c) {
+		const float* pc = p + (size_t)c * (HD + 2);
+		const float w = expf(__ldcg(pc) - mx);
+		l = fmaf(__ldcg(pc + 1), w, l);
+#pragma unroll
+		for (int d = 0; d < DPL; ++d) acc[d] = fmaf(__ldcg(pc + 2 + lane * DPL + d), w, acc[d]);
+	}
+	const float inv = 1.0f / l;
+#pragma unroll
+	for (int d = 0; d < DPL; ++d) {
+		__half hh, hl;
+		split_hl(acc[d] * inv, hh, hl);
+		const size_t o = (size_t)b * a.q_dim + (size_t)h * HD + lane * DPL + d;
+		a.Ohi[o] = hh, a.Olo[o] = hl;
+	}
+}

@@ -27,6 +27,7 @@ SYMBOLS = [
     "calm_b200_score_topk", "calm_b200_score_batch_topk", "calm_b200_score_context_topk",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
+    "calm_b200_decode_sample_n",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -39,6 +40,9 @@ TOPK_MAX = 20
 
 # the largest block calm_b200_verify_greedy takes (CALM_B200_VERIFY_MAX); decode_lookup drafts at most one fewer
 VERIFY_MAX = 16
+
+# the most sequences calm_b200_decode_sample_n samples together (CALM_B200_SAMPLE_N_MAX)
+SAMPLE_N_MAX = 16
 
 # calm_b200_read_state selectors (include/calm_b200.h)
 STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11, "pf_logits": 12}
@@ -92,6 +96,8 @@ def load() -> C.CDLL:
     L.calm_b200_verify_sample.restype = C.c_int
     L.calm_b200_decode_lookup_sample.argtypes = [T, _iptr, C.c_int, C.c_int, _iptr, C.c_int, C.c_int, C.c_float, C.c_float, _u64p, _iptr]
     L.calm_b200_decode_lookup_sample.restype = C.c_int
+    L.calm_b200_decode_sample_n.argtypes = [T, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, _u64p, _iptr]
+    L.calm_b200_decode_sample_n.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -391,6 +397,33 @@ class DeviceModel:
         rng = C.c_ulonglong(rng_state)
         self.lib.calm_b200_decode_sample(C.byref(self.transformer), token0, pos0, n, temperature, minp, C.byref(rng), out.ctypes.data_as(C.POINTER(C.c_int)))
         return out, int(rng.value)
+
+    def decode_sample_n(self, token0: int, pos0: int, n_tokens: int, temperature: float, minp: float, rng_states):
+        """calm_b200_decode_sample_n: len(rng_states) = nseq continuations of the prompt in cache slots [0, pos0), each
+        feeding token0 at pos0 and then its own samples, as decode_sample(token0, pos0, n_tokens, ..., rng_states[b])
+        would.  Returns (tokens int32[nseq, n_tokens], the nseq new generator states, served): served is 1 on the
+        shared-prompt path, 0 when nseq decode_sample runs gave them (shapes the prompt pass does not serve, or
+        pos0 + nseq * n_tokens > seq_len).  Raises ValueError for 0 or more than SAMPLE_N_MAX states, a bad state, a
+        negative n_tokens or pos0, or token0 outside the vocabulary."""
+        if rng_states is None or isinstance(rng_states, (int, np.integer)):
+            raise ValueError("decode_sample_n takes a sequence of generator states, one per sequence")
+        states = list(rng_states)
+        if not 1 <= len(states) <= SAMPLE_N_MAX:
+            raise ValueError(f"decode_sample_n samples 1 to {SAMPLE_N_MAX} sequences, got {len(states)} states")
+        for s in states:
+            _check_rng(s)
+        if not isinstance(n_tokens, (int, np.integer)) or n_tokens < 0:
+            raise ValueError(f"n_tokens must be a non-negative integer, got {n_tokens!r}")
+        if not isinstance(token0, (int, np.integer)) or not 0 <= token0 < self.vocab:
+            raise ValueError(f"token0 must be in [0, {self.vocab}), got {token0!r}")
+        if not isinstance(pos0, (int, np.integer)) or pos0 < 0:
+            raise ValueError(f"pos0 must be a non-negative integer, got {pos0!r}")
+        nseq = len(states)
+        rng = (C.c_ulonglong * nseq)(*[int(s) for s in states])
+        out = np.full((nseq, int(n_tokens)), -1, np.int32)
+        served = self.lib.calm_b200_decode_sample_n(C.byref(self.transformer), int(token0), int(pos0), int(n_tokens), nseq, temperature, minp, rng,
+                                                    out.ctypes.data_as(C.POINTER(C.c_int)))
+        return out, [int(s) for s in rng], served
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""

@@ -244,6 +244,25 @@ int calm_b200_decode_lookup_sample(struct Transformer* transformer, const int* t
                                    int n_source, int max_draft, float temperature, float minp, unsigned long long* rng_state,
                                    int* out_tokens);
 
+/* Sample nseq continuations of one prompt together: every step is one pass over the weights for all of them, and the
+ * prompt's cache entries are read once per step for all of them (DESIGN.md s.6).  The cache holds the prompt at
+ * positions [0, pos0).  Each sequence b feeds token0 at pos0 and then its own sample n_tokens - 1 times, exactly as
+ * calm_b200_decode_sample(t, token0, pos0, n_tokens, temperature, minp, &rng_states[b], ...) would, and
+ * out_tokens[b * n_tokens + i] is its sample after step i; rng_states[b] is left advanced by n_tokens draws.
+ * temperature == 0 or minp >= 1 makes every sequence the greedy stream and leaves the states alone, as sample() does.
+ * Returns 1 on the new path.  Step j writes sequence b's entries to cache slot pos0 + j * nseq + b, so the call needs
+ * pos0 + nseq * n_tokens <= seq_len; slots [0, pos0) stay bit for bit as they were and slots from pos0 on are scratch
+ * (to continue one sequence, feed its tokens again from pos0: INTEGRATION.md).  Shapes the prompt pass does not serve
+ * (as for calm_b200_verify_greedy) and calls past seq_len run calm_b200_decode_sample once per sequence, b = 0, 1, ..,
+ * each from token0 at pos0, with exactly their tokens and states, and return 0.  1 <= nseq <= CALM_B200_SAMPLE_N_MAX,
+ * n_tokens >= 0 and, for n_tokens > 0, neither array NULL, or the call aborts before any device work; n_tokens == 0
+ * does nothing and returns 1.  The first call allocates what calm_b200_verify_sample allocates, 8 bytes per cache
+ * position, and the attention's partials: 16 x n_heads x ceil((pos0 + n_tokens) / 128) x (head_dim + 2) x 4 bytes,
+ * regrown when a later call needs more (8.5 MB for Llama-3-8B at 4096 positions). */
+#define CALM_B200_SAMPLE_N_MAX 16 /* == VF_TOK, static_assert in engine.cu */
+int calm_b200_decode_sample_n(struct Transformer* transformer, int token0, int pos0, int n_tokens, int nseq, float temperature, float minp,
+                              unsigned long long* rng_states, int* out_tokens);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
@@ -288,7 +307,9 @@ void calm_b200_read_kv(struct Transformer* transformer, int layer, int kv_pos, f
  *            queries, attention output and FFN hidden matrix (the last two kept as f16 hi + lo pairs, summed here in
  *            float); rows = the pass's token tiles (a multiple of 128, at least n), of the last block of <= 2048 tokens
  *   PF_LOGITS  float[n][vocab]          the logit rows of the last calm_b200_verify_sample block that took the short-block
- *            path (n of its tokens), the values its sampler drew from */
+ *            path (n of its tokens), or of the last step of the last sampled calm_b200_decode_sample_n call that took
+ *            its new path (n = nseq, row b = sequence b), the values its sampler drew from
+ *   After calm_b200_decode_sample_n, the PF_* matrices hold its last step, row b = sequence b. */
 enum {
 	CALM_B200_STATE_X = 0, CALM_B200_STATE_XB = 1, CALM_B200_STATE_Q = 2, CALM_B200_STATE_ATT = 3, CALM_B200_STATE_HB = 4,
 	CALM_B200_STATE_MOE_SEL = 5, CALM_B200_STATE_KEYS = 6, CALM_B200_STATE_VALUES = 7,
