@@ -180,6 +180,9 @@ struct Prefill {
 	int snchunks = 0;
 	int* snpos = nullptr;    // [seq_len]: step j's rows at [j * nseq, (j + 1) * nseq)
 	int* sntok = nullptr;    // [seq_len]: step j's tokens at [j * nseq, (j + 1) * nseq)
+	// different prompts decoded together (calm_b200_decode_sample_batch), allocated on its first call: each row's prompt
+	// in the packed cache, its first slot and length (uploaded once per call)
+	int2* sbrows = nullptr; // [VF_TOK]
 };
 Prefill pf;
 
@@ -191,7 +194,7 @@ void pf_free() {
 	cudaFree(pf.topv), cudaFree(pf.topi), cudaFree(pf.top_ids), cudaFree(pf.top_lp);
 	cudaFree(pf.vacc), cudaFree(pf.vcnt);
 	cudaFree(pf.vlogits), cudaFree(pf.vtmax), cudaFree(pf.vsidx), cudaFree(pf.vsprob), cudaFree(pf.vcsum), cudaFree(pf.vcount), cudaFree(pf.vstate), cudaFree(pf.vsampled);
-	cudaFree(pf.snpart), cudaFree(pf.snpos), cudaFree(pf.sntok);
+	cudaFree(pf.snpart), cudaFree(pf.snpos), cudaFree(pf.sntok), cudaFree(pf.sbrows);
 	pf = Prefill();
 }
 
@@ -1261,42 +1264,51 @@ enum PfRows {
 	PF_SHORT,    // PF_ONE of at most VF_TOK rows (calm_b200_verify_greedy), whose GEMMs run on k_vf_gemm
 	PF_SAMPLES,  // a step of calm_b200_decode_sample_n (PfSampleStep): PF_SHORT's GEMMs, per-row RoPE positions from
 	             // pf.snpos and the shared-prompt attention of sample_n.cuh
-	PF_PACKED,   // a packed block of the scoring calls (pos0 = 0) that holds no context: per-row RoPE positions in pf.rowpos,
-	             // each row's sequence start in pf.seg
+	PF_BATCH,    // a step of calm_b200_decode_sample_batch (PfSampleStep): PF_SAMPLES, but every row continues its own prompt
+	             // (pf.sbrows) through sample_n.cuh's BATCH attention
+	PF_PACKED,   // a packed block that holds no context (the scoring calls at pos0 = 0, and decode_sample_batch's prompts at
+	             // any slot base): per-row RoPE positions in pf.rowpos, each row's sequence start (its cache slot) in pf.seg
 	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block: each row's context in pf.ctx
 };
+
+// a short block: at most VF_TOK rows whose GEMMs run on k_vf_gemm
+static bool pf_short(PfRows layout) {
+	return layout == PF_SHORT || layout == PF_SAMPLES || layout == PF_BATCH;
+}
 
 // A layer GEMM of the pass over `rows` output rows of `a` (UP: of w1 and of w3 each), whose activations are the f16 pair
 // (hi, lo) behind the tensor maps tm: on k_vf_gemm for a short block, on k_pf_gemm for any other
 template <int MODE, int DBITS, typename KVT>
 static void pf_layer_gemm(PfRows layout, const CUtensorMap* tm, const __half* hi, const __half* lo, const PfGemmArgs& a, int rows) {
-	if (layout == PF_SHORT || layout == PF_SAMPLES) vf_gemm<MODE, DBITS, KVT>(hi, lo, a, rows / VF_ROWS);
+	if (pf_short(layout)) vf_gemm<MODE, DBITS, KVT>(hi, lo, a, rows / VF_ROWS);
 	else pf_gemm<MODE, DBITS, KVT>(tm, a, rows, a.n_tokens);
 }
 
 // A step of calm_b200_decode_sample_n: its n = nseq rows are the sequences, all at RoPE position pos0 + step, row b in
-// cache slot pos0 + step * nseq + b; the prompt is in slots [0, pos0)
+// cache slot pos0 + step * nseq + b; the prompt is in slots [0, pos0).  A step of calm_b200_decode_sample_batch: the
+// same slots from pos0 = G, the end of the packed prompts, and row b at RoPE position L_b + step; lmax = max_b L_b.
 struct PfSampleStep {
-	int pos0, step, nseq;
+	int pos0, step, nseq, lmax;
 };
 
-// The shared-prompt attention of a PF_SAMPLES step (sample_n.cuh): chunk partials, then their fold into pf.Ahi / pf.Alo
-template <typename KVT, int HD>
-static void sn_attn(const SnAttnArgs& a) {
+// The attention of a PF_SAMPLES step (shared prompt) or, with BATCH, of a PF_BATCH step (a prompt per row) (sample_n.cuh):
+// chunk partials, then their fold into pf.Ahi / pf.Alo
+template <typename KVT, int HD, bool BATCH>
+static void sn_attn(const SnAttnArgs& a, int lmax) {
 	const int nkeys = a.pos0 + a.step + 1, npre = a.pos0 / SN_CHUNK, nsuf = cdiv(nkeys, SN_CHUNK) - npre;
-	const dim3 grid(npre + a.nseq * nsuf, g.cfg.n_kv_heads);
+	const dim3 grid(BATCH ? a.nseq * cdiv(lmax + a.step + 1, SN_CHUNK) : npre + a.nseq * nsuf, g.cfg.n_kv_heads);
 	auto run = [&](auto kernel, size_t smem) {
 		smem_optin(kernel, smem);
 		launch_pdl(kernel, grid, SN_WARPS * 32, smem, a);
 	};
-	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4>, sn_smem_bytes<KVT, HD, 4>());
-	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2>, sn_smem_bytes<KVT, HD, 2>());
-	else run(k_sn_attn<KVT, HD, 1>, sn_smem_bytes<KVT, HD, 1>());
-	launch_pdl(k_sn_fold<HD>, dim3(cdiv(g.cfg.n_heads, SN_WARPS), a.nseq), SN_WARPS * 32, 0, a);
+	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4, BATCH>, sn_smem_bytes<KVT, HD, 4>());
+	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2, BATCH>, sn_smem_bytes<KVT, HD, 2>());
+	else run(k_sn_attn<KVT, HD, 1, BATCH>, sn_smem_bytes<KVT, HD, 1>());
+	launch_pdl(k_sn_fold<HD, BATCH>, dim3(cdiv(g.cfg.n_heads, SN_WARPS), a.nseq), SN_WARPS * 32, 0, a);
 }
 
-// The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says (PF_SAMPLES: the step `ss`,
-// whose slot base pos0 is ss->pos0 + ss->step * n).
+// The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says (PF_SAMPLES and PF_BATCH: the
+// step `ss`, whose slot base pos0 is ss->pos0 + ss->step * n).
 template <int DBITS, typename KVT>
 static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const PfSampleStep* ss = nullptr) {
 	const bool packed = layout == PF_PACKED || layout == PF_CONTEXTS;
@@ -1304,7 +1316,7 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 	const Weights& w = g.w;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
 	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
-	if (layout == PF_SAMPLES) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.snpos + (size_t)ss->step * n, n, c.head_dim / 2);
+	if (layout == PF_SAMPLES || layout == PF_BATCH) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.snpos + (size_t)ss->step * n, n, c.head_dim / 2);
 	else if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
 	else launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
 	for (int l = 0; l < c.n_layers; ++l) {
@@ -1321,13 +1333,18 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
 		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
 		aa.seg = pf.seg, aa.ctx = pf.ctx;
-		if (layout == PF_SAMPLES) {
+		if (layout == PF_SAMPLES || layout == PF_BATCH) {
 			SnAttnArgs sa = {};
 			sa.Q = pf.Q, sa.kc = a.kc, sa.vc = a.vc, sa.part = pf.snpart, sa.Ohi = pf.Ahi, sa.Olo = pf.Alo;
 			sa.pos0 = ss->pos0, sa.step = ss->step, sa.nseq = ss->nseq, sa.seq_len = c.seq_len, sa.q_dim = g.q_dim, sa.kv_mul = g.kv_mul;
-			sa.n_heads = c.n_heads, sa.nchmax = pf.snchunks, sa.inv_sqrt_hd = aa.inv_sqrt_hd;
-			if (c.head_dim == 128) sn_attn<KVT, 128>(sa);
-			else sn_attn<KVT, 64>(sa);
+			sa.n_heads = c.n_heads, sa.nchmax = pf.snchunks, sa.inv_sqrt_hd = aa.inv_sqrt_hd, sa.rows = pf.sbrows;
+			if (layout == PF_BATCH) {
+				if (c.head_dim == 128) sn_attn<KVT, 128, true>(sa, ss->lmax);
+				else sn_attn<KVT, 64, true>(sa, ss->lmax);
+			} else {
+				if (c.head_dim == 128) sn_attn<KVT, 128, false>(sa, 0);
+				else sn_attn<KVT, 64, false>(sa, 0);
+			}
 		} else if (layout == PF_CONTEXTS) {
 			if (c.head_dim == 128) pf_attn<KVT, 128, true, true>(aa, n);
 			else pf_attn<KVT, 64, true, true>(aa, n);
@@ -1436,7 +1453,7 @@ static void pf_score(Formats<DBITS, KVT>, int n, PfRows layout, bool greedy, int
 	if (k) {
 		a.topv = pf.topv, a.topi = pf.topi, a.topk = k;
 		pf_gemm<PF_CLS_TOPK, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
-	} else if (greedy && (layout == PF_SHORT || layout == PF_SAMPLES)) {
+	} else if (greedy && pf_short(layout)) {
 		for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) {
 			if (sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
 			else vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, imin(VF_CLS_UNITS, nvt - t0), t0);
@@ -1900,9 +1917,14 @@ extern "C" int calm_b200_decode_lookup_sample(struct Transformer* transformer, c
 
 static_assert(CALM_B200_SAMPLE_N_MAX == VF_TOK, "the sequences of a step are one token tile of k_vf_gemm");
 
-// the chunk partials for `chunks` chunks per query (kept when large enough), the positions and the step tokens
-static void sn_reserve(int chunks) {
+// the pass's buffers for `rows` rows, the short block's and its sampler's, then the chunk partials for `chunks` chunks per
+// query (kept when large enough), the positions and the step tokens
+static void sn_reserve(int rows, int chunks) {
 	const Config& c = g.cfg;
+	pf_reserve(rows);
+	pf_score_reserve(true, false);
+	vf_reserve();
+	vf_sample_reserve();
 	if (!pf.snpos) {
 		pf.snpos = (int*)dev_alloc((size_t)c.seq_len * sizeof(int));
 		pf.sntok = (int*)dev_alloc((size_t)c.seq_len * sizeof(int));
@@ -1916,40 +1938,31 @@ static void sn_reserve(int chunks) {
 	pf.snpart = (float*)dev_alloc((size_t)VF_TOK * c.n_heads * chunks * (c.head_dim + 2) * sizeof(float));
 }
 
-extern "C" int calm_b200_decode_sample_n(struct Transformer* transformer, int token0, int pos0, int n_tokens, int nseq, float temperature, float minp,
-                                         unsigned long long* rng_states, int* out_tokens) {
-	if (!g.ready) CALM_FATAL("decode_sample_n before prepare_cuda");
-	if (nseq < 1 || nseq > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("decode_sample_n: nseq %d outside [1, %d]", nseq, CALM_B200_SAMPLE_N_MAX);
-	if (n_tokens < 0) CALM_FATAL("decode_sample_n: negative n_tokens %d", n_tokens);
-	if (n_tokens > 0 && (!rng_states || !out_tokens)) CALM_FATAL("decode_sample_n: rng_states or out_tokens is NULL");
-	check_call(transformer, token0, pos0);
-	if (n_tokens == 0) return 1;
-	if (!pf_supported() || (long long)pos0 + (long long)nseq * n_tokens > g.cfg.seq_len) {
-		for (int b = 0; b < nseq; ++b) calm_b200_decode_sample(transformer, token0, pos0, n_tokens, temperature, minp, &rng_states[b], out_tokens + (size_t)b * n_tokens);
-		return 0;
-	}
+// The step loop of calm_b200_decode_sample_n and calm_b200_decode_sample_batch: n_tokens short blocks of nseq rows laid
+// out as `layout`, step j at slot base s0.pos0 + j * nseq, row b fed tok0[b] at RoPE position p0[b] and then its own
+// samples at p0[b] + 1, ...; the sampled tokens go back to the next step on the device, and the tokens and states are
+// copied back once at the end.  The caller has reserved the buffers (sn_reserve).
+static void sn_decode(PfRows layout, PfSampleStep s0, const int* tok0, const int* p0, int n_tokens, float temperature, float minp,
+                      unsigned long long* rng_states, int* out_tokens) {
+	const int nseq = s0.nseq;
 	const bool greedy = temperature == 0.0f || minp >= 1.0f; // sample() is greedy there and leaves the generator alone
-	pf_reserve(nseq);
-	pf_score_reserve(true, false);
-	vf_reserve();
-	vf_sample_reserve();
-	sn_reserve(cdiv(pos0 + n_tokens, SN_CHUNK));
 	const size_t rows = (size_t)n_tokens * nseq;
-	std::vector<int> pos(rows), tok(nseq, token0);
-	for (size_t r = 0; r < rows; ++r) pos[r] = pos0 + (int)(r / nseq);
+	std::vector<int> pos(rows);
+	for (size_t r = 0; r < rows; ++r) pos[r] = p0[r % nseq] + (int)(r / nseq);
 	CUDA_CHECK(cudaMemcpyAsync(pf.snpos, pos.data(), rows * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tok.data(), nseq * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, tok0, nseq * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 	SampleState st[CALM_B200_SAMPLE_N_MAX];
 	if (!greedy) {
 		for (int b = 0; b < nseq; ++b) st[b].rng = rng_states[b], st[b].temperature = temperature, st[b].cut_delta = logf(minp) * temperature;
 		CUDA_CHECK(cudaMemcpyAsync(pf.vstate, st, nseq * sizeof(SampleState), cudaMemcpyHostToDevice, g.stream));
 	}
 	for (int j = 0; j < n_tokens; ++j) {
-		const PfSampleStep ss = {pos0, j, nseq};
+		PfSampleStep ss = s0;
+		ss.step = j;
 		int* out = pf.sntok + (size_t)j * nseq;
 		with_formats([&](auto f) {
-			pf_run(f, nseq, pos0 + j * nseq, PF_SAMPLES, &ss);
-			pf_score(f, nseq, PF_SAMPLES, true, 0, !greedy);
+			pf_run(f, nseq, s0.pos0 + j * nseq, layout, &ss);
+			pf_score(f, nseq, layout, true, 0, !greedy);
 		});
 		if (greedy) CUDA_CHECK(cudaMemcpyAsync(out, pf.greedy, nseq * sizeof(int), cudaMemcpyDeviceToDevice, g.stream));
 		else vf_sample_rows(nseq, out);
@@ -1966,6 +1979,77 @@ extern "C" int calm_b200_decode_sample_n(struct Transformer* transformer, int to
 		for (int b = 0; b < nseq; ++b) rng_states[b] = st[b].rng;
 		pf.vrows = nseq;
 	}
+}
+
+extern "C" int calm_b200_decode_sample_n(struct Transformer* transformer, int token0, int pos0, int n_tokens, int nseq, float temperature, float minp,
+                                         unsigned long long* rng_states, int* out_tokens) {
+	if (!g.ready) CALM_FATAL("decode_sample_n before prepare_cuda");
+	if (nseq < 1 || nseq > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("decode_sample_n: nseq %d outside [1, %d]", nseq, CALM_B200_SAMPLE_N_MAX);
+	if (n_tokens < 0) CALM_FATAL("decode_sample_n: negative n_tokens %d", n_tokens);
+	if (n_tokens > 0 && (!rng_states || !out_tokens)) CALM_FATAL("decode_sample_n: rng_states or out_tokens is NULL");
+	check_call(transformer, token0, pos0);
+	if (n_tokens == 0) return 1;
+	if (!pf_supported() || (long long)pos0 + (long long)nseq * n_tokens > g.cfg.seq_len) {
+		for (int b = 0; b < nseq; ++b) calm_b200_decode_sample(transformer, token0, pos0, n_tokens, temperature, minp, &rng_states[b], out_tokens + (size_t)b * n_tokens);
+		return 0;
+	}
+	sn_reserve(nseq, cdiv(pos0 + n_tokens, SN_CHUNK));
+	int tok[CALM_B200_SAMPLE_N_MAX], pos[CALM_B200_SAMPLE_N_MAX];
+	for (int b = 0; b < nseq; ++b) tok[b] = token0, pos[b] = pos0;
+	sn_decode(PF_SAMPLES, PfSampleStep{pos0, 0, nseq, 0}, tok, pos, n_tokens, temperature, minp, rng_states, out_tokens);
+	return 1;
+}
+
+// ---------------------------------------------------------------------------------------------
+// calm_b200_decode_sample_batch: nseq sequences, each with its own prompt.  The prompts go through the prompt pass packed
+// from slot 0 (PfPackedBlock, k_pf_attn<.., SEG>), then every step is one short block whose rows are the sequences
+// (PF_BATCH), each row attending over its own prompt and its own interleaved slots (sample_n.cuh, BATCH).
+
+extern "C" int calm_b200_decode_sample_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
+                                             int n_tokens, float temperature, float minp, unsigned long long* rng_states, int* out_tokens) {
+	if (!g.ready) CALM_FATAL("decode_sample_batch before prepare_cuda");
+	if (nseq < 1 || nseq > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("decode_sample_batch: nseq %d outside [1, %d]", nseq, CALM_B200_SAMPLE_N_MAX);
+	if (n_tokens < 0) CALM_FATAL("decode_sample_batch: negative n_tokens %d", n_tokens);
+	if (n_tokens == 0) return 1;
+	if (!tokens || !off || !len || !rng_states || !out_tokens) CALM_FATAL("decode_sample_batch: an array is NULL");
+	if (n < 0) CALM_FATAL("decode_sample_batch: negative n %d", n);
+	for (int b = 0; b < nseq; ++b)
+		if (len[b] < 1 || off[b] < 0 || (long)off[b] + len[b] > n) CALM_FATAL("decode_sample_batch: prompt %d (off %d, len %d) empty or outside the %d tokens", b, off[b], len[b], n);
+	check_tokens(tokens, n);
+	// prompt b's L_b = len[b] - 1 rows take ceil8(L_b) slots from s_b; the steps follow from G, nseq slots each
+	long long G = 0;
+	int lmax = 0;
+	for (int b = 0; b < nseq; ++b) G += cdiv(len[b] - 1, 8) * 8, lmax = std::max(lmax, len[b] - 1);
+	if (!pf_supported() || G + (long long)nseq * n_tokens > g.cfg.seq_len) {
+		for (int b = 0; b < nseq; ++b) {
+			const int* p = tokens + off[b];
+			forward_prefill_cuda(transformer, p, len[b] - 1, 0);
+			calm_b200_decode_sample(transformer, p[len[b] - 1], len[b] - 1, n_tokens, temperature, minp, &rng_states[b], out_tokens + (size_t)b * n_tokens);
+		}
+		return 0;
+	}
+	PfPackedBlock pb;
+	int2 rows[CALM_B200_SAMPLE_N_MAX];
+	int tok[CALM_B200_SAMPLE_N_MAX], pos[CALM_B200_SAMPLE_N_MAX];
+	for (int b = 0; b < nseq; ++b) {
+		const int* p = tokens + off[b];
+		const int L = len[b] - 1;
+		rows[b] = make_int2(pb.add(p, L, L, 0, make_int2(0, 0)), L), tok[b] = p[L], pos[b] = L;
+	}
+	const int chunk_cap = 2048;
+	sn_reserve(std::max(imin((int)G, chunk_cap), nseq), cdiv(lmax + n_tokens, SN_CHUNK));
+	if (!pf.sbrows) pf.sbrows = (int2*)dev_alloc(VF_TOK * sizeof(int2));
+	CUDA_CHECK(cudaMemcpyAsync(pf.sbrows, rows, nseq * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
+	// the prompts in blocks of at most chunk_cap rows at slot base o: pf.seg holds absolute slots, so a prompt that straddles
+	// a block edge walks its keys from s_b, which the earlier block wrote
+	for (int o = 0; o < G; o += chunk_cap) {
+		const int m = imin((int)G - o, chunk_cap);
+		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, pb.tok.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pb.pos.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		CUDA_CHECK(cudaMemcpyAsync(pf.seg, pb.seg.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		pf_block(m, o, PF_PACKED, nullptr, PfOut());
+	}
+	sn_decode(PF_BATCH, PfSampleStep{(int)G, 0, nseq, lmax}, tok, pos, n_tokens, temperature, minp, rng_states, out_tokens);
 	return 1;
 }
 
@@ -2087,8 +2171,9 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 // and into the cache slots [kv_from_pos, seq_len) of every layer and kv head.  Only data is touched: TokenParams, the
 // attention's {value, epoch} cells and counter, k_vf_gemm's arrival counters, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
 // counts (the decode's and the sampled short block's), stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
-// as do the index buffers (cand_idx, sample_idx, pf.vsidx, out_tokens, pf.tokens, pf.targets, and pf.rowpos, pf.seg and pf.ctx, read
-// as a RoPE position and as key slots of the packed attention's loop): a stale index that is read is in range,
+// as do the index buffers (cand_idx, sample_idx, pf.vsidx, out_tokens, pf.tokens, pf.targets, pf.rowpos, pf.seg and pf.ctx, read
+// as a RoPE position and as key slots of the packed attention's loop, and pf.sbrows, decode_sample_batch's key slots and
+// chunk counts): a stale index that is read is in range,
 // as after any earlier call, while 0xFFFFFFFF would send the read out of bounds.  DESIGN.md s.3 lists both groups.
 extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos) {
 	(void)transformer;

@@ -624,10 +624,12 @@ __device__ __forceinline__ void pf_load_dims(const uint8_t* p, float (&o)[DPL]) 
 }
 
 // CTA = (kv head, 8 consecutive query tokens); warp = one token with all kv_mul query heads of the kv head (KM of them per pass).
-// SEG: a packed block of the scoring calls (score_batch, score_context; pos0 = 0, row t in cache slot t).  The host starts
-// every sequence at a multiple of 8 rows, so the CTA's rows share one segment starting at row s = seg[first row], and the key
-// tiles run from s: tile j of a sequence holds the same keys in the same order as tile j of the sequence scored alone from
-// position 0, and each warp's online softmax sees exactly the values of that lone pass.
+// SEG: a packed block, row t in cache slot pos0 + t: the scoring calls' (score_batch, score_context; pos0 = 0), or one of
+// decode_sample_batch's prompt blocks (pos0 = the block's first slot of the packed prompt region).  seg[] holds absolute
+// cache slots.  The host starts every sequence at a multiple of 8 slots, so the CTA's rows share one segment starting at
+// slot s = seg[first row], and the key tiles run from s: tile j of a sequence holds the same keys in the same order as tile
+// j of the sequence run alone from position 0, and each warp's online softmax sees exactly the values of that lone pass.
+// A sequence that straddles a block edge continues in the next block from the same s, whose slots the earlier block wrote.
 // CTX (with SEG): a packed block that also holds contexts its sequences continue.  A CTA's rows start at
 // row s and continue the nc-row context at rows c0 .. c0 + nc - 1 (ctx[first row]).  The keys run over one virtual index v:
 // v < nc is row c0 + v, v >= nc is row s + v - nc; row t sees v <= nc + t - s.  A tile may straddle the two ranges, so each

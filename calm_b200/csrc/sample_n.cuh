@@ -18,6 +18,14 @@
 // A row's output depends on its query, its keys and the chunking only, never on how many rows run beside it: which chunks
 // are shared depends on pos0 and j alone, a query's arithmetic does not depend on the warp that runs it, and nothing is
 // added with atomics.
+//
+// BATCH (calm_b200_decode_sample_batch): every row continues its own prompt.  The prompts were packed by the prompt pass
+// from slot 0, row b's L_b prompt entries at slots s_b .. s_b + L_b - 1 (rows[b] = (s_b, L_b)), and the region ends at
+// slot pos0 = G.  Step j writes row b to slot G + j * nseq + b, so row b's keys at step j are v = 0 .. L_b + j: v < L_b is
+// slot s_b + v, v >= L_b is slot G + (v - L_b) * nseq + b.  No chunk is shared: CTA x is chunk x % nch of row x / nch
+// (nch = gridDim.x / nseq, the longest row's chunk count), and a CTA past its row's chunks returns.  A query's staging,
+// scores, chunk softmax, value pass and fold are the plain kernels' operations in the same order, so row b gives what
+// calm_b200_decode_sample_n gives one sequence over the same keys at pos0 = L_b.
 #pragma once
 
 #include "prefill.cuh"
@@ -34,6 +42,7 @@ struct SnAttnArgs {
 	__half* Olo;
 	int pos0, step, nseq, seq_len, q_dim, kv_mul, n_heads, nchmax;
 	float inv_sqrt_hd;
+	const int2* rows; // [nseq] (BATCH) row b's prompt: its first slot s_b and its length L_b; read by no other variant
 };
 
 // dynamic shared memory of k_sn_attn: the K tile (padded rows), the V tile, each warp's KM queries
@@ -43,8 +52,8 @@ constexpr size_t sn_smem_bytes() {
 }
 
 // grid (prompt chunks + nseq x suffix chunks, kv heads): CTA x < pos0 / SN_CHUNK is prompt chunk x for every row, the
-// others are suffix chunk x' % nsuf of row x' / nsuf (x' = x - prompt chunks)
-template <typename KVT, int HD, int KM>
+// others are suffix chunk x' % nsuf of row x' / nsuf (x' = x - prompt chunks).  BATCH: grid (nseq x nch, kv heads).
+template <typename KVT, int HD, int KM, bool BATCH = false>
 __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 	pdl_enter();
 	constexpr int DPL = HD / 32, KPL = SN_CHUNK / 32;
@@ -54,11 +63,19 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 	unsigned char* vs = ks + SN_CHUNK * KSTR;
 	float* qs = reinterpret_cast<float*>(vs + SN_CHUNK * VSTR) + (threadIdx.x >> 5) * KM * HD;
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, kvh = blockIdx.y;
-	const int nkeys = a.pos0 + a.step + 1, npre = a.pos0 / SN_CHUNK, nsuf = (nkeys + SN_CHUNK - 1) / SN_CHUNK - npre;
-	int c = blockIdx.x, b0 = 0, nrows = a.nseq;
-	if (c >= npre) {
-		const int x = c - npre;
-		b0 = x / nsuf, c = npre + x % nsuf, nrows = 1;
+	int nkeys, c, b0, nrows;
+	if constexpr (BATCH) {
+		const int nch = gridDim.x / a.nseq;
+		b0 = blockIdx.x / nch, c = blockIdx.x % nch, nrows = 1;
+		nkeys = __ldg(&a.rows[b0].y) + a.step + 1;
+		if (c * SN_CHUNK >= nkeys) return;
+	} else {
+		nkeys = a.pos0 + a.step + 1, c = blockIdx.x, b0 = 0, nrows = a.nseq;
+		const int npre = a.pos0 / SN_CHUNK, nsuf = (nkeys + SN_CHUNK - 1) / SN_CHUNK - npre;
+		if (c >= npre) {
+			const int x = c - npre;
+			b0 = x / nsuf, c = npre + x % nsuf, nrows = 1;
+		}
 	}
 	const int v0 = c * SN_CHUNK, nk = min(SN_CHUNK, nkeys - v0);
 	const KVT* kbase = reinterpret_cast<const KVT*>(a.kc) + (size_t)kvh * a.seq_len * HD;
@@ -66,7 +83,11 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 	for (int i = threadIdx.x; i < SN_CHUNK * (VSTR / 16); i += blockDim.x) {
 		const int row = i / (VSTR / 16), cc = i % (VSTR / 16), v = v0 + row;
 		const bool in = row < nk;
-		const int slot = v < a.pos0 ? v : a.pos0 + (v - a.pos0) * a.nseq + b0;
+		int slot;
+		if constexpr (BATCH) { // (read per key: held in registers through the score pass, they add spills)
+			const int2 pr = __ldg(a.rows + b0);
+			slot = v < pr.y ? pr.x + v : a.pos0 + (v - pr.y) * a.nseq + b0;
+		} else slot = v < a.pos0 ? v : a.pos0 + (v - a.pos0) * a.nseq + b0;
 		const uint4 z = make_uint4(0, 0, 0, 0);
 		*reinterpret_cast<uint4*>(ks + row * KSTR + cc * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(kbase + (size_t)slot * HD) + cc) : z;
 		*reinterpret_cast<uint4*>(vs + row * VSTR + cc * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(vbase + (size_t)slot * HD) + cc) : z;
@@ -153,13 +174,13 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 }
 
 // grid (cdiv(n_heads, SN_WARPS), nseq): warp = query head, lane = head dims [lane * DPL, lane * DPL + DPL)
-template <int HD>
+template <int HD, bool BATCH = false>
 __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_fold(const SnAttnArgs a) {
 	pdl_enter();
 	constexpr int DPL = HD / 32;
 	const int lane = threadIdx.x & 31, h = blockIdx.x * SN_WARPS + (threadIdx.x >> 5), b = blockIdx.y;
 	if (h >= a.n_heads) return;
-	const int nch = (a.pos0 + a.step + SN_CHUNK) / SN_CHUNK;
+	const int nch = ((BATCH ? a.rows[b].y : a.pos0) + a.step + SN_CHUNK) / SN_CHUNK;
 	const float* p = a.part + ((size_t)b * a.n_heads + h) * a.nchmax * (HD + 2);
 	float mx = -FLT_MAX;
 	for (int c = lane; c < nch; c += 32) mx = fmaxf(mx, __ldcg(p + (size_t)c * (HD + 2)));

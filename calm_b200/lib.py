@@ -27,7 +27,7 @@ SYMBOLS = [
     "calm_b200_score_topk", "calm_b200_score_batch_topk", "calm_b200_score_context_topk",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
-    "calm_b200_decode_sample_n",
+    "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -41,7 +41,7 @@ TOPK_MAX = 20
 # the largest block calm_b200_verify_greedy takes (CALM_B200_VERIFY_MAX); decode_lookup drafts at most one fewer
 VERIFY_MAX = 16
 
-# the most sequences calm_b200_decode_sample_n samples together (CALM_B200_SAMPLE_N_MAX)
+# the most sequences calm_b200_decode_sample_n and calm_b200_decode_sample_batch sample together (CALM_B200_SAMPLE_N_MAX)
 SAMPLE_N_MAX = 16
 
 # calm_b200_read_state selectors (include/calm_b200.h)
@@ -98,6 +98,8 @@ def load() -> C.CDLL:
     L.calm_b200_decode_lookup_sample.restype = C.c_int
     L.calm_b200_decode_sample_n.argtypes = [T, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, _u64p, _iptr]
     L.calm_b200_decode_sample_n.restype = C.c_int
+    L.calm_b200_decode_sample_batch.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, C.c_int, C.c_int, C.c_float, C.c_float, _u64p, _iptr]
+    L.calm_b200_decode_sample_batch.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -423,6 +425,42 @@ class DeviceModel:
         out = np.full((nseq, int(n_tokens)), -1, np.int32)
         served = self.lib.calm_b200_decode_sample_n(C.byref(self.transformer), int(token0), int(pos0), int(n_tokens), nseq, temperature, minp, rng,
                                                     out.ctypes.data_as(C.POINTER(C.c_int)))
+        return out, [int(s) for s in rng], served
+
+    def decode_sample_batch(self, prompts, n_tokens: int, temperature: float, minp: float, rng_states):
+        """calm_b200_decode_sample_batch: len(prompts) = nseq sequences, sequence b continuing prompts[b] (a sequence of at
+        least one token id) as forward_prefill_cuda(prompts[b][:-1], 0) and then decode_sample(prompts[b][-1], len - 1,
+        n_tokens, ..., rng_states[b]) would.  Returns (tokens int32[nseq, n_tokens], the nseq new generator states,
+        served): served is 1 on the packed path, 0 when those per-sequence pairs gave them (shapes the prompt pass does
+        not serve, or a layout past seq_len).  Raises ValueError for 0 or more than SAMPLE_N_MAX prompts, as many states
+        as prompts not given, a bad state, a negative n_tokens, an empty prompt or a token outside the vocabulary."""
+        if prompts is None or rng_states is None or isinstance(rng_states, (int, np.integer)):
+            raise ValueError("decode_sample_batch takes a list of prompts and a sequence of generator states, one per prompt")
+        prompts = [np.asarray(p) for p in prompts]
+        states = list(rng_states)
+        if not 1 <= len(prompts) <= SAMPLE_N_MAX:
+            raise ValueError(f"decode_sample_batch samples 1 to {SAMPLE_N_MAX} sequences, got {len(prompts)} prompts")
+        if len(states) != len(prompts):
+            raise ValueError(f"decode_sample_batch takes one generator state per prompt: {len(prompts)} prompts, {len(states)} states")
+        for s in states:
+            _check_rng(s)
+        if not isinstance(n_tokens, (int, np.integer)) or n_tokens < 0:
+            raise ValueError(f"n_tokens must be a non-negative integer, got {n_tokens!r}")
+        for b, p in enumerate(prompts):
+            if p.ndim != 1 or len(p) < 1 or p.dtype.kind not in "iu":
+                raise ValueError(f"prompt {b} must be a non-empty sequence of token ids")
+            if not ((p >= 0) & (p < self.vocab)).all():
+                raise ValueError(f"prompt {b} has a token outside [0, {self.vocab})")
+        nseq = len(prompts)
+        tokens = np.ascontiguousarray(np.concatenate(prompts), np.int32)
+        len_ = np.asarray([len(p) for p in prompts], np.int32)
+        off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(len_)[:-1]]), np.int32)
+        rng = (C.c_ulonglong * nseq)(*[int(s) for s in states])
+        out = np.full((nseq, int(n_tokens)), -1, np.int32)
+        ip = C.POINTER(C.c_int)
+        served = self.lib.calm_b200_decode_sample_batch(C.byref(self.transformer), tokens.ctypes.data_as(ip), len(tokens), off.ctypes.data_as(ip),
+                                                        len_.ctypes.data_as(ip), nseq, int(n_tokens), temperature, minp, rng,
+                                                        out.ctypes.data_as(ip))
         return out, [int(s) for s in rng], served
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):

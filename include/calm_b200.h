@@ -263,6 +263,27 @@ int calm_b200_decode_lookup_sample(struct Transformer* transformer, const int* t
 int calm_b200_decode_sample_n(struct Transformer* transformer, int token0, int pos0, int n_tokens, int nseq, float temperature, float minp,
                               unsigned long long* rng_states, int* out_tokens);
 
+/* Sample nseq sequences that each continue their own prompt together: the prompts go through the prompt pass packed into
+ * shared blocks, then every step is one pass over the weights for all of them (DESIGN.md s.6).  Prompt b is
+ * tokens[off[b] .. off[b] + len[b]), len[b] >= 1, as in calm_b200_score_batch.  Sequence b is, by definition, what
+ *   forward_prefill_cuda(t, prompt_b, len[b] - 1, 0);
+ *   calm_b200_decode_sample(t, prompt_b[len[b] - 1], len[b] - 1, n_tokens, temperature, minp, &rng_states[b], ...);
+ * give on a fresh cache, bit for bit: out_tokens[b * n_tokens + i] is its sample after step i, and rng_states[b] is left
+ * advanced by n_tokens draws.  temperature == 0 or minp >= 1 makes every sequence its greedy stream and leaves the states
+ * alone.  Returns 1 on the new path.  Prompt b's L_b = len[b] - 1 entries are placed at slots s_b .., each prompt taking
+ * L_b rounded up to a multiple of 8 slots, packed in input order from slot 0 up to G = sum of those; step j writes
+ * sequence b's entries to slot G + j * nseq + b, so the call needs G + nseq * n_tokens <= seq_len.  Shapes the prompt
+ * pass does not serve (as for calm_b200_verify_greedy) and calls past seq_len run the pair above for b = 0, 1, .., with
+ * exactly its tokens and states, and return 0.  The KV cache afterwards holds nothing a host can continue from (to
+ * continue one sequence, feed its prompt and tokens again: INTEGRATION.md).  1 <= nseq <= CALM_B200_SAMPLE_N_MAX and
+ * n_tokens >= 0, or the call aborts before any device work; n_tokens == 0 reads nothing else and returns 1.  Otherwise
+ * no array may be NULL, every prompt must have len[b] >= 1 and lie inside tokens[0 .. n), and every token of
+ * tokens[0 .. n) must be in the vocabulary, or the call aborts before any device work.  The first call allocates what
+ * calm_b200_decode_sample_n allocates, with the attention's partials for ceil((max L_b + n_tokens) / 128) chunks, and
+ * the prompt pass's buffers for min(G, 2048) rows. */
+int calm_b200_decode_sample_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
+                                  int n_tokens, float temperature, float minp, unsigned long long* rng_states, int* out_tokens);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
@@ -307,9 +328,11 @@ void calm_b200_read_kv(struct Transformer* transformer, int layer, int kv_pos, f
  *            queries, attention output and FFN hidden matrix (the last two kept as f16 hi + lo pairs, summed here in
  *            float); rows = the pass's token tiles (a multiple of 128, at least n), of the last block of <= 2048 tokens
  *   PF_LOGITS  float[n][vocab]          the logit rows of the last calm_b200_verify_sample block that took the short-block
- *            path (n of its tokens), or of the last step of the last sampled calm_b200_decode_sample_n call that took
- *            its new path (n = nseq, row b = sequence b), the values its sampler drew from
- *   After calm_b200_decode_sample_n, the PF_* matrices hold its last step, row b = sequence b. */
+ *            path (n of its tokens), or of the last step of the last sampled calm_b200_decode_sample_n or
+ *            calm_b200_decode_sample_batch call that took its new path (n = nseq, row b = sequence b), the values its
+ *            sampler drew from
+ *   After calm_b200_decode_sample_n or calm_b200_decode_sample_batch on its new path, the PF_* matrices hold the last
+ *   step, row b = sequence b. */
 enum {
 	CALM_B200_STATE_X = 0, CALM_B200_STATE_XB = 1, CALM_B200_STATE_Q = 2, CALM_B200_STATE_ATT = 3, CALM_B200_STATE_HB = 4,
 	CALM_B200_STATE_MOE_SEL = 5, CALM_B200_STATE_KEYS = 6, CALM_B200_STATE_VALUES = 7,
