@@ -37,6 +37,11 @@ pytestmark = pytest.mark.gpu
 MERGE_C = 2e-6
 
 
+def stage_bound(dim, amax, lse):
+    """The bound above per position: amax = max |logits of the row|, lse = ln sum exp(logits)."""
+    return 2 * pf_tol(dim) * amax + MERGE_C * np.maximum(1.0, np.abs(lse))
+
+
 def log_softmax_at(logits, targets):
     """float64 ln softmax(logits[i])[targets[i]] and the row's log-sum-exp; logits[n, vocab] (numpy or torch, any float)."""
     L = torch.as_tensor(logits).to(torch.float64)
@@ -81,7 +86,7 @@ def test_score_stage_against_float64(case):
     amax = logits.abs().amax(1).cpu().numpy()
     err = np.abs(lp.astype(np.float64) - ref)
     gemm = 2 * pf_tol(spec.dim) * amax
-    bound = gemm + MERGE_C * np.maximum(1.0, np.abs(lse))
+    bound = stage_bound(spec.dim, amax, lse)
     i = int(np.argmax(err / bound))
     excess = float(((err - gemm) / np.maximum(1.0, np.abs(lse))).max())
     worst[case] = (float(err[i] / bound[i]), excess)
