@@ -230,12 +230,13 @@ def peaked_model():
     return spec, tensors
 
 
-def coin_clear(logits, c, temperature, minp):
-    """No change of the logits within 2 TOL_SIGMA sigma moves the coin c across a bin edge (float64): no logit lies within
-    twice that of the min-p cutoff, and the coin stays inside its bin when every survivor's weight exp(l / T) moves by
-    exp(+-that / T), which bounds the odds of every cumulative share by exp(+-2 that / T)."""
+def coin_clear(logits, c, temperature, minp, d=None):
+    """No change of any logit by up to d (default 2 TOL_SIGMA sigma of the row) moves the coin c across a bin edge
+    (float64): no logit lies within 2 d of the min-p cutoff, and the coin stays inside its bin when every survivor's weight
+    exp(l / T) moves by exp(+-d / T), which bounds the odds of every cumulative share by exp(+-2 d / T)."""
     L = np.asarray(logits, np.float64)
-    d = 2 * TOL_SIGMA * L.std()
+    if d is None:
+        d = 2 * TOL_SIGMA * L.std()
     mx = L.max()
     cut = mx + math.log(minp) * temperature if minp > 0 else -np.inf
     if np.isfinite(cut) and np.abs(L - cut).min() <= 2 * d:
