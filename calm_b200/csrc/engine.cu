@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <iterator>
 #include <map>
 #include <vector>
 
@@ -183,6 +184,13 @@ struct Prefill {
 	// different prompts decoded together (calm_b200_decode_sample_batch), allocated on its first call: each row's prompt
 	// in the packed cache, its first slot and length (uploaded once per call)
 	int2* sbrows = nullptr; // [VF_TOK]
+	// requests generated from a queue (calm_b200_decode_sample_queue), allocated on its first call and regrown when a call
+	// needs more: the step's row table (written by k_sq_begin), the step's tokens, and every request's tokens and state
+	SqRows* sqrows = nullptr;
+	int* sqtok = nullptr;              // [VF_TOK]
+	int* sqout = nullptr;              // [sqout_cap]: request i's tokens from O_i = max_new[0] + .. + max_new[i - 1]
+	unsigned long long* sqst = nullptr; // [sqst_cap]: request i's generator state after its last sampled step
+	size_t sqout_cap = 0, sqst_cap = 0;
 };
 Prefill pf;
 
@@ -195,6 +203,7 @@ void pf_free() {
 	cudaFree(pf.vacc), cudaFree(pf.vcnt);
 	cudaFree(pf.vlogits), cudaFree(pf.vtmax), cudaFree(pf.vsidx), cudaFree(pf.vsprob), cudaFree(pf.vcsum), cudaFree(pf.vcount), cudaFree(pf.vstate), cudaFree(pf.vsampled);
 	cudaFree(pf.snpart), cudaFree(pf.snpos), cudaFree(pf.sntok), cudaFree(pf.sbrows);
+	cudaFree(pf.sqrows), cudaFree(pf.sqtok), cudaFree(pf.sqout), cudaFree(pf.sqst);
 	pf = Prefill();
 }
 
@@ -1243,17 +1252,18 @@ static void vf_reserve() {
 }
 
 // out = W . X^T over the rows of `a` for the n <= 16 rows of (hi, lo), in `units` row blocks of 128 (UP: of w1 and of w3
-// each); the classifier from vocabulary tile `tile0` on.  Every K-slice gets the same number of CTAs, as many as stay
-// resident together, each walking row blocks with the same stride.
+// each); the classifier from vocabulary tile `tile0` on; PF_QKV_SLOTS: row t's keys and values to cache slot slot[t].
+// Every K-slice gets the same number of CTAs, as many as stay resident together, each walking row blocks with the same
+// stride.
 template <int MODE, int DBITS, typename KVT>
-static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int units, int tile0 = 0) {
+static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int units, int tile0 = 0, const int* slot = nullptr) {
 	static int cap = 0, sms = 0;
 	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT>, VF_THREADS, 0), sms = g.sms;
 	VfArgs v = {};
 	v.xhi = hi, v.xlo = lo, v.acc = pf.vacc, v.cnt = pf.vcnt;
 	v.nsl = vf_slices(a.K), v.units = units, v.rows = (MODE == PF_UP ? 2 : 1) * units * VF_ROWS;
 	v.tile0 = tile0, v.nvt = cdiv(g.cfg.vocab_size, PF_BM);
-	v.logits = pf.vlogits, v.tmax = pf.vtmax;
+	v.logits = pf.vlogits, v.tmax = pf.vtmax, v.slot = slot;
 	const int tasks = (MODE == PF_UP ? 2 : 1) * units;
 	launch_pdl(k_vf_gemm<MODE, DBITS, KVT>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
 }
@@ -1266,6 +1276,8 @@ enum PfRows {
 	             // pf.snpos and the shared-prompt attention of sample_n.cuh
 	PF_BATCH,    // a step of calm_b200_decode_sample_batch (PfSampleStep): PF_SAMPLES, but every row continues its own prompt
 	             // (pf.sbrows) through sample_n.cuh's BATCH attention
+	PF_QUEUE,    // a step of calm_b200_decode_sample_queue (PfSampleStep): PF_BATCH, but every row has its own step count, its
+	             // own generated slots and its own RoPE position (the table pf.sqrows), and writes its keys to its own slot
 	PF_PACKED,   // a packed block that holds no context (the scoring calls at pos0 = 0, and decode_sample_batch's prompts at
 	             // any slot base): per-row RoPE positions in pf.rowpos, each row's sequence start (its cache slot) in pf.seg
 	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block: each row's context in pf.ctx
@@ -1273,7 +1285,7 @@ enum PfRows {
 
 // a short block: at most VF_TOK rows whose GEMMs run on k_vf_gemm
 static bool pf_short(PfRows layout) {
-	return layout == PF_SHORT || layout == PF_SAMPLES || layout == PF_BATCH;
+	return layout == PF_SHORT || layout == PF_SAMPLES || layout == PF_BATCH || layout == PF_QUEUE;
 }
 
 // A layer GEMM of the pass over `rows` output rows of `a` (UP: of w1 and of w3 each), whose activations are the f16 pair
@@ -1286,14 +1298,15 @@ static void pf_layer_gemm(PfRows layout, const CUtensorMap* tm, const __half* hi
 
 // A step of calm_b200_decode_sample_n: its n = nseq rows are the sequences, all at RoPE position pos0 + step, row b in
 // cache slot pos0 + step * nseq + b; the prompt is in slots [0, pos0).  A step of calm_b200_decode_sample_batch: the
-// same slots from pos0 = G, the end of the packed prompts, and row b at RoPE position L_b + step; lmax = max_b L_b.
+// same slots from pos0 = G, the end of the packed prompts, and row b at RoPE position L_b + step; lmax = max_b L_b.  A
+// step of calm_b200_decode_sample_queue: nseq rows, step 0, and lmax = the largest L + j of its rows (pf.sqrows).
 struct PfSampleStep {
 	int pos0, step, nseq, lmax;
 };
 
-// The attention of a PF_SAMPLES step (shared prompt) or, with BATCH, of a PF_BATCH step (a prompt per row) (sample_n.cuh):
-// chunk partials, then their fold into pf.Ahi / pf.Alo
-template <typename KVT, int HD, bool BATCH>
+// The attention of a PF_SAMPLES step (shared prompt) or, with BATCH, of a PF_BATCH step (a prompt per row), or with
+// QUEUE as well, of a PF_QUEUE step (sample_n.cuh): chunk partials, then their fold into pf.Ahi / pf.Alo
+template <typename KVT, int HD, bool BATCH, bool QUEUE = false>
 static void sn_attn(const SnAttnArgs& a, int lmax) {
 	const int nkeys = a.pos0 + a.step + 1, npre = a.pos0 / SN_CHUNK, nsuf = cdiv(nkeys, SN_CHUNK) - npre;
 	const dim3 grid(BATCH ? a.nseq * cdiv(lmax + a.step + 1, SN_CHUNK) : npre + a.nseq * nsuf, g.cfg.n_kv_heads);
@@ -1301,14 +1314,14 @@ static void sn_attn(const SnAttnArgs& a, int lmax) {
 		smem_optin(kernel, smem);
 		launch_pdl(kernel, grid, SN_WARPS * 32, smem, a);
 	};
-	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4, BATCH>, sn_smem_bytes<KVT, HD, 4>());
-	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2, BATCH>, sn_smem_bytes<KVT, HD, 2>());
-	else run(k_sn_attn<KVT, HD, 1, BATCH>, sn_smem_bytes<KVT, HD, 1>());
-	launch_pdl(k_sn_fold<HD, BATCH>, dim3(cdiv(g.cfg.n_heads, SN_WARPS), a.nseq), SN_WARPS * 32, 0, a);
+	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4, BATCH, QUEUE>, sn_smem_bytes<KVT, HD, 4>());
+	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2, BATCH, QUEUE>, sn_smem_bytes<KVT, HD, 2>());
+	else run(k_sn_attn<KVT, HD, 1, BATCH, QUEUE>, sn_smem_bytes<KVT, HD, 1>());
+	launch_pdl(k_sn_fold<HD, BATCH, QUEUE>, dim3(cdiv(g.cfg.n_heads, SN_WARPS), a.nseq), SN_WARPS * 32, 0, a);
 }
 
 // The pass over the n rows in pf.tokens at cache slots pos0 + t, laid out as `layout` says (PF_SAMPLES and PF_BATCH: the
-// step `ss`, whose slot base pos0 is ss->pos0 + ss->step * n).
+// step `ss`, whose slot base pos0 is ss->pos0 + ss->step * n; PF_QUEUE: the step `ss`, each row at its own slot).
 template <int DBITS, typename KVT>
 static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const PfSampleStep* ss = nullptr) {
 	const bool packed = layout == PF_PACKED || layout == PF_CONTEXTS;
@@ -1317,6 +1330,7 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
 	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
 	if (layout == PF_SAMPLES || layout == PF_BATCH) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.snpos + (size_t)ss->step * n, n, c.head_dim / 2);
+	else if (layout == PF_QUEUE) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.sqrows->pos, n, c.head_dim / 2);
 	else if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
 	else launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
 	for (int l = 0; l < c.n_layers; ++l) {
@@ -1327,18 +1341,24 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 		a.Q = pf.Q, a.q_dim = g.q_dim, a.kv_dim = g.kv_dim, a.head_dim = c.head_dim, a.seq_len = c.seq_len, a.pos0 = pos0;
 		a.bias = w.bqkv[l], a.clip = c.qkv_clip, a.rope = pf.rope;
 		a.kc = (KVT*)g.kc + l * kv_layer, a.vc = (KVT*)g.vc + l * kv_layer;
-		pf_layer_gemm<PF_QKV, DBITS, KVT>(layout, pf.tmN, pf.Nhi, pf.Nlo, a, g.q_dim + 2 * g.kv_dim);
+		if (layout == PF_QUEUE) {
+			vf_gemm<PF_QKV_SLOTS, DBITS, KVT>(pf.Nhi, pf.Nlo, a, (g.q_dim + 2 * g.kv_dim) / VF_ROWS, 0, pf.sqrows->slot);
+		} else pf_layer_gemm<PF_QKV, DBITS, KVT>(layout, pf.tmN, pf.Nhi, pf.Nlo, a, g.q_dim + 2 * g.kv_dim);
 
 		PfAttnArgs aa = {};
 		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
 		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
 		aa.seg = pf.seg, aa.ctx = pf.ctx;
-		if (layout == PF_SAMPLES || layout == PF_BATCH) {
+		if (layout == PF_SAMPLES || layout == PF_BATCH || layout == PF_QUEUE) {
 			SnAttnArgs sa = {};
 			sa.Q = pf.Q, sa.kc = a.kc, sa.vc = a.vc, sa.part = pf.snpart, sa.Ohi = pf.Ahi, sa.Olo = pf.Alo;
 			sa.pos0 = ss->pos0, sa.step = ss->step, sa.nseq = ss->nseq, sa.seq_len = c.seq_len, sa.q_dim = g.q_dim, sa.kv_mul = g.kv_mul;
 			sa.n_heads = c.n_heads, sa.nchmax = pf.snchunks, sa.inv_sqrt_hd = aa.inv_sqrt_hd, sa.rows = pf.sbrows;
-			if (layout == PF_BATCH) {
+			if (layout == PF_QUEUE) {
+				sa.qrows = pf.sqrows->q;
+				if (c.head_dim == 128) sn_attn<KVT, 128, true, true>(sa, ss->lmax);
+				else sn_attn<KVT, 64, true, true>(sa, ss->lmax);
+			} else if (layout == PF_BATCH) {
 				if (c.head_dim == 128) sn_attn<KVT, 128, true>(sa, ss->lmax);
 				else sn_attn<KVT, 64, true>(sa, ss->lmax);
 			} else {
@@ -1436,6 +1456,15 @@ static void pf_score_reserve(bool greedy, bool topk) {
 	}
 }
 
+// The merge of the classifier's tile records into each row's log-probability (pf.logprob), with `greedy` its argmax
+// (pf.greedy), with k > 0 its k largest logits (pf.top_ids / pf.top_lp)
+static void pf_merge(int n, bool greedy, int k) {
+	const int nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	const auto merge = k ? k_pf_logprob<false, true> : greedy ? k_pf_logprob<true> : k_pf_logprob<false>;
+	launch_pdl(merge, cdiv(n, 8), 256, k ? (size_t)8 * nvt : 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx,
+	           pf.greedy, (const float*)pf.topv, (const int*)pf.topi, k, pf.top_ids, pf.top_lp);
+}
+
 // After pf_run over n rows: the final norm, the classifier with its log-softmax epilogue, the merge of the tile records;
 // with `greedy` the classifier and the merge also give each row's argmax in pf.greedy, with k > 0 its k largest logits'
 // indices and log-probabilities in pf.top_ids / pf.top_lp [n][k].  A short block's greedy classifier runs on k_vf_gemm,
@@ -1464,9 +1493,7 @@ static void pf_score(Formats<DBITS, KVT>, int n, PfRows layout, bool greedy, int
 	} else {
 		pf_gemm<PF_CLS, DBITS, KVT>(pf.tmN, a, nvt * PF_BM, n);
 	}
-	const auto merge = k ? k_pf_logprob<false, true> : greedy ? k_pf_logprob<true> : k_pf_logprob<false>;
-	launch_pdl(merge, cdiv(n, 8), 256, k ? (size_t)8 * nvt : 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx,
-	           pf.greedy, (const float*)pf.topv, (const int*)pf.topi, k, pf.top_ids, pf.top_lp);
+	pf_merge(n, greedy, k);
 }
 
 // One block of the pass: the n rows the caller reserved (pf_reserve) and uploaded to pf.tokens (and, packed, to pf.rowpos,
@@ -2005,6 +2032,23 @@ extern "C" int calm_b200_decode_sample_n(struct Transformer* transformer, int to
 // from slot 0 (PfPackedBlock, k_pf_attn<.., SEG>), then every step is one short block whose rows are the sequences
 // (PF_BATCH), each row attending over its own prompt and its own interleaved slots (sample_n.cuh, BATCH).
 
+constexpr int SB_BLOCK = 2048; // rows of a block of packed prompts
+
+// The packed prompts of `pb` at cache slots base .. base + pb.rows() - 1, in blocks of at most SB_BLOCK rows at slot base
+// base + o: pf.seg holds absolute slots, so a prompt that straddles a block edge walks its keys from its first slot, which
+// the earlier block wrote.  The caller has reserved the pass for min(pb.rows(), SB_BLOCK) rows.
+static void sb_prefill(PfPackedBlock& pb, int base) {
+	for (int& s : pb.seg) s += base;
+	const int G = pb.rows();
+	for (int o = 0; o < G; o += SB_BLOCK) {
+		const int m = imin(G - o, SB_BLOCK);
+		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, pb.tok.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pb.pos.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		CUDA_CHECK(cudaMemcpyAsync(pf.seg, pb.seg.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		pf_block(m, base + o, PF_PACKED, nullptr, PfOut());
+	}
+}
+
 extern "C" int calm_b200_decode_sample_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
                                              int n_tokens, float temperature, float minp, unsigned long long* rng_states, int* out_tokens) {
 	if (!g.ready) CALM_FATAL("decode_sample_batch before prepare_cuda");
@@ -2036,20 +2080,227 @@ extern "C" int calm_b200_decode_sample_batch(struct Transformer* transformer, co
 		const int L = len[b] - 1;
 		rows[b] = make_int2(pb.add(p, L, L, 0, make_int2(0, 0)), L), tok[b] = p[L], pos[b] = L;
 	}
-	const int chunk_cap = 2048;
-	sn_reserve(std::max(imin((int)G, chunk_cap), nseq), cdiv(lmax + n_tokens, SN_CHUNK));
+	sn_reserve(std::max(imin((int)G, SB_BLOCK), nseq), cdiv(lmax + n_tokens, SN_CHUNK));
 	if (!pf.sbrows) pf.sbrows = (int2*)dev_alloc(VF_TOK * sizeof(int2));
 	CUDA_CHECK(cudaMemcpyAsync(pf.sbrows, rows, nseq * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
-	// the prompts in blocks of at most chunk_cap rows at slot base o: pf.seg holds absolute slots, so a prompt that straddles
-	// a block edge walks its keys from s_b, which the earlier block wrote
-	for (int o = 0; o < G; o += chunk_cap) {
-		const int m = imin((int)G - o, chunk_cap);
-		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, pb.tok.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pb.pos.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		CUDA_CHECK(cudaMemcpyAsync(pf.seg, pb.seg.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		pf_block(m, o, PF_PACKED, nullptr, PfOut());
-	}
+	sb_prefill(pb, 0);
 	sn_decode(PF_BATCH, PfSampleStep{(int)G, 0, nseq, lmax}, tok, pos, n_tokens, temperature, minp, rng_states, out_tokens);
+	return 1;
+}
+
+// ---------------------------------------------------------------------------------------------
+// calm_b200_decode_sample_queue: a queue of requests, at most max_rows in flight.  Before every step the requests at the
+// head of the queue that fit are admitted (a round): their prompts go through the packed prompt pass, then every step is
+// one short block over the rows in flight (PF_QUEUE), and a row retires after max_new tokens or a stop token.  Cache slots
+// are placed by SqSlots (include/calm_b200.h states the rule).
+
+static_assert(SQ_ROWS == VF_TOK, "the rows of a queue step are one token tile of k_vf_gemm");
+
+// First-fit allocation of cache slots in [0, seq_len), coalescing on release
+struct SqSlots {
+	std::map<int, int> free_; // start -> end of each free interval
+	explicit SqSlots(int n) { free_[0] = n; }
+	// the lowest start, a multiple of `align`, of n free slots, taken; -1 if there is none
+	int take(int n, int align) {
+		for (auto it = free_.begin(); it != free_.end(); ++it) {
+			const int s = it->first, e = it->second, a = cdiv(s, align) * align;
+			if (a + n > e) continue;
+			free_.erase(it);
+			if (s < a) free_[s] = a;
+			if (a + n < e) free_[a + n] = e;
+			return a;
+		}
+		return -1;
+	}
+	void give(int s, int n) {
+		if (n == 0) return;
+		int e = s + n;
+		auto nx = free_.lower_bound(s);
+		if (nx != free_.end() && nx->first == e) e = nx->second, nx = free_.erase(nx);
+		if (nx != free_.begin() && std::prev(nx)->second == s) {
+			std::prev(nx)->second = e;
+			return;
+		}
+		free_[s] = e;
+	}
+};
+
+// A request's place: its prompt's L entries at slots s .., its generated entries at slots t ..
+struct SqPlace {
+	int s, L, t;
+};
+
+// The placement of one round, the requests `rs` in input order: one extent of sum ceil8(L) slots starting at a multiple of
+// 8 for their packed prompts, then one extent of max_new slots per request.  False (and `a` spent) when one does not fit.
+static bool sq_place(SqSlots& a, const std::vector<int>& rs, const int* len, const int* max_new, std::vector<SqPlace>& out) {
+	int P = 0;
+	for (int i : rs) P += cdiv(len[i] - 1, 8) * 8;
+	int s = P ? a.take(P, 8) : 0;
+	if (s < 0) return false;
+	out.clear();
+	for (int i : rs) {
+		const int t = a.take(max_new[i], 1);
+		if (t < 0) return false;
+		out.push_back(SqPlace{s, len[i] - 1, t});
+		s += cdiv(len[i] - 1, 8) * 8;
+	}
+	return true;
+}
+
+extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nreq,
+                                             const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
+                                             int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps) {
+	if (!g.ready) CALM_FATAL("decode_sample_queue before prepare_cuda");
+	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("decode_sample_queue: max_rows %d outside [1, %d]", max_rows, CALM_B200_SAMPLE_N_MAX);
+	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("decode_sample_queue: negative nreq %d, n %d or n_stop %d", nreq, n, n_stop);
+	if (n_stop > 0 && !stop) CALM_FATAL("decode_sample_queue: stop is NULL");
+	if (nreq > 0 && (!tokens || !off || !len || !max_new || !temperature || !minp || !rng_states || !out_tokens || !out_len))
+		CALM_FATAL("decode_sample_queue: an array is NULL");
+	size_t total = 0; // sum of max_new: the output's extent
+	for (int i = 0; i < nreq; ++i) {
+		if (max_new[i] < 0) CALM_FATAL("decode_sample_queue: request %d has a negative max_new %d", i, max_new[i]);
+		if (len[i] < 1 || off[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("decode_sample_queue: prompt %d (off %d, len %d) empty or outside the %d tokens", i, off[i], len[i], n);
+		total += max_new[i];
+	}
+	if (total > 0x7fffffff) CALM_FATAL("decode_sample_queue: %zu output tokens do not fit an int index", total);
+	check_tokens(tokens, n);
+	check_tokens(stop, n_stop);
+	if (steps) *steps = 0;
+	std::vector<char> is_stop(g.cfg.vocab_size, 0);
+	for (int k = 0; k < n_stop; ++k) is_stop[stop[k]] = 1;
+	std::vector<size_t> O(nreq + 1, 0); // request i's tokens go to out_tokens[O[i] ..]
+	for (int i = 0; i < nreq; ++i) O[i + 1] = O[i] + max_new[i];
+	for (int i = 0; i < nreq; ++i)
+		if (max_new[i] == 0) out_len[i] = 0; // never admitted
+	if (total == 0) return 1;
+	auto is_greedy = [&](int i) { return temperature[i] == 0.0f || minp[i] >= 1.0f; }; // sample() is greedy there
+	bool fits = true;
+	int P = 0, chunks = 0;
+	for (int i = 0; i < nreq; ++i) {
+		if (max_new[i] == 0) continue;
+		const int L = len[i] - 1;
+		fits = fits && (long long)cdiv(L, 8) * 8 + max_new[i] <= g.cfg.seq_len;
+		P = imin(P + cdiv(L, 8) * 8, SB_BLOCK), chunks = std::max(chunks, cdiv(L + max_new[i], SN_CHUNK));
+	}
+	if (!pf_supported() || !fits) { // each request alone: decode_sample's stream, cut at its first stop token
+		for (int i = 0; i < nreq; ++i) {
+			const int* p = tokens + off[i];
+			const int L = len[i] - 1;
+			int tok = p[L], k = 0;
+			if (max_new[i] > 0) forward_prefill_cuda(transformer, p, L, 0);
+			while (k < max_new[i]) {
+				tok = calm_b200_forward_sample(transformer, tok, L + k, temperature[i], minp[i], &rng_states[i]);
+				out_tokens[O[i] + k++] = tok;
+				if (is_stop[tok]) break;
+			}
+			out_len[i] = k;
+		}
+		return 0;
+	}
+	sn_reserve(std::max(P, VF_TOK), chunks);
+	if (!pf.sqrows) {
+		pf.sqrows = (SqRows*)dev_alloc(sizeof(SqRows));
+		pf.sqtok = (int*)dev_alloc(VF_TOK * sizeof(int));
+	}
+	if (total > pf.sqout_cap || (size_t)nreq > pf.sqst_cap) { // (no step of an earlier call is still reading them)
+		CUDA_CHECK(cudaStreamSynchronize(g.stream));
+		cudaFree(pf.sqout), cudaFree(pf.sqst);
+		pf.sqout_cap = std::max(total, pf.sqout_cap), pf.sqst_cap = std::max((size_t)nreq, pf.sqst_cap);
+		pf.sqout = (int*)dev_alloc(pf.sqout_cap * sizeof(int));
+		pf.sqst = (unsigned long long*)dev_alloc(pf.sqst_cap * sizeof(unsigned long long));
+	}
+
+	SqSlots slots(g.cfg.seq_len);
+	std::vector<SqPlace> place(nreq);
+	std::vector<int> done(nreq, 0), row_of(nreq, -1); // tokens so far; row in the last step
+	std::vector<int> live;                            // requests in flight, in admission order
+	int head = 0, nsteps = 0, last_sampled = 0, tok_host[VF_TOK]; // last_sampled: the last step's rows if it sampled
+
+	for (;;) {
+		// admission: the requests at the head of the queue, in input order, while a row is free and the round's placement
+		// (recomputed with each newcomer, from the slots free before the round) fits
+		std::vector<int> round;
+		std::vector<SqPlace> rp;
+		SqSlots after = slots;
+		while (head < nreq && (int)(live.size() + round.size()) < max_rows) {
+			if (max_new[head] == 0) {
+				++head;
+				continue;
+			}
+			std::vector<int> trial = round;
+			trial.push_back(head);
+			SqSlots a = slots;
+			std::vector<SqPlace> tp;
+			if (!sq_place(a, trial, len, max_new, tp)) break;
+			round.swap(trial), rp.swap(tp), after = a, ++head;
+		}
+		if (live.empty() && round.empty()) break;
+		if (!round.empty()) {
+			slots = after;
+			PfPackedBlock pb;
+			for (size_t k = 0; k < round.size(); ++k) {
+				const int i = round[k];
+				place[i] = rp[k];
+				pb.add(tokens + off[i], rp[k].L, rp[k].L, 0, make_int2(0, 0));
+			}
+			if (pb.rows()) sb_prefill(pb, rp[0].s);
+			live.insert(live.end(), round.begin(), round.end());
+		}
+		// the step: the rows in flight, in admission order
+		SqRows r = {};
+		r.n = (int)live.size();
+		int nsampled = 0, lmax = 0;
+		for (int k = 0; k < r.n; ++k) {
+			const int i = live[k], j = done[i];
+			const SqPlace& q = place[i];
+			r.q[k] = make_int4(q.s, q.L, q.t, j), r.pos[k] = q.L + j, r.slot[k] = q.t + j;
+			r.src[k] = row_of[i], r.tok0[k] = tokens[off[i] + q.L];
+			const bool gr = is_greedy(i);
+			// (a greedy row's sampler state is never read back: any valid one will do)
+			r.st0[k].rng = gr ? 1 : rng_states[i], r.st0[k].temperature = gr ? 1.0f : temperature[i], r.st0[k].cut_delta = gr ? 0.0f : logf(minp[i]) * temperature[i];
+			r.out[k] = (int)(O[i] + j), r.req[k] = i, r.greedy[k] = gr;
+			nsampled += !gr, lmax = std::max(lmax, q.L + j), row_of[i] = k;
+		}
+		launch_pdl(k_sq_begin, 1, 32, 0, r, pf.sqrows, (const int*)pf.sqtok, pf.tokens, pf.vstate);
+		const PfSampleStep ss = {0, 0, r.n, lmax};
+		with_formats([&](auto f) {
+			pf_run(f, r.n, 0, PF_QUEUE, &ss);
+			pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
+		});
+		if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
+		if (nsampled > 0) vf_sample_rows(r.n);
+		launch_pdl(k_sq_end, 1, 32, 0, (const SqRows*)pf.sqrows, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate, pf.sqtok, pf.sqout, pf.sqst);
+		++nsteps, last_sampled = nsampled > 0 ? r.n : 0;
+		if (n_stop) { // the step's tokens decide which rows stop
+			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, r.n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+			sync_stream();
+		}
+		// retire: rows that reached max_new or emitted a stop token free their slots; the others keep their order
+		std::vector<int> keep;
+		for (int k = 0; k < r.n; ++k) {
+			const int i = live[k];
+			++done[i];
+			if (done[i] < max_new[i] && !(n_stop && is_stop[tok_host[k]])) {
+				keep.push_back(i);
+				continue;
+			}
+			out_len[i] = done[i];
+			slots.give(place[i].s, cdiv(place[i].L, 8) * 8), slots.give(place[i].t, max_new[i]);
+		}
+		live.swap(keep);
+	}
+	std::vector<int> all(total);
+	std::vector<unsigned long long> st(nreq);
+	CUDA_CHECK(cudaMemcpyAsync(all.data(), pf.sqout, total * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(st.data(), pf.sqst, nreq * sizeof(unsigned long long), cudaMemcpyDeviceToHost, g.stream));
+	sync_stream();
+	CUDA_CHECK(cudaGetLastError());
+	for (int i = 0; i < nreq; ++i) {
+		std::copy(all.begin() + O[i], all.begin() + O[i] + out_len[i], out_tokens + O[i]);
+		if (out_len[i] > 0 && !is_greedy(i)) rng_states[i] = st[i];
+	}
+	if (last_sampled) pf.vrows = last_sampled;
+	if (steps) *steps = nsteps;
 	return 1;
 }
 
@@ -2172,8 +2423,8 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 // attention's {value, epoch} cells and counter, k_vf_gemm's arrival counters, the tensor-parallel exchange area, moe_sel, the sampler's state and survivor
 // counts (the decode's and the sampled short block's), stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
 // as do the index buffers (cand_idx, sample_idx, pf.vsidx, out_tokens, pf.tokens, pf.targets, pf.rowpos, pf.seg and pf.ctx, read
-// as a RoPE position and as key slots of the packed attention's loop, and pf.sbrows, decode_sample_batch's key slots and
-// chunk counts): a stale index that is read is in range,
+// as a RoPE position and as key slots of the packed attention's loop, pf.sbrows, decode_sample_batch's key slots and
+// chunk counts, and pf.sqrows, decode_sample_queue's row table): a stale index that is read is in range,
 // as after any earlier call, while 0xFFFFFFFF would send the read out of bounds.  DESIGN.md s.3 lists both groups.
 extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos) {
 	(void)transformer;
@@ -2214,6 +2465,9 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		// decode_sample_n's chunk partials and step tokens, which every call writes before it reads them (its positions,
 		// read as RoPE positions, are an index buffer)
 		nan(pf.snpart, (size_t)VF_TOK * c.n_heads * pf.snchunks * (c.head_dim + 2) * sizeof(float)), nan(pf.sntok, (size_t)c.seq_len * sizeof(int));
+		// decode_sample_queue's step tokens and per-request tokens and states, which every call writes before it reads them
+		// (its row table, read as positions and key slots, is an index buffer)
+		nan(pf.sqtok, VF_TOK * sizeof(int)), nan(pf.sqout, pf.sqout_cap * sizeof(int)), nan(pf.sqst, pf.sqst_cap * sizeof(unsigned long long));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

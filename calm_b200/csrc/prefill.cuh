@@ -42,7 +42,8 @@
 #define PF_BN 128 // tokens per tile       (two consumer warpgroups of 64: the M of the MMA)
 #define PF_BK 64  // k per stage: 64 f16 = 128 bytes = one swizzle atom
 #define PF_THREADS 384 // warpgroup 0: dequantising producers (thread 0 also issues the TMA); warpgroups 1, 2: MMA + epilogue
-enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3, PF_CLS = 4, PF_CLS_GREEDY = 5, PF_CLS_TOPK = 6, PF_CLS_SAMPLE = 7 }; // PF_CLS_GREEDY: PF_CLS + each tile's argmax; PF_CLS_SAMPLE (k_vf_gemm only): PF_CLS_GREEDY + the logit rows
+enum { PF_QKV = 0, PF_WO = 1, PF_UP = 2, PF_DOWN = 3, PF_CLS = 4, PF_CLS_GREEDY = 5, PF_CLS_TOPK = 6, PF_CLS_SAMPLE = 7, PF_QKV_SLOTS = 8 }; // PF_CLS_GREEDY: PF_CLS + each tile's argmax; PF_CLS_SAMPLE (k_vf_gemm only): PF_CLS_GREEDY + the logit rows
+// PF_QKV_SLOTS (k_vf_gemm only): PF_QKV, but row t's keys and values go to cache slot VfArgs::slot[t] instead of pos0 + t
 #define PF_TOPK_MAX 20 // PF_CLS_TOPK: PF_CLS + each tile's k <= PF_TOPK_MAX largest logits (CALM_B200_TOPK_MAX)
 
 // ---------------------------------------------------------------- wgmma / TMA wrappers

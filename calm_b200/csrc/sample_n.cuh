@@ -26,6 +26,12 @@
 // (nch = gridDim.x / nseq, the longest row's chunk count), and a CTA past its row's chunks returns.  A query's staging,
 // scores, chunk softmax, value pass and fold are the plain kernels' operations in the same order, so row b gives what
 // calm_b200_decode_sample_n gives one sequence over the same keys at pos0 = L_b.
+//
+// QUEUE (with BATCH; calm_b200_decode_sample_queue): rows run requests that were admitted at different steps, so each row
+// has its own step count and its own generated slots.  qrows[r] = (s, L, t, j): the row's prompt entries are at slots
+// s .. s + L - 1, its generated entries at slots t, t + 1, .., and it is at its own step j, so its keys are v = 0 .. L + j:
+// v < L is slot s + v, v >= L is slot t + (v - L).  Grid, chunking and every floating-point operation are BATCH's, so a row
+// gives what decode_sample_batch gives its sequence over the same keys at step j.
 #pragma once
 
 #include "prefill.cuh"
@@ -43,6 +49,7 @@ struct SnAttnArgs {
 	int pos0, step, nseq, seq_len, q_dim, kv_mul, n_heads, nchmax;
 	float inv_sqrt_hd;
 	const int2* rows; // [nseq] (BATCH) row b's prompt: its first slot s_b and its length L_b; read by no other variant
+	const int4* qrows; // [nseq] (QUEUE) row b's (s, L, t, j); read by no other variant
 };
 
 // dynamic shared memory of k_sn_attn: the K tile (padded rows), the V tile, each warp's KM queries
@@ -52,9 +59,11 @@ constexpr size_t sn_smem_bytes() {
 }
 
 // grid (prompt chunks + nseq x suffix chunks, kv heads): CTA x < pos0 / SN_CHUNK is prompt chunk x for every row, the
-// others are suffix chunk x' % nsuf of row x' / nsuf (x' = x - prompt chunks).  BATCH: grid (nseq x nch, kv heads).
-template <typename KVT, int HD, int KM, bool BATCH = false>
+// others are suffix chunk x' % nsuf of row x' / nsuf (x' = x - prompt chunks).  BATCH (and QUEUE): grid (nseq x nch, kv
+// heads).
+template <typename KVT, int HD, int KM, bool BATCH = false, bool QUEUE = false>
 __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
+	static_assert(BATCH || !QUEUE, "a queue step is a batch step with per-row step counts");
 	pdl_enter();
 	constexpr int DPL = HD / 32, KPL = SN_CHUNK / 32;
 	constexpr int VSTR = HD * sizeof(KVT), KSTR = VSTR + 16; // padded key row, as k_pf_attn's
@@ -67,7 +76,10 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 	if constexpr (BATCH) {
 		const int nch = gridDim.x / a.nseq;
 		b0 = blockIdx.x / nch, c = blockIdx.x % nch, nrows = 1;
-		nkeys = __ldg(&a.rows[b0].y) + a.step + 1;
+		if constexpr (QUEUE) {
+			const int4 qr = __ldg(a.qrows + b0);
+			nkeys = qr.y + qr.w + 1;
+		} else nkeys = __ldg(&a.rows[b0].y) + a.step + 1;
 		if (c * SN_CHUNK >= nkeys) return;
 	} else {
 		nkeys = a.pos0 + a.step + 1, c = blockIdx.x, b0 = 0, nrows = a.nseq;
@@ -84,7 +96,11 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 		const int row = i / (VSTR / 16), cc = i % (VSTR / 16), v = v0 + row;
 		const bool in = row < nk;
 		int slot;
-		if constexpr (BATCH) { // (read per key: held in registers through the score pass, they add spills)
+		if constexpr (QUEUE) { // (scalar loads: the whole int4 held through the score pass adds spills)
+			const int* qr = reinterpret_cast<const int*>(a.qrows + b0);
+			const int L = __ldg(qr + 1);
+			slot = v < L ? __ldg(qr) + v : __ldg(qr + 2) + (v - L);
+		} else if constexpr (BATCH) { // (read per key: held in registers through the score pass, they add spills)
 			const int2 pr = __ldg(a.rows + b0);
 			slot = v < pr.y ? pr.x + v : a.pos0 + (v - pr.y) * a.nseq + b0;
 		} else slot = v < a.pos0 ? v : a.pos0 + (v - a.pos0) * a.nseq + b0;
@@ -174,13 +190,16 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 }
 
 // grid (cdiv(n_heads, SN_WARPS), nseq): warp = query head, lane = head dims [lane * DPL, lane * DPL + DPL)
-template <int HD, bool BATCH = false>
+template <int HD, bool BATCH = false, bool QUEUE = false>
 __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_fold(const SnAttnArgs a) {
 	pdl_enter();
 	constexpr int DPL = HD / 32;
 	const int lane = threadIdx.x & 31, h = blockIdx.x * SN_WARPS + (threadIdx.x >> 5), b = blockIdx.y;
 	if (h >= a.n_heads) return;
-	const int nch = ((BATCH ? a.rows[b].y : a.pos0) + a.step + SN_CHUNK) / SN_CHUNK;
+	int last; // the row's last virtual key
+	if constexpr (QUEUE) last = a.qrows[b].y + a.qrows[b].w;
+	else last = (BATCH ? a.rows[b].y : a.pos0) + a.step;
+	const int nch = (last + SN_CHUNK) / SN_CHUNK;
 	const float* p = a.part + ((size_t)b * a.n_heads + h) * a.nchmax * (HD + 2);
 	float mx = -FLT_MAX;
 	for (int c = lane; c < nch; c += 32) mx = fmaxf(mx, __ldcg(p + (size_t)c * (HD + 2)));
@@ -203,4 +222,53 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_fold(const SnAttnArgs a) {
 		const size_t o = (size_t)b * a.q_dim + (size_t)h * HD + lane * DPL + d;
 		a.Ohi[o] = hh, a.Olo[o] = hl;
 	}
+}
+
+// ---------------------------------------------------------------- calm_b200_decode_sample_queue's rows
+
+#define SQ_ROWS 16 // rows of a queue step: one token tile of k_vf_gemm
+
+// The rows of one queue step, row r in admission order.  Passed by value to k_sq_begin, which keeps it where the step's
+// kernels read it.
+struct SqRows {
+	int4 q[SQ_ROWS];          // (s, L, t, j): k_sn_attn<.., QUEUE>'s key mapping
+	int pos[SQ_ROWS];         // RoPE position L + j (k_pf_rope_rows)
+	int slot[SQ_ROWS];        // cache slot t + j of the row's keys and values (k_vf_gemm<PF_QKV_SLOTS>)
+	int src[SQ_ROWS];         // the previous step's row this row continues, or -1 for a row admitted before this step
+	int tok0[SQ_ROWS];        // (src -1) the last token of the row's prompt
+	SampleState st0[SQ_ROWS]; // (src -1) the row's sampler state
+	int out[SQ_ROWS];         // where the row's token goes in pf.sqout
+	int req[SQ_ROWS];         // the row's request, its slot in pf.sqst
+	int greedy[SQ_ROWS];      // 1: the row takes the argmax (pf.greedy), 0: the sampler's token (pf.vsampled)
+	int n;
+};
+
+// one warp, before a step: keep the table, then give each row its token and sampler state, taken from the previous step's
+// row it continues or from the table.  Rows only move down, onto rows other lanes read, so every lane reads first.
+__global__ void __launch_bounds__(32) k_sq_begin(const SqRows r, SqRows* tab, const int* prev, int* tokens, SampleState* st) {
+	pdl_enter();
+	const int i = threadIdx.x;
+	for (int k = i; k < (int)(sizeof(SqRows) / sizeof(int)); k += 32) reinterpret_cast<int*>(tab)[k] = reinterpret_cast<const int*>(&r)[k];
+	int tok = 0;
+	SampleState s = {};
+	if (i < r.n) {
+		const int from = r.src[i];
+		tok = from >= 0 ? prev[from] : r.tok0[i];
+		s = from >= 0 ? st[from] : r.st0[i];
+	}
+	__syncwarp();
+	if (i < r.n) tokens[i] = tok, st[i] = s;
+}
+
+// one warp, after a step: each row's token (the argmax or the sampler's) to the step's tokens and to the row's output
+// slot, and a sampled row's generator state to its request
+__global__ void __launch_bounds__(32) k_sq_end(const SqRows* tab, const int* greedy, const int* sampled, const SampleState* st, int* step_tok, int* out,
+                                               unsigned long long* rng) {
+	pdl_enter();
+	const int i = threadIdx.x;
+	if (i >= tab->n) return;
+	const bool gr = tab->greedy[i];
+	const int tok = gr ? greedy[i] : sampled[i];
+	step_tok[i] = tok, out[tab->out[i]] = tok;
+	if (!gr) rng[tab->req[i]] = st[i].rng;
 }

@@ -18,6 +18,7 @@
 //               PF_CLS_SAMPLE (calm_b200_verify_sample) is PF_CLS_GREEDY that also stores the fold's logits of every
 //               token row, and each tile's maximum, which k_sample_scan_rows / k_sample_pick_rows (stages.cuh) sample,
 //               all rows side by side: the same accumulator values the argmax records come from.
+//               PF_QKV_SLOTS (calm_b200_decode_sample_queue) is PF_QKV with each row's keys and values at its own slot.
 #pragma once
 
 #include "prefill.cuh"
@@ -40,6 +41,7 @@ struct VfArgs {
 	int tile0, nvt;    // CLS: the first vocabulary tile of this launch, and the tiles of the vocabulary
 	float* logits;     // PF_CLS_SAMPLE: [n_tokens][vocab] the logit rows
 	float* tmax;       // PF_CLS_SAMPLE: [n_tokens][nvt] each tile's maximum logit (the sampler's cand_val)
+	const int* slot;   // PF_QKV_SLOTS: [n_tokens] the cache slot of each row's keys and values
 };
 
 template <int DBITS>
@@ -105,7 +107,7 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 
 	// the weight row of partial-sum row r (this launch's numbering)
 	auto row_ptr = [&](int r) -> const unsigned char* {
-		if constexpr (MODE == PF_QKV) {
+		if constexpr (MODE == PF_QKV || MODE == PF_QKV_SLOTS) {
 			const void* w = r < a.q_dim ? a.w[0] : (r < a.q_dim + a.kv_dim ? a.w[1] : a.w[2]);
 			const int k = r < a.q_dim ? r : (r < a.q_dim + a.kv_dim ? r - a.q_dim : r - a.q_dim - a.kv_dim);
 			return reinterpret_cast<const unsigned char*>(w) + (size_t)k * rowbytes;
@@ -273,7 +275,7 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 			for (int j = 0; j < 4; ++j) {
 				const int t = 4 * tq + j;
 				if (t >= a.n_tokens) continue;
-				if constexpr (MODE == PF_QKV) {
+				if constexpr (MODE == PF_QKV || MODE == PF_QKV_SLOTS) {
 					float x0 = x[0][j], x1 = x[1][j];
 					const bool is_q = gr < a.q_dim, is_k = !is_q && gr < a.q_dim + a.kv_dim;
 					const int k = is_q ? gr : (is_k ? gr - a.q_dim : gr - a.q_dim - a.kv_dim);
@@ -288,8 +290,13 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 					if (is_q) {
 						*reinterpret_cast<float2*>(a.Q + (size_t)t * a.q_dim + k) = make_float2(x0, x1);
 					} else {
-						KVT* dst = reinterpret_cast<KVT*>(is_k ? a.kc : a.vc) + ((size_t)hh * a.seq_len + a.pos0 + t) * a.head_dim + d;
-						kv_store(dst, x0), kv_store(dst + 1, x1);
+						if constexpr (MODE == PF_QKV_SLOTS) { // (a statement of its own: PF_QKV's address arithmetic stays as it was)
+							KVT* dst = reinterpret_cast<KVT*>(is_k ? a.kc : a.vc) + ((size_t)hh * a.seq_len + v.slot[t]) * a.head_dim + d;
+							kv_store(dst, x0), kv_store(dst + 1, x1);
+						} else {
+							KVT* dst = reinterpret_cast<KVT*>(is_k ? a.kc : a.vc) + ((size_t)hh * a.seq_len + a.pos0 + t) * a.head_dim + d;
+							kv_store(dst, x0), kv_store(dst + 1, x1);
+						}
 					}
 				} else {
 					pf_epilogue_pair<MODE>(a, gr, t, x[0][j], x[1][j], gt[0][j], gt[1][j]);

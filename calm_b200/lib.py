@@ -27,7 +27,7 @@ SYMBOLS = [
     "calm_b200_score_topk", "calm_b200_score_batch_topk", "calm_b200_score_context_topk",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
-    "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch",
+    "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -41,7 +41,8 @@ TOPK_MAX = 20
 # the largest block calm_b200_verify_greedy takes (CALM_B200_VERIFY_MAX); decode_lookup drafts at most one fewer
 VERIFY_MAX = 16
 
-# the most sequences calm_b200_decode_sample_n and calm_b200_decode_sample_batch sample together (CALM_B200_SAMPLE_N_MAX)
+# the most sequences calm_b200_decode_sample_n and calm_b200_decode_sample_batch sample together, and the most rows
+# calm_b200_decode_sample_queue keeps in flight (CALM_B200_SAMPLE_N_MAX)
 SAMPLE_N_MAX = 16
 
 # calm_b200_read_state selectors (include/calm_b200.h)
@@ -100,6 +101,9 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_n.restype = C.c_int
     L.calm_b200_decode_sample_batch.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, C.c_int, C.c_int, C.c_float, C.c_float, _u64p, _iptr]
     L.calm_b200_decode_sample_batch.restype = C.c_int
+    L.calm_b200_decode_sample_queue.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, C.c_int, _iptr, _fptr, _fptr, _iptr, C.c_int, C.c_int, _u64p, _iptr,
+                                                _iptr, _iptr]
+    L.calm_b200_decode_sample_queue.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -462,6 +466,64 @@ class DeviceModel:
                                                         len_.ctypes.data_as(ip), nseq, int(n_tokens), temperature, minp, rng,
                                                         out.ctypes.data_as(ip))
         return out, [int(s) for s in rng], served
+
+    def decode_sample_queue(self, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states):
+        """calm_b200_decode_sample_queue: request i continues prompts[i] (a sequence of at least one token id) for at most
+        max_new[i] tokens at temperature[i] / minp[i] from rng_states[i], stopping after a token in `stop` (a sequence of
+        ids shared by all requests, possibly empty), with at most max_rows requests in flight.  Returns (tokens, states,
+        served, steps): tokens[i] is request i's int32 tokens (its out_len[i] of them), states the nreq generator states
+        after the call, served 1 on the new path and 0 when the per-request fallback gave them, steps the number of steps
+        run.  Raises ValueError where the C call would abort, and for per-request lists whose lengths differ."""
+        if prompts is None or rng_states is None or isinstance(rng_states, (int, np.integer)):
+            raise ValueError("decode_sample_queue takes a list of prompts and a sequence of generator states, one per prompt")
+        prompts = [np.asarray(p) for p in prompts]
+        nreq = len(prompts)
+        states = list(rng_states)
+        try:
+            max_new = [m for m in max_new]
+            temperature = np.ascontiguousarray(temperature, np.float32).reshape(-1)
+            minp = np.ascontiguousarray(minp, np.float32).reshape(-1)
+            stop = np.asarray([] if stop is None else stop)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"decode_sample_queue: bad per-request list: {e}") from None
+        for name, xs in (("max_new", max_new), ("temperature", temperature), ("minp", minp), ("rng_states", states)):
+            if len(xs) != nreq:
+                raise ValueError(f"decode_sample_queue takes one {name} per prompt: {nreq} prompts, {len(xs)} values")
+        if not isinstance(max_rows, (int, np.integer)) or not 1 <= max_rows <= SAMPLE_N_MAX:
+            raise ValueError(f"max_rows must be an integer in [1, {SAMPLE_N_MAX}], got {max_rows!r}")
+        for s in states:
+            _check_rng(s)
+        for i, m in enumerate(max_new):
+            if not isinstance(m, (int, np.integer)) or m < 0:
+                raise ValueError(f"max_new[{i}] must be a non-negative integer, got {m!r}")
+        for i, p in enumerate(prompts):
+            if p.ndim != 1 or len(p) < 1 or p.dtype.kind not in "iu":
+                raise ValueError(f"prompt {i} must be a non-empty sequence of token ids")
+            if not ((p >= 0) & (p < self.vocab)).all():
+                raise ValueError(f"prompt {i} has a token outside [0, {self.vocab})")
+        if stop.ndim != 1 or (len(stop) and stop.dtype.kind not in "iu"):
+            raise ValueError("stop must be a sequence of token ids")
+        if not ((stop >= 0) & (stop < self.vocab)).all():
+            raise ValueError(f"a stop id is outside [0, {self.vocab})")
+        if sum(int(m) for m in max_new) >= 1 << 31:
+            raise ValueError("decode_sample_queue: the sum of max_new does not fit an int")
+        tokens = np.ascontiguousarray(np.concatenate(prompts) if nreq else np.zeros(0), np.int32)
+        len_ = np.asarray([len(p) for p in prompts], np.int32)
+        off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(len_)[:-1]]) if nreq else np.zeros(0), np.int32)
+        mn = np.ascontiguousarray(max_new, np.int32)
+        st = np.ascontiguousarray(stop, np.int32)
+        rng = (C.c_ulonglong * max(nreq, 1))(*[int(s) for s in states])
+        out = np.full(max(int(mn.sum()), 1), -1, np.int32)
+        out_len = np.zeros(max(nreq, 1), np.int32)
+        steps = C.c_int(-1)
+        ip, fp = C.POINTER(C.c_int), C.POINTER(C.c_float)
+        served = self.lib.calm_b200_decode_sample_queue(C.byref(self.transformer), tokens.ctypes.data_as(ip), len(tokens), off.ctypes.data_as(ip),
+                                                        len_.ctypes.data_as(ip), nreq, mn.ctypes.data_as(ip), temperature.ctypes.data_as(fp),
+                                                        minp.ctypes.data_as(fp), st.ctypes.data_as(ip) if len(st) else None, len(st), int(max_rows),
+                                                        rng, out.ctypes.data_as(ip), out_len.ctypes.data_as(ip), C.byref(steps))
+        o = np.concatenate([[0], np.cumsum(mn)]).astype(np.int64)
+        toks = [out[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)]
+        return toks, [int(rng[i]) for i in range(nreq)], served, int(steps.value)
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""

@@ -284,6 +284,40 @@ int calm_b200_decode_sample_n(struct Transformer* transformer, int token0, int p
 int calm_b200_decode_sample_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
                                   int n_tokens, float temperature, float minp, unsigned long long* rng_states, int* out_tokens);
 
+/* Generate for a queue of nreq requests, at most max_rows (1 .. CALM_B200_SAMPLE_N_MAX) in flight, each with its own
+ * length, sampling settings and generator, and admit new requests as rows finish (DESIGN.md s.6).  Request i's prompt is
+ * tokens[off[i] .. off[i] + len[i]), len[i] >= 1, as in calm_b200_decode_sample_batch; it generates at most
+ * max_new[i] >= 0 tokens at temperature[i] / minp[i] from rng_states[i].  stop[0 .. n_stop) is one list of stop ids shared
+ * by all requests (NULL when n_stop == 0).  Request i writes its tokens to out_tokens[O_i ..], O_i = max_new[0] + .. +
+ * max_new[i - 1], and its count to out_len[i]: the smaller of max_new[i] and 1 + the index of its first token in stop
+ * (the stop token is emitted); out_tokens past out_len[i] are left untouched.  steps (may be NULL) receives the number of
+ * steps the call ran, each one pass over the weights for the rows in flight.
+ * Returns 1 on the new path: request i's tokens and its final rng_states[i] are then bit for bit those of
+ * calm_b200_decode_sample_batch over its prompt alone (nseq = 1) with n_tokens = out_len[i], whatever the other requests,
+ * max_rows, the admission order, the slots it was given or seq_len.  temperature[i] == 0 or minp[i] >= 1 makes request i
+ * its greedy stream and leaves its state alone; max_new[i] == 0 gives out_len[i] = 0, and the request is never admitted.
+ * Schedule.  Before every step the requests at the head of the queue are admitted in input order (no overtaking), while
+ * a row is free and the placement below of the requests admitted so far before this step (a round), with the next one
+ * added, fits.  A round's prompts go through the packed prompt pass together.  A step runs every request in flight once;
+ * its rows are in admission order, and a request retires after the step that gave its max_new-th or its stop token.
+ * Placement.  The cache slots [0, seq_len) are free at the start.  A round's placement, computed from the slots free
+ * before the round, takes first one extent of the sum of ceil8(len[i] - 1) over its requests, at the lowest free start
+ * that is a multiple of 8, holding their prompts packed in input order (request i's L_i = len[i] - 1 entries at slots
+ * s_i ..); then, in input order, one extent of max_new[i] slots per request at the lowest free start (t_i ..).  Step j of
+ * request i feeds its last token at RoPE position L_i + j and writes slot t_i + j.  A retiring request frees its
+ * ceil8(L_i) prompt slots and its max_new[i] generated slots, and adjacent free slots merge.
+ * Shapes the prompt pass does not serve (as for calm_b200_verify_greedy), and calls with a request whose
+ * ceil8(len[i] - 1) + max_new[i] > seq_len, return 0: each request then runs in input order as forward_prefill_cuda of
+ * its first len[i] - 1 tokens and calm_b200_forward_sample from its last token, token by token, until a stop token or
+ * max_new[i] (decode_sample's stream, cut), and *steps = 0.  The call aborts before any device work when an array it
+ * needs is NULL, max_rows is outside its range, nreq, n or n_stop is negative, a max_new is negative, a prompt is empty
+ * or outside tokens[0 .. n), or a token of tokens[0 .. n) or a stop id is outside the vocabulary.  The KV cache
+ * afterwards holds nothing a host can continue from.  The first call allocates what calm_b200_decode_sample_batch
+ * allocates, and room for max_new[0] + .. + max_new[nreq - 1] tokens and nreq states, regrown by a larger call. */
+int calm_b200_decode_sample_queue(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nreq,
+                                  const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
+                                  int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
@@ -330,9 +364,11 @@ void calm_b200_read_kv(struct Transformer* transformer, int layer, int kv_pos, f
  *   PF_LOGITS  float[n][vocab]          the logit rows of the last calm_b200_verify_sample block that took the short-block
  *            path (n of its tokens), or of the last step of the last sampled calm_b200_decode_sample_n or
  *            calm_b200_decode_sample_batch call that took its new path (n = nseq, row b = sequence b), the values its
- *            sampler drew from
+ *            sampler drew from, or of the last step of a calm_b200_decode_sample_queue call on its new path if that step
+ *            sampled any row (n = the rows in flight)
  *   After calm_b200_decode_sample_n or calm_b200_decode_sample_batch on its new path, the PF_* matrices hold the last
- *   step, row b = sequence b. */
+ *   step, row b = sequence b.  After calm_b200_decode_sample_queue on its new path, the PF_* matrices and PF_LOGITS hold
+ *   the last step, with the rows in flight in admission order. */
 enum {
 	CALM_B200_STATE_X = 0, CALM_B200_STATE_XB = 1, CALM_B200_STATE_Q = 2, CALM_B200_STATE_ATT = 3, CALM_B200_STATE_HB = 4,
 	CALM_B200_STATE_MOE_SEL = 5, CALM_B200_STATE_KEYS = 6, CALM_B200_STATE_VALUES = 7,
