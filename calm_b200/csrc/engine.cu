@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <iterator>
 #include <map>
+#include <set>
 #include <vector>
 
 #include "stages.cuh"
@@ -187,6 +188,7 @@ struct Prefill {
 	// requests generated from a queue (calm_b200_decode_sample_queue), allocated on its first call and regrown when a call
 	// needs more: the step's row table (written by k_sq_begin), the step's tokens, and every request's tokens and state
 	SqRows* sqrows = nullptr;
+	SqGroups* sqgroups = nullptr;      // the step's context groups (written by k_sq_groups), on steps whose rows have contexts
 	int* sqtok = nullptr;              // [VF_TOK]
 	int* sqout = nullptr;              // [sqout_cap]: request i's tokens from O_i = max_new[0] + .. + max_new[i - 1]
 	unsigned long long* sqst = nullptr; // [sqst_cap]: request i's generator state after its last sampled step
@@ -203,7 +205,7 @@ void pf_free() {
 	cudaFree(pf.vacc), cudaFree(pf.vcnt);
 	cudaFree(pf.vlogits), cudaFree(pf.vtmax), cudaFree(pf.vsidx), cudaFree(pf.vsprob), cudaFree(pf.vcsum), cudaFree(pf.vcount), cudaFree(pf.vstate), cudaFree(pf.vsampled);
 	cudaFree(pf.snpart), cudaFree(pf.snpos), cudaFree(pf.sntok), cudaFree(pf.sbrows);
-	cudaFree(pf.sqrows), cudaFree(pf.sqtok), cudaFree(pf.sqout), cudaFree(pf.sqst);
+	cudaFree(pf.sqrows), cudaFree(pf.sqgroups), cudaFree(pf.sqtok), cudaFree(pf.sqout), cudaFree(pf.sqst);
 	pf = Prefill();
 }
 
@@ -1299,24 +1301,28 @@ static void pf_layer_gemm(PfRows layout, const CUtensorMap* tm, const __half* hi
 // A step of calm_b200_decode_sample_n: its n = nseq rows are the sequences, all at RoPE position pos0 + step, row b in
 // cache slot pos0 + step * nseq + b; the prompt is in slots [0, pos0).  A step of calm_b200_decode_sample_batch: the
 // same slots from pos0 = G, the end of the packed prompts, and row b at RoPE position L_b + step; lmax = max_b L_b.  A
-// step of calm_b200_decode_sample_queue: nseq rows, step 0, and lmax = the largest L + j of its rows (pf.sqrows).
+// step of calm_b200_decode_sample_queue: nseq rows, step 0, and lmax = the largest L + j of its rows (pf.sqrows).  A queue
+// step whose rows have contexts (pf.sqgroups): nshared shared chunks and nsuf > 0 per-row chunks per row (sample_n.cuh,
+// GROUPS); nsuf = 0 on every other step.
 struct PfSampleStep {
 	int pos0, step, nseq, lmax;
+	int nshared = 0, nsuf = 0;
 };
 
 // The attention of a PF_SAMPLES step (shared prompt) or, with BATCH, of a PF_BATCH step (a prompt per row), or with
-// QUEUE as well, of a PF_QUEUE step (sample_n.cuh): chunk partials, then their fold into pf.Ahi / pf.Alo
-template <typename KVT, int HD, bool BATCH, bool QUEUE = false>
-static void sn_attn(const SnAttnArgs& a, int lmax) {
+// QUEUE as well, of a PF_QUEUE step (sample_n.cuh), with GROUPS of one whose rows have contexts: chunk partials, then
+// their fold into pf.Ahi / pf.Alo
+template <typename KVT, int HD, bool BATCH, bool QUEUE = false, bool GROUPS = false>
+static void sn_attn(const SnAttnArgs& a, const PfSampleStep& ss) {
 	const int nkeys = a.pos0 + a.step + 1, npre = a.pos0 / SN_CHUNK, nsuf = cdiv(nkeys, SN_CHUNK) - npre;
-	const dim3 grid(BATCH ? a.nseq * cdiv(lmax + a.step + 1, SN_CHUNK) : npre + a.nseq * nsuf, g.cfg.n_kv_heads);
+	const dim3 grid(GROUPS ? ss.nshared + a.nseq * ss.nsuf : BATCH ? a.nseq * cdiv(ss.lmax + a.step + 1, SN_CHUNK) : npre + a.nseq * nsuf, g.cfg.n_kv_heads);
 	auto run = [&](auto kernel, size_t smem) {
 		smem_optin(kernel, smem);
 		launch_pdl(kernel, grid, SN_WARPS * 32, smem, a);
 	};
-	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4, BATCH, QUEUE>, sn_smem_bytes<KVT, HD, 4>());
-	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2, BATCH, QUEUE>, sn_smem_bytes<KVT, HD, 2>());
-	else run(k_sn_attn<KVT, HD, 1, BATCH, QUEUE>, sn_smem_bytes<KVT, HD, 1>());
+	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4, BATCH, QUEUE, GROUPS>, sn_smem_bytes<KVT, HD, 4>());
+	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2, BATCH, QUEUE, GROUPS>, sn_smem_bytes<KVT, HD, 2>());
+	else run(k_sn_attn<KVT, HD, 1, BATCH, QUEUE, GROUPS>, sn_smem_bytes<KVT, HD, 1>());
 	launch_pdl(k_sn_fold<HD, BATCH, QUEUE>, dim3(cdiv(g.cfg.n_heads, SN_WARPS), a.nseq), SN_WARPS * 32, 0, a);
 }
 
@@ -1354,16 +1360,20 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 			sa.Q = pf.Q, sa.kc = a.kc, sa.vc = a.vc, sa.part = pf.snpart, sa.Ohi = pf.Ahi, sa.Olo = pf.Alo;
 			sa.pos0 = ss->pos0, sa.step = ss->step, sa.nseq = ss->nseq, sa.seq_len = c.seq_len, sa.q_dim = g.q_dim, sa.kv_mul = g.kv_mul;
 			sa.n_heads = c.n_heads, sa.nchmax = pf.snchunks, sa.inv_sqrt_hd = aa.inv_sqrt_hd, sa.rows = pf.sbrows;
-			if (layout == PF_QUEUE) {
+			if (layout == PF_QUEUE && ss->nsuf) {
+				sa.qrows = pf.sqrows->q, sa.groups = pf.sqgroups;
+				if (c.head_dim == 128) sn_attn<KVT, 128, true, true, true>(sa, *ss);
+				else sn_attn<KVT, 64, true, true, true>(sa, *ss);
+			} else if (layout == PF_QUEUE) {
 				sa.qrows = pf.sqrows->q;
-				if (c.head_dim == 128) sn_attn<KVT, 128, true, true>(sa, ss->lmax);
-				else sn_attn<KVT, 64, true, true>(sa, ss->lmax);
+				if (c.head_dim == 128) sn_attn<KVT, 128, true, true>(sa, *ss);
+				else sn_attn<KVT, 64, true, true>(sa, *ss);
 			} else if (layout == PF_BATCH) {
-				if (c.head_dim == 128) sn_attn<KVT, 128, true>(sa, ss->lmax);
-				else sn_attn<KVT, 64, true>(sa, ss->lmax);
+				if (c.head_dim == 128) sn_attn<KVT, 128, true>(sa, *ss);
+				else sn_attn<KVT, 64, true>(sa, *ss);
 			} else {
-				if (c.head_dim == 128) sn_attn<KVT, 128, false>(sa, 0);
-				else sn_attn<KVT, 64, false>(sa, 0);
+				if (c.head_dim == 128) sn_attn<KVT, 128, false>(sa, *ss);
+				else sn_attn<KVT, 64, false>(sa, *ss);
 			}
 		} else if (layout == PF_CONTEXTS) {
 			if (c.head_dim == 128) pf_attn<KVT, 128, true, true>(aa, n);
@@ -2036,16 +2046,21 @@ constexpr int SB_BLOCK = 2048; // rows of a block of packed prompts
 
 // The packed prompts of `pb` at cache slots base .. base + pb.rows() - 1, in blocks of at most SB_BLOCK rows at slot base
 // base + o: pf.seg holds absolute slots, so a prompt that straddles a block edge walks its keys from its first slot, which
-// the earlier block wrote.  The caller has reserved the pass for min(pb.rows(), SB_BLOCK) rows.
+// the earlier block wrote.  Rows that continue a context (calm_b200_decode_sample_queue_context) carry its absolute first
+// slot in pb.ctx; a block that holds such a row uploads pf.ctx and runs the context walk (PF_CONTEXTS), which reads the
+// context's slots wherever an earlier block or an earlier call of this function wrote them.  The caller has reserved the
+// pass for min(pb.rows(), SB_BLOCK) rows.
 static void sb_prefill(PfPackedBlock& pb, int base) {
 	for (int& s : pb.seg) s += base;
 	const int G = pb.rows();
 	for (int o = 0; o < G; o += SB_BLOCK) {
 		const int m = imin(G - o, SB_BLOCK);
+		const bool contexts = std::any_of(pb.ctx.begin() + o, pb.ctx.begin() + o + m, [](int2 c) { return c.y > 0; });
 		CUDA_CHECK(cudaMemcpyAsync(pf.tokens, pb.tok.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 		CUDA_CHECK(cudaMemcpyAsync(pf.rowpos, pb.pos.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 		CUDA_CHECK(cudaMemcpyAsync(pf.seg, pb.seg.data() + o, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		pf_block(m, base + o, PF_PACKED, nullptr, PfOut());
+		if (contexts) CUDA_CHECK(cudaMemcpyAsync(pf.ctx, pb.ctx.data() + o, (size_t)m * sizeof(int2), cudaMemcpyHostToDevice, g.stream));
+		pf_block(m, base + o, contexts ? PF_CONTEXTS : PF_PACKED, nullptr, PfOut());
 	}
 }
 
@@ -2125,47 +2140,75 @@ struct SqSlots {
 	}
 };
 
-// A request's place: its prompt's L entries at slots s .., its generated entries at slots t ..
+// A request's place: its context's nc entries at slots c .. (nc = 0: none), its own prompt entries (L - nc of them) at
+// slots s .., its generated entries at slots t ..
 struct SqPlace {
-	int s, L, t;
+	int s, L, t, c, nc;
 };
 
-// The placement of one round, the requests `rs` in input order: one extent of sum ceil8(L) slots starting at a multiple of
-// 8 for their packed prompts, then one extent of max_new slots per request.  False (and `a` spent) when one does not fit.
-static bool sq_place(SqSlots& a, const std::vector<int>& rs, const int* len, const int* max_new, std::vector<SqPlace>& out) {
+using SqCtx = std::pair<int, int>; // a context by (ctx_off, ctx_len): requests share it exactly when these are equal
+
+// The placement of one round, the requests `rs` in input order, with the contexts `resident` holds at their first slots:
+// one extent starting at a multiple of 8 that holds, request by request, the request's context (ceil8(ctx_len) slots) if
+// it is neither resident nor placed by an earlier request of the round, then its own prompt (ceil8(len - 1) slots); then
+// one extent of max_new slots per request.  False (and `a` spent) when one does not fit; `base` gets the first extent's
+// first slot.
+static bool sq_place(SqSlots& a, const std::vector<int>& rs, const int* ctx_off, const int* ctx_len, const int* len, const int* max_new,
+                     const std::map<SqCtx, int>& resident, std::vector<SqPlace>& out, int& base) {
+	std::map<SqCtx, int> placed; // contexts of this round, by their offset in the extent
 	int P = 0;
-	for (int i : rs) P += cdiv(len[i] - 1, 8) * 8;
-	int s = P ? a.take(P, 8) : 0;
-	if (s < 0) return false;
-	out.clear();
 	for (int i : rs) {
+		const SqCtx k(ctx_off[i], ctx_len[i]);
+		if (ctx_len[i] && !resident.count(k) && !placed.count(k)) placed[k] = P, P += cdiv(ctx_len[i], 8) * 8;
+		P += cdiv(len[i] - 1, 8) * 8;
+	}
+	const int s0 = base = P ? a.take(P, 8) : 0;
+	if (s0 < 0) return false;
+	out.clear();
+	std::set<SqCtx> seen;
+	int s = s0;
+	for (int i : rs) {
+		const SqCtx k(ctx_off[i], ctx_len[i]);
+		int c = 0;
+		if (ctx_len[i]) {
+			const auto r = resident.find(k);
+			c = r != resident.end() ? r->second : s0 + placed.at(k);
+			if (r == resident.end() && seen.insert(k).second) s += cdiv(ctx_len[i], 8) * 8;
+		}
 		const int t = a.take(max_new[i], 1);
 		if (t < 0) return false;
-		out.push_back(SqPlace{s, len[i] - 1, t});
+		out.push_back(SqPlace{s, ctx_len[i] + len[i] - 1, t, c, ctx_len[i]});
 		s += cdiv(len[i] - 1, 8) * 8;
 	}
 	return true;
 }
 
-extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nreq,
-                                             const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
-                                             int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps) {
-	if (!g.ready) CALM_FATAL("decode_sample_queue before prepare_cuda");
-	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("decode_sample_queue: max_rows %d outside [1, %d]", max_rows, CALM_B200_SAMPLE_N_MAX);
-	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("decode_sample_queue: negative nreq %d, n %d or n_stop %d", nreq, n, n_stop);
-	if (n_stop > 0 && !stop) CALM_FATAL("decode_sample_queue: stop is NULL");
-	if (nreq > 0 && (!tokens || !off || !len || !max_new || !temperature || !minp || !rng_states || !out_tokens || !out_len))
-		CALM_FATAL("decode_sample_queue: an array is NULL");
+// calm_b200_decode_sample_queue_context, and calm_b200_decode_sample_queue with every ctx_len 0 (`who` names the call in
+// error messages): a round's extent goes through the packed prompt pass (sb_prefill), each request's own rows continuing
+// its context at positions ctx_len .. (PF_CONTEXTS where a block holds such rows); a step whose rows have contexts runs
+// k_sn_attn's GROUPS variant, every other step exactly the QUEUE kernels.
+static int sq_run(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off,
+                  const int* len, int nreq, const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
+                  int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows) {
+	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
+	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, max_rows, CALM_B200_SAMPLE_N_MAX);
+	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, n_stop);
+	if (n_stop > 0 && !stop) CALM_FATAL("%s: stop is NULL", who);
+	if (nreq > 0 && (!tokens || !ctx_off || !ctx_len || !off || !len || !max_new || !temperature || !minp || !rng_states || !out_tokens || !out_len))
+		CALM_FATAL("%s: an array is NULL", who);
 	size_t total = 0; // sum of max_new: the output's extent
 	for (int i = 0; i < nreq; ++i) {
-		if (max_new[i] < 0) CALM_FATAL("decode_sample_queue: request %d has a negative max_new %d", i, max_new[i]);
-		if (len[i] < 1 || off[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("decode_sample_queue: prompt %d (off %d, len %d) empty or outside the %d tokens", i, off[i], len[i], n);
+		if (max_new[i] < 0) CALM_FATAL("%s: request %d has a negative max_new %d", who, i, max_new[i]);
+		if (len[i] < 1 || off[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("%s: prompt %d (off %d, len %d) empty or outside the %d tokens", who, i, off[i], len[i], n);
+		if (ctx_off[i] < 0 || ctx_len[i] < 0 || (long)ctx_off[i] + ctx_len[i] > n)
+			CALM_FATAL("%s: context of request %d (off %d, len %d) outside the %d tokens", who, i, ctx_off[i], ctx_len[i], n);
 		total += max_new[i];
 	}
-	if (total > 0x7fffffff) CALM_FATAL("decode_sample_queue: %zu output tokens do not fit an int index", total);
+	if (total > 0x7fffffff) CALM_FATAL("%s: %zu output tokens do not fit an int index", who, total);
 	check_tokens(tokens, n);
 	check_tokens(stop, n_stop);
 	if (steps) *steps = 0;
+	if (prompt_rows) *prompt_rows = 0;
 	std::vector<char> is_stop(g.cfg.vocab_size, 0);
 	for (int k = 0; k < n_stop; ++k) is_stop[stop[k]] = 1;
 	std::vector<size_t> O(nreq + 1, 0); // request i's tokens go to out_tokens[O[i] ..]
@@ -2178,16 +2221,17 @@ extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, co
 	int P = 0, chunks = 0;
 	for (int i = 0; i < nreq; ++i) {
 		if (max_new[i] == 0) continue;
-		const int L = len[i] - 1;
-		fits = fits && (long long)cdiv(L, 8) * 8 + max_new[i] <= g.cfg.seq_len;
-		P = imin(P + cdiv(L, 8) * 8, SB_BLOCK), chunks = std::max(chunks, cdiv(L + max_new[i], SN_CHUNK));
+		const int Rc = cdiv(ctx_len[i], 8) * 8, L = ctx_len[i] + len[i] - 1;
+		fits = fits && (long long)Rc + cdiv(len[i] - 1, 8) * 8 + max_new[i] <= g.cfg.seq_len;
+		P = imin(P + Rc + cdiv(len[i] - 1, 8) * 8, SB_BLOCK), chunks = std::max(chunks, cdiv(L + max_new[i], SN_CHUNK));
 	}
-	if (!pf_supported() || !fits) { // each request alone: decode_sample's stream, cut at its first stop token
+	if (!pf_supported() || !fits) { // each request alone over ctx ++ prompt: decode_sample's stream, cut at its first stop token
 		for (int i = 0; i < nreq; ++i) {
-			const int* p = tokens + off[i];
-			const int L = len[i] - 1;
+			std::vector<int> p(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
+			p.insert(p.end(), tokens + off[i], tokens + off[i] + len[i]);
+			const int L = (int)p.size() - 1;
 			int tok = p[L], k = 0;
-			if (max_new[i] > 0) forward_prefill_cuda(transformer, p, L, 0);
+			if (max_new[i] > 0) forward_prefill_cuda(transformer, p.data(), L, 0);
 			while (k < max_new[i]) {
 				tok = calm_b200_forward_sample(transformer, tok, L + k, temperature[i], minp[i], &rng_states[i]);
 				out_tokens[O[i] + k++] = tok;
@@ -2200,6 +2244,7 @@ extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, co
 	sn_reserve(std::max(P, VF_TOK), chunks);
 	if (!pf.sqrows) {
 		pf.sqrows = (SqRows*)dev_alloc(sizeof(SqRows));
+		pf.sqgroups = (SqGroups*)dev_alloc(sizeof(SqGroups));
 		pf.sqtok = (int*)dev_alloc(VF_TOK * sizeof(int));
 	}
 	if (total > pf.sqout_cap || (size_t)nreq > pf.sqst_cap) { // (no step of an earlier call is still reading them)
@@ -2211,16 +2256,18 @@ extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, co
 	}
 
 	SqSlots slots(g.cfg.seq_len);
+	std::map<SqCtx, int> resident; // contexts in the cache, at their first slot
 	std::vector<SqPlace> place(nreq);
 	std::vector<int> done(nreq, 0), row_of(nreq, -1); // tokens so far; row in the last step
 	std::vector<int> live;                            // requests in flight, in admission order
-	int head = 0, nsteps = 0, last_sampled = 0, tok_host[VF_TOK]; // last_sampled: the last step's rows if it sampled
-
-	for (;;) {
-		// admission: the requests at the head of the queue, in input order, while a row is free and the round's placement
-		// (recomputed with each newcomer, from the slots free before the round) fits
-		std::vector<int> round;
-		std::vector<SqPlace> rp;
+	int head = 0, nsteps = 0, last_sampled = 0, rows_computed = 0, tok_host[VF_TOK]; // last_sampled: the last step's rows if it sampled
+	std::vector<int> round;
+	std::vector<SqPlace> rp;
+	int rbase = 0; // the round's prompt extent's first slot
+	// admission: the requests at the head of the queue, in input order, while a row is free and the round's placement
+	// (recomputed with each newcomer, from the slots free before the round) fits
+	auto admit = [&]() {
+		round.clear(), rp.clear();
 		SqSlots after = slots;
 		while (head < nreq && (int)(live.size() + round.size()) < max_rows) {
 			if (max_new[head] == 0) {
@@ -2231,38 +2278,88 @@ extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, co
 			trial.push_back(head);
 			SqSlots a = slots;
 			std::vector<SqPlace> tp;
-			if (!sq_place(a, trial, len, max_new, tp)) break;
-			round.swap(trial), rp.swap(tp), after = a, ++head;
+			int tb;
+			if (!sq_place(a, trial, ctx_off, ctx_len, len, max_new, resident, tp, tb)) break;
+			round.swap(trial), rp.swap(tp), after = a, rbase = tb, ++head;
 		}
-		if (live.empty() && round.empty()) break;
+		slots = after;
+	};
+	// release: a resident context that no request in flight or of the round names frees its slots
+	auto release = [&]() {
+		std::set<SqCtx> named;
+		for (int i : live) named.insert(SqCtx(ctx_off[i], ctx_len[i]));
+		for (int i : round) named.insert(SqCtx(ctx_off[i], ctx_len[i]));
+		for (auto it = resident.begin(); it != resident.end();) {
+			if (named.count(it->first)) {
+				++it;
+				continue;
+			}
+			slots.give(it->second, cdiv(it->first.second, 8) * 8);
+			it = resident.erase(it);
+		}
+	};
+
+	for (;;) {
+		admit();
+		release();
+		if (live.empty() && round.empty()) { // the cache is empty now: the head fits
+			admit();
+			if (round.empty()) break;
+		}
 		if (!round.empty()) {
-			slots = after;
 			PfPackedBlock pb;
 			for (size_t k = 0; k < round.size(); ++k) {
 				const int i = round[k];
-				place[i] = rp[k];
-				pb.add(tokens + off[i], rp[k].L, rp[k].L, 0, make_int2(0, 0));
+				const SqPlace& q = rp[k];
+				place[i] = q;
+				const SqCtx key(ctx_off[i], ctx_len[i]);
+				if (q.nc && !resident.count(key)) { // placed by this round, at the extent's next rows
+					resident[key] = q.c;
+					pb.add(tokens + ctx_off[i], q.nc, q.nc - 1, 0, make_int2(0, 0));
+				}
+				pb.add(tokens + off[i], len[i] - 1, len[i] - 1, q.nc, make_int2(q.c, q.nc));
 			}
-			if (pb.rows()) sb_prefill(pb, rp[0].s);
+			if (pb.rows()) sb_prefill(pb, rbase);
+			rows_computed += pb.rows();
 			live.insert(live.end(), round.begin(), round.end());
 		}
 		// the step: the rows in flight, in admission order
 		SqRows r = {};
+		SqGroups grp = {};
 		r.n = (int)live.size();
-		int nsampled = 0, lmax = 0;
+		int nsampled = 0, lmax = 0, nsuf = 0;
+		std::map<int, std::vector<int>> groups; // rows by their context's first slot
+		std::vector<int> gorder;                // group slots in order of their first row
 		for (int k = 0; k < r.n; ++k) {
 			const int i = live[k], j = done[i];
 			const SqPlace& q = place[i];
 			r.q[k] = make_int4(q.s, q.L, q.t, j), r.pos[k] = q.L + j, r.slot[k] = q.t + j;
-			r.src[k] = row_of[i], r.tok0[k] = tokens[off[i] + q.L];
+			r.src[k] = row_of[i], r.tok0[k] = tokens[off[i] + len[i] - 1];
 			const bool gr = is_greedy(i);
 			// (a greedy row's sampler state is never read back: any valid one will do)
 			r.st0[k].rng = gr ? 1 : rng_states[i], r.st0[k].temperature = gr ? 1.0f : temperature[i], r.st0[k].cut_delta = gr ? 0.0f : logf(minp[i]) * temperature[i];
 			r.out[k] = (int)(O[i] + j), r.req[k] = i, r.greedy[k] = gr;
 			nsampled += !gr, lmax = std::max(lmax, q.L + j), row_of[i] = k;
+			grp.ctx[k] = make_int2(q.c, q.nc);
+			nsuf = std::max(nsuf, cdiv(q.L + j + 1, SN_CHUNK) - q.nc / SN_CHUNK);
+			if (q.nc) {
+				if (!groups.count(q.c)) gorder.push_back(q.c);
+				groups[q.c].push_back(k);
+			}
 		}
 		launch_pdl(k_sq_begin, 1, 32, 0, r, pf.sqrows, (const int*)pf.sqtok, pf.tokens, pf.vstate);
-		const PfSampleStep ss = {0, 0, r.n, lmax};
+		PfSampleStep ss = {0, 0, r.n, lmax};
+		if (!gorder.empty()) { // rows with contexts: the groups table, and the GROUPS attention
+			for (int c : gorder) {
+				const std::vector<int>& rows = groups[c];
+				grp.first[grp.ng + 1] = grp.first[grp.ng] + (int)rows.size();
+				grp.chunk0[grp.ng + 1] = grp.chunk0[grp.ng] + grp.ctx[rows[0]].y / SN_CHUNK;
+				std::copy(rows.begin(), rows.end(), grp.rows + grp.first[grp.ng]);
+				++grp.ng;
+			}
+			launch_pdl(k_sq_groups, 1, 32, 0, grp, pf.sqgroups);
+			ss.nshared = grp.chunk0[grp.ng], ss.nsuf = nsuf;
+		}
 		with_formats([&](auto f) {
 			pf_run(f, r.n, 0, PF_QUEUE, &ss);
 			pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
@@ -2275,7 +2372,7 @@ extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, co
 			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, r.n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 			sync_stream();
 		}
-		// retire: rows that reached max_new or emitted a stop token free their slots; the others keep their order
+		// retire: rows that reached max_new or emitted a stop token free their own slots; the others keep their order
 		std::vector<int> keep;
 		for (int k = 0; k < r.n; ++k) {
 			const int i = live[k];
@@ -2285,7 +2382,7 @@ extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, co
 				continue;
 			}
 			out_len[i] = done[i];
-			slots.give(place[i].s, cdiv(place[i].L, 8) * 8), slots.give(place[i].t, max_new[i]);
+			slots.give(place[i].s, cdiv(len[i] - 1, 8) * 8), slots.give(place[i].t, max_new[i]);
 		}
 		live.swap(keep);
 	}
@@ -2301,7 +2398,24 @@ extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, co
 	}
 	if (last_sampled) pf.vrows = last_sampled;
 	if (steps) *steps = nsteps;
+	if (prompt_rows) *prompt_rows = rows_computed;
 	return 1;
+}
+
+extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nreq,
+                                             const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
+                                             int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps) {
+	const std::vector<int> empty(nreq > 0 ? nreq : 0);
+	return sq_run("decode_sample_queue", transformer, tokens, n, empty.data(), empty.data(), off, len, nreq, max_new, temperature, minp, stop, n_stop,
+	              max_rows, rng_states, out_tokens, out_len, steps, nullptr);
+}
+
+extern "C" int calm_b200_decode_sample_queue_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                                     const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                                     const float* minp, const int* stop, int n_stop, int max_rows, unsigned long long* rng_states,
+                                                     int* out_tokens, int* out_len, int* steps, int* prompt_rows) {
+	return sq_run("decode_sample_queue_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nreq, max_new, temperature, minp, stop, n_stop,
+	              max_rows, rng_states, out_tokens, out_len, steps, prompt_rows);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -2424,7 +2538,7 @@ extern "C" void calm_b200_fill_kv(struct Transformer* transformer, int n_pos, ui
 // counts (the decode's and the sampled short block's), stamps, the watchdog words, the weights and rope_freq steer control flow, waits or addresses and stay as they are,
 // as do the index buffers (cand_idx, sample_idx, pf.vsidx, out_tokens, pf.tokens, pf.targets, pf.rowpos, pf.seg and pf.ctx, read
 // as a RoPE position and as key slots of the packed attention's loop, pf.sbrows, decode_sample_batch's key slots and
-// chunk counts, and pf.sqrows, decode_sample_queue's row table): a stale index that is read is in range,
+// chunk counts, pf.sqrows, decode_sample_queue's row table, and pf.sqgroups, its context groups): a stale index that is read is in range,
 // as after any earlier call, while 0xFFFFFFFF would send the read out of bounds.  DESIGN.md s.3 lists both groups.
 extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_from_pos) {
 	(void)transformer;

@@ -32,12 +32,33 @@
 // s .. s + L - 1, its generated entries at slots t, t + 1, .., and it is at its own step j, so its keys are v = 0 .. L + j:
 // v < L is slot s + v, v >= L is slot t + (v - L).  Grid, chunking and every floating-point operation are BATCH's, so a row
 // gives what decode_sample_batch gives its sequence over the same keys at step j.
+//
+// GROUPS (with QUEUE; calm_b200_decode_sample_queue_context): a row's prompt is a context of nc entries at slots c ..
+// followed by its own L - nc entries at slots s .., so v < nc is slot c + v, nc <= v < L is slot s + (v - nc) and v >= L is
+// slot t + (v - L) (SqGroups.ctx[r] = (c, nc); nc = 0 is QUEUE's mapping).  The rows in flight that name one context form
+// a group.  A chunk wholly inside the context, (k + 1) * SN_CHUNK <= nc, holds the same keys for every row of the group,
+// so one CTA per (group, chunk, kv head) stages it once and writes the partials of every row of the group, as the shared
+// prompt chunks above; every other chunk is computed per row, over the row's own virtual keys.  Grid (shared chunks +
+// nseq x nsuf, kv heads): CTA x < the shared chunks' count is shared chunk x - chunk0[g] of the group g that holds it, the
+// others are per-row chunk nc / SN_CHUNK + x' % nsuf of row x' / nsuf.  Which chunks are shared depends on nc alone and a
+// query's arithmetic does not depend on the CTA or warp that runs it, so a row gives what QUEUE gives it over the same keys.
 #pragma once
 
 #include "prefill.cuh"
 
 #define SN_CHUNK 128 // virtual keys per chunk: four per lane in the score pass
 #define SN_WARPS 8
+#define SQ_ROWS 16   // rows of a queue step: one token tile of k_vf_gemm
+
+// The context groups of one queue step (GROUPS), rows in the step's admission order.  Passed by value to k_sq_groups,
+// which keeps it where k_sn_attn reads it.
+struct SqGroups {
+	int2 ctx[SQ_ROWS];        // row r's context: its first slot and its length nc (0: none)
+	int chunk0[SQ_ROWS + 1];  // group g's shared chunks are the CTAs chunk0[g] .. chunk0[g + 1] - 1
+	int first[SQ_ROWS + 1];   // group g's rows are rows[first[g] .. first[g + 1])
+	int rows[SQ_ROWS];
+	int ng;                   // groups; chunk0[ng] is the shared chunks' count
+};
 
 struct SnAttnArgs {
 	const float* Q;  // [nseq][q_dim] the step's rotated queries
@@ -50,6 +71,7 @@ struct SnAttnArgs {
 	float inv_sqrt_hd;
 	const int2* rows; // [nseq] (BATCH) row b's prompt: its first slot s_b and its length L_b; read by no other variant
 	const int4* qrows; // [nseq] (QUEUE) row b's (s, L, t, j); read by no other variant
+	const SqGroups* groups; // (GROUPS) the step's contexts and groups; read by no other variant
 };
 
 // dynamic shared memory of k_sn_attn: the K tile (padded rows), the V tile, each warp's KM queries
@@ -60,10 +82,11 @@ constexpr size_t sn_smem_bytes() {
 
 // grid (prompt chunks + nseq x suffix chunks, kv heads): CTA x < pos0 / SN_CHUNK is prompt chunk x for every row, the
 // others are suffix chunk x' % nsuf of row x' / nsuf (x' = x - prompt chunks).  BATCH (and QUEUE): grid (nseq x nch, kv
-// heads).
-template <typename KVT, int HD, int KM, bool BATCH = false, bool QUEUE = false>
+// heads).  GROUPS: the grid above its header comment says.
+template <typename KVT, int HD, int KM, bool BATCH = false, bool QUEUE = false, bool GROUPS = false>
 __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 	static_assert(BATCH || !QUEUE, "a queue step is a batch step with per-row step counts");
+	static_assert(QUEUE || !GROUPS, "context groups are rows of a queue step");
 	pdl_enter();
 	constexpr int DPL = HD / 32, KPL = SN_CHUNK / 32;
 	constexpr int VSTR = HD * sizeof(KVT), KSTR = VSTR + 16; // padded key row, as k_pf_attn's
@@ -72,8 +95,24 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 	unsigned char* vs = ks + SN_CHUNK * KSTR;
 	float* qs = reinterpret_cast<float*>(vs + SN_CHUNK * VSTR) + (threadIdx.x >> 5) * KM * HD;
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, kvh = blockIdx.y;
-	int nkeys, c, b0, nrows;
-	if constexpr (BATCH) {
+	int nkeys, c, b0, nrows; // (GROUPS) b0 = -1 - f for a shared chunk, whose rows are groups->rows[f ..]
+	if constexpr (GROUPS) {
+		const SqGroups* gt = a.groups;
+		const int nsh = __ldg(gt->chunk0 + __ldg(&gt->ng));
+		if ((int)blockIdx.x < nsh) { // chunk c of group gi's context, for every row of the group
+			int gi = 0;
+			while ((int)blockIdx.x >= __ldg(gt->chunk0 + gi + 1)) ++gi;
+			const int f = __ldg(gt->first + gi);
+			c = blockIdx.x - __ldg(gt->chunk0 + gi), nrows = __ldg(gt->first + gi + 1) - f;
+			b0 = -1 - f, nkeys = (c + 1) * SN_CHUNK;
+		} else {
+			const int nsuf = (gridDim.x - nsh) / a.nseq, x = blockIdx.x - nsh;
+			b0 = x / nsuf, nrows = 1;
+			const int4 qr = __ldg(a.qrows + b0);
+			nkeys = qr.y + qr.w + 1, c = __ldg(&gt->ctx[b0].y) / SN_CHUNK + x % nsuf;
+			if (c * SN_CHUNK >= nkeys) return;
+		}
+	} else if constexpr (BATCH) {
 		const int nch = gridDim.x / a.nseq;
 		b0 = blockIdx.x / nch, c = blockIdx.x % nch, nrows = 1;
 		if constexpr (QUEUE) {
@@ -96,7 +135,13 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 		const int row = i / (VSTR / 16), cc = i % (VSTR / 16), v = v0 + row;
 		const bool in = row < nk;
 		int slot;
-		if constexpr (QUEUE) { // (scalar loads: the whole int4 held through the score pass adds spills)
+		if constexpr (GROUPS) { // (a shared chunk maps its keys through its group's first row: they are in its context)
+			const int br = b0 >= 0 ? b0 : __ldg(a.groups->rows - 1 - b0);
+			const int* qr = reinterpret_cast<const int*>(a.qrows + br);
+			const int2 cx = __ldg(a.groups->ctx + br);
+			const int L = __ldg(qr + 1);
+			slot = v < cx.y ? cx.x + v : v < L ? __ldg(qr) + (v - cx.y) : __ldg(qr + 2) + (v - L);
+		} else if constexpr (QUEUE) { // (scalar loads: the whole int4 held through the score pass adds spills)
 			const int* qr = reinterpret_cast<const int*>(a.qrows + b0);
 			const int L = __ldg(qr + 1);
 			slot = v < L ? __ldg(qr) + v : __ldg(qr + 2) + (v - L);
@@ -112,7 +157,7 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 
 	const int groups = nrows * a.kv_mul / KM;
 	for (int gq = warp; gq < groups; gq += SN_WARPS) {
-		const int b = b0 + gq * KM / a.kv_mul, h0 = kvh * a.kv_mul + gq * KM % a.kv_mul;
+		const int b = GROUPS && b0 < 0 ? __ldg(a.groups->rows + (-1 - b0) + gq * KM / a.kv_mul) : b0 + gq * KM / a.kv_mul, h0 = kvh * a.kv_mul + gq * KM % a.kv_mul;
 		__syncwarp(); // the previous group's queries are no longer being read
 		for (int i = lane; i < KM * HD; i += 32) qs[i] = a.Q[(size_t)b * a.q_dim + (size_t)h0 * HD + i];
 		__syncwarp();
@@ -226,8 +271,6 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_fold(const SnAttnArgs a) {
 
 // ---------------------------------------------------------------- calm_b200_decode_sample_queue's rows
 
-#define SQ_ROWS 16 // rows of a queue step: one token tile of k_vf_gemm
-
 // The rows of one queue step, row r in admission order.  Passed by value to k_sq_begin, which keeps it where the step's
 // kernels read it.
 struct SqRows {
@@ -258,6 +301,12 @@ __global__ void __launch_bounds__(32) k_sq_begin(const SqRows r, SqRows* tab, co
 	}
 	__syncwarp();
 	if (i < r.n) tokens[i] = tok, st[i] = s;
+}
+
+// one warp, before a step whose rows have contexts: keep the step's groups table
+__global__ void __launch_bounds__(32) k_sq_groups(const SqGroups gr, SqGroups* tab) {
+	pdl_enter();
+	for (int k = threadIdx.x; k < (int)(sizeof(SqGroups) / sizeof(int)); k += 32) reinterpret_cast<int*>(tab)[k] = reinterpret_cast<const int*>(&gr)[k];
 }
 
 // one warp, after a step: each row's token (the argmax or the sampler's) to the step's tokens and to the row's output

@@ -28,6 +28,7 @@ SYMBOLS = [
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
     "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
+    "calm_b200_decode_sample_queue_context",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -104,6 +105,9 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_queue.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, C.c_int, _iptr, _fptr, _fptr, _iptr, C.c_int, C.c_int, _u64p, _iptr,
                                                 _iptr, _iptr]
     L.calm_b200_decode_sample_queue.restype = C.c_int
+    L.calm_b200_decode_sample_queue_context.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, _iptr, _iptr, C.c_int, _iptr, _fptr, _fptr, _iptr, C.c_int, C.c_int,
+                                                        _u64p, _iptr, _iptr, _iptr, _iptr]
+    L.calm_b200_decode_sample_queue_context.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -467,15 +471,11 @@ class DeviceModel:
                                                         out.ctypes.data_as(ip))
         return out, [int(s) for s in rng], served
 
-    def decode_sample_queue(self, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states):
-        """calm_b200_decode_sample_queue: request i continues prompts[i] (a sequence of at least one token id) for at most
-        max_new[i] tokens at temperature[i] / minp[i] from rng_states[i], stopping after a token in `stop` (a sequence of
-        ids shared by all requests, possibly empty), with at most max_rows requests in flight.  Returns (tokens, states,
-        served, steps): tokens[i] is request i's int32 tokens (its out_len[i] of them), states the nreq generator states
-        after the call, served 1 on the new path and 0 when the per-request fallback gave them, steps the number of steps
-        run.  Raises ValueError where the C call would abort, and for per-request lists whose lengths differ."""
+    def _queue_args(self, who, prompts, max_new, temperature, minp, stop, max_rows, rng_states):
+        """The queue calls' checked per-request arrays (prompts, max_new, temperature, minp, stop, states), or ValueError
+        wherever the C call would abort, and for per-request lists whose lengths differ."""
         if prompts is None or rng_states is None or isinstance(rng_states, (int, np.integer)):
-            raise ValueError("decode_sample_queue takes a list of prompts and a sequence of generator states, one per prompt")
+            raise ValueError(f"{who} takes a list of prompts and a sequence of generator states, one per prompt")
         prompts = [np.asarray(p) for p in prompts]
         nreq = len(prompts)
         states = list(rng_states)
@@ -485,10 +485,10 @@ class DeviceModel:
             minp = np.ascontiguousarray(minp, np.float32).reshape(-1)
             stop = np.asarray([] if stop is None else stop)
         except (TypeError, ValueError) as e:
-            raise ValueError(f"decode_sample_queue: bad per-request list: {e}") from None
+            raise ValueError(f"{who}: bad per-request list: {e}") from None
         for name, xs in (("max_new", max_new), ("temperature", temperature), ("minp", minp), ("rng_states", states)):
             if len(xs) != nreq:
-                raise ValueError(f"decode_sample_queue takes one {name} per prompt: {nreq} prompts, {len(xs)} values")
+                raise ValueError(f"{who} takes one {name} per prompt: {nreq} prompts, {len(xs)} values")
         if not isinstance(max_rows, (int, np.integer)) or not 1 <= max_rows <= SAMPLE_N_MAX:
             raise ValueError(f"max_rows must be an integer in [1, {SAMPLE_N_MAX}], got {max_rows!r}")
         for s in states:
@@ -506,24 +506,84 @@ class DeviceModel:
         if not ((stop >= 0) & (stop < self.vocab)).all():
             raise ValueError(f"a stop id is outside [0, {self.vocab})")
         if sum(int(m) for m in max_new) >= 1 << 31:
-            raise ValueError("decode_sample_queue: the sum of max_new does not fit an int")
-        tokens = np.ascontiguousarray(np.concatenate(prompts) if nreq else np.zeros(0), np.int32)
-        len_ = np.asarray([len(p) for p in prompts], np.int32)
-        off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(len_)[:-1]]) if nreq else np.zeros(0), np.int32)
+            raise ValueError(f"{who}: the sum of max_new does not fit an int")
+        return prompts, max_new, temperature, minp, stop, states
+
+    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states):
+        """Run a queue call over the laid-out tokens; ctx is (ctx_off, ctx_len) or None.  Returns (tokens, states, served,
+        steps, prompt_rows)."""
+        nreq = len(len_)
         mn = np.ascontiguousarray(max_new, np.int32)
         st = np.ascontiguousarray(stop, np.int32)
         rng = (C.c_ulonglong * max(nreq, 1))(*[int(s) for s in states])
         out = np.full(max(int(mn.sum()), 1), -1, np.int32)
         out_len = np.zeros(max(nreq, 1), np.int32)
-        steps = C.c_int(-1)
+        steps, rows = C.c_int(-1), C.c_int(-1)
         ip, fp = C.POINTER(C.c_int), C.POINTER(C.c_float)
-        served = self.lib.calm_b200_decode_sample_queue(C.byref(self.transformer), tokens.ctypes.data_as(ip), len(tokens), off.ctypes.data_as(ip),
-                                                        len_.ctypes.data_as(ip), nreq, mn.ctypes.data_as(ip), temperature.ctypes.data_as(fp),
-                                                        minp.ctypes.data_as(fp), st.ctypes.data_as(ip) if len(st) else None, len(st), int(max_rows),
-                                                        rng, out.ctypes.data_as(ip), out_len.ctypes.data_as(ip), C.byref(steps))
+        args = [C.byref(self.transformer), tokens.ctypes.data_as(ip), len(tokens)]
+        if ctx is not None:
+            args += [ctx[0].ctypes.data_as(ip), ctx[1].ctypes.data_as(ip)]
+        args += [off.ctypes.data_as(ip), len_.ctypes.data_as(ip), nreq, mn.ctypes.data_as(ip), temperature.ctypes.data_as(fp), minp.ctypes.data_as(fp),
+                 st.ctypes.data_as(ip) if len(st) else None, len(st), int(max_rows), rng, out.ctypes.data_as(ip), out_len.ctypes.data_as(ip), C.byref(steps)]
+        if ctx is not None:
+            args.append(C.byref(rows))
+        served = fn(*args)
         o = np.concatenate([[0], np.cumsum(mn)]).astype(np.int64)
         toks = [out[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)]
-        return toks, [int(rng[i]) for i in range(nreq)], served, int(steps.value)
+        return toks, [int(rng[i]) for i in range(nreq)], served, int(steps.value), int(rows.value)
+
+    def decode_sample_queue(self, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states):
+        """calm_b200_decode_sample_queue: request i continues prompts[i] (a sequence of at least one token id) for at most
+        max_new[i] tokens at temperature[i] / minp[i] from rng_states[i], stopping after a token in `stop` (a sequence of
+        ids shared by all requests, possibly empty), with at most max_rows requests in flight.  Returns (tokens, states,
+        served, steps): tokens[i] is request i's int32 tokens (its out_len[i] of them), states the nreq generator states
+        after the call, served 1 on the new path and 0 when the per-request fallback gave them, steps the number of steps
+        run.  Raises ValueError where the C call would abort, and for per-request lists whose lengths differ."""
+        prompts, max_new, temperature, minp, stop, states = self._queue_args("decode_sample_queue", prompts, max_new, temperature, minp, stop, max_rows,
+                                                                             rng_states)
+        nreq = len(prompts)
+        tokens = np.ascontiguousarray(np.concatenate(prompts) if nreq else np.zeros(0), np.int32)
+        len_ = np.asarray([len(p) for p in prompts], np.int32)
+        off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(len_)[:-1]]) if nreq else np.zeros(0), np.int32)
+        return self._queue_call(self.lib.calm_b200_decode_sample_queue, tokens, None, off, len_, max_new, temperature, minp, stop, max_rows, states)[:4]
+
+    def decode_sample_queue_context(self, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states):
+        """calm_b200_decode_sample_queue_context: decode_sample_queue where request i's prompt is contexts[ctx_of[i]] ++
+        prompts[i] (ctx_of[i] == -1: prompts[i] alone).  Each context (a sequence of token ids, possibly empty) is laid
+        out once, so the requests that name it share it.  Returns (tokens, states, served, steps, prompt_rows), prompt_rows
+        being the rows the call's prompt passes computed.  Raises ValueError where the C call would abort, for an index
+        outside contexts and for per-request lists whose lengths differ."""
+        prompts, max_new, temperature, minp, stop, states = self._queue_args("decode_sample_queue_context", prompts, max_new, temperature, minp, stop,
+                                                                             max_rows, rng_states)
+        if contexts is None or ctx_of is None:
+            raise ValueError("decode_sample_queue_context takes a list of contexts and one context index per prompt")
+        contexts = [np.asarray(c) for c in contexts]
+        try:
+            ctx_of = [c for c in ctx_of]
+        except TypeError as e:
+            raise ValueError(f"decode_sample_queue_context: bad ctx_of: {e}") from None
+        nreq = len(prompts)
+        if len(ctx_of) != nreq:
+            raise ValueError(f"decode_sample_queue_context takes one ctx_of per prompt: {nreq} prompts, {len(ctx_of)} values")
+        for i, c in enumerate(ctx_of):
+            if not isinstance(c, (int, np.integer)) or not -1 <= c < len(contexts):
+                raise ValueError(f"ctx_of[{i}] must be -1 or an index into the {len(contexts)} contexts, got {c!r}")
+        for k, c in enumerate(contexts):
+            if c.ndim != 1 or (len(c) and c.dtype.kind not in "iu"):
+                raise ValueError(f"context {k} must be a sequence of token ids")
+            if not ((c >= 0) & (c < self.vocab)).all():
+                raise ValueError(f"context {k} has a token outside [0, {self.vocab})")
+        pieces = contexts + prompts
+        starts = np.concatenate([[0], np.cumsum([len(p) for p in pieces])]).astype(np.int64)
+        if starts[-1] >= 1 << 31:
+            raise ValueError("decode_sample_queue_context: the tokens do not fit an int index")
+        tokens = np.ascontiguousarray(np.concatenate(pieces) if len(pieces) else np.zeros(0), np.int32)
+        ctx_off = np.asarray([starts[c] if c >= 0 else 0 for c in ctx_of], np.int32)
+        ctx_len = np.asarray([len(contexts[c]) if c >= 0 else 0 for c in ctx_of], np.int32)
+        off = np.asarray(starts[len(contexts):len(contexts) + nreq], np.int32)
+        len_ = np.asarray([len(p) for p in prompts], np.int32)
+        return self._queue_call(self.lib.calm_b200_decode_sample_queue_context, tokens, (ctx_off, ctx_len), off, len_, max_new, temperature, minp, stop,
+                                max_rows, states)
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""

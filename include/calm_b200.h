@@ -318,6 +318,38 @@ int calm_b200_decode_sample_queue(struct Transformer* transformer, const int* to
                                   const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
                                   int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps);
 
+/* calm_b200_decode_sample_queue for requests whose prompts share prefixes: each shared context is computed once by the
+ * prompt pass while its requests are in flight, and every step reads a context's whole chunks once for all of them
+ * (DESIGN.md s.6).  Request i's prompt is the context tokens[ctx_off[i] .. ctx_off[i] + ctx_len[i]) followed by its own
+ * tokens[off[i] .. off[i] + len[i]), len[i] >= 1; ctx_len[i] == 0 means no context.  Requests share a context exactly
+ * when they name the same (ctx_off, ctx_len), as in calm_b200_score_context; equal contents at different offsets are
+ * correct but computed separately.  Every other argument and output is calm_b200_decode_sample_queue's; prompt_rows
+ * (may be NULL) receives the number of rows the call's prompt passes computed.
+ * Returns 1 on the new path: request i's tokens and final rng_states[i] are then bit for bit those of
+ * calm_b200_decode_sample_batch over its concatenated prompt alone (nseq = 1) with n_tokens = out_len[i], whatever the
+ * other requests, which of them share its context, max_rows, the slots it was given or seq_len.
+ * Schedule and placement.  calm_b200_decode_sample_queue's, with contexts: a context is resident from the round that
+ * places it until it is released.  Admission: before every step the requests at the head of the queue are admitted in
+ * input order while a row is free and the round's placement, computed from the slots free before the round, fits.  A
+ * round's placement takes first one extent at the lowest free start that is a multiple of 8 holding, request by request
+ * in input order, the request's context (ceil8(ctx_len[i]) slots, at RoPE positions 0 ..) unless that context is
+ * resident or placed by an earlier request of the round, then its own prompt (ceil8(len[i] - 1) slots, at positions
+ * ctx_len[i] ..); then, in input order, one extent of max_new[i] slots per request at the lowest free start.  A request
+ * whose context is resident reads it there.  The extent goes through the packed prompt pass.  Release: after admission,
+ * a resident context that no request in flight names (those admitted by the round included) frees its slots; if then
+ * nothing is in flight, admission runs again on the empty cache.  Retire: a request retires after the step that gave its
+ * max_new-th or its stop token and frees its own ceil8(len[i] - 1) prompt slots and its max_new[i] generated slots.
+ * Step j of request i feeds its last token at RoPE position ctx_len[i] + len[i] - 1 + j and writes slot t_i + j.  With
+ * every ctx_len 0 this is calm_b200_decode_sample_queue's rule exactly, and the call is that call.
+ * Shapes the prompt pass does not serve, and calls with a request whose ceil8(ctx_len[i]) + ceil8(len[i] - 1) +
+ * max_new[i] > seq_len, return 0: calm_b200_decode_sample_queue's fallback over each request's concatenated prompt,
+ * with *steps = 0 and *prompt_rows = 0.  The call aborts before any device work where calm_b200_decode_sample_queue
+ * does, and when a context lies outside tokens[0 .. n) or ctx_off / ctx_len is NULL. */
+int calm_b200_decode_sample_queue_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                          const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                          const float* minp, const int* stop, int n_stop, int max_rows, unsigned long long* rng_states,
+                                          int* out_tokens, int* out_len, int* steps, int* prompt_rows);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
