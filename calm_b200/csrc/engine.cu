@@ -193,6 +193,16 @@ struct Prefill {
 	int* sqout = nullptr;              // [sqout_cap]: request i's tokens from O_i = max_new[0] + .. + max_new[i - 1]
 	unsigned long long* sqst = nullptr; // [sqst_cap]: request i's generator state after its last sampled step
 	size_t sqout_cap = 0, sqst_cap = 0;
+	// the queue's log-probabilities (calm_b200_decode_sample_queue_logprobs), allocated on its first call: a step's tile
+	// lists and merged top-k for VF_TOK rows and the largest k, and every request's outputs, regrown like pf.sqout
+	float* sqtopv = nullptr; // [VF_TOK][cdiv(vocab, PF_BM)][PF_TOPK_MAX]
+	int* sqtopi = nullptr;
+	int* sqtid = nullptr;    // [VF_TOK][PF_TOPK_MAX]
+	float* sqtlp = nullptr;
+	float* sqlp = nullptr;   // [sqlp_cap]: request i's log-probabilities from O_i
+	int* sqoid = nullptr;    // [sqtop_cap]: request i's top-k ids and log-probabilities from O_i * k
+	float* sqolp = nullptr;
+	size_t sqlp_cap = 0, sqtop_cap = 0;
 };
 Prefill pf;
 
@@ -206,6 +216,7 @@ void pf_free() {
 	cudaFree(pf.vlogits), cudaFree(pf.vtmax), cudaFree(pf.vsidx), cudaFree(pf.vsprob), cudaFree(pf.vcsum), cudaFree(pf.vcount), cudaFree(pf.vstate), cudaFree(pf.vsampled);
 	cudaFree(pf.snpart), cudaFree(pf.snpos), cudaFree(pf.sntok), cudaFree(pf.sbrows);
 	cudaFree(pf.sqrows), cudaFree(pf.sqgroups), cudaFree(pf.sqtok), cudaFree(pf.sqout), cudaFree(pf.sqst);
+	cudaFree(pf.sqtopv), cudaFree(pf.sqtopi), cudaFree(pf.sqtid), cudaFree(pf.sqtlp), cudaFree(pf.sqlp), cudaFree(pf.sqoid), cudaFree(pf.sqolp);
 	pf = Prefill();
 }
 
@@ -1257,17 +1268,17 @@ static void vf_reserve() {
 // each); the classifier from vocabulary tile `tile0` on; PF_QKV_SLOTS: row t's keys and values to cache slot slot[t].
 // Every K-slice gets the same number of CTAs, as many as stay resident together, each walking row blocks with the same
 // stride.
-template <int MODE, int DBITS, typename KVT>
+template <int MODE, int DBITS, typename KVT, bool TOPK = false>
 static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int units, int tile0 = 0, const int* slot = nullptr) {
 	static int cap = 0, sms = 0;
-	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT>, VF_THREADS, 0), sms = g.sms;
+	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT, TOPK>, VF_THREADS, 0), sms = g.sms;
 	VfArgs v = {};
 	v.xhi = hi, v.xlo = lo, v.acc = pf.vacc, v.cnt = pf.vcnt;
 	v.nsl = vf_slices(a.K), v.units = units, v.rows = (MODE == PF_UP ? 2 : 1) * units * VF_ROWS;
 	v.tile0 = tile0, v.nvt = cdiv(g.cfg.vocab_size, PF_BM);
 	v.logits = pf.vlogits, v.tmax = pf.vtmax, v.slot = slot;
 	const int tasks = (MODE == PF_UP ? 2 : 1) * units;
-	launch_pdl(k_vf_gemm<MODE, DBITS, KVT>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
+	launch_pdl(k_vf_gemm<MODE, DBITS, KVT, TOPK>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
 }
 
 // What the rows of a prompt-pass block are
@@ -1562,6 +1573,21 @@ extern "C" int forward_prefill_cuda(struct Transformer* transformer, const int* 
 	return 1;
 }
 
+// The decode path's log-softmax of one logit row l[0 .. vocab), in double: *logprob = l[target] - M - ln S, and with k > 0
+// the k largest logits, equal logits by index ascending (the same order as the tensor-core pass), and theirs
+static void host_logprobs(const float* l, int vocab, int target, int k, float* logprob, int* top_ids, float* top_logprobs) {
+	double mx = l[0], s = 0.0;
+	for (int v = 1; v < vocab; ++v) mx = l[v] > mx ? l[v] : mx;
+	for (int v = 0; v < vocab; ++v) s += exp((double)l[v] - mx);
+	*logprob = (float)((double)l[target] - mx - log(s));
+	if (k) {
+		std::vector<int> idx(vocab);
+		for (int v = 0; v < vocab; ++v) idx[v] = v;
+		std::partial_sort(idx.begin(), idx.begin() + k, idx.end(), [l](int a, int b) { return l[a] > l[b] || (l[a] == l[b] && a < b); });
+		for (int r = 0; r < k; ++r) top_ids[r] = idx[r], top_logprobs[r] = (float)((double)l[idx[r]] - mx - log(s));
+	}
+}
+
 // Score tokens[1 .. n) given what precedes each (the reference's study(), run.c:291-308): tokens[0 .. n - 1) go through
 // the prompt pass and logprobs[i] = ln softmax(logits after tokens[i])[tokens[i + 1]].  The cache is left as
 // forward_prefill_cuda(tokens, n - 1, pos0) leaves it.  Shapes the pass does not serve go one position at a time through
@@ -1578,24 +1604,12 @@ static int pf_score_one(struct Transformer* transformer, const int* tokens, int 
 			launch_token(1);
 			sync_stream();
 			const float* l = g.logits_host;
-			double mx = l[0], s = 0.0;
-			for (int v = 1; v < vocab; ++v) mx = l[v] > mx ? l[v] : mx;
-			for (int v = 0; v < vocab; ++v) s += exp((double)l[v] - mx);
-			x.logprobs[i] = (float)((double)l[tokens[i + 1]] - mx - log(s));
+			host_logprobs(l, vocab, tokens[i + 1], x.k, &x.logprobs[i], x.top_ids + (size_t)i * x.k, x.top_logprobs + (size_t)i * x.k);
 			if (x.greedy) { // first maximum (sampler.c:34-42), as calm_b200_forward_argmax
 				int best = 0;
 				for (int v = 1; v < vocab; ++v)
 					if (l[v] > l[best]) best = v;
 				x.greedy[i] = best;
-			}
-			if (x.k) { // the k largest logits, equal logits by index ascending: the same order as the tensor-core pass
-				std::vector<int> idx(vocab);
-				for (int v = 0; v < vocab; ++v) idx[v] = v;
-				std::partial_sort(idx.begin(), idx.begin() + x.k, idx.end(), [l](int a, int b) { return l[a] > l[b] || (l[a] == l[b] && a < b); });
-				for (int r = 0; r < x.k; ++r) {
-					x.top_ids[(size_t)i * x.k + r] = idx[r];
-					x.top_logprobs[(size_t)i * x.k + r] = (float)((double)l[idx[r]] - mx - log(s));
-				}
 			}
 		}
 		CUDA_CHECK(cudaGetLastError());
@@ -2183,13 +2197,79 @@ static bool sq_place(SqSlots& a, const std::vector<int>& rs, const int* ctx_off,
 	return true;
 }
 
+// The log-probability outputs of calm_b200_decode_sample_queue_logprobs: request i step j writes logprobs[O_i + j] and
+// top_ids / top_logprobs[(O_i + j) * k ..]
+struct SqLogprobs {
+	int k;
+	float* logprobs;
+	int* top_ids;
+	float* top_logprobs;
+};
+
+// a step's tile lists and merged top-k for VF_TOK rows and the largest k, and room for `total` tokens' outputs at k
+static void sq_lp_reserve(size_t total, int k) {
+	const size_t nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	if (!pf.sqtopv) {
+		pf.sqtopv = (float*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(float));
+		pf.sqtopi = (int*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
+		pf.sqtid = (int*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(int));
+		pf.sqtlp = (float*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(float));
+	}
+	if (total > pf.sqlp_cap) { // (no step of an earlier call is still reading them)
+		CUDA_CHECK(cudaStreamSynchronize(g.stream));
+		cudaFree(pf.sqlp);
+		pf.sqlp_cap = total;
+		pf.sqlp = (float*)dev_alloc(total * sizeof(float));
+	}
+	if (total * k > pf.sqtop_cap) {
+		CUDA_CHECK(cudaStreamSynchronize(g.stream));
+		cudaFree(pf.sqoid), cudaFree(pf.sqolp);
+		pf.sqtop_cap = total * k;
+		pf.sqoid = (int*)dev_alloc(pf.sqtop_cap * sizeof(int));
+		pf.sqolp = (float*)dev_alloc(pf.sqtop_cap * sizeof(float));
+	}
+}
+
+// A queue step's final norm and short-block classifier with its log-probability epilogue: pf_score's greedy (or, with
+// `sample`, sampled) classifier on the n rows, with k > 0 its TOPK variant writing each tile's top-k lists to pf.sqtopv /
+// pf.sqtopi.  The merge is left to sq_merge, after each row's target is set.
+template <int DBITS, typename KVT>
+static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample) {
+	const Config& c = g.cfg;
+	const int nvt = cdiv(c.vocab_size, PF_BM);
+	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)g.w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
+	PfGemmArgs a = {};
+	a.n_tokens = n, a.w[0] = g.w.wcls, a.K = c.dim;
+	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
+	a.topv = pf.sqtopv, a.topi = pf.sqtopi, a.topk = k;
+	for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) {
+		const int units = imin(VF_CLS_UNITS, nvt - t0);
+		if (sample && k) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		else if (sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
+		else if (k) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		else vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
+	}
+}
+
+// The merge of a step with log-probabilities: pf_merge's greedy merge (k > 0: with the top-k lists of pf.sqtopv into
+// pf.sqtid / pf.sqtlp), every row's log-probability that of its target
+static void sq_merge(int n, int k) {
+	const int nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	const auto merge = k ? k_pf_logprob<true, true> : k_pf_logprob<true>;
+	launch_pdl(merge, cdiv(n, 8), 256, k ? (size_t)8 * nvt : 0, (const float2*)pf.part, (const float*)pf.tgt, pf.logprob, n, nvt, (const int*)pf.gidx,
+	           pf.greedy, (const float*)pf.sqtopv, (const int*)pf.sqtopi, k, pf.sqtid, pf.sqtlp);
+}
+
 // calm_b200_decode_sample_queue_context, and calm_b200_decode_sample_queue with every ctx_len 0 (`who` names the call in
 // error messages): a round's extent goes through the packed prompt pass (sb_prefill), each request's own rows continuing
 // its context at positions ctx_len .. (PF_CONTEXTS where a block holds such rows); a step whose rows have contexts runs
-// k_sn_attn's GROUPS variant, every other step exactly the QUEUE kernels.
+// k_sn_attn's GROUPS variant, every other step exactly the QUEUE kernels.  With `lp` (calm_b200_decode_sample_queue_logprobs)
+// a step's classifier also runs the TOPK epilogue (k > 0), the merge runs after the sampler with each row's target set to
+// its token (k_sq_tgt), and k_sq_lp stores the results; the tokens are the same bits.
 static int sq_run(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off,
                   const int* len, int nreq, const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
-                  int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows) {
+                  int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows,
+                  const SqLogprobs* lp = nullptr) {
 	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
 	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, max_rows, CALM_B200_SAMPLE_N_MAX);
 	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, n_stop);
@@ -2205,6 +2285,12 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		total += max_new[i];
 	}
 	if (total > 0x7fffffff) CALM_FATAL("%s: %zu output tokens do not fit an int index", who, total);
+	if (lp) {
+		const int kmax = imin(CALM_B200_TOPK_MAX, g.cfg.vocab_size);
+		if (lp->k < 0 || lp->k > kmax) CALM_FATAL("%s: k %d outside [0, %d]", who, lp->k, kmax);
+		if (total > 0 && !lp->logprobs) CALM_FATAL("%s: logprobs is NULL", who);
+		if (total > 0 && lp->k > 0 && (!lp->top_ids || !lp->top_logprobs)) CALM_FATAL("%s: top_ids or top_logprobs is NULL", who);
+	}
 	check_tokens(tokens, n);
 	check_tokens(stop, n_stop);
 	if (steps) *steps = 0;
@@ -2232,8 +2318,14 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			const int L = (int)p.size() - 1;
 			int tok = p[L], k = 0;
 			if (max_new[i] > 0) forward_prefill_cuda(transformer, p.data(), L, 0);
+			std::vector<float> logits(lp ? g.cfg.vocab_size : 0);
 			while (k < max_new[i]) {
 				tok = calm_b200_forward_sample(transformer, tok, L + k, temperature[i], minp[i], &rng_states[i]);
+				if (lp) { // the step's device logits, through pf_score_one's decode-path log-softmax
+					const size_t o = O[i] + k;
+					calm_b200_read_device_logits(logits.data());
+					host_logprobs(logits.data(), g.cfg.vocab_size, tok, lp->k, lp->logprobs + o, lp->top_ids + o * lp->k, lp->top_logprobs + o * lp->k);
+				}
 				out_tokens[O[i] + k++] = tok;
 				if (is_stop[tok]) break;
 			}
@@ -2254,6 +2346,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		pf.sqout = (int*)dev_alloc(pf.sqout_cap * sizeof(int));
 		pf.sqst = (unsigned long long*)dev_alloc(pf.sqst_cap * sizeof(unsigned long long));
 	}
+	if (lp) sq_lp_reserve(total, lp->k);
 
 	SqSlots slots(g.cfg.seq_len);
 	std::map<SqCtx, int> resident; // contexts in the cache, at their first slot
@@ -2362,11 +2455,22 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		}
 		with_formats([&](auto f) {
 			pf_run(f, r.n, 0, PF_QUEUE, &ss);
-			pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
+			if (lp) sq_classify(f, r.n, lp->k, nsampled > 0);
+			else pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
 		});
-		if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
-		if (nsampled > 0) vf_sample_rows(r.n);
+		if (lp) { // the sampler, then every row's target and the merge, whose argmax is the greedy rows' token as above
+			if (nsampled > 0) vf_sample_rows(r.n);
+			launch_pdl(k_sq_tgt, r.n, 32, 0, (const SqRows*)pf.sqrows, (const float2*)pf.part, cdiv(g.cfg.vocab_size, PF_BM), (const float*)pf.vlogits,
+			           g.cfg.vocab_size, (const int*)pf.vsampled, pf.tgt);
+			sq_merge(r.n, lp->k);
+		} else {
+			if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
+			if (nsampled > 0) vf_sample_rows(r.n);
+		}
 		launch_pdl(k_sq_end, 1, 32, 0, (const SqRows*)pf.sqrows, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate, pf.sqtok, pf.sqout, pf.sqst);
+		if (lp)
+			launch_pdl(k_sq_lp, 1, 32, 0, (const SqRows*)pf.sqrows, (const float*)pf.logprob, (const int*)pf.sqtid, (const float*)pf.sqtlp, lp->k, pf.sqlp,
+			           pf.sqoid, pf.sqolp);
 		++nsteps, last_sampled = nsampled > 0 ? r.n : 0;
 		if (n_stop) { // the step's tokens decide which rows stop
 			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, r.n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
@@ -2390,11 +2494,26 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 	std::vector<unsigned long long> st(nreq);
 	CUDA_CHECK(cudaMemcpyAsync(all.data(), pf.sqout, total * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 	CUDA_CHECK(cudaMemcpyAsync(st.data(), pf.sqst, nreq * sizeof(unsigned long long), cudaMemcpyDeviceToHost, g.stream));
+	const size_t k = lp ? lp->k : 0;
+	std::vector<float> lps(lp ? total : 0), tlp(total * k);
+	std::vector<int> tid(total * k);
+	if (lp) {
+		CUDA_CHECK(cudaMemcpyAsync(lps.data(), pf.sqlp, total * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+		if (k) {
+			CUDA_CHECK(cudaMemcpyAsync(tid.data(), pf.sqoid, total * k * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+			CUDA_CHECK(cudaMemcpyAsync(tlp.data(), pf.sqolp, total * k * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+		}
+	}
 	sync_stream();
 	CUDA_CHECK(cudaGetLastError());
 	for (int i = 0; i < nreq; ++i) {
 		std::copy(all.begin() + O[i], all.begin() + O[i] + out_len[i], out_tokens + O[i]);
 		if (out_len[i] > 0 && !is_greedy(i)) rng_states[i] = st[i];
+		if (lp) { // (slots past out_len[i] are left untouched)
+			std::copy(lps.begin() + O[i], lps.begin() + O[i] + out_len[i], lp->logprobs + O[i]);
+			std::copy(tid.begin() + O[i] * k, tid.begin() + (O[i] + out_len[i]) * k, lp->top_ids + O[i] * k);
+			std::copy(tlp.begin() + O[i] * k, tlp.begin() + (O[i] + out_len[i]) * k, lp->top_logprobs + O[i] * k);
+		}
 	}
 	if (last_sampled) pf.vrows = last_sampled;
 	if (steps) *steps = nsteps;
@@ -2416,6 +2535,18 @@ extern "C" int calm_b200_decode_sample_queue_context(struct Transformer* transfo
                                                      int* out_tokens, int* out_len, int* steps, int* prompt_rows) {
 	return sq_run("decode_sample_queue_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nreq, max_new, temperature, minp, stop, n_stop,
 	              max_rows, rng_states, out_tokens, out_len, steps, prompt_rows);
+}
+
+extern "C" int calm_b200_decode_sample_queue_logprobs(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                                      const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                                      const float* minp, const int* stop, int n_stop, int max_rows, unsigned long long* rng_states,
+                                                      int* out_tokens, int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
+                                                      float* top_logprobs) {
+	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
+	const bool none = !ctx_off && !ctx_len;
+	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
+	return sq_run("decode_sample_queue_logprobs", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
+	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, &lp);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -2582,6 +2713,11 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		// decode_sample_queue's step tokens and per-request tokens and states, which every call writes before it reads them
 		// (its row table, read as positions and key slots, is an index buffer)
 		nan(pf.sqtok, VF_TOK * sizeof(int)), nan(pf.sqout, pf.sqout_cap * sizeof(int)), nan(pf.sqst, pf.sqst_cap * sizeof(unsigned long long));
+		// and its log-probability call's tile lists, merged top-k and per-request outputs (ids only compared and copied out)
+		const size_t nvt = cdiv(c.vocab_size, PF_BM);
+		nan(pf.sqtopv, VF_TOK * nvt * PF_TOPK_MAX * sizeof(float)), nan(pf.sqtopi, VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
+		nan(pf.sqtid, VF_TOK * PF_TOPK_MAX * sizeof(int)), nan(pf.sqtlp, VF_TOK * PF_TOPK_MAX * sizeof(float));
+		nan(pf.sqlp, pf.sqlp_cap * sizeof(float)), nan(pf.sqoid, pf.sqtop_cap * sizeof(int)), nan(pf.sqolp, pf.sqtop_cap * sizeof(float));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

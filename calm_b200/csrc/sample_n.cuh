@@ -321,3 +321,36 @@ __global__ void __launch_bounds__(32) k_sq_end(const SqRows* tab, const int* gre
 	step_tok[i] = tok, out[tab->out[i]] = tok;
 	if (!gr) rng[tab->req[i]] = st[i].rng;
 }
+
+// ---------------------------------------------------------------- calm_b200_decode_sample_queue_logprobs
+
+// one warp per row, after the sampler and before the merge of a step with log-probabilities: the row's target logit
+// becomes its emitted token's, so that k_pf_logprob's tgt - M - ln S is that token's log-probability.  A sampled row's
+// logit is its sampled token's entry of its logit row; a greedy row's token is the argmax, whose logit is the largest tile
+// maximum (fmaxf is exact, so the order of the maxima does not matter).
+__global__ void __launch_bounds__(32) k_sq_tgt(const SqRows* tab, const float2* part, int nvt, const float* logits, int vocab, const int* sampled,
+                                               float* tgt) {
+	pdl_enter();
+	const int i = blockIdx.x, lane = threadIdx.x;
+	if (tab->greedy[i]) {
+		float m = -FLT_MAX;
+		for (int v = lane; v < nvt; v += 32) m = fmaxf(m, part[(size_t)i * nvt + v].x);
+		m = warp_max(m);
+		if (lane == 0) tgt[i] = m;
+	} else if (lane == 0) {
+		tgt[i] = logits[(size_t)i * vocab + sampled[i]];
+	}
+}
+
+// one warp, after the merge of a step with log-probabilities: each row's log-probability, and its k top ids and
+// log-probabilities, to the row's output slot (its token's slot in pf.sqout; the top-k entries at k times that)
+__global__ void __launch_bounds__(32) k_sq_lp(const SqRows* tab, const float* logprob, const int* top_ids, const float* top_lp, int k, float* out_lp,
+                                              int* out_ids, float* out_tlp) {
+	pdl_enter();
+	const int n = tab->n;
+	for (int i = threadIdx.x; i < n; i += 32) out_lp[tab->out[i]] = logprob[i];
+	for (int e = threadIdx.x; e < n * k; e += 32) {
+		const size_t o = (size_t)tab->out[e / k] * k + e % k;
+		out_ids[o] = top_ids[e], out_tlp[o] = top_lp[e];
+	}
+}

@@ -19,6 +19,9 @@
 //               token row, and each tile's maximum, which k_sample_scan_rows / k_sample_pick_rows (stages.cuh) sample,
 //               all rows side by side: the same accumulator values the argmax records come from.
 //               PF_QKV_SLOTS (calm_b200_decode_sample_queue) is PF_QKV with each row's keys and values at its own slot.
+//               TOPK (with PF_CLS_GREEDY or PF_CLS_SAMPLE; calm_b200_decode_sample_queue_logprobs) computes every record
+//               above with the same operations and then each tile's a.topk largest logits of every token row, in
+//               PF_CLS_TOPK's layout and by its rule, which the unchanged k_pf_logprob<.., true> merges.
 #pragma once
 
 #include "prefill.cuh"
@@ -93,10 +96,11 @@ __device__ __forceinline__ void vf_dequant(const uint32_t (&w)[VfFmt<DBITS>::WOR
 	}
 }
 
-template <int MODE, int DBITS, typename KVT>
+template <int MODE, int DBITS, typename KVT, bool TOPK = false>
 __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, const VfArgs v) {
 	constexpr int W = VfFmt<DBITS>::WORDS, U = VfFmt<DBITS>::U;
 	constexpr bool CLS = MODE == PF_CLS_GREEDY || MODE == PF_CLS_SAMPLE;
+	static_assert(CLS || !TOPK, "the top-k lists are a classifier epilogue");
 	__shared__ __align__(16) __half xs[2][VF_TOK][VF_XSTR];
 	__shared__ unsigned last_s;
 	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
@@ -265,6 +269,44 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 							if (rbase + r < a.vocab) v.logits[(size_t)t * a.vocab + rbase + r] = lg[t][r];
 						}
 						if (lane == 0) v.tmax[(size_t)t * v.nvt + tile] = m;
+					}
+				}
+			}
+			if constexpr (TOPK) { // PF_CLS_TOPK's selection over the same logits, one per round: each lane offers its largest
+				// logit not yet taken (a strict > over its ascending rows keeps the lowest index of equal values), the butterfly
+				// keeps the larger value or, on equal values, the lower index, and the owner marks it taken.  The warp's two
+				// tokens go through the rounds together, so that their independent butterflies overlap.
+				const int tw = 2 * warp;
+				if (tw < a.n_tokens) {
+					uint32_t taken[2] = {0, 0}; // bit i: this lane's row lane + 32 i
+					for (int r = 0; r < a.topk; ++r) {
+						float bv[2];
+						int bi[2], bp[2], mine[2];
+#pragma unroll
+						for (int h = 0; h < 2; ++h) {
+							bv[h] = -INFINITY, bi[h] = INT_MAX, bp[h] = 0;
+#pragma unroll
+							for (int i = 0; i < 4; ++i) {
+								const int rr = lane + 32 * i;
+								const float x = lg[tw + h][rr];
+								if (rbase + rr < a.vocab && !((taken[h] >> i) & 1u) && x > bv[h]) bv[h] = x, bi[h] = rbase + rr, bp[h] = i;
+							}
+							mine[h] = bi[h];
+						}
+#pragma unroll
+						for (int o = 1; o < 32; o <<= 1)
+#pragma unroll
+							for (int h = 0; h < 2; ++h) {
+								const float v2 = __shfl_xor_sync(0xffffffffu, bv[h], o);
+								const int i2 = __shfl_xor_sync(0xffffffffu, bi[h], o);
+								if (v2 > bv[h] || (v2 == bv[h] && i2 < bi[h])) bv[h] = v2, bi[h] = i2;
+							}
+#pragma unroll
+						for (int h = 0; h < 2; ++h) {
+							if (bi[h] == mine[h]) taken[h] |= 1u << bp[h]; // (a lane with nothing left re-marks a taken or invalid bit)
+							const size_t rec = ((size_t)(tw + h) * v.nvt + tile) * a.topk;
+							if (lane == 0 && tw + h < a.n_tokens) a.topv[rec + r] = bv[h], a.topi[rec + r] = bi[h];
+						}
 					}
 				}
 			}

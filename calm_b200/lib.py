@@ -28,7 +28,7 @@ SYMBOLS = [
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
     "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
-    "calm_b200_decode_sample_queue_context",
+    "calm_b200_decode_sample_queue_context", "calm_b200_decode_sample_queue_logprobs",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -108,6 +108,8 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_queue_context.argtypes = [T, _iptr, C.c_int, _iptr, _iptr, _iptr, _iptr, C.c_int, _iptr, _fptr, _fptr, _iptr, C.c_int, C.c_int,
                                                         _u64p, _iptr, _iptr, _iptr, _iptr]
     L.calm_b200_decode_sample_queue_context.restype = C.c_int
+    L.calm_b200_decode_sample_queue_logprobs.argtypes = L.calm_b200_decode_sample_queue_context.argtypes + [C.c_int, _fptr, _iptr, _fptr]
+    L.calm_b200_decode_sample_queue_logprobs.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -509,28 +511,72 @@ class DeviceModel:
             raise ValueError(f"{who}: the sum of max_new does not fit an int")
         return prompts, max_new, temperature, minp, stop, states
 
-    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states):
-        """Run a queue call over the laid-out tokens; ctx is (ctx_off, ctx_len) or None.  Returns (tokens, states, served,
-        steps, prompt_rows)."""
+    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None):
+        """Run a queue call over the laid-out tokens; ctx is (ctx_off, ctx_len), either of them None for a NULL array, or
+        None for a call without those arguments.  Returns (tokens, states, served, steps, prompt_rows), and with `k` (the
+        log-probability call) also each request's float32[out_len] log-probabilities and, for k > 0, its top ids and
+        log-probabilities [out_len, k] (None for k == 0)."""
         nreq = len(len_)
         mn = np.ascontiguousarray(max_new, np.int32)
         st = np.ascontiguousarray(stop, np.int32)
         rng = (C.c_ulonglong * max(nreq, 1))(*[int(s) for s in states])
-        out = np.full(max(int(mn.sum()), 1), -1, np.int32)
+        total = max(int(mn.sum()), 1)
+        out = np.full(total, -1, np.int32)
         out_len = np.zeros(max(nreq, 1), np.int32)
         steps, rows = C.c_int(-1), C.c_int(-1)
         ip, fp = C.POINTER(C.c_int), C.POINTER(C.c_float)
         args = [C.byref(self.transformer), tokens.ctypes.data_as(ip), len(tokens)]
         if ctx is not None:
-            args += [ctx[0].ctypes.data_as(ip), ctx[1].ctypes.data_as(ip)]
+            args += [None if c is None else c.ctypes.data_as(ip) for c in ctx]
         args += [off.ctypes.data_as(ip), len_.ctypes.data_as(ip), nreq, mn.ctypes.data_as(ip), temperature.ctypes.data_as(fp), minp.ctypes.data_as(fp),
                  st.ctypes.data_as(ip) if len(st) else None, len(st), int(max_rows), rng, out.ctypes.data_as(ip), out_len.ctypes.data_as(ip), C.byref(steps)]
         if ctx is not None:
             args.append(C.byref(rows))
+        if k is not None:
+            lp = np.full(total, np.nan, np.float32)
+            ids = np.full((total, k), -1, np.int32) if k else None
+            tlp = np.full((total, k), np.nan, np.float32) if k else None
+            args += [k, lp.ctypes.data_as(fp), ids.ctypes.data_as(ip) if k else None, tlp.ctypes.data_as(fp) if k else None]
         served = fn(*args)
         o = np.concatenate([[0], np.cumsum(mn)]).astype(np.int64)
         toks = [out[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)]
-        return toks, [int(rng[i]) for i in range(nreq)], served, int(steps.value), int(rows.value)
+        res = (toks, [int(rng[i]) for i in range(nreq)], served, int(steps.value), int(rows.value))
+        if k is None:
+            return res
+        cut = lambda a: [a[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)] if a is not None else None  # noqa: E731
+        return res + (cut(lp), cut(ids), cut(tlp))
+
+    def _context_layout(self, who, contexts, ctx_of, prompts):
+        """The context calls' laid-out tokens and (ctx_off, ctx_len, off, len) for contexts / ctx_of / prompts (each
+        context once), or ValueError for an index outside contexts or a bad context."""
+        if contexts is None or ctx_of is None:
+            raise ValueError(f"{who} takes a list of contexts and one context index per prompt")
+        contexts = [np.asarray(c) for c in contexts]
+        try:
+            ctx_of = [c for c in ctx_of]
+        except TypeError as e:
+            raise ValueError(f"{who}: bad ctx_of: {e}") from None
+        nreq = len(prompts)
+        if len(ctx_of) != nreq:
+            raise ValueError(f"{who} takes one ctx_of per prompt: {nreq} prompts, {len(ctx_of)} values")
+        for i, c in enumerate(ctx_of):
+            if not isinstance(c, (int, np.integer)) or not -1 <= c < len(contexts):
+                raise ValueError(f"ctx_of[{i}] must be -1 or an index into the {len(contexts)} contexts, got {c!r}")
+        for k, c in enumerate(contexts):
+            if c.ndim != 1 or (len(c) and c.dtype.kind not in "iu"):
+                raise ValueError(f"context {k} must be a sequence of token ids")
+            if not ((c >= 0) & (c < self.vocab)).all():
+                raise ValueError(f"context {k} has a token outside [0, {self.vocab})")
+        pieces = contexts + prompts
+        starts = np.concatenate([[0], np.cumsum([len(p) for p in pieces])]).astype(np.int64)
+        if starts[-1] >= 1 << 31:
+            raise ValueError(f"{who}: the tokens do not fit an int index")
+        tokens = np.ascontiguousarray(np.concatenate(pieces) if len(pieces) else np.zeros(0), np.int32)
+        ctx_off = np.asarray([starts[c] if c >= 0 else 0 for c in ctx_of], np.int32)
+        ctx_len = np.asarray([len(contexts[c]) if c >= 0 else 0 for c in ctx_of], np.int32)
+        off = np.asarray(starts[len(contexts):len(contexts) + nreq], np.int32)
+        len_ = np.asarray([len(p) for p in prompts], np.int32)
+        return tokens, ctx_off, ctx_len, off, len_
 
     def decode_sample_queue(self, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states):
         """calm_b200_decode_sample_queue: request i continues prompts[i] (a sequence of at least one token id) for at most
@@ -555,35 +601,33 @@ class DeviceModel:
         outside contexts and for per-request lists whose lengths differ."""
         prompts, max_new, temperature, minp, stop, states = self._queue_args("decode_sample_queue_context", prompts, max_new, temperature, minp, stop,
                                                                              max_rows, rng_states)
-        if contexts is None or ctx_of is None:
-            raise ValueError("decode_sample_queue_context takes a list of contexts and one context index per prompt")
-        contexts = [np.asarray(c) for c in contexts]
-        try:
-            ctx_of = [c for c in ctx_of]
-        except TypeError as e:
-            raise ValueError(f"decode_sample_queue_context: bad ctx_of: {e}") from None
-        nreq = len(prompts)
-        if len(ctx_of) != nreq:
-            raise ValueError(f"decode_sample_queue_context takes one ctx_of per prompt: {nreq} prompts, {len(ctx_of)} values")
-        for i, c in enumerate(ctx_of):
-            if not isinstance(c, (int, np.integer)) or not -1 <= c < len(contexts):
-                raise ValueError(f"ctx_of[{i}] must be -1 or an index into the {len(contexts)} contexts, got {c!r}")
-        for k, c in enumerate(contexts):
-            if c.ndim != 1 or (len(c) and c.dtype.kind not in "iu"):
-                raise ValueError(f"context {k} must be a sequence of token ids")
-            if not ((c >= 0) & (c < self.vocab)).all():
-                raise ValueError(f"context {k} has a token outside [0, {self.vocab})")
-        pieces = contexts + prompts
-        starts = np.concatenate([[0], np.cumsum([len(p) for p in pieces])]).astype(np.int64)
-        if starts[-1] >= 1 << 31:
-            raise ValueError("decode_sample_queue_context: the tokens do not fit an int index")
-        tokens = np.ascontiguousarray(np.concatenate(pieces) if len(pieces) else np.zeros(0), np.int32)
-        ctx_off = np.asarray([starts[c] if c >= 0 else 0 for c in ctx_of], np.int32)
-        ctx_len = np.asarray([len(contexts[c]) if c >= 0 else 0 for c in ctx_of], np.int32)
-        off = np.asarray(starts[len(contexts):len(contexts) + nreq], np.int32)
-        len_ = np.asarray([len(p) for p in prompts], np.int32)
+        tokens, ctx_off, ctx_len, off, len_ = self._context_layout("decode_sample_queue_context", contexts, ctx_of, prompts)
         return self._queue_call(self.lib.calm_b200_decode_sample_queue_context, tokens, (ctx_off, ctx_len), off, len_, max_new, temperature, minp, stop,
                                 max_rows, states)
+
+    def decode_sample_queue_logprobs(self, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states, k: int = 0):
+        """calm_b200_decode_sample_queue_logprobs: decode_sample_queue_context (contexts and ctx_of both None: no
+        contexts, decode_sample_queue), returning its tuple and each request's log-probabilities of its tokens and the k
+        most likely tokens at each step: (tokens, states, served, steps, prompt_rows, logprobs, top_ids, top_logprobs)
+        with logprobs[i] float32[out_len[i]] and, for k > 0, top_ids[i] int32 / top_logprobs[i] float32 [out_len[i], k]
+        (None for k == 0).  The numbers are the log-softmax of the step's logits at temperature 1 without the min-p cut.
+        Raises ValueError where the C call would abort (k outside [0, min(TOPK_MAX, vocab)] included)."""
+        who = "decode_sample_queue_logprobs"
+        kmax = min(TOPK_MAX, self.vocab)
+        if not isinstance(k, (int, np.integer)) or isinstance(k, bool) or not 0 <= k <= kmax:
+            raise ValueError(f"k must be an integer in [0, {kmax}], got {k!r}")
+        prompts, max_new, temperature, minp, stop, states = self._queue_args(who, prompts, max_new, temperature, minp, stop, max_rows, rng_states)
+        if contexts is None and ctx_of is None:
+            nreq = len(prompts)
+            tokens = np.ascontiguousarray(np.concatenate(prompts) if nreq else np.zeros(0), np.int32)
+            len_ = np.asarray([len(p) for p in prompts], np.int32)
+            off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(len_)[:-1]]) if nreq else np.zeros(0), np.int32)
+            ctx = (None, None)
+        else:
+            tokens, ctx_off, ctx_len, off, len_ = self._context_layout(who, contexts, ctx_of, prompts)
+            ctx = (ctx_off, ctx_len)
+        return self._queue_call(self.lib.calm_b200_decode_sample_queue_logprobs, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states,
+                                k=int(k))
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""

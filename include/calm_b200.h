@@ -350,6 +350,40 @@ int calm_b200_decode_sample_queue_context(struct Transformer* transformer, const
                                           const float* minp, const int* stop, int n_stop, int max_rows, unsigned long long* rng_states,
                                           int* out_tokens, int* out_len, int* steps, int* prompt_rows);
 
+/* calm_b200_decode_sample_queue_context that also returns every generated token's log-probability and the k most likely
+ * tokens at its step, with theirs (an OpenAI-style response's logprobs / top_logprobs, best_of, RL rollouts;
+ * INTEGRATION.md).  ctx_off and ctx_len may both be NULL: no request has a context.
+ * Unchanged outputs.  out_tokens, out_len, rng_states, steps, prompt_rows and the return value are bit for bit those of
+ * calm_b200_decode_sample_queue_context with the same arguments (with no contexts, those of
+ * calm_b200_decode_sample_queue), on the new path and on the fallback alike.
+ * What the numbers are.  The model's own distribution, as in the scoring calls: the log-softmax of the step's fp32
+ * logits at temperature 1 and without the min-p cut, whatever the request's temperature / minp.  A sampled token can
+ * therefore have any log-probability and can lie outside the top k.
+ * Where they go.  Request i's token of step j is out_tokens[O_i + j]; the same slot gets logprobs[O_i + j] = l[tok] - M
+ * - ln S, with M and S the maximum and sum the scoring calls' merge gives that step's logits l (the expression of
+ * calm_b200_score's logprobs), and for k >= 1 top_ids[(O_i + j)*k + r] and top_logprobs[(O_i + j)*k + r], r in [0, k),
+ * by the _topk scoring calls' rule: logit descending, equal logits lowest index first, log-probabilities by the same
+ * expression with the same M and S.  Where top_ids holds the emitted token, top_logprobs == logprobs bit for bit; a
+ * greedy request's top_ids[.. + 0] is its token.  Slots past out_len[i] are left untouched.
+ * Independence.  On the new path request i's logprobs / top_* do not depend on the other requests, max_rows, the slots
+ * or seq_len, as its tokens do not: they come from the same logits.
+ * Arguments.  0 <= k <= min(CALM_B200_TOPK_MAX, vocab_size); logprobs not NULL when any max_new[i] > 0, and top_ids /
+ * top_logprobs not NULL when also k > 0 (either may be NULL when k == 0).  They hold max_new[0] + .. + max_new[nreq - 1]
+ * and k times that entries.  Otherwise, and wherever calm_b200_decode_sample_queue_context aborts, the call aborts
+ * before any device work.
+ * Fallback (return 0; MoE, tensor parallelism, other shapes the prompt pass does not serve, requests that do not fit
+ * seq_len): after each token of the queue's fallback, its device logits (those calm_b200_read_device_logits reads) go
+ * through calm_b200_score's decode-path log-softmax in double and top-k, written as float.
+ * The first call allocates what calm_b200_decode_sample_queue_context allocates, the step's tile lists for 16 rows:
+ * 16 x ceil(vocab_size / 128) x CALM_B200_TOPK_MAX x 8 bytes (2.6 MB at a 128256-token vocabulary; not the scoring
+ * calls' 2048-row lists), and room for the outputs, 4 + 8 k bytes per token of max_new[0] + .. + max_new[nreq - 1],
+ * regrown by a larger call. */
+int calm_b200_decode_sample_queue_logprobs(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                           const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                           const float* minp, const int* stop, int n_stop, int max_rows, unsigned long long* rng_states,
+                                           int* out_tokens, int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
+                                           float* top_logprobs);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
