@@ -203,6 +203,17 @@ struct Prefill {
 	int* sqoid = nullptr;    // [sqtop_cap]: request i's top-k ids and log-probabilities from O_i * k
 	float* sqolp = nullptr;
 	size_t sqlp_cap = 0, sqtop_cap = 0;
+	// the queue's logit processing (calm_b200_decode_sample_queue_penalties), allocated on its first call with a
+	// non-neutral request: each of the 16 lanes' count and bias rows and parameters (VfArgs::pcnt / pbias / ppar), and
+	// the call's tokens and bias lists, uploaded once per call and regrown like pf.sqout
+	int* sqpcnt = nullptr;    // [16][vocab]
+	float* sqpbias = nullptr; // [16][vocab]
+	float4* sqppar = nullptr; // [16]
+	int* sqlanes = nullptr;   // [16] the step's lane of each row (k_sq_lanes)
+	int* sqptok = nullptr;    // [sqptok_cap]
+	int* sqpbid = nullptr;    // [sqpb_cap]
+	float* sqpbval = nullptr;
+	size_t sqptok_cap = 0, sqpb_cap = 0;
 };
 Prefill pf;
 
@@ -217,6 +228,7 @@ void pf_free() {
 	cudaFree(pf.snpart), cudaFree(pf.snpos), cudaFree(pf.sntok), cudaFree(pf.sbrows);
 	cudaFree(pf.sqrows), cudaFree(pf.sqgroups), cudaFree(pf.sqtok), cudaFree(pf.sqout), cudaFree(pf.sqst);
 	cudaFree(pf.sqtopv), cudaFree(pf.sqtopi), cudaFree(pf.sqtid), cudaFree(pf.sqtlp), cudaFree(pf.sqlp), cudaFree(pf.sqoid), cudaFree(pf.sqolp);
+	cudaFree(pf.sqpcnt), cudaFree(pf.sqpbias), cudaFree(pf.sqppar), cudaFree(pf.sqlanes), cudaFree(pf.sqptok), cudaFree(pf.sqpbid), cudaFree(pf.sqpbval);
 	pf = Prefill();
 }
 
@@ -1267,18 +1279,19 @@ static void vf_reserve() {
 // out = W . X^T over the rows of `a` for the n <= 16 rows of (hi, lo), in `units` row blocks of 128 (UP: of w1 and of w3
 // each); the classifier from vocabulary tile `tile0` on; PF_QKV_SLOTS: row t's keys and values to cache slot slot[t].
 // Every K-slice gets the same number of CTAs, as many as stay resident together, each walking row blocks with the same
-// stride.
-template <int MODE, int DBITS, typename KVT, bool TOPK = false>
+// stride.  PEN: the rows' lanes as k_sq_lanes left them in pf.sqlanes.
+template <int MODE, int DBITS, typename KVT, bool TOPK = false, bool PEN = false>
 static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int units, int tile0 = 0, const int* slot = nullptr) {
 	static int cap = 0, sms = 0;
-	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT, TOPK>, VF_THREADS, 0), sms = g.sms;
+	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT, TOPK, PEN>, VF_THREADS, 0), sms = g.sms;
 	VfArgs v = {};
 	v.xhi = hi, v.xlo = lo, v.acc = pf.vacc, v.cnt = pf.vcnt;
 	v.nsl = vf_slices(a.K), v.units = units, v.rows = (MODE == PF_UP ? 2 : 1) * units * VF_ROWS;
 	v.tile0 = tile0, v.nvt = cdiv(g.cfg.vocab_size, PF_BM);
 	v.logits = pf.vlogits, v.tmax = pf.vtmax, v.slot = slot;
+	if constexpr (PEN) v.lane = pf.sqlanes, v.pcnt = pf.sqpcnt, v.pbias = pf.sqpbias, v.ppar = pf.sqppar;
 	const int tasks = (MODE == PF_UP ? 2 : 1) * units;
-	launch_pdl(k_vf_gemm<MODE, DBITS, KVT, TOPK>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
+	launch_pdl(k_vf_gemm<MODE, DBITS, KVT, TOPK, PEN>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
 }
 
 // What the rows of a prompt-pass block are
@@ -2232,9 +2245,10 @@ static void sq_lp_reserve(size_t total, int k) {
 
 // A queue step's final norm and short-block classifier with its log-probability epilogue: pf_score's greedy (or, with
 // `sample`, sampled) classifier on the n rows, with k > 0 its TOPK variant writing each tile's top-k lists to pf.sqtopv /
-// pf.sqtopi.  The merge is left to sq_merge, after each row's target is set.
+// pf.sqtopi.  The merge is left to sq_merge, after each row's target is set.  With `pen` (a step with non-neutral rows of
+// calm_b200_decode_sample_queue_penalties) the TOPK variant with PEN runs whatever k is, and processes those rows' logits.
 template <int DBITS, typename KVT>
-static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample) {
+static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample, bool pen = false) {
 	const Config& c = g.cfg;
 	const int nvt = cdiv(c.vocab_size, PF_BM);
 	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)g.w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
@@ -2244,7 +2258,9 @@ static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample) {
 	a.topv = pf.sqtopv, a.topi = pf.sqtopi, a.topk = k;
 	for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) {
 		const int units = imin(VF_CLS_UNITS, nvt - t0);
-		if (sample && k) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		if (pen && sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		else if (pen) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		else if (sample && k) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
 		else if (sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
 		else if (k) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
 		else vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
@@ -2260,16 +2276,72 @@ static void sq_merge(int n, int k) {
 	           pf.greedy, (const float*)pf.sqtopv, (const int*)pf.sqtopi, k, pf.sqtid, pf.sqtlp);
 }
 
+// The logit processing of calm_b200_decode_sample_queue_penalties (include/calm_b200.h): presence / frequency /
+// repetition may each be NULL (0, 0, 1), bias_off / bias_len both NULL when n_bias == 0
+struct SqPenalties {
+	const float* presence;
+	const float* frequency;
+	const float* repetition;
+	const int* bias_off;
+	const int* bias_len;
+	const int* bias_ids;
+	const float* bias_val;
+	int n_bias;
+	float p(int i) const { return presence ? presence[i] : 0.0f; }
+	float f(int i) const { return frequency ? frequency[i] : 0.0f; }
+	float r(int i) const { return repetition ? repetition[i] : 1.0f; }
+	int nb(int i) const { return bias_len ? bias_len[i] : 0; }
+	bool neutral(int i) const { return p(i) == 0.0f && f(i) == 0.0f && r(i) == 1.0f && nb(i) == 0; }
+};
+
+// sq_pen_logit on the host, for the fallback: the same IEEE operations, one per statement (no contraction)
+static float sq_pen_logit_host(float l, int c, bool seen, float b, float p, float f, float r) {
+	float l1 = l;
+	if (seen && r != 1.0f) l1 = l > 0.0f ? l / r : l * r;
+	const float fc = f * (float)c;
+	const float bf = b - fc;
+	const float a = bf - (c > 0 ? p : 0.0f);
+	return a == 0.0f ? l1 : l1 + a;
+}
+
+// The lanes' rows and parameters (first use), and room for the call's n tokens and n_bias bias entries
+static void sq_pen_reserve(int n, int n_bias) {
+	const size_t vocab = g.cfg.vocab_size;
+	if (!pf.sqpcnt) {
+		pf.sqpcnt = (int*)dev_alloc(SQ_ROWS * vocab * sizeof(int));
+		pf.sqpbias = (float*)dev_alloc(SQ_ROWS * vocab * sizeof(float));
+		pf.sqppar = (float4*)dev_alloc(SQ_ROWS * sizeof(float4));
+		pf.sqlanes = (int*)dev_alloc(SQ_ROWS * sizeof(int));
+	}
+	if ((size_t)n > pf.sqptok_cap) { // (no step of an earlier call is still reading them)
+		CUDA_CHECK(cudaStreamSynchronize(g.stream));
+		cudaFree(pf.sqptok);
+		pf.sqptok_cap = n;
+		pf.sqptok = (int*)dev_alloc((size_t)n * sizeof(int));
+	}
+	if ((size_t)n_bias > pf.sqpb_cap) {
+		CUDA_CHECK(cudaStreamSynchronize(g.stream));
+		cudaFree(pf.sqpbid), cudaFree(pf.sqpbval);
+		pf.sqpb_cap = n_bias;
+		pf.sqpbid = (int*)dev_alloc((size_t)n_bias * sizeof(int));
+		pf.sqpbval = (float*)dev_alloc((size_t)n_bias * sizeof(float));
+	}
+}
+
 // calm_b200_decode_sample_queue_context, and calm_b200_decode_sample_queue with every ctx_len 0 (`who` names the call in
 // error messages): a round's extent goes through the packed prompt pass (sb_prefill), each request's own rows continuing
 // its context at positions ctx_len .. (PF_CONTEXTS where a block holds such rows); a step whose rows have contexts runs
 // k_sn_attn's GROUPS variant, every other step exactly the QUEUE kernels.  With `lp` (calm_b200_decode_sample_queue_logprobs)
 // a step's classifier also runs the TOPK epilogue (k > 0), the merge runs after the sampler with each row's target set to
-// its token (k_sq_tgt), and k_sq_lp stores the results; the tokens are the same bits.
+// its token (k_sq_tgt), and k_sq_lp stores the results; the tokens are the same bits.  With `pen`
+// (calm_b200_decode_sample_queue_penalties) each non-neutral request holds a lane from admission to retirement, cleared
+// and filled by k_sq_pen_admit; a step with such rows passes their lanes to k_sq_lanes, runs sq_classify's PEN classifier
+// and after k_sq_end k_sq_pen_step, every
+// other step exactly the kernels it runs without `pen`.
 static int sq_run(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off,
                   const int* len, int nreq, const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
                   int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows,
-                  const SqLogprobs* lp = nullptr) {
+                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr) {
 	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
 	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, max_rows, CALM_B200_SAMPLE_N_MAX);
 	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, n_stop);
@@ -2290,6 +2362,30 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		if (lp->k < 0 || lp->k > kmax) CALM_FATAL("%s: k %d outside [0, %d]", who, lp->k, kmax);
 		if (total > 0 && !lp->logprobs) CALM_FATAL("%s: logprobs is NULL", who);
 		if (total > 0 && lp->k > 0 && (!lp->top_ids || !lp->top_logprobs)) CALM_FATAL("%s: top_ids or top_logprobs is NULL", who);
+	}
+	if (pen) { // bounds that keep every processed logit finite
+		const float big = 1e6f;
+		const int vocab = g.cfg.vocab_size;
+		if (pen->n_bias < 0) CALM_FATAL("%s: negative n_bias %d", who, pen->n_bias);
+		if (!pen->bias_off != !pen->bias_len || (!pen->bias_off && pen->n_bias > 0)) CALM_FATAL("%s: bias_off or bias_len is NULL", who);
+		if (pen->n_bias > 0 && (!pen->bias_ids || !pen->bias_val)) CALM_FATAL("%s: bias_ids or bias_val is NULL", who);
+		std::vector<int> listed(vocab, -1); // the request whose list last named the id
+		for (int i = 0; i < nreq; ++i) {
+			const float p = pen->p(i), f = pen->f(i), r = pen->r(i);
+			if (!std::isfinite(p) || !std::isfinite(f) || !std::isfinite(r) || fabsf(p) > big || fabsf(f) > big || !(r >= 1e-6f && r <= big))
+				CALM_FATAL("%s: request %d's presence %g, frequency %g or repetition %g is not finite or out of bounds", who, i, p, f, r);
+			if (!pen->bias_off) continue;
+			const int bo = pen->bias_off[i], bl = pen->bias_len[i];
+			if (bo < 0 || bl < 0 || (long)bo + bl > pen->n_bias) CALM_FATAL("%s: bias list %d (off %d, len %d) outside the %d entries", who, i, bo, bl, pen->n_bias);
+			for (int e = bo; e < bo + bl; ++e) {
+				const int id = pen->bias_ids[e];
+				const float b = pen->bias_val[e];
+				if (id < 0 || id >= vocab) CALM_FATAL("%s: request %d's bias id %d outside [0, %d)", who, i, id, vocab);
+				if (listed[id] == i) CALM_FATAL("%s: request %d's bias list repeats id %d", who, i, id);
+				if (!std::isfinite(b) || fabsf(b) > big) CALM_FATAL("%s: request %d's bias %g for id %d is not finite or out of bounds", who, i, b, id);
+				listed[id] = i;
+			}
+		}
 	}
 	check_tokens(tokens, n);
 	check_tokens(stop, n_stop);
@@ -2318,8 +2414,30 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			const int L = (int)p.size() - 1;
 			int tok = p[L], k = 0;
 			if (max_new[i] > 0) forward_prefill_cuda(transformer, p.data(), L, 0);
-			std::vector<float> logits(lp ? g.cfg.vocab_size : 0);
+			const bool processed = pen && !pen->neutral(i);
+			std::vector<float> logits(lp || processed ? g.cfg.vocab_size : 0);
+			std::vector<int> cnt(processed ? g.cfg.vocab_size : 0);
+			std::vector<float> bias(processed ? g.cfg.vocab_size : 0);
+			std::vector<char> seen(processed ? g.cfg.vocab_size : 0);
+			if (processed) {
+				for (int t : p) seen[t] = 1;
+				for (int e = 0; e < pen->nb(i); ++e) bias[pen->bias_ids[pen->bias_off[i] + e]] = pen->bias_val[pen->bias_off[i] + e];
+			}
 			while (k < max_new[i]) {
+				if (processed) { // the decode path's device logits (its argmax discarded), processed and sampled on the host
+					unsigned long long unused = 1;
+					calm_b200_forward_sample(transformer, tok, L + k, 0.0f, 0.0f, &unused);
+					calm_b200_read_device_logits(logits.data());
+					for (int v = 0; v < g.cfg.vocab_size; ++v)
+						logits[v] = sq_pen_logit_host(logits[v], cnt[v], seen[v] || cnt[v] > 0, bias[v], pen->p(i), pen->f(i), pen->r(i));
+					tok = calm_b200_sample_logits(logits.data(), g.cfg.vocab_size, temperature[i], minp[i], &rng_states[i], nullptr); // (greedy: first maximum)
+					++cnt[tok];
+					if (lp) host_logprobs(logits.data(), g.cfg.vocab_size, tok, lp->k, lp->logprobs + O[i] + k, lp->top_ids + (O[i] + k) * lp->k,
+					                      lp->top_logprobs + (O[i] + k) * lp->k);
+					out_tokens[O[i] + k++] = tok;
+					if (is_stop[tok]) break;
+					continue;
+				}
 				tok = calm_b200_forward_sample(transformer, tok, L + k, temperature[i], minp[i], &rng_states[i]);
 				if (lp) { // the step's device logits, through pf_score_one's decode-path log-softmax
 					const size_t o = O[i] + k;
@@ -2347,6 +2465,18 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		pf.sqst = (unsigned long long*)dev_alloc(pf.sqst_cap * sizeof(unsigned long long));
 	}
 	if (lp) sq_lp_reserve(total, lp->k);
+	bool any_pen = false; // a request with max_new > 0 is not neutral: the lanes are used
+	for (int i = 0; pen && i < nreq; ++i) any_pen = any_pen || (max_new[i] > 0 && !pen->neutral(i));
+	if (any_pen) { // the call's tokens and bias lists, once
+		sq_pen_reserve(n, pen->n_bias);
+		CUDA_CHECK(cudaMemcpyAsync(pf.sqptok, tokens, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		if (pen->n_bias) {
+			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbid, pen->bias_ids, (size_t)pen->n_bias * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbval, pen->bias_val, (size_t)pen->n_bias * sizeof(float), cudaMemcpyHostToDevice, g.stream));
+		}
+	}
+	std::vector<int> lane_of(nreq, -1); // a non-neutral request's lane while it is in flight
+	unsigned lanes_free = (1u << SQ_ROWS) - 1;
 
 	SqSlots slots(g.cfg.seq_len);
 	std::map<SqCtx, int> resident; // contexts in the cache, at their first slot
@@ -2411,6 +2541,14 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 					pb.add(tokens + ctx_off[i], q.nc, q.nc - 1, 0, make_int2(0, 0));
 				}
 				pb.add(tokens + off[i], len[i] - 1, len[i] - 1, q.nc, make_int2(q.c, q.nc));
+				if (pen && !pen->neutral(i)) { // the lowest free lane, cleared and filled for the request
+					const int ln = __builtin_ctz(lanes_free);
+					lanes_free &= ~(1u << ln), lane_of[i] = ln;
+					const SqPenAdmit qa = {ln, ctx_off[i], ctx_len[i], off[i], len[i], pen->bias_off ? pen->bias_off[i] : 0, pen->nb(i),
+					                       make_float4(pen->p(i), pen->f(i), pen->r(i), 0.0f)};
+					launch_pdl(k_sq_pen_admit, cdiv(g.cfg.vocab_size, SQ_PEN_SPAN), 256, 0, qa, (const int*)pf.sqptok, (const int*)pf.sqpbid,
+					           (const float*)pf.sqpbval, g.cfg.vocab_size, pf.sqpcnt, pf.sqpbias, pf.sqppar);
+				}
 			}
 			if (pb.rows()) sb_prefill(pb, rbase);
 			rows_computed += pb.rows();
@@ -2419,6 +2557,8 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		// the step: the rows in flight, in admission order
 		SqRows r = {};
 		SqGroups grp = {};
+		SqLanes lanes;
+		bool pen_step = false; // a row of the step is a non-neutral request's
 		r.n = (int)live.size();
 		int nsampled = 0, lmax = 0, nsuf = 0;
 		std::map<int, std::vector<int>> groups; // rows by their context's first slot
@@ -2432,6 +2572,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			// (a greedy row's sampler state is never read back: any valid one will do)
 			r.st0[k].rng = gr ? 1 : rng_states[i], r.st0[k].temperature = gr ? 1.0f : temperature[i], r.st0[k].cut_delta = gr ? 0.0f : logf(minp[i]) * temperature[i];
 			r.out[k] = (int)(O[i] + j), r.req[k] = i, r.greedy[k] = gr;
+			lanes.lane[k] = lane_of[i], pen_step = pen_step || lane_of[i] >= 0;
 			nsampled += !gr, lmax = std::max(lmax, q.L + j), row_of[i] = k;
 			grp.ctx[k] = make_int2(q.c, q.nc);
 			nsuf = std::max(nsuf, cdiv(q.L + j + 1, SN_CHUNK) - q.nc / SN_CHUNK);
@@ -2440,7 +2581,9 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 				groups[q.c].push_back(k);
 			}
 		}
+		std::fill(lanes.lane + r.n, lanes.lane + SQ_ROWS, -1);
 		launch_pdl(k_sq_begin, 1, 32, 0, r, pf.sqrows, (const int*)pf.sqtok, pf.tokens, pf.vstate);
+		if (pen_step) launch_pdl(k_sq_lanes, 1, 32, 0, lanes, pf.sqlanes);
 		PfSampleStep ss = {0, 0, r.n, lmax};
 		if (!gorder.empty()) { // rows with contexts: the groups table, and the GROUPS attention
 			for (int c : gorder) {
@@ -2455,7 +2598,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		}
 		with_formats([&](auto f) {
 			pf_run(f, r.n, 0, PF_QUEUE, &ss);
-			if (lp) sq_classify(f, r.n, lp->k, nsampled > 0);
+			if (lp || pen_step) sq_classify(f, r.n, lp ? lp->k : 0, nsampled > 0, pen_step);
 			else pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
 		});
 		if (lp) { // the sampler, then every row's target and the merge, whose argmax is the greedy rows' token as above
@@ -2464,6 +2607,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			           g.cfg.vocab_size, (const int*)pf.vsampled, pf.tgt);
 			sq_merge(r.n, lp->k);
 		} else {
+			if (pen_step && nsampled == 0) pf_merge(r.n, true, 0); // pf_score's merge, which sq_classify leaves out
 			if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
 			if (nsampled > 0) vf_sample_rows(r.n);
 		}
@@ -2471,6 +2615,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		if (lp)
 			launch_pdl(k_sq_lp, 1, 32, 0, (const SqRows*)pf.sqrows, (const float*)pf.logprob, (const int*)pf.sqtid, (const float*)pf.sqtlp, lp->k, pf.sqlp,
 			           pf.sqoid, pf.sqolp);
+		if (pen_step) launch_pdl(k_sq_pen_step, 1, 32, 0, (const int*)pf.sqlanes, (const int*)pf.sqtok, g.cfg.vocab_size, pf.sqpcnt);
 		++nsteps, last_sampled = nsampled > 0 ? r.n : 0;
 		if (n_stop) { // the step's tokens decide which rows stop
 			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, r.n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
@@ -2487,6 +2632,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			}
 			out_len[i] = done[i];
 			slots.give(place[i].s, cdiv(len[i] - 1, 8) * 8), slots.give(place[i].t, max_new[i]);
+			if (lane_of[i] >= 0) lanes_free |= 1u << lane_of[i], lane_of[i] = -1;
 		}
 		live.swap(keep);
 	}
@@ -2547,6 +2693,22 @@ extern "C" int calm_b200_decode_sample_queue_logprobs(struct Transformer* transf
 	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
 	return sq_run("decode_sample_queue_logprobs", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
 	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, &lp);
+}
+
+extern "C" int calm_b200_decode_sample_queue_penalties(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                                       const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                                       const float* minp, const float* presence, const float* frequency, const float* repetition,
+                                                       const int* bias_off, const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias,
+                                                       const int* stop, int n_stop, int max_rows, unsigned long long* rng_states, int* out_tokens,
+                                                       int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
+                                                       float* top_logprobs) {
+	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
+	const bool none = !ctx_off && !ctx_len;
+	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
+	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
+	return sq_run("decode_sample_queue_penalties", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
+	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
+	              logprobs || k ? &lp : nullptr, &pen);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -2718,6 +2880,11 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		nan(pf.sqtopv, VF_TOK * nvt * PF_TOPK_MAX * sizeof(float)), nan(pf.sqtopi, VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
 		nan(pf.sqtid, VF_TOK * PF_TOPK_MAX * sizeof(int)), nan(pf.sqtlp, VF_TOK * PF_TOPK_MAX * sizeof(float));
 		nan(pf.sqlp, pf.sqlp_cap * sizeof(float)), nan(pf.sqoid, pf.sqtop_cap * sizeof(int)), nan(pf.sqolp, pf.sqtop_cap * sizeof(float));
+		// and its penalty call's lanes, which k_sq_pen_admit rewrites whole for each request it admits (a poisoned count
+		// word reads as seen with count 0x3fffffff), and its uploaded bias values (the uploaded tokens and bias ids and the
+		// step's lanes, pf.sqlanes, read as addresses into the lanes, are index buffers)
+		nan(pf.sqpcnt, SQ_ROWS * (size_t)c.vocab_size * sizeof(int)), nan(pf.sqpbias, SQ_ROWS * (size_t)c.vocab_size * sizeof(float));
+		nan(pf.sqppar, SQ_ROWS * sizeof(float4)), nan(pf.sqpbval, pf.sqpb_cap * sizeof(float));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

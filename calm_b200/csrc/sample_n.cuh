@@ -354,3 +354,56 @@ __global__ void __launch_bounds__(32) k_sq_lp(const SqRows* tab, const float* lo
 		out_ids[o] = top_ids[e], out_tlp[o] = top_lp[e];
 	}
 }
+
+// ---------------------------------------------------------------- calm_b200_decode_sample_queue_penalties
+
+// A step's penalty lane of each row (-1: a neutral request's row), passed by value to k_sq_lanes
+struct SqLanes {
+	int lane[SQ_ROWS];
+};
+
+// one warp, before a step with non-neutral rows: keep the step's lanes where k_vf_gemm<.., PEN> and k_sq_pen_step read them
+__global__ void __launch_bounds__(32) k_sq_lanes(const SqLanes l, int* lanes) {
+	pdl_enter();
+	if (threadIdx.x < SQ_ROWS) lanes[threadIdx.x] = l.lane[threadIdx.x];
+}
+
+// What k_sq_pen_admit needs of the request it admits to a lane: where its context, prompt and bias list lie in the
+// call's uploaded tokens and bias arrays, and its (presence, frequency, repetition, 0)
+struct SqPenAdmit {
+	int lane, ctx_off, ctx_len, off, len, bias_off, bias_len;
+	float4 par;
+};
+
+#define SQ_PEN_SPAN 1024 // vocabulary entries per CTA of k_sq_pen_admit
+
+// one launch per non-neutral request a round admits, CTA b owning the lane's entries [b SQ_PEN_SPAN, (b + 1) SQ_PEN_SPAN):
+// it clears them in the count and bias rows, then marks the tokens of ctx ++ prompt that fall among them seen and writes
+// the bias list's values there (ids are distinct within a list), so that nothing of the lane's previous occupant
+// remains.  Each entry is written by its own CTA only, the marks after the clear (__syncthreads orders a block's writes).
+__global__ void __launch_bounds__(256) k_sq_pen_admit(const SqPenAdmit q, const int* tokens, const int* bias_ids, const float* bias_val, int vocab, int* cnt,
+                                                      float* bias, float4* par) {
+	pdl_enter();
+	const int v0 = blockIdx.x * SQ_PEN_SPAN, v1 = min(v0 + SQ_PEN_SPAN, vocab);
+	int* c = cnt + (size_t)q.lane * vocab;
+	float* b = bias + (size_t)q.lane * vocab;
+	for (int v = v0 + threadIdx.x; v < v1; v += blockDim.x) c[v] = 0, b[v] = 0.0f;
+	__syncthreads();
+	for (int i = threadIdx.x; i < q.ctx_len + q.len; i += blockDim.x) {
+		const int tok = i < q.ctx_len ? tokens[q.ctx_off + i] : tokens[q.off + i - q.ctx_len];
+		if (tok >= v0 && tok < v1) c[tok] = SQ_PEN_SEEN;
+	}
+	for (int i = threadIdx.x; i < q.bias_len; i += blockDim.x) {
+		const int id = bias_ids[q.bias_off + i];
+		if (id >= v0 && id < v1) b[id] = bias_val[q.bias_off + i];
+	}
+	if (blockIdx.x == 0 && threadIdx.x == 0) par[q.lane] = q.par;
+}
+
+// one warp, after k_sq_end of a step with non-neutral rows: each such row's token counts once more in its lane, so the
+// next step's classifier sees c(v) over the tokens of steps 0 .. j (a count > 0 also makes the token seen)
+__global__ void __launch_bounds__(32) k_sq_pen_step(const int* lanes, const int* step_tok, int vocab, int* cnt) {
+	pdl_enter();
+	const int i = threadIdx.x;
+	if (i < SQ_ROWS && lanes[i] >= 0) ++cnt[(size_t)lanes[i] * vocab + step_tok[i]];
+}

@@ -22,6 +22,10 @@
 //               TOPK (with PF_CLS_GREEDY or PF_CLS_SAMPLE; calm_b200_decode_sample_queue_logprobs) computes every record
 //               above with the same operations and then each tile's a.topk largest logits of every token row, in
 //               PF_CLS_TOPK's layout and by its rule, which the unchanged k_pf_logprob<.., true> merges.
+//               PEN (with TOPK, whose lists are empty at a.topk == 0; calm_b200_decode_sample_queue_penalties) replaces
+//               each logit of a row whose v.lane[t] is non-negative by the request's processed logit (sq_pen_logit)
+//               before any record is formed, so the argmax records, logit rows, tile maxima, (max, sum) records and top-k
+//               lists all see the processed values.  Other rows are not touched.
 #pragma once
 
 #include "prefill.cuh"
@@ -45,7 +49,23 @@ struct VfArgs {
 	float* logits;     // PF_CLS_SAMPLE: [n_tokens][vocab] the logit rows
 	float* tmax;       // PF_CLS_SAMPLE: [n_tokens][nvt] each tile's maximum logit (the sampler's cand_val)
 	const int* slot;   // PF_QKV_SLOTS: [n_tokens] the cache slot of each row's keys and values
+	// PEN: the lanes' state (sq_pen_logit), and row t's lane, or -1 for a row left as it is
+	const int* lane;    // [VF_TOK] (k_sq_lanes)
+	const int* pcnt;    // [16][vocab] count of the token among the request's generated tokens, | SQ_PEN_SEEN if in ctx ++ prompt
+	const float* pbias; // [16][vocab] b(v): the request's logit bias, 0 off its list
+	const float4* ppar; // [16] (presence, frequency, repetition, 0)
 };
+
+#define SQ_PEN_SEEN (1 << 30) // a count row's mark of a token in the request's ctx ++ prompt; the count is the bits below
+
+// One logit of a non-neutral request through its processing (include/calm_b200.h), each operation one IEEE fp32
+// operation rounded to nearest: w is the token's count word, b its bias, par (presence, frequency, repetition, 0).
+__device__ __forceinline__ float sq_pen_logit(float l, int w, float b, float4 par) {
+	const int c = w & (SQ_PEN_SEEN - 1);
+	const float l1 = w != 0 && par.z != 1.0f ? (l > 0.0f ? __fdiv_rn(l, par.z) : __fmul_rn(l, par.z)) : l; // seen: in ctx ++ prompt, or c > 0
+	const float a = __fsub_rn(__fsub_rn(b, __fmul_rn(par.y, (float)c)), c > 0 ? par.x : 0.0f);
+	return a == 0.0f ? l1 : __fadd_rn(l1, a);
+}
 
 template <int DBITS>
 struct VfFmt {
@@ -96,11 +116,12 @@ __device__ __forceinline__ void vf_dequant(const uint32_t (&w)[VfFmt<DBITS>::WOR
 	}
 }
 
-template <int MODE, int DBITS, typename KVT, bool TOPK = false>
+template <int MODE, int DBITS, typename KVT, bool TOPK = false, bool PEN = false>
 __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, const VfArgs v) {
 	constexpr int W = VfFmt<DBITS>::WORDS, U = VfFmt<DBITS>::U;
 	constexpr bool CLS = MODE == PF_CLS_GREEDY || MODE == PF_CLS_SAMPLE;
 	static_assert(CLS || !TOPK, "the top-k lists are a classifier epilogue");
+	static_assert(TOPK || !PEN, "the processed logits come with the top-k epilogue (a.topk may be 0)");
 	__shared__ __align__(16) __half xs[2][VF_TOK][VF_XSTR];
 	__shared__ unsigned last_s;
 	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
@@ -229,6 +250,17 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 #pragma unroll
 			for (int j = 0; j < 4; ++j) lg[4 * tq + j][2 * rp] = x[0][j], lg[4 * tq + j][2 * rp + 1] = x[1][j];
 			__syncthreads();
+			if constexpr (PEN) { // consecutive threads on consecutive vocabulary entries of a row, so the lane rows load coalesced
+				const int pbase = (v.tile0 + fu) * VF_ROWS;
+				for (int e = tid; e < VF_TOK * VF_ROWS; e += VF_THREADS) {
+					const int t = e / VF_ROWS, r = e % VF_ROWS, ln = v.lane[t];
+					if (t < a.n_tokens && ln >= 0 && pbase + r < a.vocab) {
+						const size_t o = (size_t)ln * a.vocab + pbase + r;
+						lg[t][r] = sq_pen_logit(lg[t][r], v.pcnt[o], v.pbias[o], v.ppar[ln]);
+					}
+				}
+				__syncthreads();
+			}
 			// warp w: tokens 2 w, 2 w + 1.  Lane: rows lane + 32 i, ascending, so a strict > keeps the lowest index of the
 			// maximum; the butterfly gives a tie to the lower index.  Then sum exp(logit - max) over the tile's rows.
 			const int tile = v.tile0 + fu, rbase = tile * VF_ROWS;

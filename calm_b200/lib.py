@@ -28,7 +28,7 @@ SYMBOLS = [
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
     "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
-    "calm_b200_decode_sample_queue_context", "calm_b200_decode_sample_queue_logprobs",
+    "calm_b200_decode_sample_queue_context", "calm_b200_decode_sample_queue_logprobs", "calm_b200_decode_sample_queue_penalties",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -110,6 +110,10 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_queue_context.restype = C.c_int
     L.calm_b200_decode_sample_queue_logprobs.argtypes = L.calm_b200_decode_sample_queue_context.argtypes + [C.c_int, _fptr, _iptr, _fptr]
     L.calm_b200_decode_sample_queue_logprobs.restype = C.c_int
+    ctx_args = L.calm_b200_decode_sample_queue_context.argtypes
+    L.calm_b200_decode_sample_queue_penalties.argtypes = (ctx_args[:11] + [_fptr, _fptr, _fptr, _iptr, _iptr, _iptr, _fptr, C.c_int] + ctx_args[11:]
+                                                          + [C.c_int, _fptr, _iptr, _fptr])
+    L.calm_b200_decode_sample_queue_penalties.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -511,11 +515,12 @@ class DeviceModel:
             raise ValueError(f"{who}: the sum of max_new does not fit an int")
         return prompts, max_new, temperature, minp, stop, states
 
-    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None):
+    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None, pen=None):
         """Run a queue call over the laid-out tokens; ctx is (ctx_off, ctx_len), either of them None for a NULL array, or
         None for a call without those arguments.  Returns (tokens, states, served, steps, prompt_rows), and with `k` (the
         log-probability call) also each request's float32[out_len] log-probabilities and, for k > 0, its top ids and
-        log-probabilities [out_len, k] (None for k == 0)."""
+        log-probabilities [out_len, k] (None for k == 0).  `pen` (the penalty call) is the list of its arguments after
+        minp; without `k` that call gets k 0 and NULL outputs."""
         nreq = len(len_)
         mn = np.ascontiguousarray(max_new, np.int32)
         st = np.ascontiguousarray(stop, np.int32)
@@ -528,8 +533,9 @@ class DeviceModel:
         args = [C.byref(self.transformer), tokens.ctypes.data_as(ip), len(tokens)]
         if ctx is not None:
             args += [None if c is None else c.ctypes.data_as(ip) for c in ctx]
-        args += [off.ctypes.data_as(ip), len_.ctypes.data_as(ip), nreq, mn.ctypes.data_as(ip), temperature.ctypes.data_as(fp), minp.ctypes.data_as(fp),
-                 st.ctypes.data_as(ip) if len(st) else None, len(st), int(max_rows), rng, out.ctypes.data_as(ip), out_len.ctypes.data_as(ip), C.byref(steps)]
+        args += [off.ctypes.data_as(ip), len_.ctypes.data_as(ip), nreq, mn.ctypes.data_as(ip), temperature.ctypes.data_as(fp), minp.ctypes.data_as(fp)]
+        args += pen or []
+        args += [st.ctypes.data_as(ip) if len(st) else None, len(st), int(max_rows), rng, out.ctypes.data_as(ip), out_len.ctypes.data_as(ip), C.byref(steps)]
         if ctx is not None:
             args.append(C.byref(rows))
         if k is not None:
@@ -537,6 +543,8 @@ class DeviceModel:
             ids = np.full((total, k), -1, np.int32) if k else None
             tlp = np.full((total, k), np.nan, np.float32) if k else None
             args += [k, lp.ctypes.data_as(fp), ids.ctypes.data_as(ip) if k else None, tlp.ctypes.data_as(fp) if k else None]
+        elif pen is not None:
+            args += [0, None, None, None]
         served = fn(*args)
         o = np.concatenate([[0], np.cumsum(mn)]).astype(np.int64)
         toks = [out[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)]
@@ -578,6 +586,24 @@ class DeviceModel:
         len_ = np.asarray([len(p) for p in prompts], np.int32)
         return tokens, ctx_off, ctx_len, off, len_
 
+    def _optional_context_layout(self, who, contexts, ctx_of, prompts):
+        """_context_layout, or with contexts and ctx_of both None the prompts alone: (tokens, (ctx_off, ctx_len), off, len)
+        with (None, None) for NULL context arrays."""
+        if contexts is None and ctx_of is None:
+            nreq = len(prompts)
+            tokens = np.ascontiguousarray(np.concatenate(prompts) if nreq else np.zeros(0), np.int32)
+            len_ = np.asarray([len(p) for p in prompts], np.int32)
+            off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(len_)[:-1]]) if nreq else np.zeros(0), np.int32)
+            return tokens, (None, None), off, len_
+        tokens, ctx_off, ctx_len, off, len_ = self._context_layout(who, contexts, ctx_of, prompts)
+        return tokens, (ctx_off, ctx_len), off, len_
+
+    def _check_queue_k(self, k):
+        """The queue calls' check on k (0 allowed), raised before the library would abort the process."""
+        kmax = min(TOPK_MAX, self.vocab)
+        if not isinstance(k, (int, np.integer)) or isinstance(k, bool) or not 0 <= k <= kmax:
+            raise ValueError(f"k must be an integer in [0, {kmax}], got {k!r}")
+
     def decode_sample_queue(self, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states):
         """calm_b200_decode_sample_queue: request i continues prompts[i] (a sequence of at least one token id) for at most
         max_new[i] tokens at temperature[i] / minp[i] from rng_states[i], stopping after a token in `stop` (a sequence of
@@ -613,21 +639,73 @@ class DeviceModel:
         (None for k == 0).  The numbers are the log-softmax of the step's logits at temperature 1 without the min-p cut.
         Raises ValueError where the C call would abort (k outside [0, min(TOPK_MAX, vocab)] included)."""
         who = "decode_sample_queue_logprobs"
-        kmax = min(TOPK_MAX, self.vocab)
-        if not isinstance(k, (int, np.integer)) or isinstance(k, bool) or not 0 <= k <= kmax:
-            raise ValueError(f"k must be an integer in [0, {kmax}], got {k!r}")
+        self._check_queue_k(k)
         prompts, max_new, temperature, minp, stop, states = self._queue_args(who, prompts, max_new, temperature, minp, stop, max_rows, rng_states)
-        if contexts is None and ctx_of is None:
-            nreq = len(prompts)
-            tokens = np.ascontiguousarray(np.concatenate(prompts) if nreq else np.zeros(0), np.int32)
-            len_ = np.asarray([len(p) for p in prompts], np.int32)
-            off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(len_)[:-1]]) if nreq else np.zeros(0), np.int32)
-            ctx = (None, None)
-        else:
-            tokens, ctx_off, ctx_len, off, len_ = self._context_layout(who, contexts, ctx_of, prompts)
-            ctx = (ctx_off, ctx_len)
+        tokens, ctx, off, len_ = self._optional_context_layout(who, contexts, ctx_of, prompts)
         return self._queue_call(self.lib.calm_b200_decode_sample_queue_logprobs, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states,
                                 k=int(k))
+
+    def decode_sample_queue_penalties(self, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states, presence=None,
+                                      frequency=None, repetition=None, logit_bias=None, k=None):
+        """calm_b200_decode_sample_queue_penalties: decode_sample_queue_logprobs (contexts and ctx_of both None: no
+        contexts) where request i's logits go through its presence[i], frequency[i] and repetition[i] penalties and its
+        logit_bias[i] ({token id: value}, or None) before its token is chosen, as include/calm_b200.h states.  presence /
+        frequency / repetition None mean 0 / 0 / 1 for every request, logit_bias None no bias.  k None: no
+        log-probabilities, and the return value is decode_sample_queue_context's (tokens, states, served, steps,
+        prompt_rows); otherwise decode_sample_queue_logprobs' tuple, of the processed logits.  Raises ValueError where
+        the C call would abort."""
+        who = "decode_sample_queue_penalties"
+        if k is not None:
+            self._check_queue_k(k)
+        prompts, max_new, temperature, minp, stop, states = self._queue_args(who, prompts, max_new, temperature, minp, stop, max_rows, rng_states)
+        nreq = len(prompts)
+        fp, ip = C.POINTER(C.c_float), C.POINTER(C.c_int)
+        keep = []  # the arrays the C call reads
+
+        def per_request(name, xs, lo, hi):
+            if xs is None:
+                return None
+            try:
+                a = np.ascontiguousarray(xs, np.float32).reshape(-1)
+            except (TypeError, ValueError) as e:
+                raise ValueError(f"{who}: bad {name}: {e}") from None
+            if len(a) != nreq:
+                raise ValueError(f"{who} takes one {name} per prompt: {nreq} prompts, {len(a)} values")
+            if not (np.isfinite(a) & (a >= lo) & (a <= hi)).all():
+                raise ValueError(f"{who}: every {name} must be finite and in [{lo:g}, {hi:g}]")
+            keep.append(a)
+            return a.ctypes.data_as(fp)
+
+        pen = [per_request("presence", presence, -1e6, 1e6), per_request("frequency", frequency, -1e6, 1e6),
+               per_request("repetition", repetition, np.float32(1e-6), 1e6)]
+        if logit_bias is None:
+            pen += [None, None, None, None, 0]
+        else:
+            logit_bias = list(logit_bias)
+            if len(logit_bias) != nreq:
+                raise ValueError(f"{who} takes one logit_bias per prompt: {nreq} prompts, {len(logit_bias)} values")
+            ids, vals, blen = [], [], []
+            for i, d in enumerate(logit_bias):
+                d = {} if d is None else d
+                if not isinstance(d, dict):
+                    raise ValueError(f"logit_bias[{i}] must be a dict of token id: value, or None")
+                for t, b in d.items():
+                    if not isinstance(t, (int, np.integer)) or isinstance(t, bool) or not 0 <= t < self.vocab:
+                        raise ValueError(f"logit_bias[{i}] has an id outside [0, {self.vocab}): {t!r}")
+                    b32 = np.float32(b)
+                    if not np.isfinite(b32) or abs(b32) > 1e6:
+                        raise ValueError(f"logit_bias[{i}][{t}] must be finite and in [-1e6, 1e6], got {b!r}")
+                    ids.append(int(t)), vals.append(b32)
+                blen.append(len(d))
+            b_len = np.asarray(blen, np.int32)
+            b_off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(b_len)[:-1]]) if nreq else np.zeros(0), np.int32)
+            b_ids, b_val = np.asarray(ids, np.int32), np.asarray(vals, np.float32)
+            keep += [b_len, b_off, b_ids, b_val]
+            pen += [b_off.ctypes.data_as(ip), b_len.ctypes.data_as(ip), b_ids.ctypes.data_as(ip) if len(ids) else None,
+                    b_val.ctypes.data_as(fp) if len(ids) else None, len(ids)]
+        tokens, ctx, off, len_ = self._optional_context_layout(who, contexts, ctx_of, prompts)
+        return self._queue_call(self.lib.calm_b200_decode_sample_queue_penalties, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows,
+                                states, k=None if k is None else int(k), pen=pen)
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""

@@ -384,6 +384,46 @@ int calm_b200_decode_sample_queue_logprobs(struct Transformer* transformer, cons
                                            int* out_tokens, int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
                                            float* top_logprobs);
 
+/* calm_b200_decode_sample_queue_logprobs where each request's logits first go through its own logit bias and presence,
+ * frequency and repetition penalties (OpenAI's logit_bias / presence_penalty / frequency_penalty, the repetition_penalty
+ * of Hugging Face generate; INTEGRATION.md).
+ * Settings.  Request i has presence p = presence[i], frequency f = frequency[i], repetition r = repetition[i] (each
+ * array may be NULL: 0, 0 and 1 for every request) and the bias list bias_ids / bias_val[bias_off[i] .. + bias_len[i]);
+ * b(v) is the list's value for id v, 0 off the list.  bias_off and bias_len may both be NULL when n_bias == 0.
+ * Processing.  At request i's step j, with l(v) the step's fp32 logit as calm_b200_decode_sample_queue_logprobs
+ * computes it, c(v) how many of the request's tokens of steps 0 .. j-1 equal v (generated tokens only) and seen(v)
+ * true when v is among the ctx_len[i] + len[i] tokens of ctx ++ prompt (the last one included) or c(v) > 0:
+ *     l1 = (seen(v) && r != 1) ? (l > 0 ? l / r : l * r) : l
+ *     a  = (b(v) - f * (float)c(v)) - (c(v) > 0 ? p : 0)
+ *     l2 = (a == 0) ? l1 : l1 + a
+ * each operation one IEEE fp32 operation rounded to nearest, with no contraction (numpy float32 gives the same bits).
+ * l2 replaces l for everything the step does: a greedy request's token is the first maximum of l2, a sampled one's the
+ * reference's sample() at its temperature / minp over l2, and logprobs / top_ids / top_logprobs are those of l2
+ * (processed log-probabilities) by the _logprobs call's rules.
+ * Neutral requests.  A request with p == 0, f == 0, r == 1 and an empty list is neutral: its outputs are the bits
+ * calm_b200_decode_sample_queue_logprobs gives it, whatever shares its steps.
+ * Arguments.  logprobs == NULL with k == 0: no log-probability work (the call then launches what
+ * calm_b200_decode_sample_queue_context launches while no non-neutral request is in flight); otherwise the _logprobs
+ * rules apply.  Contexts, the schedule, placement, stops, steps, prompt_rows and independence are the context call's:
+ * request i's outputs do not depend on the other requests, max_rows, its slots, seq_len or an earlier call.  The call
+ * aborts before any device work where calm_b200_decode_sample_queue_logprobs aborts, and when n_bias < 0, a bias list
+ * lies outside [0, n_bias), a bias id is outside [0, vocab_size) or repeats within one list, a value is not finite,
+ * |p|, |f| or |b| exceeds 1e6, or r lies outside [1e-6, 1e6] (bounds that keep every l2 finite).
+ * Fallback (return 0; as the context call: MoE, tensor parallelism, shapes the prompt pass does not serve, requests
+ * that do not fit seq_len).  A neutral request runs the context call's fallback.  A non-neutral one decodes on the
+ * decode path and takes each step's device logits; the host applies the expression above and takes the first maximum
+ * (greedy) or calls calm_b200_sample_logits with the request's state, and log-probabilities come from l2 in double as in
+ * calm_b200_decode_sample_queue_logprobs' fallback.
+ * Memory.  The first call with a non-neutral request allocates 16 lanes of 8 bytes per vocabulary entry, a count and
+ * a bias row (16.4 MB at a 128256-token vocabulary), and room for the call's tokens and bias lists (4 bytes per token
+ * of n, 8 per entry of n_bias), regrown by a larger call. */
+int calm_b200_decode_sample_queue_penalties(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                            const int* off, const int* len, int nreq, const int* max_new, const float* temperature, const float* minp,
+                                            const float* presence, const float* frequency, const float* repetition, const int* bias_off,
+                                            const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias, const int* stop, int n_stop,
+                                            int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps,
+                                            int* prompt_rows, int k, float* logprobs, int* top_ids, float* top_logprobs);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
@@ -431,7 +471,8 @@ void calm_b200_read_kv(struct Transformer* transformer, int layer, int kv_pos, f
  *            path (n of its tokens), or of the last step of the last sampled calm_b200_decode_sample_n or
  *            calm_b200_decode_sample_batch call that took its new path (n = nseq, row b = sequence b), the values its
  *            sampler drew from, or of the last step of a calm_b200_decode_sample_queue call on its new path if that step
- *            sampled any row (n = the rows in flight)
+ *            sampled any row (n = the rows in flight).  After calm_b200_decode_sample_queue_penalties the rows of
+ *            non-neutral requests hold their processed logits l2, the values the sampler drew from
  *   After calm_b200_decode_sample_n or calm_b200_decode_sample_batch on its new path, the PF_* matrices hold the last
  *   step, row b = sequence b.  After calm_b200_decode_sample_queue on its new path, the PF_* matrices and PF_LOGITS hold
  *   the last step, with the rows in flight in admission order. */
