@@ -209,11 +209,15 @@ struct Prefill {
 	int* sqpcnt = nullptr;    // [16][vocab]
 	float* sqpbias = nullptr; // [16][vocab]
 	float4* sqppar = nullptr; // [16]
-	int* sqlanes = nullptr;   // [16] the step's lane of each row (k_sq_lanes)
+	int* sqlanes = nullptr;   // [32] the step's lane of each row (k_sq_lanes), and its automaton state (k_sq_mask_lanes) from 16
 	int* sqptok = nullptr;    // [sqptok_cap]
 	int* sqpbid = nullptr;    // [sqpb_cap]
 	float* sqpbval = nullptr;
 	size_t sqptok_cap = 0, sqpb_cap = 0;
+	// the automaton of calm_b200_decode_sample_queue_constrained: its states' bitmasks (VfArgs::allow), uploaded once per
+	// call with a constrained request and regrown like pf.sqout
+	uint32_t* sqallow = nullptr; // [sqallow_cap]
+	size_t sqallow_cap = 0;
 };
 Prefill pf;
 
@@ -229,6 +233,7 @@ void pf_free() {
 	cudaFree(pf.sqrows), cudaFree(pf.sqgroups), cudaFree(pf.sqtok), cudaFree(pf.sqout), cudaFree(pf.sqst);
 	cudaFree(pf.sqtopv), cudaFree(pf.sqtopi), cudaFree(pf.sqtid), cudaFree(pf.sqtlp), cudaFree(pf.sqlp), cudaFree(pf.sqoid), cudaFree(pf.sqolp);
 	cudaFree(pf.sqpcnt), cudaFree(pf.sqpbias), cudaFree(pf.sqppar), cudaFree(pf.sqlanes), cudaFree(pf.sqptok), cudaFree(pf.sqpbid), cudaFree(pf.sqpbval);
+	cudaFree(pf.sqallow);
 	pf = Prefill();
 }
 
@@ -1128,7 +1133,9 @@ static unsigned long long xorshift_step(unsigned long long s) {
 
 // The device sampler on its own: logits given by the host, any vocabulary size; returns the token and advances *rng_state.
 // Same kernels as the decode loop (k_sample_scan + k_sample_pick); device_us (optional) receives their mean duration.
-extern "C" int calm_b200_sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us) {
+// `masked` (the fallback of calm_b200_decode_sample_queue_constrained): k_sample_scan_rows_masked on the one row instead
+// of k_sample_scan, so that a -inf logit never survives.
+static int sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us, bool masked) {
 	select_device();
 	if (vocab <= 0) CALM_FATAL("sample_logits: empty vocabulary");
 	if (temperature == 0.0f || minp >= 1.0f) { // greedy, first maximum (sampler.c:34-42); the generator is not touched
@@ -1165,7 +1172,8 @@ extern "C" int calm_b200_sample_logits(const float* logits_host, int vocab, floa
 		CUDA_CHECK(cudaMemcpyAsync(sst, &hs, sizeof(hs), cudaMemcpyHostToDevice, st));
 		k_chunk_max<<<nchunks, 256, 0, st>>>(logits, vocab, cmax);
 		CUDA_CHECK(cudaEventRecord(e0, st));
-		k_sample_scan<<<nchunks, 256, 0, st>>>(sa);
+		if (masked) k_sample_scan_rows_masked<<<dim3(nchunks, 1), 256, 0, st>>>(sa);
+		else k_sample_scan<<<nchunks, 256, 0, st>>>(sa);
 		k_sample_pick<<<1, 256, 0, st>>>(sa, sst, tp, nullptr, tok, 0);
 		CUDA_CHECK(cudaEventRecord(e1, st));
 		CUDA_CHECK(cudaEventSynchronize(e1));
@@ -1181,6 +1189,10 @@ extern "C" int calm_b200_sample_logits(const float* logits_host, int vocab, floa
 	cudaFree(logits), cudaFree(cmax), cudaFree(sst), cudaFree(count), cudaFree(csum), cudaFree(sidx), cudaFree(sprob), cudaFree(tok), cudaFree(tp);
 	cudaEventDestroy(e0), cudaEventDestroy(e1), cudaStreamDestroy(st);
 	return htok;
+}
+
+extern "C" int calm_b200_sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us) {
+	return sample_logits(logits_host, vocab, temperature, minp, rng_state, device_us, false);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1279,19 +1291,20 @@ static void vf_reserve() {
 // out = W . X^T over the rows of `a` for the n <= 16 rows of (hi, lo), in `units` row blocks of 128 (UP: of w1 and of w3
 // each); the classifier from vocabulary tile `tile0` on; PF_QKV_SLOTS: row t's keys and values to cache slot slot[t].
 // Every K-slice gets the same number of CTAs, as many as stay resident together, each walking row blocks with the same
-// stride.  PEN: the rows' lanes as k_sq_lanes left them in pf.sqlanes.
-template <int MODE, int DBITS, typename KVT, bool TOPK = false, bool PEN = false>
+// stride.  PEN: the rows' lanes as k_sq_lanes left them in pf.sqlanes; MASK: also their automaton states, after them.
+template <int MODE, int DBITS, typename KVT, bool TOPK = false, bool PEN = false, bool MASK = false>
 static void vf_gemm(const __half* hi, const __half* lo, const PfGemmArgs& a, int units, int tile0 = 0, const int* slot = nullptr) {
 	static int cap = 0, sms = 0;
-	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT, TOPK, PEN>, VF_THREADS, 0), sms = g.sms;
+	if (sms != g.sms) cap = max_ctas(k_vf_gemm<MODE, DBITS, KVT, TOPK, PEN, MASK>, VF_THREADS, 0), sms = g.sms;
 	VfArgs v = {};
 	v.xhi = hi, v.xlo = lo, v.acc = pf.vacc, v.cnt = pf.vcnt;
 	v.nsl = vf_slices(a.K), v.units = units, v.rows = (MODE == PF_UP ? 2 : 1) * units * VF_ROWS;
 	v.tile0 = tile0, v.nvt = cdiv(g.cfg.vocab_size, PF_BM);
 	v.logits = pf.vlogits, v.tmax = pf.vtmax, v.slot = slot;
 	if constexpr (PEN) v.lane = pf.sqlanes, v.pcnt = pf.sqpcnt, v.pbias = pf.sqpbias, v.ppar = pf.sqppar;
+	if constexpr (MASK) v.mstate = pf.sqlanes + SQ_ROWS, v.allow = pf.sqallow;
 	const int tasks = (MODE == PF_UP ? 2 : 1) * units;
-	launch_pdl(k_vf_gemm<MODE, DBITS, KVT, TOPK, PEN>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
+	launch_pdl(k_vf_gemm<MODE, DBITS, KVT, TOPK, PEN, MASK>, dim3(balanced_grid(tasks, cap / v.nsl > 0 ? cap / v.nsl : 1), v.nsl), VF_THREADS, 0, a, v);
 }
 
 // What the rows of a prompt-pass block are
@@ -1841,13 +1854,14 @@ static void vf_sample_reserve() {
 
 // The n rows of the last PF_CLS_SAMPLE classifier through the decode's sampler, side by side: row i is k_sample_scan +
 // k_sample_pick on its own lists and its own SampleState pf.vstate[i] (k_sample_scan_rows / k_sample_pick_rows), and its
-// token goes to out[i] (default pf.vsampled[i])
-static void vf_sample_rows(int n, int* out = nullptr) {
+// token goes to out[i] (default pf.vsampled[i]).  `masked`: k_sample_scan_rows_masked, where -inf never survives.
+static void vf_sample_rows(int n, int* out = nullptr, bool masked = false) {
 	const int vocab = g.cfg.vocab_size, nvt = cdiv(vocab, PF_BM), nch = g.sample_chunks;
 	SampleArgs sa;
 	sa.logits = pf.vlogits, sa.cand_val = pf.vtmax, sa.ncand = nvt, sa.vocab = vocab, sa.nchunks = nch;
 	sa.st = pf.vstate, sa.count = pf.vcount, sa.csum = pf.vcsum, sa.sidx = pf.vsidx, sa.sprob = pf.vsprob;
-	launch_pdl(k_sample_scan_rows, dim3(nch, n), 256, 0, sa);
+	if (masked) launch_pdl(k_sample_scan_rows_masked, dim3(nch, n), 256, 0, sa);
+	else launch_pdl(k_sample_scan_rows, dim3(nch, n), 256, 0, sa);
 	launch_pdl(k_sample_pick_rows, n, 256, 0, sa, pf.vstate, out ? out : pf.vsampled);
 }
 
@@ -2246,9 +2260,10 @@ static void sq_lp_reserve(size_t total, int k) {
 // A queue step's final norm and short-block classifier with its log-probability epilogue: pf_score's greedy (or, with
 // `sample`, sampled) classifier on the n rows, with k > 0 its TOPK variant writing each tile's top-k lists to pf.sqtopv /
 // pf.sqtopi.  The merge is left to sq_merge, after each row's target is set.  With `pen` (a step with non-neutral rows of
-// calm_b200_decode_sample_queue_penalties) the TOPK variant with PEN runs whatever k is, and processes those rows' logits.
+// calm_b200_decode_sample_queue_penalties) the TOPK variant with PEN runs whatever k is, and processes those rows' logits;
+// with `mask` (a step with a constrained row) its MASK variant also masks them.
 template <int DBITS, typename KVT>
-static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample, bool pen = false) {
+static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample, bool pen = false, bool mask = false) {
 	const Config& c = g.cfg;
 	const int nvt = cdiv(c.vocab_size, PF_BM);
 	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)g.w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
@@ -2258,7 +2273,9 @@ static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample, bool pen
 	a.topv = pf.sqtopv, a.topi = pf.sqtopi, a.topk = k;
 	for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) {
 		const int units = imin(VF_CLS_UNITS, nvt - t0);
-		if (pen && sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		if (mask && sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		else if (mask) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
+		else if (pen && sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
 		else if (pen) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
 		else if (sample && k) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
 		else if (sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
@@ -2311,8 +2328,8 @@ static void sq_pen_reserve(int n, int n_bias) {
 		pf.sqpcnt = (int*)dev_alloc(SQ_ROWS * vocab * sizeof(int));
 		pf.sqpbias = (float*)dev_alloc(SQ_ROWS * vocab * sizeof(float));
 		pf.sqppar = (float4*)dev_alloc(SQ_ROWS * sizeof(float4));
-		pf.sqlanes = (int*)dev_alloc(SQ_ROWS * sizeof(int));
 	}
+	if (!pf.sqlanes) pf.sqlanes = (int*)dev_alloc(2 * SQ_ROWS * sizeof(int));
 	if ((size_t)n > pf.sqptok_cap) { // (no step of an earlier call is still reading them)
 		CUDA_CHECK(cudaStreamSynchronize(g.stream));
 		cudaFree(pf.sqptok);
@@ -2328,6 +2345,70 @@ static void sq_pen_reserve(int n, int n_bias) {
 	}
 }
 
+// The token automaton of calm_b200_decode_sample_queue_constrained (include/calm_b200.h) and each request's start state
+// (start NULL: no request is constrained).  sq_run checks it and fills `fin`, which states are final.
+struct SqAutomaton {
+	int n_states;
+	const uint32_t* allow;
+	const int* next_default;
+	const int* exc_off;
+	const int* exc_tok;
+	const int* exc_next;
+	const int* start;
+	int* out_state;
+	int words;             // ceil(vocab / 32): one state's bitmask
+	std::vector<char> fin; // [n_states] no token allowed
+	int s0(int i) const { return start ? start[i] : -1; }
+	bool allowed(int s, int v) const { return (allow[(size_t)s * words + (v >> 5)] >> (v & 31)) & 1u; }
+	// the state after allowed token v in state s: its exception, else the default.  v comes from the device (or the
+	// fallback's sampler), which never draws a masked token; one that did would be a bug, so it aborts here rather than
+	// taking a default that may be -1 and leaving the request unconstrained.
+	int next(int s, int v) const {
+		if (v < 0 || v >= words * 32 || !allowed(s, v)) CALM_FATAL("constrained queue: token %d is not allowed in state %d", v, s);
+		const int* b = exc_tok + exc_off[s];
+		const int* e = exc_tok + exc_off[s + 1];
+		const int* x = std::lower_bound(b, e, v);
+		return x != e && *x == v ? exc_next[x - exc_tok] : next_default[s];
+	}
+};
+
+// Abort unless `a` is a well-formed automaton for a vocabulary of `vocab` tokens with valid start states (the automaton
+// itself is read only when some request is constrained); fills a.words and a.fin
+static void sq_check_automaton(const char* who, SqAutomaton& a, int nreq, const int* max_new, int vocab) {
+	if (a.n_states < 0) CALM_FATAL("%s: negative n_states %d", who, a.n_states);
+	a.words = cdiv(vocab, 32);
+	bool any = false;
+	for (int i = 0; i < nreq; ++i) {
+		if (a.s0(i) < -1 || a.s0(i) >= a.n_states) CALM_FATAL("%s: request %d's start state %d outside [-1, %d)", who, i, a.s0(i), a.n_states);
+		any = any || a.s0(i) >= 0;
+	}
+	if (!any) return;
+	if (!a.allow || !a.next_default || !a.exc_off || !a.exc_tok || !a.exc_next) CALM_FATAL("%s: an automaton array is NULL", who);
+	if (a.exc_off[0] != 0) CALM_FATAL("%s: exc_off[0] is %d, not 0", who, a.exc_off[0]);
+	const uint32_t tail = vocab % 32 ? ~0u << (vocab % 32) : 0u; // the last word's bits past the vocabulary
+	a.fin.assign(a.n_states, 0);
+	for (int s = 0; s < a.n_states; ++s) {
+		const uint32_t* w = a.allow + (size_t)s * a.words;
+		if (w[a.words - 1] & tail) CALM_FATAL("%s: state %d allows a token past the %d-token vocabulary", who, s, vocab);
+		long allowed = 0;
+		for (int j = 0; j < a.words; ++j) allowed += __builtin_popcount(w[j]);
+		a.fin[s] = allowed == 0;
+		const int e0 = a.exc_off[s], e1 = a.exc_off[s + 1];
+		if (e1 < e0) CALM_FATAL("%s: exc_off decreases at state %d (%d, %d)", who, s, e0, e1);
+		for (int e = e0; e < e1; ++e) {
+			const int v = a.exc_tok[e];
+			if (v < 0 || v >= vocab || !a.allowed(s, v)) CALM_FATAL("%s: state %d's exception token %d is not allowed in it", who, s, v);
+			if (e > e0 && v <= a.exc_tok[e - 1]) CALM_FATAL("%s: state %d's exception tokens are not strictly ascending at %d", who, s, v);
+			if (a.exc_next[e] < 0 || a.exc_next[e] >= a.n_states) CALM_FATAL("%s: state %d's exception next state %d outside [0, %d)", who, s, a.exc_next[e], a.n_states);
+		}
+		const int d = a.next_default[s];
+		if (d < -1 || d >= a.n_states) CALM_FATAL("%s: state %d's default next state %d outside [-1, %d)", who, s, d, a.n_states);
+		if (d == -1 && allowed > e1 - e0) CALM_FATAL("%s: state %d allows a token outside its exception list and has no default next state", who, s);
+	}
+	for (int i = 0; i < nreq; ++i)
+		if (max_new[i] > 0 && a.s0(i) >= 0 && a.fin[a.s0(i)]) CALM_FATAL("%s: request %d starts in final state %d", who, i, a.s0(i));
+}
+
 // calm_b200_decode_sample_queue_context, and calm_b200_decode_sample_queue with every ctx_len 0 (`who` names the call in
 // error messages): a round's extent goes through the packed prompt pass (sb_prefill), each request's own rows continuing
 // its context at positions ctx_len .. (PF_CONTEXTS where a block holds such rows); a step whose rows have contexts runs
@@ -2337,11 +2418,14 @@ static void sq_pen_reserve(int n, int n_bias) {
 // (calm_b200_decode_sample_queue_penalties) each non-neutral request holds a lane from admission to retirement, cleared
 // and filled by k_sq_pen_admit; a step with such rows passes their lanes to k_sq_lanes, runs sq_classify's PEN classifier
 // and after k_sq_end k_sq_pen_step, every
-// other step exactly the kernels it runs without `pen`.
+// other step exactly the kernels it runs without `pen`.  With `aut` (calm_b200_decode_sample_queue_constrained, with
+// `pen`) the host follows each constrained request's state from the step's tokens, read back as the stop list's are; a
+// step with a constrained row passes the rows' lanes and states to k_sq_mask_lanes, runs sq_classify's MASK classifier
+// and, when such a row samples, k_sample_scan_rows_masked; every other step exactly the kernels it runs without `aut`.
 static int sq_run(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off,
                   const int* len, int nreq, const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
                   int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows,
-                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr) {
+                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr, SqAutomaton* aut = nullptr) {
 	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
 	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, max_rows, CALM_B200_SAMPLE_N_MAX);
 	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, n_stop);
@@ -2387,16 +2471,21 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			}
 		}
 	}
+	if (aut) sq_check_automaton(who, *aut, nreq, max_new, g.cfg.vocab_size);
 	check_tokens(tokens, n);
 	check_tokens(stop, n_stop);
 	if (steps) *steps = 0;
 	if (prompt_rows) *prompt_rows = 0;
+	std::vector<int> cur(nreq, -1); // a constrained request's automaton state after its tokens so far
+	for (int i = 0; aut && i < nreq; ++i) cur[i] = aut->s0(i);
+	auto ends = [&](int i) { return cur[i] >= 0 && aut->fin[cur[i]]; }; // the request's last token led to a final state
 	std::vector<char> is_stop(g.cfg.vocab_size, 0);
 	for (int k = 0; k < n_stop; ++k) is_stop[stop[k]] = 1;
 	std::vector<size_t> O(nreq + 1, 0); // request i's tokens go to out_tokens[O[i] ..]
 	for (int i = 0; i < nreq; ++i) O[i + 1] = O[i] + max_new[i];
 	for (int i = 0; i < nreq; ++i)
 		if (max_new[i] == 0) out_len[i] = 0; // never admitted
+	if (aut && aut->out_state) std::copy(cur.begin(), cur.end(), aut->out_state); // (each request's final value below)
 	if (total == 0) return 1;
 	auto is_greedy = [&](int i) { return temperature[i] == 0.0f || minp[i] >= 1.0f; }; // sample() is greedy there
 	bool fits = true;
@@ -2414,8 +2503,8 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			const int L = (int)p.size() - 1;
 			int tok = p[L], k = 0;
 			if (max_new[i] > 0) forward_prefill_cuda(transformer, p.data(), L, 0);
-			const bool processed = pen && !pen->neutral(i);
-			std::vector<float> logits(lp || processed ? g.cfg.vocab_size : 0);
+			const bool processed = pen && !pen->neutral(i), masked = cur[i] >= 0;
+			std::vector<float> logits(lp || processed || masked ? g.cfg.vocab_size : 0);
 			std::vector<int> cnt(processed ? g.cfg.vocab_size : 0);
 			std::vector<float> bias(processed ? g.cfg.vocab_size : 0);
 			std::vector<char> seen(processed ? g.cfg.vocab_size : 0);
@@ -2424,18 +2513,26 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 				for (int e = 0; e < pen->nb(i); ++e) bias[pen->bias_ids[pen->bias_off[i] + e]] = pen->bias_val[pen->bias_off[i] + e];
 			}
 			while (k < max_new[i]) {
-				if (processed) { // the decode path's device logits (its argmax discarded), processed and sampled on the host
+				if (processed || masked) { // the decode path's device logits (its argmax discarded), processed, masked and sampled on the host
 					unsigned long long unused = 1;
 					calm_b200_forward_sample(transformer, tok, L + k, 0.0f, 0.0f, &unused);
 					calm_b200_read_device_logits(logits.data());
-					for (int v = 0; v < g.cfg.vocab_size; ++v)
+					for (int v = 0; processed && v < g.cfg.vocab_size; ++v)
 						logits[v] = sq_pen_logit_host(logits[v], cnt[v], seen[v] || cnt[v] > 0, bias[v], pen->p(i), pen->f(i), pen->r(i));
-					tok = calm_b200_sample_logits(logits.data(), g.cfg.vocab_size, temperature[i], minp[i], &rng_states[i], nullptr); // (greedy: first maximum)
-					++cnt[tok];
-					if (lp) host_logprobs(logits.data(), g.cfg.vocab_size, tok, lp->k, lp->logprobs + O[i] + k, lp->top_ids + (O[i] + k) * lp->k,
-					                      lp->top_logprobs + (O[i] + k) * lp->k);
+					for (int v = 0; masked && v < g.cfg.vocab_size; ++v)
+						if (!aut->allowed(cur[i], v)) logits[v] = -INFINITY;
+					// (greedy: the first maximum; sampled: through k_sample_scan_rows_masked where the row is masked)
+					tok = sample_logits(logits.data(), g.cfg.vocab_size, temperature[i], minp[i], &rng_states[i], nullptr, masked);
+					if (processed) ++cnt[tok];
+					if (lp) {
+						const size_t o = O[i] + k;
+						host_logprobs(logits.data(), g.cfg.vocab_size, tok, lp->k, lp->logprobs + o, lp->top_ids + o * lp->k, lp->top_logprobs + o * lp->k);
+						for (size_t e = o * lp->k; masked && e < (o + 1) * lp->k; ++e) // ranks past the allowed tokens
+							if (lp->top_logprobs[e] == -INFINITY) lp->top_ids[e] = -1;
+					}
 					out_tokens[O[i] + k++] = tok;
-					if (is_stop[tok]) break;
+					if (masked) cur[i] = aut->next(cur[i], tok);
+					if (is_stop[tok] || ends(i)) break;
 					continue;
 				}
 				tok = calm_b200_forward_sample(transformer, tok, L + k, temperature[i], minp[i], &rng_states[i]);
@@ -2448,6 +2545,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 				if (is_stop[tok]) break;
 			}
 			out_len[i] = k;
+			if (aut && aut->out_state) aut->out_state[i] = cur[i];
 		}
 		return 0;
 	}
@@ -2474,6 +2572,19 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbid, pen->bias_ids, (size_t)pen->n_bias * sizeof(int), cudaMemcpyHostToDevice, g.stream));
 			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbval, pen->bias_val, (size_t)pen->n_bias * sizeof(float), cudaMemcpyHostToDevice, g.stream));
 		}
+	}
+	bool any_aut = false; // a request with max_new > 0 is constrained: the automaton is uploaded, once
+	for (int i = 0; aut && i < nreq; ++i) any_aut = any_aut || (max_new[i] > 0 && cur[i] >= 0);
+	if (any_aut) {
+		const size_t words = (size_t)aut->n_states * aut->words;
+		if (!pf.sqlanes) pf.sqlanes = (int*)dev_alloc(2 * SQ_ROWS * sizeof(int));
+		if (words > pf.sqallow_cap) { // (no step of an earlier call is still reading it)
+			CUDA_CHECK(cudaStreamSynchronize(g.stream));
+			cudaFree(pf.sqallow);
+			pf.sqallow_cap = words;
+			pf.sqallow = (uint32_t*)dev_alloc(words * sizeof(uint32_t));
+		}
+		CUDA_CHECK(cudaMemcpyAsync(pf.sqallow, aut->allow, words * sizeof(uint32_t), cudaMemcpyHostToDevice, g.stream));
 	}
 	std::vector<int> lane_of(nreq, -1); // a non-neutral request's lane while it is in flight
 	unsigned lanes_free = (1u << SQ_ROWS) - 1;
@@ -2558,7 +2669,10 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		SqRows r = {};
 		SqGroups grp = {};
 		SqLanes lanes;
-		bool pen_step = false; // a row of the step is a non-neutral request's
+		SqMaskLanes ml;
+		bool pen_step = false;     // a row of the step is a non-neutral request's
+		bool mask_step = false;    // a row of the step is a constrained request's
+		bool mask_sampled = false; // .. that samples
 		r.n = (int)live.size();
 		int nsampled = 0, lmax = 0, nsuf = 0;
 		std::map<int, std::vector<int>> groups; // rows by their context's first slot
@@ -2573,6 +2687,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			r.st0[k].rng = gr ? 1 : rng_states[i], r.st0[k].temperature = gr ? 1.0f : temperature[i], r.st0[k].cut_delta = gr ? 0.0f : logf(minp[i]) * temperature[i];
 			r.out[k] = (int)(O[i] + j), r.req[k] = i, r.greedy[k] = gr;
 			lanes.lane[k] = lane_of[i], pen_step = pen_step || lane_of[i] >= 0;
+			ml.lane[k] = lane_of[i], ml.state[k] = cur[i], mask_step = mask_step || cur[i] >= 0, mask_sampled = mask_sampled || (cur[i] >= 0 && !gr);
 			nsampled += !gr, lmax = std::max(lmax, q.L + j), row_of[i] = k;
 			grp.ctx[k] = make_int2(q.c, q.nc);
 			nsuf = std::max(nsuf, cdiv(q.L + j + 1, SN_CHUNK) - q.nc / SN_CHUNK);
@@ -2582,8 +2697,10 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			}
 		}
 		std::fill(lanes.lane + r.n, lanes.lane + SQ_ROWS, -1);
+		std::fill(ml.lane + r.n, ml.lane + SQ_ROWS, -1), std::fill(ml.state + r.n, ml.state + SQ_ROWS, -1);
 		launch_pdl(k_sq_begin, 1, 32, 0, r, pf.sqrows, (const int*)pf.sqtok, pf.tokens, pf.vstate);
-		if (pen_step) launch_pdl(k_sq_lanes, 1, 32, 0, lanes, pf.sqlanes);
+		if (mask_step) launch_pdl(k_sq_mask_lanes, 1, 32, 0, ml, pf.sqlanes);
+		else if (pen_step) launch_pdl(k_sq_lanes, 1, 32, 0, lanes, pf.sqlanes);
 		PfSampleStep ss = {0, 0, r.n, lmax};
 		if (!gorder.empty()) { // rows with contexts: the groups table, and the GROUPS attention
 			for (int c : gorder) {
@@ -2598,18 +2715,18 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		}
 		with_formats([&](auto f) {
 			pf_run(f, r.n, 0, PF_QUEUE, &ss);
-			if (lp || pen_step) sq_classify(f, r.n, lp ? lp->k : 0, nsampled > 0, pen_step);
+			if (lp || pen_step || mask_step) sq_classify(f, r.n, lp ? lp->k : 0, nsampled > 0, pen_step || mask_step, mask_step);
 			else pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
 		});
 		if (lp) { // the sampler, then every row's target and the merge, whose argmax is the greedy rows' token as above
-			if (nsampled > 0) vf_sample_rows(r.n);
+			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled);
 			launch_pdl(k_sq_tgt, r.n, 32, 0, (const SqRows*)pf.sqrows, (const float2*)pf.part, cdiv(g.cfg.vocab_size, PF_BM), (const float*)pf.vlogits,
 			           g.cfg.vocab_size, (const int*)pf.vsampled, pf.tgt);
 			sq_merge(r.n, lp->k);
 		} else {
-			if (pen_step && nsampled == 0) pf_merge(r.n, true, 0); // pf_score's merge, which sq_classify leaves out
+			if ((pen_step || mask_step) && nsampled == 0) pf_merge(r.n, true, 0); // pf_score's merge, which sq_classify leaves out
 			if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
-			if (nsampled > 0) vf_sample_rows(r.n);
+			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled);
 		}
 		launch_pdl(k_sq_end, 1, 32, 0, (const SqRows*)pf.sqrows, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate, pf.sqtok, pf.sqout, pf.sqst);
 		if (lp)
@@ -2617,7 +2734,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			           pf.sqoid, pf.sqolp);
 		if (pen_step) launch_pdl(k_sq_pen_step, 1, 32, 0, (const int*)pf.sqlanes, (const int*)pf.sqtok, g.cfg.vocab_size, pf.sqpcnt);
 		++nsteps, last_sampled = nsampled > 0 ? r.n : 0;
-		if (n_stop) { // the step's tokens decide which rows stop
+		if (n_stop || mask_step) { // the step's tokens decide which rows stop, and the constrained rows' next states
 			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, r.n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 			sync_stream();
 		}
@@ -2626,13 +2743,15 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		for (int k = 0; k < r.n; ++k) {
 			const int i = live[k];
 			++done[i];
-			if (done[i] < max_new[i] && !(n_stop && is_stop[tok_host[k]])) {
+			if (cur[i] >= 0) cur[i] = aut->next(cur[i], tok_host[k]);
+			if (done[i] < max_new[i] && !(n_stop && is_stop[tok_host[k]]) && !ends(i)) {
 				keep.push_back(i);
 				continue;
 			}
 			out_len[i] = done[i];
 			slots.give(place[i].s, cdiv(len[i] - 1, 8) * 8), slots.give(place[i].t, max_new[i]);
 			if (lane_of[i] >= 0) lanes_free |= 1u << lane_of[i], lane_of[i] = -1;
+			if (aut && aut->out_state) aut->out_state[i] = cur[i];
 		}
 		live.swap(keep);
 	}
@@ -2659,6 +2778,9 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			std::copy(lps.begin() + O[i], lps.begin() + O[i] + out_len[i], lp->logprobs + O[i]);
 			std::copy(tid.begin() + O[i] * k, tid.begin() + (O[i] + out_len[i]) * k, lp->top_ids + O[i] * k);
 			std::copy(tlp.begin() + O[i] * k, tlp.begin() + (O[i] + out_len[i]) * k, lp->top_logprobs + O[i] * k);
+			if (aut && aut->s0(i) >= 0) // the merge's entry past a list's allowed tokens is (-inf, INT_MAX): id -1 there
+				for (size_t e = O[i] * k; e < (O[i] + out_len[i]) * k; ++e)
+					if (lp->top_ids[e] == INT_MAX) lp->top_ids[e] = -1;
 		}
 	}
 	if (last_sampled) pf.vrows = last_sampled;
@@ -2709,6 +2831,24 @@ extern "C" int calm_b200_decode_sample_queue_penalties(struct Transformer* trans
 	return sq_run("decode_sample_queue_penalties", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
 	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
 	              logprobs || k ? &lp : nullptr, &pen);
+}
+
+extern "C" int calm_b200_decode_sample_queue_constrained(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                                         const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                                         const float* minp, const float* presence, const float* frequency, const float* repetition,
+                                                         const int* bias_off, const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias,
+                                                         const int* stop, int n_stop, int max_rows, unsigned long long* rng_states, int* out_tokens,
+                                                         int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
+                                                         float* top_logprobs, int n_states, const uint32_t* allow, const int* next_default,
+                                                         const int* exc_off, const int* exc_tok, const int* exc_next, const int* start, int* out_state) {
+	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
+	const bool none = !ctx_off && !ctx_len;
+	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
+	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
+	SqAutomaton aut{n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state, 0, {}};
+	return sq_run("decode_sample_queue_constrained", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len,
+	              nreq, max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
+	              logprobs || k ? &lp : nullptr, &pen, &aut);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -2885,6 +3025,9 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		// step's lanes, pf.sqlanes, read as addresses into the lanes, are index buffers)
 		nan(pf.sqpcnt, SQ_ROWS * (size_t)c.vocab_size * sizeof(int)), nan(pf.sqpbias, SQ_ROWS * (size_t)c.vocab_size * sizeof(float));
 		nan(pf.sqppar, SQ_ROWS * sizeof(float4)), nan(pf.sqpbval, pf.sqpb_cap * sizeof(float));
+		// and its constrained call's uploaded automaton, which every such call rewrites before a step reads it (a poisoned
+		// word allows every token of its 32)
+		nan(pf.sqallow, pf.sqallow_cap * sizeof(uint32_t));
 	}
 	if (kv_from_pos < c.seq_len) { // the cache is [layer][kv head][seq_len][head_dim]: the tail of every (layer, head) row
 		const size_t slot = (size_t)c.head_dim * (g.kvbits / 8), pitch = c.seq_len * slot, width = (c.seq_len - kv_from_pos) * slot;

@@ -1255,7 +1255,9 @@ struct SampleArgs {
 	float* sprob;
 };
 
-// one chunk of the vocabulary: its survivors, in index order, and their sequential sum
+// one chunk of the vocabulary: its survivors, in index order, and their sequential sum.  MASK: a logit of -inf (a token
+// its row's automaton does not allow) never survives, also where the cut is -inf (minp 0)
+template <bool MASK = false>
 __device__ __forceinline__ void sample_scan(const SampleArgs& a, const unsigned chunk) {
 	__shared__ float red[8];
 	__shared__ int wcount[8];
@@ -1277,6 +1279,7 @@ __device__ __forceinline__ void sample_scan(const SampleArgs& a, const unsigned 
 	for (int k = 0; k < 4; ++k) {
 		float l = base + k < a.vocab ? a.logits[base + k] : -FLT_MAX;
 		bool s = base + k < a.vocab && l >= cutoff;
+		if constexpr (MASK) s = s && l != -INFINITY;
 		p[k] = s ? expf((l - mx) / temp) : -1.f;
 		keep += s;
 	}
@@ -1424,6 +1427,12 @@ __device__ __forceinline__ SampleArgs sample_row(const SampleArgs& a, int r) {
 __global__ void __launch_bounds__(256) k_sample_scan_rows(const SampleArgs a) {
 	pdl_enter();
 	sample_scan(sample_row(a, blockIdx.y), blockIdx.x);
+}
+
+// k_sample_scan_rows where masked tokens (-inf) never survive (calm_b200_decode_sample_queue_constrained)
+__global__ void __launch_bounds__(256) k_sample_scan_rows_masked(const SampleArgs a) {
+	pdl_enter();
+	sample_scan<true>(sample_row(a, blockIdx.y), blockIdx.x);
 }
 
 __global__ void __launch_bounds__(256) k_sample_pick_rows(const SampleArgs a, SampleState* st, int* tokens) {

@@ -26,6 +26,10 @@
 //               each logit of a row whose v.lane[t] is non-negative by the request's processed logit (sq_pen_logit)
 //               before any record is formed, so the argmax records, logit rows, tile maxima, (max, sum) records and top-k
 //               lists all see the processed values.  Other rows are not touched.
+//               MASK (with TOPK and PEN; calm_b200_decode_sample_queue_constrained) then sets to -inf each logit of a row
+//               whose v.mstate[t] is non-negative at every token its automaton state does not allow (v.allow), in the
+//               same pass, so every record sees the masked values.  A tile with no allowed entry gives (m = -FLT_MAX,
+//               sum = 0, gi = INT_MAX), its top-k lists (-inf, INT_MAX).
 #pragma once
 
 #include "prefill.cuh"
@@ -54,6 +58,9 @@ struct VfArgs {
 	const int* pcnt;    // [16][vocab] count of the token among the request's generated tokens, | SQ_PEN_SEEN if in ctx ++ prompt
 	const float* pbias; // [16][vocab] b(v): the request's logit bias, 0 off its list
 	const float4* ppar; // [16] (presence, frequency, repetition, 0)
+	// MASK: row t's automaton state, or -1 for a row left as it is, and the states' bitmasks
+	const int* mstate;       // [VF_TOK] (k_sq_mask_lanes)
+	const uint32_t* allow;   // [n_states][ceil(vocab / 32)] bit v % 32 of word v / 32: token v is allowed
 };
 
 #define SQ_PEN_SEEN (1 << 30) // a count row's mark of a token in the request's ctx ++ prompt; the count is the bits below
@@ -116,12 +123,13 @@ __device__ __forceinline__ void vf_dequant(const uint32_t (&w)[VfFmt<DBITS>::WOR
 	}
 }
 
-template <int MODE, int DBITS, typename KVT, bool TOPK = false, bool PEN = false>
+template <int MODE, int DBITS, typename KVT, bool TOPK = false, bool PEN = false, bool MASK = false>
 __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, const VfArgs v) {
 	constexpr int W = VfFmt<DBITS>::WORDS, U = VfFmt<DBITS>::U;
 	constexpr bool CLS = MODE == PF_CLS_GREEDY || MODE == PF_CLS_SAMPLE;
 	static_assert(CLS || !TOPK, "the top-k lists are a classifier epilogue");
 	static_assert(TOPK || !PEN, "the processed logits come with the top-k epilogue (a.topk may be 0)");
+	static_assert(PEN || !MASK, "the mask comes with the processed logits (every lane may be -1)");
 	__shared__ __align__(16) __half xs[2][VF_TOK][VF_XSTR];
 	__shared__ unsigned last_s;
 	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
@@ -257,6 +265,14 @@ __global__ void __launch_bounds__(VF_THREADS, 2) k_vf_gemm(const PfGemmArgs a, c
 					if (t < a.n_tokens && ln >= 0 && pbase + r < a.vocab) {
 						const size_t o = (size_t)ln * a.vocab + pbase + r;
 						lg[t][r] = sq_pen_logit(lg[t][r], v.pcnt[o], v.pbias[o], v.ppar[ln]);
+					}
+				}
+				if constexpr (MASK) { // each entry by the thread that processed it; pbase is a multiple of 128, so a row's tile is 4 words
+					const int words = (a.vocab + 31) >> 5;
+					for (int e = tid; e < VF_TOK * VF_ROWS; e += VF_THREADS) {
+						const int t = e / VF_ROWS, r = e % VF_ROWS, s = v.mstate[t];
+						if (t < a.n_tokens && s >= 0 && pbase + r < a.vocab && !((v.allow[(size_t)s * words + ((pbase + r) >> 5)] >> (r & 31)) & 1u))
+							lg[t][r] = -INFINITY;
 					}
 				}
 				__syncthreads();

@@ -29,6 +29,7 @@ SYMBOLS = [
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
     "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
     "calm_b200_decode_sample_queue_context", "calm_b200_decode_sample_queue_logprobs", "calm_b200_decode_sample_queue_penalties",
+    "calm_b200_decode_sample_queue_constrained",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -114,6 +115,9 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_queue_penalties.argtypes = (ctx_args[:11] + [_fptr, _fptr, _fptr, _iptr, _iptr, _iptr, _fptr, C.c_int] + ctx_args[11:]
                                                           + [C.c_int, _fptr, _iptr, _fptr])
     L.calm_b200_decode_sample_queue_penalties.restype = C.c_int
+    L.calm_b200_decode_sample_queue_constrained.argtypes = (L.calm_b200_decode_sample_queue_penalties.argtypes
+                                                            + [C.c_int, C.POINTER(C.c_uint32), _iptr, _iptr, _iptr, _iptr, _iptr, _iptr])
+    L.calm_b200_decode_sample_queue_constrained.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -155,6 +159,113 @@ def _check_rng(rng_state):
     """A generator state the C calls can take (a NULL state would abort the process)."""
     if not isinstance(rng_state, (int, np.integer)) or not 0 <= rng_state < 1 << 64:
         raise ValueError(f"rng_state must be an unsigned 64-bit integer, got {rng_state!r}")
+
+
+class TokenAutomaton:
+    """A finite token automaton for DeviceModel.decode_sample_queue_constrained, checked as the C call checks it.
+
+    States are 0 .. n_states-1.  `allow` says which tokens each state allows: a bool array [n_states, vocab], or the C
+    call's own bitmask, uint32 [n_states, ceil(vocab / 32)] with bit v % 32 of word v / 32 for token v.  After an
+    allowed token v, state s moves to exceptions[s][v] when v is a key of that dict (exceptions may be None, and any
+    entry None: no exceptions), otherwise to next_default[s]; -1 there means every allowed token is an exception.  A
+    state that allows no token is final.  Raises ValueError for an automaton the C call would abort on."""
+
+    def __init__(self, vocab: int, allow, next_default, exceptions=None):
+        if not isinstance(vocab, (int, np.integer)) or isinstance(vocab, bool) or vocab < 1:
+            raise ValueError(f"vocab must be a positive integer, got {vocab!r}")
+        self.vocab, self.words = int(vocab), (int(vocab) + 31) // 32
+        a = np.asarray(allow)
+        if a.ndim != 2:
+            raise ValueError("allow must be a 2-D array, one row per state")
+        if a.dtype == np.bool_:
+            if a.shape[1] != self.vocab:
+                raise ValueError(f"a bool allow has one column per token: {a.shape[1]} columns, {self.vocab} tokens")
+            bits = np.zeros((a.shape[0], self.words * 32), np.uint8)
+            bits[:, :self.vocab] = a
+            a = np.packbits(bits.reshape(a.shape[0], self.words, 4, 8), axis=-1, bitorder="little").reshape(a.shape[0], -1).view("<u4")
+        elif a.dtype != np.uint32 or a.shape[1] != self.words:
+            raise ValueError(f"allow must be bool [n_states, {self.vocab}] or uint32 [n_states, {self.words}], got {a.dtype} {a.shape}")
+        self.allow = np.ascontiguousarray(a, np.uint32)
+        self.n_states = n = self.allow.shape[0]
+        if self.vocab % 32 and (self.allow[:, -1] >> np.uint32(self.vocab % 32)).any():
+            raise ValueError(f"allow has a bit set past the {self.vocab}-token vocabulary")
+        nd = np.asarray(next_default)
+        if nd.shape != (n,) or (n and nd.dtype.kind not in "iu"):
+            raise ValueError(f"next_default must hold one integer per state ({n})")
+        if ((nd < -1) | (nd >= n)).any():
+            raise ValueError(f"a default next state is outside [-1, {n})")
+        self.next_default = np.ascontiguousarray(nd, np.int32)
+        exceptions = [None] * n if exceptions is None else list(exceptions)
+        if len(exceptions) != n:
+            raise ValueError(f"exceptions must hold one dict (or None) per state ({n}), got {len(exceptions)}")
+        off, tok, nxt = [0], [], []
+        self.allowed_count = np.array([int(np.unpackbits(r.view(np.uint8)).sum()) for r in self.allow], np.int64)
+        for s, d in enumerate(exceptions):
+            d = {} if d is None else d
+            if not isinstance(d, dict):
+                raise ValueError(f"exceptions[{s}] must be a dict of token: next state, or None")
+            for v in sorted(d):
+                t = d[v]
+                if not isinstance(v, (int, np.integer)) or isinstance(v, bool) or not 0 <= v < self.vocab or not self._bit(s, v):
+                    raise ValueError(f"state {s}'s exception token {v!r} is not a token it allows")
+                if not isinstance(t, (int, np.integer)) or isinstance(t, bool) or not 0 <= t < n:
+                    raise ValueError(f"state {s}'s exception for token {v} goes to {t!r}, outside [0, {n})")
+                tok.append(int(v)), nxt.append(int(t))
+            off.append(len(tok))
+            if self.next_default[s] == -1 and self.allowed_count[s] > len(d):
+                raise ValueError(f"state {s} allows a token outside its exceptions and has no default next state")
+        self.exc_off, self.exc_tok, self.exc_next = (np.asarray(x, np.int32) for x in (off, tok, nxt))
+        self.final = self.allowed_count == 0
+
+    def _bit(self, s, v):
+        return bool((int(self.allow[s, v >> 5]) >> (v & 31)) & 1)
+
+    def allowed(self, s: int) -> np.ndarray:
+        """The ids state s allows, ascending."""
+        bits = np.unpackbits(self.allow[s].view(np.uint8), bitorder="little")[:self.vocab]
+        return np.flatnonzero(bits)
+
+    def next(self, s: int, token: int) -> int:
+        """The state after `token` in state s, or ValueError if s does not allow it."""
+        if not 0 <= s < self.n_states or not 0 <= token < self.vocab or not self._bit(s, token):
+            raise ValueError(f"state {s} does not allow token {token}")
+        lo, hi = self.exc_off[s], self.exc_off[s + 1]
+        j = lo + int(np.searchsorted(self.exc_tok[lo:hi], token))
+        return int(self.exc_next[j]) if j < hi and self.exc_tok[j] == token else int(self.next_default[s])
+
+    @classmethod
+    def choices(cls, seqs, vocab: int) -> "TokenAutomaton":
+        """guided_choice: a trie over the token sequences `seqs`, from state 0, whose every leaf is the one final state,
+        so that a constrained request emits exactly one of them.  ValueError for an empty list, an empty sequence, an id
+        outside [0, vocab) or a sequence that is a proper prefix of another (it could not both end and go on)."""
+        seqs = [[int(t) for t in q] for q in seqs]
+        if not seqs or any(len(q) == 0 for q in seqs):
+            raise ValueError("choices takes at least one sequence, none of them empty")
+        if any(not 0 <= t < vocab for q in seqs for t in q):
+            raise ValueError(f"a choice has a token outside [0, {vocab})")
+        END = -1
+        nodes = [{}]  # node -> {token: child node, or END}
+        for q in seqs:
+            u = 0
+            for j, t in enumerate(q):
+                last = j == len(q) - 1
+                c = nodes[u].get(t)
+                if (c == END) != last and c is not None:
+                    raise ValueError(f"choice {q} and another: one is a proper prefix of the other")
+                if last:
+                    nodes[u][t] = END
+                else:
+                    if c is None:
+                        c = nodes[u][t] = len(nodes)
+                        nodes.append({})
+                    u = c
+        fin = len(nodes)
+        allow = np.zeros((fin + 1, vocab), bool)
+        exc = [None] * (fin + 1)
+        for u, ch in enumerate(nodes):
+            allow[u, list(ch)] = True
+            exc[u] = {t: (fin if c == END else c) for t, c in ch.items()}
+        return cls(vocab, allow, np.full(fin + 1, -1, np.int32), exc)
 
 
 class DeviceModel:
@@ -515,12 +626,13 @@ class DeviceModel:
             raise ValueError(f"{who}: the sum of max_new does not fit an int")
         return prompts, max_new, temperature, minp, stop, states
 
-    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None, pen=None):
+    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None, pen=None, aut=None):
         """Run a queue call over the laid-out tokens; ctx is (ctx_off, ctx_len), either of them None for a NULL array, or
         None for a call without those arguments.  Returns (tokens, states, served, steps, prompt_rows), and with `k` (the
         log-probability call) also each request's float32[out_len] log-probabilities and, for k > 0, its top ids and
         log-probabilities [out_len, k] (None for k == 0).  `pen` (the penalty call) is the list of its arguments after
-        minp; without `k` that call gets k 0 and NULL outputs."""
+        minp; without `k` that call gets k 0 and NULL outputs.  `aut` (the constrained call) is the list of its automaton
+        arguments before out_state; the return value then ends with each request's final state."""
         nreq = len(len_)
         mn = np.ascontiguousarray(max_new, np.int32)
         st = np.ascontiguousarray(stop, np.int32)
@@ -545,14 +657,19 @@ class DeviceModel:
             args += [k, lp.ctypes.data_as(fp), ids.ctypes.data_as(ip) if k else None, tlp.ctypes.data_as(fp) if k else None]
         elif pen is not None:
             args += [0, None, None, None]
+        out_state = np.full(max(nreq, 1), -2, np.int32)
+        if aut is not None:
+            args += aut + [out_state.ctypes.data_as(ip)]
         served = fn(*args)
         o = np.concatenate([[0], np.cumsum(mn)]).astype(np.int64)
         toks = [out[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)]
         res = (toks, [int(rng[i]) for i in range(nreq)], served, int(steps.value), int(rows.value))
-        if k is None:
-            return res
-        cut = lambda a: [a[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)] if a is not None else None  # noqa: E731
-        return res + (cut(lp), cut(ids), cut(tlp))
+        if k is not None:
+            cut = lambda a: [a[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)] if a is not None else None  # noqa: E731
+            res += (cut(lp), cut(ids), cut(tlp))
+        if aut is not None:
+            res += ([int(x) for x in out_state[:nreq]],)
+        return res
 
     def _context_layout(self, who, contexts, ctx_of, prompts):
         """The context calls' laid-out tokens and (ctx_off, ctx_len, off, len) for contexts / ctx_of / prompts (each
@@ -658,9 +775,16 @@ class DeviceModel:
         if k is not None:
             self._check_queue_k(k)
         prompts, max_new, temperature, minp, stop, states = self._queue_args(who, prompts, max_new, temperature, minp, stop, max_rows, rng_states)
-        nreq = len(prompts)
-        fp, ip = C.POINTER(C.c_float), C.POINTER(C.c_int)
         keep = []  # the arrays the C call reads
+        pen = self._penalty_args(who, len(prompts), presence, frequency, repetition, logit_bias, keep)
+        tokens, ctx, off, len_ = self._optional_context_layout(who, contexts, ctx_of, prompts)
+        return self._queue_call(self.lib.calm_b200_decode_sample_queue_penalties, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows,
+                                states, k=None if k is None else int(k), pen=pen)
+
+    def _penalty_args(self, who, nreq, presence, frequency, repetition, logit_bias, keep):
+        """The penalty calls' arguments after minp (presence .. n_bias), or ValueError wherever the C call would abort;
+        the arrays they point to go to `keep`."""
+        fp, ip = C.POINTER(C.c_float), C.POINTER(C.c_int)
 
         def per_request(name, xs, lo, hi):
             if xs is None:
@@ -703,9 +827,50 @@ class DeviceModel:
             keep += [b_len, b_off, b_ids, b_val]
             pen += [b_off.ctypes.data_as(ip), b_len.ctypes.data_as(ip), b_ids.ctypes.data_as(ip) if len(ids) else None,
                     b_val.ctypes.data_as(fp) if len(ids) else None, len(ids)]
+        return pen
+
+    def decode_sample_queue_constrained(self, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states,
+                                        automaton=None, start=None, presence=None, frequency=None, repetition=None, logit_bias=None, k=None):
+        """calm_b200_decode_sample_queue_constrained: decode_sample_queue_penalties where request i with start[i] >= 0 is
+        constrained to `automaton` (a TokenAutomaton over this model's vocabulary) from state start[i]: at each step only
+        the tokens its state allows can be chosen, and it retires after a token that leads to a final state.  start None
+        (or every entry -1) constrains no request.  Returns decode_sample_queue_penalties' tuple followed by each request's
+        state after its last token (-1 for an unconstrained request).  Raises ValueError where the C call would abort."""
+        who = "decode_sample_queue_constrained"
+        if k is not None:
+            self._check_queue_k(k)
+        prompts, max_new, temperature, minp, stop, states = self._queue_args(who, prompts, max_new, temperature, minp, stop, max_rows, rng_states)
+        nreq = len(prompts)
+        if automaton is not None:
+            if not isinstance(automaton, TokenAutomaton):
+                raise ValueError(f"{who}: automaton must be a TokenAutomaton or None")
+            if automaton.vocab != self.vocab:
+                raise ValueError(f"{who}: the automaton's vocabulary has {automaton.vocab} tokens, the model's {self.vocab}")
+        st = None
+        if start is not None:
+            st = list(start)
+            if len(st) != nreq:
+                raise ValueError(f"{who} takes one start state per prompt: {nreq} prompts, {len(st)} values")
+            n_states = automaton.n_states if automaton is not None else 0
+            for i, s0 in enumerate(st):
+                if not isinstance(s0, (int, np.integer)) or isinstance(s0, bool) or not -1 <= s0 < n_states:
+                    raise ValueError(f"start[{i}] must be -1 or a state in [0, {n_states}), got {s0!r}")
+                if s0 >= 0 and max_new[i] > 0 and automaton.final[s0]:
+                    raise ValueError(f"request {i} starts in final state {s0}")
+            st = np.ascontiguousarray(st, np.int32)
+        keep = [st]
+        pen = self._penalty_args(who, nreq, presence, frequency, repetition, logit_bias, keep)
+        ip = C.POINTER(C.c_int)
+        if automaton is None:
+            aut = [0, None, None, None, None, None]
+        else:
+            a = automaton
+            aut = [a.n_states, a.allow.ctypes.data_as(C.POINTER(C.c_uint32)), a.next_default.ctypes.data_as(ip), a.exc_off.ctypes.data_as(ip),
+                   a.exc_tok.ctypes.data_as(ip), a.exc_next.ctypes.data_as(ip)]
+        aut.append(None if st is None else st.ctypes.data_as(ip))
         tokens, ctx, off, len_ = self._optional_context_layout(who, contexts, ctx_of, prompts)
-        return self._queue_call(self.lib.calm_b200_decode_sample_queue_penalties, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows,
-                                states, k=None if k is None else int(k), pen=pen)
+        return self._queue_call(self.lib.calm_b200_decode_sample_queue_constrained, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows,
+                                states, k=None if k is None else int(k), pen=pen, aut=aut)
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""

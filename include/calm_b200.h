@@ -424,6 +424,58 @@ int calm_b200_decode_sample_queue_penalties(struct Transformer* transformer, con
                                             int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps,
                                             int* prompt_rows, int k, float* logprobs, int* top_ids, float* top_logprobs);
 
+/* calm_b200_decode_sample_queue_penalties where each request may be constrained to a finite token automaton: structured
+ * output (JSON mode, JSON schemas, regular expressions, guided choices; INTEGRATION.md "Structured output").
+ * The automaton.  One for the whole call, with states 0 .. n_states-1 and W = ceil(vocab_size / 32) words per state:
+ * allow[s*W + v/32] bit v%32 set means token v is allowed in state s (bits at or past vocab_size are 0).  After an
+ * allowed token v the next state is exc_next[e] when exc_tok[e] == v for some e in [exc_off[s], exc_off[s+1]) (exc_tok
+ * strictly ascending within a state, every listed token allowed in s), otherwise next_default[s].  A state with no
+ * allowed token is final.
+ * Start states.  start[i] == -1: request i is unconstrained; start == NULL: no request is (the call is then
+ * calm_b200_decode_sample_queue_penalties exactly).  The automaton arrays are read only when some start[i] >= 0.
+ * Processing.  At request i's step j in state s, with l2 the _penalties call's processed logit:
+ *     l3(v) = l2(v) if v is allowed in s, otherwise -inf
+ * and l3 replaces l2 for everything the step does: a greedy request's token is the first maximum of l3; logprobs is
+ * l3[tok] - M - ln S over the allowed tokens, a masked token's log-probability -inf; when fewer than k tokens are
+ * allowed, top_ids / top_logprobs hold -1 / -inf at the ranks past them.
+ * Sampling.  A token whose l3 is -inf never survives the min-p cut (at minp == 0 the reference's
+ * logit >= max + log(0) * T would keep it, and its rounding fallback could land on it).  With at most 2048 survivors the
+ * drawn token is exactly the reference's sample() over the allowed tokens alone, in ascending id order; beyond 2048 it is
+ * the device sampler's chunk-by-chunk rule over the full row with the masked entries left out.  One coin is drawn per
+ * step, as without a constraint, also for a forced token (a state with one allowed token).
+ * Retirement.  A request retires after the step that gives its max_new-th token, a stop token, or a token whose next
+ * state is final; that token is emitted and counted in out_len.  out_state[i] (out_state may be NULL) receives the state
+ * after the request's last token (start[i] when max_new[i] == 0), or -1 for an unconstrained request: a final state
+ * tells a completed structure from one cut off by max_new.
+ * Invariants.  An unconstrained request gets exactly the bits of the _penalties call, whatever shares its steps; with
+ * start NULL or all -1 the call launches exactly what _penalties launches.  Request i's outputs do not depend on the
+ * other requests, max_rows, its slots, seq_len or an earlier call.  The host follows each constrained request's state
+ * from the step's tokens, which it reads back after each step with a constrained row, as it does with a stop list.
+ * Aborts, before any device work: where calm_b200_decode_sample_queue_penalties aborts, and when n_states < 0, an
+ * automaton array is NULL while some start[i] >= 0, a start lies outside [-1, n_states), allow has a bit set past the
+ * vocabulary, exc_off[0] != 0 or exc_off decreases, an exception token is not strictly ascending or not allowed in its
+ * state, an exception's next state lies outside [0, n_states), next_default[s] lies outside [-1, n_states), a state
+ * allows a token outside its exception list while next_default[s] == -1, or a request with max_new > 0 starts in a
+ * final state.
+ * Fallback (return 0; as the _penalties call).  A constrained request decodes on the decode path and takes each step's
+ * device logits; the host applies l2, then the mask, takes the first allowed maximum (greedy) or runs the masked sampler
+ * kernels on the processed row with the request's state, and computes log-probabilities in double as the _logprobs
+ * call's fallback does.
+ * Memory.  A call with a constrained request uploads the bitmasks once, 4 W bytes per state (16 KB at a 128256-token
+ * vocabulary), regrown by a larger call; the exception lists and default next states stay on the host.
+ * Cost per call.  Nothing is kept between calls: each call with a constrained request checks the whole automaton on the
+ * host (every bitmask word read and popcounted, every exception checked: n_states x W words, 16 MB for 1000 states at
+ * 128256 tokens) and uploads every bitmask, before its first step.  A host that reuses a large automaton across many
+ * short calls pays both every time; that cost has not been measured. */
+int calm_b200_decode_sample_queue_constrained(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                              const int* off, const int* len, int nreq, const int* max_new, const float* temperature, const float* minp,
+                                              const float* presence, const float* frequency, const float* repetition, const int* bias_off,
+                                              const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias, const int* stop, int n_stop,
+                                              int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps,
+                                              int* prompt_rows, int k, float* logprobs, int* top_ids, float* top_logprobs, int n_states,
+                                              const uint32_t* allow, const int* next_default, const int* exc_off, const int* exc_tok,
+                                              const int* exc_next, const int* start, int* out_state);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
