@@ -1131,13 +1131,37 @@ static unsigned long long xorshift_step(unsigned long long s) {
 	return s;
 }
 
+// k_sample_trunc_rows over grid (TRUNC_CTAS, rows) on `st`, each CTA staging its ceil(vocab / TRUNC_CTAS) logits
+static void trunc_launch(dim3 grid, cudaStream_t st, const SampleArgs& sa, const TruncRows& tr, int vocab) {
+	const size_t smem = (size_t)(cdiv(vocab, TRUNC_CTAS) + 8) * sizeof(float);
+	static size_t opted = 0;
+	if (smem > opted) {
+		CUDA_CHECK(cudaFuncSetAttribute(k_sample_trunc_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+		opted = smem;
+	}
+	if (st == g.stream) {
+		launch_pdl(k_sample_trunc_rows, grid, 256, smem, sa, tr);
+		return;
+	}
+	k_sample_trunc_rows<<<grid, 256, smem, st>>>(sa, tr);
+}
+
+// abort unless top_k >= 0 and top_p is finite in (0, 1] (request i's, in `who`)
+static void trunc_check(const char* who, int i, int top_k, float top_p) {
+	if (top_k < 0) CALM_FATAL("%s: request %d's top_k %d is negative", who, i, top_k);
+	if (!(top_p > 0.0f && top_p <= 1.0f)) CALM_FATAL("%s: request %d's top_p %g is not in (0, 1]", who, i, (double)top_p);
+}
+
 // The device sampler on its own: logits given by the host, any vocabulary size; returns the token and advances *rng_state.
 // Same kernels as the decode loop (k_sample_scan + k_sample_pick); device_us (optional) receives their mean duration.
 // `masked` (the fallback of calm_b200_decode_sample_queue_constrained): k_sample_scan_rows_masked on the one row instead
-// of k_sample_scan, so that a -inf logit never survives.
-static int sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us, bool masked) {
+// of k_sample_scan, so that a -inf logit never survives.  top_k > 0 or top_p < 1 (calm_b200_sample_logits_truncated):
+// k_sample_trunc_rows on the row first, then the masked scan; out_row (may be NULL) receives the row it left.
+static int sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us, bool masked,
+                         int top_k = 0, float top_p = 1.0f, float* out_row = nullptr) {
 	select_device();
 	if (vocab <= 0) CALM_FATAL("sample_logits: empty vocabulary");
+	if (out_row) std::copy(logits_host, logits_host + vocab, out_row);
 	if (temperature == 0.0f || minp >= 1.0f) { // greedy, first maximum (sampler.c:34-42); the generator is not touched
 		int best = 0;
 		for (int i = 1; i < vocab; ++i)
@@ -1145,6 +1169,9 @@ static int sample_logits(const float* logits_host, int vocab, float temperature,
 		if (device_us) *device_us = 0.f;
 		return best;
 	}
+	const bool trunc = top_k > 0 || top_p < 1.0f;
+	if (trunc && vocab > TRUNC_VOCAB_MAX) CALM_FATAL("sample_logits: truncation serves vocabularies up to %d tokens, not %d", TRUNC_VOCAB_MAX, vocab);
+	masked = masked || trunc;
 	const int nchunks = cdiv(vocab, SAMPLE_CHUNK);
 	cudaStream_t st;
 	CUDA_CHECK(cudaStreamCreate(&st));
@@ -1170,8 +1197,15 @@ static int sample_logits(const float* logits_host, int vocab, float temperature,
 	float ms = 0;
 	for (int r = 0; r < reps; ++r) { // every repetition restarts from the caller's generator state: same draw
 		CUDA_CHECK(cudaMemcpyAsync(sst, &hs, sizeof(hs), cudaMemcpyHostToDevice, st));
+		if (trunc) CUDA_CHECK(cudaMemcpyAsync(logits, logits_host, (size_t)vocab * sizeof(float), cudaMemcpyHostToDevice, st)); // (truncated in place)
 		k_chunk_max<<<nchunks, 256, 0, st>>>(logits, vocab, cmax);
 		CUDA_CHECK(cudaEventRecord(e0, st));
+		if (trunc) {
+			TruncRows tr = {};
+			tr.top_k[0] = top_k, tr.top_p[0] = top_p;
+			trunc_launch(dim3(TRUNC_CTAS, 1), st, sa, tr, vocab);
+			g_launches += 1;
+		}
 		if (masked) k_sample_scan_rows_masked<<<dim3(nchunks, 1), 256, 0, st>>>(sa);
 		else k_sample_scan<<<nchunks, 256, 0, st>>>(sa);
 		k_sample_pick<<<1, 256, 0, st>>>(sa, sst, tp, nullptr, tok, 0);
@@ -1185,6 +1219,7 @@ static int sample_logits(const float* logits_host, int vocab, float temperature,
 	int htok = 0;
 	CUDA_CHECK(cudaMemcpy(&htok, tok, sizeof(int), cudaMemcpyDeviceToHost));
 	CUDA_CHECK(cudaMemcpy(&hs, sst, sizeof(hs), cudaMemcpyDeviceToHost));
+	if (trunc && out_row) CUDA_CHECK(cudaMemcpy(out_row, logits, (size_t)vocab * sizeof(float), cudaMemcpyDeviceToHost));
 	*rng_state = hs.rng;
 	cudaFree(logits), cudaFree(cmax), cudaFree(sst), cudaFree(count), cudaFree(csum), cudaFree(sidx), cudaFree(sprob), cudaFree(tok), cudaFree(tp);
 	cudaEventDestroy(e0), cudaEventDestroy(e1), cudaStreamDestroy(st);
@@ -1193,6 +1228,12 @@ static int sample_logits(const float* logits_host, int vocab, float temperature,
 
 extern "C" int calm_b200_sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us) {
 	return sample_logits(logits_host, vocab, temperature, minp, rng_state, device_us, false);
+}
+
+extern "C" int calm_b200_sample_logits_truncated(const float* logits_host, int vocab, float temperature, float minp, int top_k, float top_p,
+                                                 unsigned long long* rng_state, float* out_row, float* device_us) {
+	trunc_check("sample_logits_truncated", 0, top_k, top_p);
+	return sample_logits(logits_host, vocab, temperature, minp, rng_state, device_us, false, top_k, top_p, out_row);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1855,11 +1896,14 @@ static void vf_sample_reserve() {
 // The n rows of the last PF_CLS_SAMPLE classifier through the decode's sampler, side by side: row i is k_sample_scan +
 // k_sample_pick on its own lists and its own SampleState pf.vstate[i] (k_sample_scan_rows / k_sample_pick_rows), and its
 // token goes to out[i] (default pf.vsampled[i]).  `masked`: k_sample_scan_rows_masked, where -inf never survives.
-static void vf_sample_rows(int n, int* out = nullptr, bool masked = false) {
+// `trunc` (calm_b200_decode_sample_queue_truncated): its ntrunc rows first go through k_sample_trunc_rows, which writes
+// -inf over their dropped entries, and the scan is the masked one.
+static void vf_sample_rows(int n, int* out = nullptr, bool masked = false, const TruncRows* trunc = nullptr, int ntrunc = 0) {
 	const int vocab = g.cfg.vocab_size, nvt = cdiv(vocab, PF_BM), nch = g.sample_chunks;
 	SampleArgs sa;
 	sa.logits = pf.vlogits, sa.cand_val = pf.vtmax, sa.ncand = nvt, sa.vocab = vocab, sa.nchunks = nch;
 	sa.st = pf.vstate, sa.count = pf.vcount, sa.csum = pf.vcsum, sa.sidx = pf.vsidx, sa.sprob = pf.vsprob;
+	if (trunc) trunc_launch(dim3(TRUNC_CTAS, ntrunc), g.stream, sa, *trunc, vocab), masked = true;
 	if (masked) launch_pdl(k_sample_scan_rows_masked, dim3(nch, n), 256, 0, sa);
 	else launch_pdl(k_sample_scan_rows, dim3(nch, n), 256, 0, sa);
 	launch_pdl(k_sample_pick_rows, n, 256, 0, sa, pf.vstate, out ? out : pf.vsampled);
@@ -2295,6 +2339,14 @@ static void sq_merge(int n, int k) {
 
 // The logit processing of calm_b200_decode_sample_queue_penalties (include/calm_b200.h): presence / frequency /
 // repetition may each be NULL (0, 0, 1), bias_off / bias_len both NULL when n_bias == 0
+// calm_b200_decode_sample_queue_truncated's per-request top_k / top_p (either array may be NULL: 0 / 1 for every request)
+struct SqTrunc {
+	const int* top_k;
+	const float* top_p;
+	int k(int i) const { return top_k ? top_k[i] : 0; }
+	float p(int i) const { return top_p ? top_p[i] : 1.0f; }
+};
+
 struct SqPenalties {
 	const float* presence;
 	const float* frequency;
@@ -2425,7 +2477,7 @@ static void sq_check_automaton(const char* who, SqAutomaton& a, int nreq, const 
 static int sq_run(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off,
                   const int* len, int nreq, const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
                   int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows,
-                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr, SqAutomaton* aut = nullptr) {
+                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr, SqAutomaton* aut = nullptr, const SqTrunc* tr = nullptr) {
 	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
 	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, max_rows, CALM_B200_SAMPLE_N_MAX);
 	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, n_stop);
@@ -2472,6 +2524,14 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		}
 	}
 	if (aut) sq_check_automaton(who, *aut, nreq, max_new, g.cfg.vocab_size);
+	auto truncated = [&](int i) { // a sampled request with top-k or top-p (sample() is greedy at T 0 or minp >= 1)
+		return tr && !(temperature[i] == 0.0f || minp[i] >= 1.0f) && (tr->k(i) > 0 || tr->p(i) < 1.0f);
+	};
+	for (int i = 0; tr && i < nreq; ++i) {
+		trunc_check(who, i, tr->k(i), tr->p(i));
+		if (max_new[i] > 0 && truncated(i) && g.cfg.vocab_size > TRUNC_VOCAB_MAX)
+			CALM_FATAL("%s: request %d is truncated, and truncation serves vocabularies up to %d tokens, not %d", who, i, TRUNC_VOCAB_MAX, g.cfg.vocab_size);
+	}
 	check_tokens(tokens, n);
 	check_tokens(stop, n_stop);
 	if (steps) *steps = 0;
@@ -2503,8 +2563,8 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			const int L = (int)p.size() - 1;
 			int tok = p[L], k = 0;
 			if (max_new[i] > 0) forward_prefill_cuda(transformer, p.data(), L, 0);
-			const bool processed = pen && !pen->neutral(i), masked = cur[i] >= 0;
-			std::vector<float> logits(lp || processed || masked ? g.cfg.vocab_size : 0);
+			const bool processed = pen && !pen->neutral(i), masked = cur[i] >= 0, cut = truncated(i);
+			std::vector<float> logits(lp || processed || masked || cut ? g.cfg.vocab_size : 0);
 			std::vector<int> cnt(processed ? g.cfg.vocab_size : 0);
 			std::vector<float> bias(processed ? g.cfg.vocab_size : 0);
 			std::vector<char> seen(processed ? g.cfg.vocab_size : 0);
@@ -2513,7 +2573,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 				for (int e = 0; e < pen->nb(i); ++e) bias[pen->bias_ids[pen->bias_off[i] + e]] = pen->bias_val[pen->bias_off[i] + e];
 			}
 			while (k < max_new[i]) {
-				if (processed || masked) { // the decode path's device logits (its argmax discarded), processed, masked and sampled on the host
+				if (processed || masked || cut) { // the decode path's device logits (its argmax discarded), processed, masked and sampled on the host
 					unsigned long long unused = 1;
 					calm_b200_forward_sample(transformer, tok, L + k, 0.0f, 0.0f, &unused);
 					calm_b200_read_device_logits(logits.data());
@@ -2521,8 +2581,10 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 						logits[v] = sq_pen_logit_host(logits[v], cnt[v], seen[v] || cnt[v] > 0, bias[v], pen->p(i), pen->f(i), pen->r(i));
 					for (int v = 0; masked && v < g.cfg.vocab_size; ++v)
 						if (!aut->allowed(cur[i], v)) logits[v] = -INFINITY;
-					// (greedy: the first maximum; sampled: through k_sample_scan_rows_masked where the row is masked)
-					tok = sample_logits(logits.data(), g.cfg.vocab_size, temperature[i], minp[i], &rng_states[i], nullptr, masked);
+					// (greedy: the first maximum; sampled: through k_sample_scan_rows_masked where the row is masked, after
+					// k_sample_trunc_rows where it is truncated)
+					tok = sample_logits(logits.data(), g.cfg.vocab_size, temperature[i], minp[i], &rng_states[i], nullptr, masked, cut ? tr->k(i) : 0,
+					                    cut ? tr->p(i) : 1.0f);
 					if (processed) ++cnt[tok];
 					if (lp) {
 						const size_t o = O[i] + k;
@@ -2673,6 +2735,8 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		bool pen_step = false;     // a row of the step is a non-neutral request's
 		bool mask_step = false;    // a row of the step is a constrained request's
 		bool mask_sampled = false; // .. that samples
+		TruncRows trows = {};      // the step's truncated rows
+		int ntrunc = 0;
 		r.n = (int)live.size();
 		int nsampled = 0, lmax = 0, nsuf = 0;
 		std::map<int, std::vector<int>> groups; // rows by their context's first slot
@@ -2688,6 +2752,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			r.out[k] = (int)(O[i] + j), r.req[k] = i, r.greedy[k] = gr;
 			lanes.lane[k] = lane_of[i], pen_step = pen_step || lane_of[i] >= 0;
 			ml.lane[k] = lane_of[i], ml.state[k] = cur[i], mask_step = mask_step || cur[i] >= 0, mask_sampled = mask_sampled || (cur[i] >= 0 && !gr);
+			if (truncated(i)) trows.row[ntrunc] = k, trows.top_k[ntrunc] = tr->k(i), trows.top_p[ntrunc++] = tr->p(i);
 			nsampled += !gr, lmax = std::max(lmax, q.L + j), row_of[i] = k;
 			grp.ctx[k] = make_int2(q.c, q.nc);
 			nsuf = std::max(nsuf, cdiv(q.L + j + 1, SN_CHUNK) - q.nc / SN_CHUNK);
@@ -2719,14 +2784,14 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			else pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
 		});
 		if (lp) { // the sampler, then every row's target and the merge, whose argmax is the greedy rows' token as above
-			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled);
+			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled, ntrunc ? &trows : nullptr, ntrunc);
 			launch_pdl(k_sq_tgt, r.n, 32, 0, (const SqRows*)pf.sqrows, (const float2*)pf.part, cdiv(g.cfg.vocab_size, PF_BM), (const float*)pf.vlogits,
 			           g.cfg.vocab_size, (const int*)pf.vsampled, pf.tgt);
 			sq_merge(r.n, lp->k);
 		} else {
 			if ((pen_step || mask_step) && nsampled == 0) pf_merge(r.n, true, 0); // pf_score's merge, which sq_classify leaves out
 			if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
-			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled);
+			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled, ntrunc ? &trows : nullptr, ntrunc);
 		}
 		launch_pdl(k_sq_end, 1, 32, 0, (const SqRows*)pf.sqrows, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate, pf.sqtok, pf.sqout, pf.sqst);
 		if (lp)
@@ -2849,6 +2914,26 @@ extern "C" int calm_b200_decode_sample_queue_constrained(struct Transformer* tra
 	return sq_run("decode_sample_queue_constrained", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len,
 	              nreq, max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
 	              logprobs || k ? &lp : nullptr, &pen, &aut);
+}
+
+extern "C" int calm_b200_decode_sample_queue_truncated(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                                       const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                                       const float* minp, const float* presence, const float* frequency, const float* repetition,
+                                                       const int* bias_off, const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias,
+                                                       const int* stop, int n_stop, int max_rows, unsigned long long* rng_states, int* out_tokens,
+                                                       int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
+                                                       float* top_logprobs, int n_states, const uint32_t* allow, const int* next_default,
+                                                       const int* exc_off, const int* exc_tok, const int* exc_next, const int* start, int* out_state,
+                                                       const int* top_k, const float* top_p) {
+	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
+	const bool none = !ctx_off && !ctx_len;
+	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
+	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
+	SqAutomaton aut{n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state, 0, {}};
+	const SqTrunc tr{top_k, top_p};
+	return sq_run("decode_sample_queue_truncated", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len,
+	              nreq, max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
+	              logprobs || k ? &lp : nullptr, &pen, &aut, &tr);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests

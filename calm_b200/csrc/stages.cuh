@@ -11,6 +11,8 @@
 
 #include "common.cuh"
 
+#include <cooperative_groups.h>
+
 #define CALM_MAX_ACTIVE 8 // experts evaluated per token (Mixtral: 2)
 
 struct MoeSel { // router decision of the current layer, written by k_ffn_up, read by k_matres
@@ -1439,6 +1441,259 @@ __global__ void __launch_bounds__(256) k_sample_pick_rows(const SampleArgs a, Sa
 	pdl_enter();
 	const int r = blockIdx.x;
 	sample_pick(sample_row(a, r), st + r, nullptr, nullptr, tokens + r, 0);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Top-k / top-p truncation of sampled rows (calm_b200_decode_sample_queue_truncated; the rule is include/calm_b200.h's).
+// One cluster of TRUNC_CTAS CTAs per row: CTA c stages ids [c S, (c + 1) S), S = ceil(vocab / TRUNC_CTAS), into shared
+// memory with one bulk copy, then radix-selects over the order-preserving key of each allowed logit, 8 bits a round.  A
+// round's histograms (a count and a 2^40-scaled mass per bucket) are built per warp, summed per CTA, and every CTA sums
+// all TRUNC_CTAS of them through distributed shared memory, so every CTA takes the same decision with integer sums.
+// Finally each CTA writes -inf over its dropped entries of the row, in place: what the masked scan then leaves out.
+
+#define TRUNC_CTAS 8
+#define TRUNC_VOCAB_MAX (TRUNC_CTAS * 32768) // 128 KB of staged logits per CTA (the sampler's exact-table limit too)
+
+// a step's truncated sampled rows: row[i] with its request's top_k[i] (0: off) and top_p[i] (1: off), by value
+struct TruncRows {
+	int row[16];
+	int top_k[16];
+	float top_p[16];
+};
+
+__device__ __forceinline__ uint32_t trunc_key(float l) { // larger logit, larger key
+	const uint32_t u = __float_as_uint(l);
+	return (u & 0x80000000u) ? ~u : u | 0x80000000u;
+}
+__device__ __forceinline__ float trunc_logit(uint32_t k) {
+	return __uint_as_float((k & 0x80000000u) ? k & 0x7fffffffu : ~k);
+}
+// m(v) = floor(expf((l - M) / T) * 2^40): the sampler's survivor weight, exactly scaled to an integer
+__device__ __forceinline__ unsigned long long trunc_mass(float l, float mx, float temp) {
+	return (unsigned long long)(expf((l - mx) / temp) * 1099511627776.0f);
+}
+// ceil(z * p) for 0 < p <= 1 taken exactly, p = mant 2^e
+__device__ __forceinline__ unsigned long long trunc_target(unsigned long long z, float p) {
+	const uint32_t u = __float_as_uint(p);
+	const int be = (u >> 23) & 0xff;
+	const unsigned long long mant = be ? (u & 0x7fffffu) | 0x800000u : u & 0x7fffffu;
+	const int sh = (be ? be : 1) - 150; // p = mant 2^sh, sh <= -23
+	const unsigned __int128 prod = (unsigned __int128)z * mant;
+	if (-sh >= 128) return prod ? 1 : 0;
+	const unsigned __int128 q = prod >> -sh;
+	return (unsigned long long)q + ((q << -sh) != prod ? 1 : 0);
+}
+
+struct TruncHist {
+	unsigned cnt[256];
+	unsigned long long mass[256];
+};
+
+__global__ void __cluster_dims__(TRUNC_CTAS, 1, 1) __launch_bounds__(256) k_sample_trunc_rows(const SampleArgs a0, const TruncRows t) {
+	namespace cg = cooperative_groups;
+	extern __shared__ __align__(16) float seg_raw[]; // [S + 8]: the segment from seg_raw[4 - h] on
+	__shared__ TruncHist wh[8];                      // per warp
+	__shared__ TruncHist ch[2];                      // the CTA's, ping-pong between rounds (read by the whole cluster)
+	__shared__ unsigned long long cz[2];             // the CTA's part of a cluster sum
+	__shared__ unsigned ctie[2];
+	__shared__ __align__(8) uint64_t bar;
+	__shared__ uint32_t sel_key;
+	__shared__ unsigned sel_rem;
+	__shared__ unsigned long long sel_above;
+	__shared__ unsigned sel_group;
+	__shared__ unsigned wscan[8];
+	pdl_enter();
+	cg::cluster_group cluster = cg::this_cluster();
+	const int c = (int)cluster.block_rank(), tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int row = t.row[blockIdx.y], K = t.top_k[blockIdx.y];
+	const float P = t.top_p[blockIdx.y];
+	const SampleArgs a = sample_row(a0, row);
+	float* logits = const_cast<float*>(a.logits); // the step's own row of pf.vlogits, truncated in place
+	const int S = (a.vocab + TRUNC_CTAS - 1) / TRUNC_CTAS, lo = c * S, n = max(0, min(S, a.vocab - lo));
+
+	// the segment, aligned part by one bulk copy, the <= 3 entries on each side of it by plain loads
+	const float* gp = logits + lo;
+	const int h = n ? (int)(((16 - ((uintptr_t)gp & 15)) & 15) >> 2) : 0, hb = min(h, n);
+	const int nb = n > hb ? ((n - hb) >> 2) << 2 : 0;
+	float* seg = seg_raw + 4 - h;
+	if (tid == 0) {
+		mbar_init(&bar, 1);
+		mbar_init_fence();
+	}
+	__syncthreads();
+	if (tid == 0) {
+		mbar_expect_tx(&bar, nb * 4u);
+		if (nb) tma_load_1d(seg + hb, gp + hb, nb * 4u, &bar);
+	}
+	if (tid < hb) seg[tid] = gp[tid];
+	if (tid < n - hb - nb) seg[hb + nb + tid] = gp[hb + nb + tid];
+
+	float mx = -FLT_MAX; // M and T as sample_scan forms them
+	for (int i = tid; i < a.ncand; i += 256) mx = fmaxf(mx, a.cand_val[i]);
+	mx = warp_max(mx);
+	if (lane == 0) wscan[warp] = __float_as_uint(mx);
+	mbar_wait(&bar, 0);
+	__syncthreads();
+	mx = __uint_as_float(wscan[0]);
+	for (int i = 1; i < 8; ++i) mx = fmaxf(mx, __uint_as_float(wscan[i]));
+	const float temp = a.st->temperature;
+
+	// sums x over the cluster (every CTA gets the total); slot `s` alternates between consecutive calls
+	int zs = 0;
+	auto cluster_sum = [&](unsigned long long x) {
+		for (int m = 16; m > 0; m >>= 1) x += __shfl_xor_sync(0xffffffffu, x, m);
+		if (lane == 0) wh[warp].mass[0] = x;
+		__syncthreads();
+		if (tid == 0) {
+			unsigned long long s = 0;
+			for (int w = 0; w < 8; ++w) s += wh[w].mass[0];
+			cz[zs] = s;
+		}
+		cluster.sync();
+		unsigned long long tot = 0;
+		for (int r = 0; r < TRUNC_CTAS; ++r) tot += *cluster.map_shared_rank(&cz[zs], r);
+		zs ^= 1;
+		return tot;
+	};
+
+	// One radix round over the allowed entries whose key agrees with `pre` above bit `shift + 8` and that `in` admits:
+	// the cluster's count and mass histograms of their next digit, then the walk from the top bucket that stops where
+	// the running count (BY_MASS: mass) reaches `need`.  The mass of the excluded top-k tie group (key kx, rx of its
+	// tokens in the set) is added back by every CTA alike.  Leaves the chosen digit in sel_key, the remainder in
+	// sel_rem / sel_above (what lies above the chosen bucket) and the bucket's count in sel_group.
+	int hs = 0;
+	auto radix_round = [&](uint32_t pre, int shift, auto in, bool by_mass, unsigned long long need, uint32_t kx, unsigned rx, unsigned long long mxk) {
+		TruncHist& w = wh[warp];
+		for (int b = lane; b < 256; b += 32) w.cnt[b] = 0, w.mass[b] = 0;
+		__syncwarp();
+		const uint32_t hmask = shift == 24 ? 0u : ~0u << (shift + 8);
+		for (int i = tid; i < n; i += 256) {
+			const float l = seg[i];
+			const uint32_t k = trunc_key(l);
+			if (l == -INFINITY || (k & hmask) != (pre & hmask) || !in(k)) continue;
+			const int b = (k >> shift) & 255;
+			atomicAdd(&w.cnt[b], 1u);
+			if (by_mass) atomicAdd(&w.mass[b], trunc_mass(l, mx, temp));
+		}
+		__syncthreads();
+		TruncHist& o = ch[hs];
+		{
+			unsigned cn = 0;
+			unsigned long long ms = 0;
+			for (int v = 0; v < 8; ++v) cn += wh[v].cnt[tid], ms += wh[v].mass[tid];
+			o.cnt[tid] = cn, o.mass[tid] = ms;
+		}
+		cluster.sync();
+		unsigned cn = 0;
+		unsigned long long ms = 0;
+		for (int r = 0; r < TRUNC_CTAS; ++r) {
+			const TruncHist* rh = cluster.map_shared_rank(&o, r);
+			cn += rh->cnt[tid], ms += rh->mass[tid];
+		}
+		if (rx && (kx & hmask) == (pre & hmask) && (int)((kx >> shift) & 255) == tid) cn += rx, ms += rx * mxk;
+		wh[0].cnt[tid] = cn, wh[0].mass[tid] = ms; // (every warp is past reading wh: the cluster barrier)
+		hs ^= 1;
+		__syncthreads();
+		if (tid == 0) {
+			unsigned long long acc = 0;
+			int b = 255;
+			for (; b > 0; --b) {
+				const unsigned long long x = by_mass ? wh[0].mass[b] : wh[0].cnt[b];
+				if (acc + x >= need) break;
+				acc += x;
+			}
+			sel_key = (pre & hmask) | ((uint32_t)b << shift);
+			sel_above = acc, sel_group = wh[0].cnt[b];
+		}
+		__syncthreads();
+	};
+
+	// top-k: (vk, rk), the K-th rank's key and how many of its tied tokens the set keeps; off (vk 0) when K >= allowed
+	uint32_t vk = 0, sel = 0;
+	unsigned rk = 0;
+	const unsigned long long allowed = cluster_sum([&] {
+		unsigned x = 0;
+		for (int i = tid; i < n; i += 256) x += seg[i] != -INFINITY;
+		return (unsigned long long)x;
+	}());
+	auto all = [](uint32_t) { return true; };
+	if (K > 0 && (unsigned long long)K < allowed) {
+		unsigned long long need = K;
+		for (int shift = 24; shift >= 0; shift -= 8) {
+			radix_round(sel, shift, all, false, need, 0, 0, 0);
+			sel = sel_key, need -= sel_above;
+		}
+		vk = sel, rk = (unsigned)need;
+	}
+	uint32_t v = vk; // the kept set: keys above v, and the first r tokens of key v
+	unsigned r = rk;
+	if (P < 1.0f) {
+		const unsigned long long mk = vk ? trunc_mass(trunc_logit(vk), mx, temp) : 0;
+		unsigned long long z = 0;
+		for (int i = tid; i < n; i += 256) {
+			const float l = seg[i];
+			if (l != -INFINITY && trunc_key(l) > vk) z += trunc_mass(l, mx, temp);
+		}
+		z = cluster_sum(z) + rk * mk;
+		unsigned long long need = trunc_target(z, P);
+		auto above_k = [vk](uint32_t k) { return k > vk; };
+		sel = 0;
+		for (int shift = 24; shift >= 0; shift -= 8) {
+			radix_round(sel, shift, above_k, true, need, vk, rk, mk);
+			sel = sel_key, need -= sel_above;
+		}
+		const unsigned long long mp = trunc_mass(trunc_logit(sel), mx, temp); // > 0: the walk stops at a bucket with mass
+		v = sel, r = (unsigned)min((unsigned long long)sel_group, (need + mp - 1) / mp);
+	}
+	if (v) {
+		// this CTA's tied tokens before those of the CTAs below it
+		unsigned ties = 0;
+		for (int i = tid; i < n; i += 256) ties += trunc_key(seg[i]) == v && seg[i] != -INFINITY;
+		for (int m = 16; m > 0; m >>= 1) ties += __shfl_xor_sync(0xffffffffu, ties, m);
+		if (lane == 0) wscan[warp] = ties;
+		__syncthreads();
+		if (tid == 0) {
+			unsigned s = 0;
+			for (int w = 0; w < 8; ++w) s += wscan[w];
+			ctie[zs] = s;
+		}
+		cluster.sync();
+		unsigned before = 0;
+		for (int q = 0; q < c; ++q) before += *cluster.map_shared_rank(&ctie[zs], q);
+		const int keep = (int)min(max((long long)r - before, 0ll), (long long)ctie[zs]);
+		// in id order: 4 consecutive entries per thread, 1024 a pass, the tied ones ranked by a block scan
+		int seen = 0;
+		for (int base = 0; base < n; base += 1024) {
+			const int i0 = base + tid * 4;
+			bool tie[4], drop[4];
+			int nt = 0;
+#pragma unroll
+			for (int j = 0; j < 4; ++j) {
+				const float l = i0 + j < n ? seg[i0 + j] : -INFINITY;
+				const uint32_t k = trunc_key(l);
+				tie[j] = l != -INFINITY && k == v;
+				drop[j] = l != -INFINITY && k < v;
+				nt += tie[j];
+			}
+			int incl = nt;
+			for (int m = 1; m < 32; m <<= 1) {
+				const int x = __shfl_up_sync(0xffffffffu, incl, m);
+				if (lane >= m) incl += x;
+			}
+			__syncthreads(); // (the previous pass is done with wscan)
+			if (lane == 31) wscan[warp] = incl;
+			__syncthreads();
+			int rank = seen + incl - nt;
+			for (int w = 0; w < warp; ++w) rank += wscan[w];
+			for (int w = 0; w < 8; ++w) seen += wscan[w];
+#pragma unroll
+			for (int j = 0; j < 4; ++j) {
+				if (tie[j]) drop[j] = rank++ >= keep;
+				if (drop[j]) logits[lo + i0 + j] = -INFINITY;
+			}
+		}
+	}
+	cluster.sync(); // no CTA leaves while another may still read its shared memory
 }
 
 // per-chunk maxima of a logits vector (stand-alone sampler entry point: what k_output's candidates are in a token)

@@ -29,16 +29,20 @@ SYMBOLS = [
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
     "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
     "calm_b200_decode_sample_queue_context", "calm_b200_decode_sample_queue_logprobs", "calm_b200_decode_sample_queue_penalties",
-    "calm_b200_decode_sample_queue_constrained",
+    "calm_b200_decode_sample_queue_constrained", "calm_b200_decode_sample_queue_truncated",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
     "calm_b200_tp_unique_id", "calm_b200_tp_init", "calm_b200_tp_world", "calm_b200_tp_mode",
     "calm_b200_decode_sample", "calm_b200_forward_sample", "calm_b200_read_device_logits", "calm_b200_sample_logits",
+    "calm_b200_sample_logits_truncated",
 ]
 
 # the largest k calm_b200_score_topk and its siblings accept (CALM_B200_TOPK_MAX)
 TOPK_MAX = 20
+
+# the largest vocabulary calm_b200_decode_sample_queue_truncated and calm_b200_sample_logits_truncated truncate
+TRUNC_VOCAB_MAX = 262144
 
 # the largest block calm_b200_verify_greedy takes (CALM_B200_VERIFY_MAX); decode_lookup drafts at most one fewer
 VERIFY_MAX = 16
@@ -118,6 +122,8 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_queue_constrained.argtypes = (L.calm_b200_decode_sample_queue_penalties.argtypes
                                                             + [C.c_int, C.POINTER(C.c_uint32), _iptr, _iptr, _iptr, _iptr, _iptr, _iptr])
     L.calm_b200_decode_sample_queue_constrained.restype = C.c_int
+    L.calm_b200_decode_sample_queue_truncated.argtypes = L.calm_b200_decode_sample_queue_constrained.argtypes + [_iptr, _fptr]
+    L.calm_b200_decode_sample_queue_truncated.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -144,6 +150,8 @@ def load() -> C.CDLL:
     L.calm_b200_read_device_logits.argtypes, L.calm_b200_read_device_logits.restype = [_fptr], None
     L.calm_b200_sample_logits.argtypes = [_fptr, C.c_int, C.c_float, C.c_float, C.POINTER(C.c_ulonglong), _fptr]
     L.calm_b200_sample_logits.restype = C.c_int
+    L.calm_b200_sample_logits_truncated.argtypes = [_fptr, C.c_int, C.c_float, C.c_float, C.c_int, C.c_float, C.POINTER(C.c_ulonglong), _fptr, _fptr]
+    L.calm_b200_sample_logits_truncated.restype = C.c_int
     _lib = L
     return L
 
@@ -626,13 +634,14 @@ class DeviceModel:
             raise ValueError(f"{who}: the sum of max_new does not fit an int")
         return prompts, max_new, temperature, minp, stop, states
 
-    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None, pen=None, aut=None):
+    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None, pen=None, aut=None, trunc=None):
         """Run a queue call over the laid-out tokens; ctx is (ctx_off, ctx_len), either of them None for a NULL array, or
         None for a call without those arguments.  Returns (tokens, states, served, steps, prompt_rows), and with `k` (the
         log-probability call) also each request's float32[out_len] log-probabilities and, for k > 0, its top ids and
         log-probabilities [out_len, k] (None for k == 0).  `pen` (the penalty call) is the list of its arguments after
         minp; without `k` that call gets k 0 and NULL outputs.  `aut` (the constrained call) is the list of its automaton
-        arguments before out_state; the return value then ends with each request's final state."""
+        arguments before out_state; the return value then ends with each request's final state.  `trunc` (the truncated
+        call) is its (top_k, top_p) pointers, after out_state."""
         nreq = len(len_)
         mn = np.ascontiguousarray(max_new, np.int32)
         st = np.ascontiguousarray(stop, np.int32)
@@ -660,6 +669,8 @@ class DeviceModel:
         out_state = np.full(max(nreq, 1), -2, np.int32)
         if aut is not None:
             args += aut + [out_state.ctypes.data_as(ip)]
+        if trunc is not None:
+            args += trunc
         served = fn(*args)
         o = np.concatenate([[0], np.cumsum(mn)]).astype(np.int64)
         toks = [out[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)]
@@ -836,7 +847,52 @@ class DeviceModel:
         the tokens its state allows can be chosen, and it retires after a token that leads to a final state.  start None
         (or every entry -1) constrains no request.  Returns decode_sample_queue_penalties' tuple followed by each request's
         state after its last token (-1 for an unconstrained request).  Raises ValueError where the C call would abort."""
-        who = "decode_sample_queue_constrained"
+        return self._constrained_call("decode_sample_queue_constrained", contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows,
+                                      rng_states, automaton, start, presence, frequency, repetition, logit_bias, k)
+
+    def decode_sample_queue_truncated(self, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states, top_k=None,
+                                      top_p=None, automaton=None, start=None, presence=None, frequency=None, repetition=None, logit_bias=None, k=None):
+        """calm_b200_decode_sample_queue_truncated: decode_sample_queue_constrained where sampled request i keeps only its
+        top_k[i] most likely tokens (0: off) and the shortest prefix of those whose probability reaches top_p[i] (1: off)
+        before the draw, by include/calm_b200.h's rule.  top_k / top_p None mean off for every request.  Returns
+        decode_sample_queue_constrained's tuple; log-probabilities stay those before truncation.  Raises ValueError where
+        the C call would abort."""
+        who = "decode_sample_queue_truncated"
+        nreq = len(prompts)
+        keep = []
+        trunc = []
+        for name, xs, dt in (("top_k", top_k, np.int32), ("top_p", top_p, np.float32)):
+            if xs is None:
+                trunc.append(None)
+                continue
+            try:
+                a = np.asarray(xs)
+                if name == "top_k" and (a.dtype.kind not in "iu" or a.ndim != 1):
+                    raise TypeError("not a sequence of integers")
+                a = np.ascontiguousarray(a, dt).reshape(-1)
+            except (TypeError, ValueError) as e:
+                raise ValueError(f"{who}: bad {name}: {e}") from None
+            if len(a) != nreq:
+                raise ValueError(f"{who} takes one {name} per prompt: {nreq} prompts, {len(a)} values")
+            if name == "top_k" and not (a >= 0).all():
+                raise ValueError(f"{who}: every top_k must be >= 0")
+            if name == "top_p" and not (np.isfinite(a) & (a > 0) & (a <= 1)).all():
+                raise ValueError(f"{who}: every top_p must be finite and in (0, 1]")
+            keep.append(a)
+            trunc.append(a.ctypes.data_as(C.POINTER(C.c_int) if name == "top_k" else _fptr))
+        if self.vocab > TRUNC_VOCAB_MAX and nreq:
+            t = np.ascontiguousarray(temperature, np.float32).reshape(-1)
+            m = np.ascontiguousarray(minp, np.float32).reshape(-1)
+            for i in range(min(nreq, len(t), len(m), len(max_new))):
+                on = (top_k is not None and keep[0][i] > 0) or (top_p is not None and keep[-1][i] < 1)
+                if on and max_new[i] > 0 and t[i] != 0 and m[i] < 1:
+                    raise ValueError(f"{who}: truncation serves vocabularies up to {TRUNC_VOCAB_MAX} tokens, not {self.vocab}")
+        return self._constrained_call(who, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows, rng_states, automaton, start,
+                                      presence, frequency, repetition, logit_bias, k, trunc=trunc, keep=keep)
+
+    def _constrained_call(self, who, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows, rng_states, automaton, start, presence,
+                          frequency, repetition, logit_bias, k, trunc=None, keep=None):
+        """decode_sample_queue_constrained (trunc None) or _truncated (trunc: its top_k / top_p pointers, their arrays in keep)."""
         if k is not None:
             self._check_queue_k(k)
         prompts, max_new, temperature, minp, stop, states = self._queue_args(who, prompts, max_new, temperature, minp, stop, max_rows, rng_states)
@@ -858,7 +914,7 @@ class DeviceModel:
                 if s0 >= 0 and max_new[i] > 0 and automaton.final[s0]:
                     raise ValueError(f"request {i} starts in final state {s0}")
             st = np.ascontiguousarray(st, np.int32)
-        keep = [st]
+        keep = (keep or []) + [st]
         pen = self._penalty_args(who, nreq, presence, frequency, repetition, logit_bias, keep)
         ip = C.POINTER(C.c_int)
         if automaton is None:
@@ -869,8 +925,9 @@ class DeviceModel:
                    a.exc_tok.ctypes.data_as(ip), a.exc_next.ctypes.data_as(ip)]
         aut.append(None if st is None else st.ctypes.data_as(ip))
         tokens, ctx, off, len_ = self._optional_context_layout(who, contexts, ctx_of, prompts)
-        return self._queue_call(self.lib.calm_b200_decode_sample_queue_constrained, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows,
-                                states, k=None if k is None else int(k), pen=pen, aut=aut)
+        fn = self.lib.calm_b200_decode_sample_queue_constrained if trunc is None else self.lib.calm_b200_decode_sample_queue_truncated
+        return self._queue_call(fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None if k is None else int(k), pen=pen,
+                                aut=aut, trunc=trunc)
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""
@@ -957,3 +1014,27 @@ def sample_logits(logits: np.ndarray, temperature: float, minp: float, rng_state
     us = C.c_float(0)
     tok = L.calm_b200_sample_logits(buf.ctypes.data_as(_fptr), len(buf), temperature, minp, C.byref(rng), C.byref(us) if timed else None)
     return (tok, int(rng.value), us.value) if timed else (tok, int(rng.value))
+
+
+def sample_logits_truncated(logits: np.ndarray, temperature: float, minp: float, top_k: int, top_p: float, rng_state: int, timed: bool = False):
+    """calm_b200_sample_logits_truncated: the device sampler on host logits after top_k (0: off) / top_p (1: off)
+    truncation by include/calm_b200.h's rule; returns (token, new rng state, the row after truncation with -inf at the
+    dropped ids[, microseconds of the kernels]).  Raises ValueError where the C call would abort."""
+    buf = np.ascontiguousarray(logits, np.float32).reshape(-1)
+    if not len(buf):
+        raise ValueError("sample_logits_truncated: empty vocabulary")
+    if not isinstance(top_k, (int, np.integer)) or isinstance(top_k, bool) or top_k < 0:
+        raise ValueError(f"top_k must be a non-negative integer, got {top_k!r}")
+    p32 = np.float32(top_p)
+    if not (np.isfinite(p32) and 0 < p32 <= 1):
+        raise ValueError(f"top_p must be finite and in (0, 1], got {top_p!r}")
+    _check_rng(rng_state)
+    if (top_k > 0 or p32 < 1) and np.float32(temperature) != 0 and np.float32(minp) < 1 and len(buf) > TRUNC_VOCAB_MAX:
+        raise ValueError(f"sample_logits_truncated: truncation serves vocabularies up to {TRUNC_VOCAB_MAX} tokens, not {len(buf)}")
+    L = load()
+    rng = C.c_ulonglong(rng_state)
+    us = C.c_float(0)
+    row = np.empty_like(buf)
+    tok = L.calm_b200_sample_logits_truncated(buf.ctypes.data_as(_fptr), len(buf), temperature, minp, int(top_k), float(p32), C.byref(rng),
+                                              row.ctypes.data_as(_fptr), C.byref(us) if timed else None)
+    return (tok, int(rng.value), row, us.value) if timed else (tok, int(rng.value), row)

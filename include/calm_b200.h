@@ -476,6 +476,47 @@ int calm_b200_decode_sample_queue_constrained(struct Transformer* transformer, c
                                               const uint32_t* allow, const int* next_default, const int* exc_off, const int* exc_tok,
                                               const int* exc_next, const int* start, int* out_state);
 
+/* calm_b200_decode_sample_queue_constrained where each sampled request may also truncate its distribution to top-k
+ * and top-p (nucleus) before the draw: top_k[i] (0 = off) and top_p[i] (1 = off), either array NULL meaning off for
+ * every request (INTEGRATION.md "Top-k and top-p").
+ * The rule.  At request i's step j, sampled (temperature T > 0, minp < 1), let l3 be the _constrained call's
+ * processed and masked logits and M = max l3.
+ *   Rank order: the allowed tokens (l3 != -inf) by l3 descending, equal logits lowest id first (the _topk calls' rule).
+ *   Mass: q(v) = expf((l3(v) - M) / T), the exact fp32 value the sampler forms for a survivor, and
+ *     m(v) = floor(q(v) * 2^40) as an unsigned 64-bit integer (m(argmax) = 2^40; sums are exact and associative).
+ *   top_k = K > 0: keep the first K ranks.
+ *   top_p = P < 1: with Z the total mass of the top-K set (of every allowed token when K is off) and
+ *     target = ceil(Z * P) in exact integer arithmetic (P the fp32 value taken exactly), keep the shortest rank prefix
+ *     of that set, at least one token, whose mass sum is >= target.  The nucleus is normalised over the top-k set:
+ *     temperature -> top-k -> top-p -> min-p, Hugging Face's warper order and vLLM's top-k-then-top-p.
+ *   Min-p: the reference's cut l >= M + log(minp) * T applies on top, unchanged; M is always kept.
+ *   The draw: the survivors go through exactly the masked sampler (index order, the reference's fp32 additions, one
+ *     coin per step): a truncated token behaves exactly like a token the automaton masked.
+ * Greedy requests take the first maximum, which every truncation keeps: their top_k / top_p change nothing.
+ * What truncation does not change: logprobs, top_ids and top_logprobs stay the _constrained call's, the model's
+ * processed distribution at temperature 1 before min-p, top-k and top-p; penalty counts and automaton states
+ * advance from the emitted token, as before.
+ * Invariants.  A request with top_k 0 and top_p 1 gets the _constrained call's bits whatever shares its steps; with
+ * top_k and top_p NULL, or all neutral, the call launches exactly what _constrained launches.  Request i's outputs do
+ * not depend on the other requests, max_rows, its slots, seq_len or an earlier call.
+ * Device work.  A step with a truncated sampled row runs k_sample_trunc_rows (one 8-CTA thread-block cluster per such
+ * row: a radix select over its logits staged in shared memory) after the classifier, which writes -inf over the
+ * row's dropped entries, then the masked sampler scan.  Truncation serves vocabularies up to 262144 tokens.
+ * Aborts, before any device work: where _constrained aborts, and when a top_k is negative, a top_p is not finite or
+ * outside (0, 1], or a request with max_new > 0 is sampled with top_k > 0 or top_p < 1 on a vocabulary larger than
+ * 262144 tokens.
+ * Fallback (return 0; as the _constrained call).  A truncated request decodes on the decode path; the host applies
+ * l2 and the mask to each step's device logits and draws with calm_b200_sample_logits_truncated's kernels and the
+ * request's state. */
+int calm_b200_decode_sample_queue_truncated(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                            const int* off, const int* len, int nreq, const int* max_new, const float* temperature, const float* minp,
+                                            const float* presence, const float* frequency, const float* repetition, const int* bias_off,
+                                            const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias, const int* stop, int n_stop,
+                                            int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps,
+                                            int* prompt_rows, int k, float* logprobs, int* top_ids, float* top_logprobs, int n_states,
+                                            const uint32_t* allow, const int* next_default, const int* exc_off, const int* exc_tok,
+                                            const int* exc_next, const int* start, int* out_state, const int* top_k, const float* top_p);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
@@ -490,6 +531,14 @@ void calm_b200_read_device_logits(float* out_vocab);
 /* The same sampler kernels on logits supplied by the host (any vocabulary size, no model needed): returns the token,
  * advances *rng_state exactly as sample() does; *device_us (optional) = duration of the two sampler kernels. */
 int calm_b200_sample_logits(const float* logits_host, int vocab, float temperature, float minp, unsigned long long* rng_state, float* device_us);
+
+/* calm_b200_sample_logits with calm_b200_decode_sample_queue_truncated's top-k / top-p rule on one host row: chunk
+ * maxima, k_sample_trunc_rows, the masked scan and the pick (a -inf logit never survives).  top_k 0 and top_p 1 mean
+ * off; with both off the row still goes through the masked scan.  out_row (may be NULL) receives the row after
+ * truncation, -inf at the dropped ids (for a greedy draw, the row unchanged).  Aborts when top_k < 0, top_p is not
+ * finite or outside (0, 1], or a sampled draw with truncation has a vocabulary above 262144 tokens. */
+int calm_b200_sample_logits_truncated(const float* logits_host, int vocab, float temperature, float minp, int top_k, float top_p,
+                                      unsigned long long* rng_state, float* out_row, float* device_us);
 
 /* Device timer on the library's stream (CUDA events): start, ..., stop -> ms. */
 void calm_b200_timer_start(void);
