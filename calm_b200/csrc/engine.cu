@@ -189,7 +189,7 @@ struct Prefill {
 	// needs more: the step's row table (written by k_sq_begin), the step's tokens, and every request's tokens and state
 	SqRows* sqrows = nullptr;
 	SqGroups* sqgroups = nullptr;      // the step's context groups (written by k_sq_groups), on steps whose rows have contexts
-	int* sqtok = nullptr;              // [VF_TOK]
+	int* sqtok = nullptr;              // [2 VF_TOK]: the step's tokens, then (k_sq_accept) each row's emitted flag
 	int* sqout = nullptr;              // [sqout_cap]: request i's tokens from O_i = max_new[0] + .. + max_new[i - 1]
 	unsigned long long* sqst = nullptr; // [sqst_cap]: request i's generator state after its last sampled step
 	size_t sqout_cap = 0, sqst_cap = 0;
@@ -2461,6 +2461,14 @@ static void sq_check_automaton(const char* who, SqAutomaton& a, int nreq, const 
 		if (max_new[i] > 0 && a.s0(i) >= 0 && a.fin[a.s0(i)]) CALM_FATAL("%s: request %d starts in final state %d", who, i, a.s0(i));
 }
 
+// The prompt-lookup drafts of calm_b200_decode_sample_queue_lookup: up to max_draft draft rows per request and step, and
+// where the call counts the draft rows it ran and the drafts it accepted (either may be NULL)
+struct SqLookup {
+	int max_draft;
+	int* drafted;
+	int* accepted;
+};
+
 // calm_b200_decode_sample_queue_context, and calm_b200_decode_sample_queue with every ctx_len 0 (`who` names the call in
 // error messages): a round's extent goes through the packed prompt pass (sb_prefill), each request's own rows continuing
 // its context at positions ctx_len .. (PF_CONTEXTS where a block holds such rows); a step whose rows have contexts runs
@@ -2474,10 +2482,16 @@ static void sq_check_automaton(const char* who, SqAutomaton& a, int nreq, const 
 // `pen`) the host follows each constrained request's state from the step's tokens, read back as the stop list's are; a
 // step with a constrained row passes the rows' lanes and states to k_sq_mask_lanes, runs sq_classify's MASK classifier
 // and, when such a row samples, k_sample_scan_rows_masked; every other step exactly the kernels it runs without `aut`.
+// With `lk` and max_draft > 0 (calm_b200_decode_sample_queue_lookup) the rows a step's requests leave free carry drafts:
+// a request's draft rows follow its row, each one more queue row at its own step j + d, fed the draft's d-th token with
+// the request's generator advanced d times and its automaton state advanced through the draft; a step with a draft row
+// ends with k_sq_accept instead of k_sq_end, and every step's tokens and emitted flags are read back, from which the host
+// takes the emitted tokens, the next drafts and each request's next row source.
 static int sq_run(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off,
                   const int* len, int nreq, const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
                   int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows,
-                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr, SqAutomaton* aut = nullptr, const SqTrunc* tr = nullptr) {
+                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr, SqAutomaton* aut = nullptr, const SqTrunc* tr = nullptr,
+                  const SqLookup* lk = nullptr) {
 	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
 	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, max_rows, CALM_B200_SAMPLE_N_MAX);
 	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, n_stop);
@@ -2532,10 +2546,13 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		if (max_new[i] > 0 && truncated(i) && g.cfg.vocab_size > TRUNC_VOCAB_MAX)
 			CALM_FATAL("%s: request %d is truncated, and truncation serves vocabularies up to %d tokens, not %d", who, i, TRUNC_VOCAB_MAX, g.cfg.vocab_size);
 	}
+	if (lk && (lk->max_draft < 0 || lk->max_draft > SQ_ROWS - 1)) CALM_FATAL("%s: max_draft %d outside [0, %d]", who, lk->max_draft, SQ_ROWS - 1);
 	check_tokens(tokens, n);
 	check_tokens(stop, n_stop);
 	if (steps) *steps = 0;
 	if (prompt_rows) *prompt_rows = 0;
+	if (lk && lk->drafted) *lk->drafted = 0;
+	if (lk && lk->accepted) *lk->accepted = 0;
 	std::vector<int> cur(nreq, -1); // a constrained request's automaton state after its tokens so far
 	for (int i = 0; aut && i < nreq; ++i) cur[i] = aut->s0(i);
 	auto ends = [&](int i) { return cur[i] >= 0 && aut->fin[cur[i]]; }; // the request's last token led to a final state
@@ -2615,7 +2632,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 	if (!pf.sqrows) {
 		pf.sqrows = (SqRows*)dev_alloc(sizeof(SqRows));
 		pf.sqgroups = (SqGroups*)dev_alloc(sizeof(SqGroups));
-		pf.sqtok = (int*)dev_alloc(VF_TOK * sizeof(int));
+		pf.sqtok = (int*)dev_alloc(2 * VF_TOK * sizeof(int));
 	}
 	if (total > pf.sqout_cap || (size_t)nreq > pf.sqst_cap) { // (no step of an earlier call is still reading them)
 		CUDA_CHECK(cudaStreamSynchronize(g.stream));
@@ -2649,6 +2666,10 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		CUDA_CHECK(cudaMemcpyAsync(pf.sqallow, aut->allow, words * sizeof(uint32_t), cudaMemcpyHostToDevice, g.stream));
 	}
 	std::vector<int> lane_of(nreq, -1); // a non-neutral request's lane while it is in flight
+	const bool drafting = lk && lk->max_draft > 0;
+	std::vector<std::vector<int>> corpus(drafting ? nreq : 0); // (drafting) ctx ++ prompt ++ tokens so far: the lookup's sequence
+	std::vector<unsigned long long> hst(rng_states, rng_states + nreq); // a sampled request's state after its tokens so far
+	int ndrafted = 0, naccepted = 0;
 	unsigned lanes_free = (1u << SQ_ROWS) - 1;
 
 	SqSlots slots(g.cfg.seq_len);
@@ -2656,7 +2677,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 	std::vector<SqPlace> place(nreq);
 	std::vector<int> done(nreq, 0), row_of(nreq, -1); // tokens so far; row in the last step
 	std::vector<int> live;                            // requests in flight, in admission order
-	int head = 0, nsteps = 0, last_sampled = 0, rows_computed = 0, tok_host[VF_TOK]; // last_sampled: the last step's rows if it sampled
+	int head = 0, nsteps = 0, last_sampled = 0, rows_computed = 0, tok_host[2 * VF_TOK]; // last_sampled: the last step's rows if it sampled
 	std::vector<int> round;
 	std::vector<SqPlace> rp;
 	int rbase = 0; // the round's prompt extent's first slot
@@ -2714,6 +2735,10 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 					pb.add(tokens + ctx_off[i], q.nc, q.nc - 1, 0, make_int2(0, 0));
 				}
 				pb.add(tokens + off[i], len[i] - 1, len[i] - 1, q.nc, make_int2(q.c, q.nc));
+				if (drafting) {
+					corpus[i].assign(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
+					corpus[i].insert(corpus[i].end(), tokens + off[i], tokens + off[i] + len[i]);
+				}
 				if (pen && !pen->neutral(i)) { // the lowest free lane, cleared and filled for the request
 					const int ln = __builtin_ctz(lanes_free);
 					lanes_free &= ~(1u << ln), lane_of[i] = ln;
@@ -2727,7 +2752,7 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			rows_computed += pb.rows();
 			live.insert(live.end(), round.begin(), round.end());
 		}
-		// the step: the rows in flight, in admission order
+		// the step: the rows in flight, in admission order, each request's draft rows after its row
 		SqRows r = {};
 		SqGroups grp = {};
 		SqLanes lanes;
@@ -2737,30 +2762,58 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 		bool mask_sampled = false; // .. that samples
 		TruncRows trows = {};      // the step's truncated rows
 		int ntrunc = 0;
-		r.n = (int)live.size();
-		int nsampled = 0, lmax = 0, nsuf = 0;
+		const int nlive = (int)live.size();
+		int nsampled = 0, lmax = 0, nsuf = 0, nfree = SQ_ROWS - nlive; // nfree: rows left for drafts
+		int first[SQ_ROWS + 1]; // request k's rows are first[k] .. first[k + 1] - 1
+		SqNext nx = {};         // the draft each row's successor is fed, -1 after a request's last row
 		std::map<int, std::vector<int>> groups; // rows by their context's first slot
 		std::vector<int> gorder;                // group slots in order of their first row
-		for (int k = 0; k < r.n; ++k) {
+		for (int k = 0; k < nlive; ++k) {
 			const int i = live[k], j = done[i];
 			const SqPlace& q = place[i];
-			r.q[k] = make_int4(q.s, q.L, q.t, j), r.pos[k] = q.L + j, r.slot[k] = q.t + j;
-			r.src[k] = row_of[i], r.tok0[k] = tokens[off[i] + len[i] - 1];
 			const bool gr = is_greedy(i);
-			// (a greedy row's sampler state is never read back: any valid one will do)
-			r.st0[k].rng = gr ? 1 : rng_states[i], r.st0[k].temperature = gr ? 1.0f : temperature[i], r.st0[k].cut_delta = gr ? 0.0f : logf(minp[i]) * temperature[i];
-			r.out[k] = (int)(O[i] + j), r.req[k] = i, r.greedy[k] = gr;
-			lanes.lane[k] = lane_of[i], pen_step = pen_step || lane_of[i] >= 0;
-			ml.lane[k] = lane_of[i], ml.state[k] = cur[i], mask_step = mask_step || cur[i] >= 0, mask_sampled = mask_sampled || (cur[i] >= 0 && !gr);
-			if (truncated(i)) trows.row[ntrunc] = k, trows.top_k[ntrunc] = tr->k(i), trows.top_p[ntrunc++] = tr->p(i);
-			nsampled += !gr, lmax = std::max(lmax, q.L + j), row_of[i] = k;
-			grp.ctx[k] = make_int2(q.c, q.nc);
-			nsuf = std::max(nsuf, cdiv(q.L + j + 1, SN_CHUNK) - q.nc / SN_CHUNK);
-			if (q.nc) {
-				if (!groups.count(q.c)) gorder.push_back(q.c);
-				groups[q.c].push_back(k);
+			int draft[SQ_ROWS], sd[SQ_ROWS]; // the draft, and a constrained request's state before each of its rows
+			int nd = 0;
+			sd[0] = cur[i];
+			if (drafting && !(pen && !pen->neutral(i))) {
+				nd = vf_lookup(corpus[i], nullptr, 0, imin(imin(lk->max_draft, max_new[i] - j - 1), nfree), draft);
+				// no draft row follows its request's end: the draft stops before a stop token, a token the state disallows
+				// and a token that leads to a final state
+				for (int d = 0; d < nd; ++d) {
+					const int v = draft[d];
+					if (is_stop[v] || (sd[d] >= 0 && (!aut->allowed(sd[d], v) || aut->fin[aut->next(sd[d], v)]))) {
+						nd = d;
+						break;
+					}
+					sd[d + 1] = sd[d] >= 0 ? aut->next(sd[d], v) : -1;
+				}
+				nfree -= nd;
+			}
+			first[k] = r.n;
+			unsigned long long s = hst[i]; // row d draws the coin after the d coins before it
+			for (int d = 0; d <= nd; ++d, s = xorshift_step(s)) {
+				const int b = r.n++;
+				r.q[b] = make_int4(q.s, q.L, q.t, j + d), r.pos[b] = q.L + j + d, r.slot[b] = q.t + j + d;
+				r.src[b] = d ? -1 : row_of[i], r.tok0[b] = d ? draft[d - 1] : tokens[off[i] + len[i] - 1];
+				// (a greedy row's sampler state is never read back: any valid one will do)
+				r.st0[b].rng = gr ? 1 : d ? s : rng_states[i], r.st0[b].temperature = gr ? 1.0f : temperature[i];
+				r.st0[b].cut_delta = gr ? 0.0f : logf(minp[i]) * temperature[i];
+				r.out[b] = (int)(O[i] + j + d), r.req[b] = i, r.greedy[b] = gr;
+				lanes.lane[b] = lane_of[i], pen_step = pen_step || lane_of[i] >= 0;
+				ml.lane[b] = lane_of[i], ml.state[b] = sd[d], mask_step = mask_step || sd[d] >= 0, mask_sampled = mask_sampled || (sd[d] >= 0 && !gr);
+				if (truncated(i)) trows.row[ntrunc] = b, trows.top_k[ntrunc] = tr->k(i), trows.top_p[ntrunc++] = tr->p(i);
+				nsampled += !gr, lmax = std::max(lmax, q.L + j + d);
+				grp.ctx[b] = make_int2(q.c, q.nc);
+				nsuf = std::max(nsuf, cdiv(q.L + j + d + 1, SN_CHUNK) - q.nc / SN_CHUNK);
+				if (q.nc) {
+					if (!groups.count(q.c)) gorder.push_back(q.c);
+					groups[q.c].push_back(b);
+				}
+				nx.tok[b] = d < nd ? draft[d] : -1;
 			}
 		}
+		first[nlive] = r.n;
+		const bool draft_step = r.n > nlive;
 		std::fill(lanes.lane + r.n, lanes.lane + SQ_ROWS, -1);
 		std::fill(ml.lane + r.n, ml.lane + SQ_ROWS, -1), std::fill(ml.state + r.n, ml.state + SQ_ROWS, -1);
 		launch_pdl(k_sq_begin, 1, 32, 0, r, pf.sqrows, (const int*)pf.sqtok, pf.tokens, pf.vstate);
@@ -2793,23 +2846,39 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
 			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled, ntrunc ? &trows : nullptr, ntrunc);
 		}
-		launch_pdl(k_sq_end, 1, 32, 0, (const SqRows*)pf.sqrows, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate, pf.sqtok, pf.sqout, pf.sqst);
+		if (draft_step)
+			launch_pdl(k_sq_accept, 1, 32, 0, (const SqRows*)pf.sqrows, nx, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate,
+			           pf.sqtok, pf.sqtok + VF_TOK, pf.sqout, pf.sqst);
+		else
+			launch_pdl(k_sq_end, 1, 32, 0, (const SqRows*)pf.sqrows, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate, pf.sqtok, pf.sqout, pf.sqst);
 		if (lp)
 			launch_pdl(k_sq_lp, 1, 32, 0, (const SqRows*)pf.sqrows, (const float*)pf.logprob, (const int*)pf.sqtid, (const float*)pf.sqtlp, lp->k, pf.sqlp,
 			           pf.sqoid, pf.sqolp);
 		if (pen_step) launch_pdl(k_sq_pen_step, 1, 32, 0, (const int*)pf.sqlanes, (const int*)pf.sqtok, g.cfg.vocab_size, pf.sqpcnt);
 		++nsteps, last_sampled = nsampled > 0 ? r.n : 0;
-		if (n_stop || mask_step) { // the step's tokens decide which rows stop, and the constrained rows' next states
-			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, r.n * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+		// the step's tokens decide which rows stop, the constrained rows' next states and the next drafts; with drafts, one
+		// copy also brings the emitted flags
+		if (n_stop || mask_step || drafting) {
+			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, (drafting ? 2 * VF_TOK : r.n) * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 			sync_stream();
 		}
-		// retire: rows that reached max_new or emitted a stop token free their own slots; the others keep their order
+		// retire: requests that reached max_new or emitted a stop token free their own slots; the others keep their order
 		std::vector<int> keep;
-		for (int k = 0; k < r.n; ++k) {
-			const int i = live[k];
-			++done[i];
-			if (cur[i] >= 0) cur[i] = aut->next(cur[i], tok_host[k]);
-			if (done[i] < max_new[i] && !(n_stop && is_stop[tok_host[k]]) && !ends(i)) {
+		for (int k = 0; k < nlive; ++k) {
+			const int i = live[k], f = first[k], nr = first[k + 1] - f;
+			int a = 0; // accepted drafts: the request emits its rows 0 .. a
+			while (a < nr - 1 && tok_host[f + a] == nx.tok[f + a]) ++a;
+			for (int d = 1; d < nr; ++d)
+				if (tok_host[VF_TOK + f + d] != (d <= a)) CALM_FATAL("%s: row %d's emitted flag disagrees with the step's tokens", who, f + d);
+			ndrafted += nr - 1, naccepted += a;
+			for (int d = 0; d <= a; ++d) {
+				++done[i];
+				if (cur[i] >= 0) cur[i] = aut->next(cur[i], tok_host[f + d]);
+				if (drafting) corpus[i].push_back(tok_host[f + d]);
+				if (!is_greedy(i)) hst[i] = xorshift_step(hst[i]);
+			}
+			row_of[i] = f + a;
+			if (done[i] < max_new[i] && !(n_stop && is_stop[tok_host[f + a]]) && !ends(i)) {
 				keep.push_back(i);
 				continue;
 			}
@@ -2851,6 +2920,8 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 	if (last_sampled) pf.vrows = last_sampled;
 	if (steps) *steps = nsteps;
 	if (prompt_rows) *prompt_rows = rows_computed;
+	if (lk && lk->drafted) *lk->drafted = ndrafted;
+	if (lk && lk->accepted) *lk->accepted = naccepted;
 	return 1;
 }
 
@@ -2934,6 +3005,27 @@ extern "C" int calm_b200_decode_sample_queue_truncated(struct Transformer* trans
 	return sq_run("decode_sample_queue_truncated", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len,
 	              nreq, max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
 	              logprobs || k ? &lp : nullptr, &pen, &aut, &tr);
+}
+
+extern "C" int calm_b200_decode_sample_queue_lookup(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                                    const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
+                                                    const float* minp, const float* presence, const float* frequency, const float* repetition,
+                                                    const int* bias_off, const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias,
+                                                    const int* stop, int n_stop, int max_rows, unsigned long long* rng_states, int* out_tokens,
+                                                    int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
+                                                    float* top_logprobs, int n_states, const uint32_t* allow, const int* next_default,
+                                                    const int* exc_off, const int* exc_tok, const int* exc_next, const int* start, int* out_state,
+                                                    const int* top_k, const float* top_p, int max_draft, int* drafted, int* accepted) {
+	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
+	const bool none = !ctx_off && !ctx_len;
+	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
+	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
+	SqAutomaton aut{n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state, 0, {}};
+	const SqTrunc tr{top_k, top_p};
+	const SqLookup lk{max_draft, drafted, accepted};
+	return sq_run("decode_sample_queue_lookup", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
+	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, logprobs || k ? &lp : nullptr,
+	              &pen, &aut, &tr, &lk);
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
@@ -3099,7 +3191,7 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		nan(pf.snpart, (size_t)VF_TOK * c.n_heads * pf.snchunks * (c.head_dim + 2) * sizeof(float)), nan(pf.sntok, (size_t)c.seq_len * sizeof(int));
 		// decode_sample_queue's step tokens and per-request tokens and states, which every call writes before it reads them
 		// (its row table, read as positions and key slots, is an index buffer)
-		nan(pf.sqtok, VF_TOK * sizeof(int)), nan(pf.sqout, pf.sqout_cap * sizeof(int)), nan(pf.sqst, pf.sqst_cap * sizeof(unsigned long long));
+		nan(pf.sqtok, 2 * VF_TOK * sizeof(int)), nan(pf.sqout, pf.sqout_cap * sizeof(int)), nan(pf.sqst, pf.sqst_cap * sizeof(unsigned long long));
 		// and its log-probability call's tile lists, merged top-k and per-request outputs (ids only compared and copied out)
 		const size_t nvt = cdiv(c.vocab_size, PF_BM);
 		nan(pf.sqtopv, VF_TOK * nvt * PF_TOPK_MAX * sizeof(float)), nan(pf.sqtopi, VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));

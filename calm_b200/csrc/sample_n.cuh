@@ -322,6 +322,39 @@ __global__ void __launch_bounds__(32) k_sq_end(const SqRows* tab, const int* gre
 	if (!gr) rng[tab->req[i]] = st[i].rng;
 }
 
+// ---------------------------------------------------------------- calm_b200_decode_sample_queue_lookup
+
+// The token each row's successor was fed, its draft (src -1 in SqRows), or -1 for a request's last row.  Passed by value
+// to k_sq_accept.
+struct SqNext {
+	int tok[SQ_ROWS];
+};
+
+// one warp, in place of k_sq_end after a step with draft rows (a request's rows are contiguous, its draft rows after its
+// first): row i is emitted when every earlier row of its request gave the token its successor was fed.  A row whose token
+// differs from its successor's draft, or a request's last row, ends its request's run, so row i is emitted exactly when
+// the nearest earlier run end (the ballot's highest bit below i) belongs to another request or there is none.  Every row's
+// token goes to the step's tokens and its emitted flag to emitted[i]; an emitted row's token goes to its output slot, and
+// a sampled request's generator state comes from its last emitted row alone, so each word has one writer.
+__global__ void __launch_bounds__(32) k_sq_accept(const SqRows* tab, const SqNext nx, const int* greedy, const int* sampled, const SampleState* st,
+                                                  int* step_tok, int* emitted, int* out, unsigned long long* rng) {
+	pdl_enter();
+	const int i = threadIdx.x;
+	const bool in = i < tab->n;
+	const bool gr = in && tab->greedy[i];
+	const int tok = !in ? -1 : gr ? greedy[i] : sampled[i], req = in ? tab->req[i] : -1;
+	const bool ends = in && tok != nx.tok[i];
+	const unsigned below = __ballot_sync(0xffffffffu, ends) & ((1u << i) - 1u);
+	const int h = 31 - __clz(below); // -1: no earlier run end
+	const int hreq = __shfl_sync(0xffffffffu, req, h < 0 ? 0 : h);
+	if (!in) return;
+	const bool em = h < 0 || hreq != req;
+	step_tok[i] = tok, emitted[i] = em;
+	if (!em) return;
+	out[tab->out[i]] = tok;
+	if (ends && !gr) rng[req] = st[i].rng;
+}
+
 // ---------------------------------------------------------------- calm_b200_decode_sample_queue_logprobs
 
 // one warp per row, after the sampler and before the merge of a step with log-probabilities: the row's target logit

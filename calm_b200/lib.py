@@ -29,7 +29,7 @@ SYMBOLS = [
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
     "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
     "calm_b200_decode_sample_queue_context", "calm_b200_decode_sample_queue_logprobs", "calm_b200_decode_sample_queue_penalties",
-    "calm_b200_decode_sample_queue_constrained", "calm_b200_decode_sample_queue_truncated",
+    "calm_b200_decode_sample_queue_constrained", "calm_b200_decode_sample_queue_truncated", "calm_b200_decode_sample_queue_lookup",
     "calm_b200_timer_start", "calm_b200_timer_stop",
     "calm_b200_stream", "calm_b200_launch_count", "calm_b200_read_kv", "calm_b200_read_state", "calm_b200_poison_state", "calm_b200_fill_kv", "calm_b200_matvec",
     "calm_b200_set_perf", "calm_b200_stage_stats", "calm_b200_perf_token_ms", "calm_b200_debug_stamps",
@@ -124,6 +124,8 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_queue_constrained.restype = C.c_int
     L.calm_b200_decode_sample_queue_truncated.argtypes = L.calm_b200_decode_sample_queue_constrained.argtypes + [_iptr, _fptr]
     L.calm_b200_decode_sample_queue_truncated.restype = C.c_int
+    L.calm_b200_decode_sample_queue_lookup.argtypes = L.calm_b200_decode_sample_queue_truncated.argtypes + [C.c_int, _iptr, _iptr]
+    L.calm_b200_decode_sample_queue_lookup.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -634,14 +636,16 @@ class DeviceModel:
             raise ValueError(f"{who}: the sum of max_new does not fit an int")
         return prompts, max_new, temperature, minp, stop, states
 
-    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None, pen=None, aut=None, trunc=None):
+    def _queue_call(self, fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None, pen=None, aut=None, trunc=None,
+                    max_draft=None):
         """Run a queue call over the laid-out tokens; ctx is (ctx_off, ctx_len), either of them None for a NULL array, or
         None for a call without those arguments.  Returns (tokens, states, served, steps, prompt_rows), and with `k` (the
         log-probability call) also each request's float32[out_len] log-probabilities and, for k > 0, its top ids and
         log-probabilities [out_len, k] (None for k == 0).  `pen` (the penalty call) is the list of its arguments after
         minp; without `k` that call gets k 0 and NULL outputs.  `aut` (the constrained call) is the list of its automaton
         arguments before out_state; the return value then ends with each request's final state.  `trunc` (the truncated
-        call) is its (top_k, top_p) pointers, after out_state."""
+        call) is its (top_k, top_p) pointers, after out_state.  `max_draft` (the lookup call) follows them; the return value
+        then ends with (drafted, accepted)."""
         nreq = len(len_)
         mn = np.ascontiguousarray(max_new, np.int32)
         st = np.ascontiguousarray(stop, np.int32)
@@ -671,6 +675,9 @@ class DeviceModel:
             args += aut + [out_state.ctypes.data_as(ip)]
         if trunc is not None:
             args += trunc
+        drafted, accepted = C.c_int(-1), C.c_int(-1)
+        if max_draft is not None:
+            args += [int(max_draft), C.byref(drafted), C.byref(accepted)]
         served = fn(*args)
         o = np.concatenate([[0], np.cumsum(mn)]).astype(np.int64)
         toks = [out[o[i]:o[i] + out_len[i]].copy() for i in range(nreq)]
@@ -680,6 +687,8 @@ class DeviceModel:
             res += (cut(lp), cut(ids), cut(tlp))
         if aut is not None:
             res += ([int(x) for x in out_state[:nreq]],)
+        if max_draft is not None:
+            res += (int(drafted.value), int(accepted.value))
         return res
 
     def _context_layout(self, who, contexts, ctx_of, prompts):
@@ -857,7 +866,25 @@ class DeviceModel:
         before the draw, by include/calm_b200.h's rule.  top_k / top_p None mean off for every request.  Returns
         decode_sample_queue_constrained's tuple; log-probabilities stay those before truncation.  Raises ValueError where
         the C call would abort."""
-        who = "decode_sample_queue_truncated"
+        return self._truncated_call("decode_sample_queue_truncated", contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows, rng_states,
+                                    top_k, top_p, automaton, start, presence, frequency, repetition, logit_bias, k)
+
+    def decode_sample_queue_lookup(self, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows: int, rng_states, max_draft: int = 7,
+                                   top_k=None, top_p=None, automaton=None, start=None, presence=None, frequency=None, repetition=None, logit_bias=None,
+                                   k=None):
+        """calm_b200_decode_sample_queue_lookup: decode_sample_queue_truncated, with the rows its steps leave free holding
+        prompt-lookup drafts of each request's own tokens (up to max_draft per request and step, in [0, 15]) that the same
+        step verifies.  Returns decode_sample_queue_truncated's tuple, bit for bit except that steps may be fewer, followed
+        by (drafted, accepted): the draft rows the call ran and the drafts it accepted.  Raises ValueError where the C call
+        would abort."""
+        if not isinstance(max_draft, (int, np.integer)) or isinstance(max_draft, bool) or not 0 <= max_draft <= VERIFY_MAX - 1:
+            raise ValueError(f"max_draft must be an integer in [0, {VERIFY_MAX - 1}], got {max_draft!r}")
+        return self._truncated_call("decode_sample_queue_lookup", contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows, rng_states,
+                                    top_k, top_p, automaton, start, presence, frequency, repetition, logit_bias, k, max_draft=int(max_draft))
+
+    def _truncated_call(self, who, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows, rng_states, top_k, top_p, automaton, start,
+                        presence, frequency, repetition, logit_bias, k, max_draft=None):
+        """decode_sample_queue_truncated (max_draft None) or _lookup: the top_k / top_p checks, then _constrained_call."""
         nreq = len(prompts)
         keep = []
         trunc = []
@@ -888,11 +915,12 @@ class DeviceModel:
                 if on and max_new[i] > 0 and t[i] != 0 and m[i] < 1:
                     raise ValueError(f"{who}: truncation serves vocabularies up to {TRUNC_VOCAB_MAX} tokens, not {self.vocab}")
         return self._constrained_call(who, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows, rng_states, automaton, start,
-                                      presence, frequency, repetition, logit_bias, k, trunc=trunc, keep=keep)
+                                      presence, frequency, repetition, logit_bias, k, trunc=trunc, keep=keep, max_draft=max_draft)
 
     def _constrained_call(self, who, contexts, ctx_of, prompts, max_new, temperature, minp, stop, max_rows, rng_states, automaton, start, presence,
-                          frequency, repetition, logit_bias, k, trunc=None, keep=None):
-        """decode_sample_queue_constrained (trunc None) or _truncated (trunc: its top_k / top_p pointers, their arrays in keep)."""
+                          frequency, repetition, logit_bias, k, trunc=None, keep=None, max_draft=None):
+        """decode_sample_queue_constrained (trunc None), _truncated (trunc: its top_k / top_p pointers, their arrays in
+        keep) or, with max_draft, _lookup."""
         if k is not None:
             self._check_queue_k(k)
         prompts, max_new, temperature, minp, stop, states = self._queue_args(who, prompts, max_new, temperature, minp, stop, max_rows, rng_states)
@@ -926,8 +954,10 @@ class DeviceModel:
         aut.append(None if st is None else st.ctypes.data_as(ip))
         tokens, ctx, off, len_ = self._optional_context_layout(who, contexts, ctx_of, prompts)
         fn = self.lib.calm_b200_decode_sample_queue_constrained if trunc is None else self.lib.calm_b200_decode_sample_queue_truncated
+        if max_draft is not None:
+            fn = self.lib.calm_b200_decode_sample_queue_lookup
         return self._queue_call(fn, tokens, ctx, off, len_, max_new, temperature, minp, stop, max_rows, states, k=None if k is None else int(k), pen=pen,
-                                aut=aut, trunc=trunc)
+                                aut=aut, trunc=trunc, max_draft=max_draft)
 
     def forward_sample(self, token: int, pos: int, temperature: float, minp: float, rng_state: int):
         """calm_b200_forward_sample: one token, sampled on the device; returns (token, new rng state)."""

@@ -517,6 +517,41 @@ int calm_b200_decode_sample_queue_truncated(struct Transformer* transformer, con
                                             const uint32_t* allow, const int* next_default, const int* exc_off, const int* exc_tok,
                                             const int* exc_next, const int* start, int* out_state, const int* top_k, const float* top_p);
 
+/* calm_b200_decode_sample_queue_truncated that fills the rows a step leaves free (16 per step, less the requests in
+ * flight) with prompt-lookup drafts of the requests' own tokens, verified in the same step (DESIGN.md s.6; INTEGRATION.md
+ * "Lookup drafts in the queue").  It takes every argument of the _truncated call, then max_draft, drafted and accepted.
+ * Outputs.  out_tokens, out_len, rng_states, logprobs, top_ids, top_logprobs, out_state, prompt_rows and the return value
+ * are bit for bit what calm_b200_decode_sample_queue_truncated gives with the same arguments; only *steps may be smaller.
+ * *drafted (drafted may be NULL) receives the draft rows the call ran, *accepted (may be NULL) the drafts it accepted.
+ * Slots past out_len[i] are left untouched, as in the _truncated call.
+ * max_draft in [0, 15].  0: no drafts; the call launches exactly what _truncated launches and takes the same steps.
+ * The draft rule (calm_b200_decode_lookup's with source == NULL).  Over request i's sequence ctx ++ prompt ++ its tokens so
+ * far, the key is the last 3 tokens, else 2, else 1, and the draft is what follows the key's rightmost occurrence that
+ * some token follows.
+ * Which requests draft.  After a step's admission, the requests in flight in admission order each take up to
+ * min(max_draft, max_new[i] - out_so_far - 1, rows still free of 16) draft rows, right after the request's own row.
+ * The draft then stops before its first stop token, and for a constrained request before the first token its state
+ * disallows and before the first token that leads to a final state: no draft row continues a finished request.  A
+ * request with non-neutral penalties or bias never drafts.  max_rows counts requests, not rows.
+ * Acceptance.  Draft row d of request i is the request at its step j + d, fed the draft's d-th token, and draws with the
+ * coin after the d coins before it.  Row d + 1's token is accepted when row d's token equals it; the request emits the
+ * tokens of its rows 0 .. a, a the accepted drafts, and draws one coin per emitted token.  Each emitted token is the one
+ * the _truncated call gives at that step, since a row's result depends on its own keys, token, position and state alone.
+ * Cost.  With max_draft > 0, every step copies its tokens and emitted flags back and synchronises, so that the host can
+ * look up the next drafts.  Rejected draft rows leave cache slots and device-side outputs at or past the request's
+ * position, which later steps overwrite; the host copies only each request's first out_len[i] outputs.
+ * Aborts, before any device work: where the _truncated call aborts, and when max_draft is outside [0, 15].
+ * Fallback (return 0; as the _truncated call): the _truncated call's fallback, with *steps, *drafted and *accepted 0. */
+int calm_b200_decode_sample_queue_lookup(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
+                                         const int* off, const int* len, int nreq, const int* max_new, const float* temperature, const float* minp,
+                                         const float* presence, const float* frequency, const float* repetition, const int* bias_off,
+                                         const int* bias_len, const int* bias_ids, const float* bias_val, int n_bias, const int* stop, int n_stop,
+                                         int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps,
+                                         int* prompt_rows, int k, float* logprobs, int* top_ids, float* top_logprobs, int n_states,
+                                         const uint32_t* allow, const int* next_default, const int* exc_off, const int* exc_tok,
+                                         const int* exc_next, const int* start, int* out_state, const int* top_k, const float* top_p,
+                                         int max_draft, int* drafted, int* accepted);
+
 /* The reference's sample() (sampler.c:80-90) on the device: temperature / min-p sampling with the reference's
  * xorshift* generator (sampler.c:7-17), no logits transfer and no host scan of the vocabulary per token.
  * temperature == 0 or minp >= 1 is greedy and leaves *rng_state alone, as in the reference.  Survivors are added
