@@ -209,7 +209,7 @@ struct Prefill {
 	int* sqpcnt = nullptr;    // [16][vocab]
 	float* sqpbias = nullptr; // [16][vocab]
 	float4* sqppar = nullptr; // [16]
-	int* sqlanes = nullptr;   // [32] the step's lane of each row (k_sq_lanes), and its automaton state (k_sq_mask_lanes) from 16
+	int* sqlanes = nullptr;   // [32] the step's lane of each row, and its automaton state from 16 (k_sq_lanes), allocated with pf.sqrows
 	int* sqptok = nullptr;    // [sqptok_cap]
 	int* sqpbid = nullptr;    // [sqpb_cap]
 	float* sqpbval = nullptr;
@@ -2233,18 +2233,28 @@ struct SqPlace {
 
 using SqCtx = std::pair<int, int>; // a context by (ctx_off, ctx_len): requests share it exactly when these are equal
 
+// The requests' contexts.  Both arrays NULL: no request has a context, except where `required` (the context call).
+struct SqContexts {
+	const int *ctx_off, *ctx_len;
+	bool required;
+	int off(int i) const { return ctx_off ? ctx_off[i] : 0; }
+	int len(int i) const { return ctx_len ? ctx_len[i] : 0; }
+	SqCtx key(int i) const { return SqCtx(off(i), len(i)); }
+	bool missing() const { return !ctx_off != !ctx_len || (required && !ctx_off); }
+};
+
 // The placement of one round, the requests `rs` in input order, with the contexts `resident` holds at their first slots:
 // one extent starting at a multiple of 8 that holds, request by request, the request's context (ceil8(ctx_len) slots) if
 // it is neither resident nor placed by an earlier request of the round, then its own prompt (ceil8(len - 1) slots); then
 // one extent of max_new slots per request.  False (and `a` spent) when one does not fit; `base` gets the first extent's
 // first slot.
-static bool sq_place(SqSlots& a, const std::vector<int>& rs, const int* ctx_off, const int* ctx_len, const int* len, const int* max_new,
-                     const std::map<SqCtx, int>& resident, std::vector<SqPlace>& out, int& base) {
+static bool sq_place(SqSlots& a, const std::vector<int>& rs, const SqContexts& ctx, const int* len, const int* max_new, const std::map<SqCtx, int>& resident,
+                     std::vector<SqPlace>& out, int& base) {
 	std::map<SqCtx, int> placed; // contexts of this round, by their offset in the extent
 	int P = 0;
 	for (int i : rs) {
-		const SqCtx k(ctx_off[i], ctx_len[i]);
-		if (ctx_len[i] && !resident.count(k) && !placed.count(k)) placed[k] = P, P += cdiv(ctx_len[i], 8) * 8;
+		const SqCtx k = ctx.key(i);
+		if (ctx.len(i) && !resident.count(k) && !placed.count(k)) placed[k] = P, P += cdiv(ctx.len(i), 8) * 8;
 		P += cdiv(len[i] - 1, 8) * 8;
 	}
 	const int s0 = base = P ? a.take(P, 8) : 0;
@@ -2253,61 +2263,54 @@ static bool sq_place(SqSlots& a, const std::vector<int>& rs, const int* ctx_off,
 	std::set<SqCtx> seen;
 	int s = s0;
 	for (int i : rs) {
-		const SqCtx k(ctx_off[i], ctx_len[i]);
+		const SqCtx k = ctx.key(i);
 		int c = 0;
-		if (ctx_len[i]) {
+		if (ctx.len(i)) {
 			const auto r = resident.find(k);
 			c = r != resident.end() ? r->second : s0 + placed.at(k);
-			if (r == resident.end() && seen.insert(k).second) s += cdiv(ctx_len[i], 8) * 8;
+			if (r == resident.end() && seen.insert(k).second) s += cdiv(ctx.len(i), 8) * 8;
 		}
 		const int t = a.take(max_new[i], 1);
 		if (t < 0) return false;
-		out.push_back(SqPlace{s, ctx_len[i] + len[i] - 1, t, c, ctx_len[i]});
+		out.push_back(SqPlace{s, ctx.len(i) + len[i] - 1, t, c, ctx.len(i)});
 		s += cdiv(len[i] - 1, 8) * 8;
 	}
 	return true;
 }
 
 // The log-probability outputs of calm_b200_decode_sample_queue_logprobs: request i step j writes logprobs[O_i + j] and
-// top_ids / top_logprobs[(O_i + j) * k ..]
+// top_ids / top_logprobs[(O_i + j) * k ..] (off: none, and k is 0)
 struct SqLogprobs {
+	bool on;
 	int k;
 	float* logprobs;
 	int* top_ids;
 	float* top_logprobs;
 };
 
-// a step's tile lists and merged top-k for VF_TOK rows and the largest k, and room for `total` tokens' outputs at k
-static void sq_lp_reserve(size_t total, int k) {
-	const size_t nvt = cdiv(g.cfg.vocab_size, PF_BM);
-	if (!pf.sqtopv) {
-		pf.sqtopv = (float*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(float));
-		pf.sqtopi = (int*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
-		pf.sqtid = (int*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(int));
-		pf.sqtlp = (float*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(float));
-	}
-	if (total > pf.sqlp_cap) { // (no step of an earlier call is still reading them)
-		CUDA_CHECK(cudaStreamSynchronize(g.stream));
-		cudaFree(pf.sqlp);
-		pf.sqlp_cap = total;
-		pf.sqlp = (float*)dev_alloc(total * sizeof(float));
-	}
-	if (total * k > pf.sqtop_cap) {
-		CUDA_CHECK(cudaStreamSynchronize(g.stream));
-		cudaFree(pf.sqoid), cudaFree(pf.sqolp);
-		pf.sqtop_cap = total * k;
-		pf.sqoid = (int*)dev_alloc(pf.sqtop_cap * sizeof(int));
-		pf.sqolp = (float*)dev_alloc(pf.sqtop_cap * sizeof(float));
-	}
+// Queue buffers sharing capacity `cap` regrown to `need` elements, after the stream: no earlier call still reads them
+template <typename... T>
+static void sq_grow(size_t& cap, size_t need, T*&... bufs) {
+	if (need <= cap) return;
+	CUDA_CHECK(cudaStreamSynchronize(g.stream));
+	cap = need;
+	((cudaFree(bufs), bufs = (T*)dev_alloc(need * sizeof(T))), ...);
 }
 
-// A queue step's final norm and short-block classifier with its log-probability epilogue: pf_score's greedy (or, with
-// `sample`, sampled) classifier on the n rows, with k > 0 its TOPK variant writing each tile's top-k lists to pf.sqtopv /
-// pf.sqtopi.  The merge is left to sq_merge, after each row's target is set.  With `pen` (a step with non-neutral rows of
-// calm_b200_decode_sample_queue_penalties) the TOPK variant with PEN runs whatever k is, and processes those rows' logits;
-// with `mask` (a step with a constrained row) its MASK variant also masks them.
+// One launch of a queue step's classifier: MASK (with PEN, TOPK) if `mask`, else PEN (with TOPK) if `pen`, else TOPK if k > 0
+template <int MODE, int DBITS, typename KVT>
+static void sq_gemm(const PfGemmArgs& a, int units, int t0, int k, bool pen, bool mask) {
+	if (mask) vf_gemm<MODE, DBITS, KVT, true, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
+	else if (pen) vf_gemm<MODE, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
+	else if (k) vf_gemm<MODE, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
+	else vf_gemm<MODE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
+}
+
+// A queue step's final norm and short-block classifier: greedy (or, with `sample`, sampled) on the n rows, with k > 0
+// writing each tile's top-k lists to pf.sqtopv / pf.sqtopi, with `pen` (a step with non-neutral rows) processing those
+// rows' logits and with `mask` (a step with a constrained row) also masking them.  The merge is left to the caller.
 template <int DBITS, typename KVT>
-static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample, bool pen = false, bool mask = false) {
+static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample, bool pen, bool mask) {
 	const Config& c = g.cfg;
 	const int nvt = cdiv(c.vocab_size, PF_BM);
 	launch_pdl(k_pf_norm, n, 256, 0, (const float*)pf.X, (const float*)g.w.rms_final_weight, pf.Nhi, pf.Nlo, n, c.dim, c.norm_eps, (int)c.norm_ln);
@@ -2315,17 +2318,8 @@ static void sq_classify(Formats<DBITS, KVT>, int n, int k, bool sample, bool pen
 	a.n_tokens = n, a.w[0] = g.w.wcls, a.K = c.dim;
 	a.targets = pf.targets, a.part = pf.part, a.tgt = pf.tgt, a.vocab = c.vocab_size, a.gidx = pf.gidx;
 	a.topv = pf.sqtopv, a.topi = pf.sqtopi, a.topk = k;
-	for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) {
-		const int units = imin(VF_CLS_UNITS, nvt - t0);
-		if (mask && sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
-		else if (mask) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
-		else if (pen && sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
-		else if (pen) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true, true>(pf.Nhi, pf.Nlo, a, units, t0);
-		else if (sample && k) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
-		else if (sample) vf_gemm<PF_CLS_SAMPLE, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
-		else if (k) vf_gemm<PF_CLS_GREEDY, DBITS, KVT, true>(pf.Nhi, pf.Nlo, a, units, t0);
-		else vf_gemm<PF_CLS_GREEDY, DBITS, KVT>(pf.Nhi, pf.Nlo, a, units, t0);
-	}
+	const auto gemm = sample ? sq_gemm<PF_CLS_SAMPLE, DBITS, KVT> : sq_gemm<PF_CLS_GREEDY, DBITS, KVT>;
+	for (int t0 = 0; t0 < nvt; t0 += VF_CLS_UNITS) gemm(a, imin(VF_CLS_UNITS, nvt - t0), t0, k, pen, mask);
 }
 
 // The merge of a step with log-probabilities: pf_merge's greedy merge (k > 0: with the top-k lists of pf.sqtopv into
@@ -2373,32 +2367,8 @@ static float sq_pen_logit_host(float l, int c, bool seen, float b, float p, floa
 	return a == 0.0f ? l1 : l1 + a;
 }
 
-// The lanes' rows and parameters (first use), and room for the call's n tokens and n_bias bias entries
-static void sq_pen_reserve(int n, int n_bias) {
-	const size_t vocab = g.cfg.vocab_size;
-	if (!pf.sqpcnt) {
-		pf.sqpcnt = (int*)dev_alloc(SQ_ROWS * vocab * sizeof(int));
-		pf.sqpbias = (float*)dev_alloc(SQ_ROWS * vocab * sizeof(float));
-		pf.sqppar = (float4*)dev_alloc(SQ_ROWS * sizeof(float4));
-	}
-	if (!pf.sqlanes) pf.sqlanes = (int*)dev_alloc(2 * SQ_ROWS * sizeof(int));
-	if ((size_t)n > pf.sqptok_cap) { // (no step of an earlier call is still reading them)
-		CUDA_CHECK(cudaStreamSynchronize(g.stream));
-		cudaFree(pf.sqptok);
-		pf.sqptok_cap = n;
-		pf.sqptok = (int*)dev_alloc((size_t)n * sizeof(int));
-	}
-	if ((size_t)n_bias > pf.sqpb_cap) {
-		CUDA_CHECK(cudaStreamSynchronize(g.stream));
-		cudaFree(pf.sqpbid), cudaFree(pf.sqpbval);
-		pf.sqpb_cap = n_bias;
-		pf.sqpbid = (int*)dev_alloc((size_t)n_bias * sizeof(int));
-		pf.sqpbval = (float*)dev_alloc((size_t)n_bias * sizeof(float));
-	}
-}
-
 // The token automaton of calm_b200_decode_sample_queue_constrained (include/calm_b200.h) and each request's start state
-// (start NULL: no request is constrained).  sq_run checks it and fills `fin`, which states are final.
+// (start NULL: no request is constrained).  sq_check checks it and fills `fin`, which states are final.
 struct SqAutomaton {
 	int n_states;
 	const uint32_t* allow;
@@ -2411,6 +2381,7 @@ struct SqAutomaton {
 	int words;             // ceil(vocab / 32): one state's bitmask
 	std::vector<char> fin; // [n_states] no token allowed
 	int s0(int i) const { return start ? start[i] : -1; }
+	bool ends(int s) const { return s >= 0 && fin[s]; } // a token that led to state s ends its request
 	bool allowed(int s, int v) const { return (allow[(size_t)s * words + (v >> 5)] >> (v & 31)) & 1u; }
 	// the state after allowed token v in state s: its exception, else the default.  v comes from the device (or the
 	// fallback's sampler), which never draws a masked token; one that did would be a bug, so it aborts here rather than
@@ -2469,225 +2440,232 @@ struct SqLookup {
 	int* accepted;
 };
 
-// calm_b200_decode_sample_queue_context, and calm_b200_decode_sample_queue with every ctx_len 0 (`who` names the call in
-// error messages): a round's extent goes through the packed prompt pass (sb_prefill), each request's own rows continuing
-// its context at positions ctx_len .. (PF_CONTEXTS where a block holds such rows); a step whose rows have contexts runs
-// k_sn_attn's GROUPS variant, every other step exactly the QUEUE kernels.  With `lp` (calm_b200_decode_sample_queue_logprobs)
-// a step's classifier also runs the TOPK epilogue (k > 0), the merge runs after the sampler with each row's target set to
-// its token (k_sq_tgt), and k_sq_lp stores the results; the tokens are the same bits.  With `pen`
-// (calm_b200_decode_sample_queue_penalties) each non-neutral request holds a lane from admission to retirement, cleared
-// and filled by k_sq_pen_admit; a step with such rows passes their lanes to k_sq_lanes, runs sq_classify's PEN classifier
-// and after k_sq_end k_sq_pen_step, every
-// other step exactly the kernels it runs without `pen`.  With `aut` (calm_b200_decode_sample_queue_constrained, with
-// `pen`) the host follows each constrained request's state from the step's tokens, read back as the stop list's are; a
-// step with a constrained row passes the rows' lanes and states to k_sq_mask_lanes, runs sq_classify's MASK classifier
-// and, when such a row samples, k_sample_scan_rows_masked; every other step exactly the kernels it runs without `aut`.
-// With `lk` and max_draft > 0 (calm_b200_decode_sample_queue_lookup) the rows a step's requests leave free carry drafts:
-// a request's draft rows follow its row, each one more queue row at its own step j + d, fed the draft's d-th token with
-// the request's generator advanced d times and its automaton state advanced through the draft; a step with a draft row
-// ends with k_sq_accept instead of k_sq_end, and every step's tokens and emitted flags are read back, from which the host
-// takes the emitted tokens, the next drafts and each request's next row source.
-static int sq_run(const char* who, struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len, const int* off,
-                  const int* len, int nreq, const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
-                  int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps, int* prompt_rows,
-                  const SqLogprobs* lp = nullptr, const SqPenalties* pen = nullptr, SqAutomaton* aut = nullptr, const SqTrunc* tr = nullptr,
-                  const SqLookup* lk = nullptr) {
+// One queue call: its requests and every option, each option neutral (all-zero) where the entry point has none of it
+struct SqCall {
+	const char* who; // the entry point, in error messages
+	struct Transformer* transformer;
+	const int* tokens;
+	int n;
+	SqContexts ctx;
+	const int *off, *len;
+	int nreq;
+	const int* max_new;
+	const float *temperature, *minp;
+	const int* stop;
+	int n_stop, max_rows;
+	unsigned long long* rng_states;
+	int *out_tokens, *out_len, *steps, *prompt_rows;
+	SqLogprobs lp = {};
+	SqPenalties pen = {};
+	SqAutomaton aut = {};
+	SqTrunc tr = {};
+	SqLookup lk = {};
+	bool greedy(int i) const { return temperature[i] == 0.0f || minp[i] >= 1.0f; } // sample() is greedy there
+	bool truncated(int i) const { return !greedy(i) && (tr.k(i) > 0 || tr.p(i) < 1.0f); } // a sampled request with top-k or top-p
+};
+
+// Abort on a bad argument, before any device work; fills c.aut's words and final states, returns the sum of max_new
+static size_t sq_check(SqCall& c) {
+	const char* who = c.who;
+	const int nreq = c.nreq, n = c.n;
 	if (!g.ready) CALM_FATAL("%s before prepare_cuda", who);
-	if (max_rows < 1 || max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, max_rows, CALM_B200_SAMPLE_N_MAX);
-	if (nreq < 0 || n < 0 || n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, n_stop);
-	if (n_stop > 0 && !stop) CALM_FATAL("%s: stop is NULL", who);
-	if (nreq > 0 && (!tokens || !ctx_off || !ctx_len || !off || !len || !max_new || !temperature || !minp || !rng_states || !out_tokens || !out_len))
+	if (c.max_rows < 1 || c.max_rows > CALM_B200_SAMPLE_N_MAX) CALM_FATAL("%s: max_rows %d outside [1, %d]", who, c.max_rows, CALM_B200_SAMPLE_N_MAX);
+	if (nreq < 0 || n < 0 || c.n_stop < 0) CALM_FATAL("%s: negative nreq %d, n %d or n_stop %d", who, nreq, n, c.n_stop);
+	if (c.n_stop > 0 && !c.stop) CALM_FATAL("%s: stop is NULL", who);
+	if (nreq > 0 && (!c.tokens || c.ctx.missing() || !c.off || !c.len || !c.max_new || !c.temperature || !c.minp || !c.rng_states || !c.out_tokens ||
+	                 !c.out_len))
 		CALM_FATAL("%s: an array is NULL", who);
 	size_t total = 0; // sum of max_new: the output's extent
 	for (int i = 0; i < nreq; ++i) {
-		if (max_new[i] < 0) CALM_FATAL("%s: request %d has a negative max_new %d", who, i, max_new[i]);
-		if (len[i] < 1 || off[i] < 0 || (long)off[i] + len[i] > n) CALM_FATAL("%s: prompt %d (off %d, len %d) empty or outside the %d tokens", who, i, off[i], len[i], n);
-		if (ctx_off[i] < 0 || ctx_len[i] < 0 || (long)ctx_off[i] + ctx_len[i] > n)
-			CALM_FATAL("%s: context of request %d (off %d, len %d) outside the %d tokens", who, i, ctx_off[i], ctx_len[i], n);
-		total += max_new[i];
+		const int mn = c.max_new[i], o = c.off[i], l = c.len[i], co = c.ctx.off(i), cl = c.ctx.len(i);
+		if (mn < 0) CALM_FATAL("%s: request %d has a negative max_new %d", who, i, mn);
+		if (l < 1 || o < 0 || (long)o + l > n) CALM_FATAL("%s: prompt %d (off %d, len %d) empty or outside the %d tokens", who, i, o, l, n);
+		if (co < 0 || cl < 0 || (long)co + cl > n) CALM_FATAL("%s: context of request %d (off %d, len %d) outside the %d tokens", who, i, co, cl, n);
+		total += mn;
 	}
 	if (total > 0x7fffffff) CALM_FATAL("%s: %zu output tokens do not fit an int index", who, total);
-	if (lp) {
-		const int kmax = imin(CALM_B200_TOPK_MAX, g.cfg.vocab_size);
-		if (lp->k < 0 || lp->k > kmax) CALM_FATAL("%s: k %d outside [0, %d]", who, lp->k, kmax);
-		if (total > 0 && !lp->logprobs) CALM_FATAL("%s: logprobs is NULL", who);
-		if (total > 0 && lp->k > 0 && (!lp->top_ids || !lp->top_logprobs)) CALM_FATAL("%s: top_ids or top_logprobs is NULL", who);
+	const SqPenalties& pen = c.pen;
+	const int vocab = g.cfg.vocab_size;
+	if (c.lp.on) {
+		const int kmax = imin(CALM_B200_TOPK_MAX, vocab);
+		if (c.lp.k < 0 || c.lp.k > kmax) CALM_FATAL("%s: k %d outside [0, %d]", who, c.lp.k, kmax);
+		if (total > 0 && !c.lp.logprobs) CALM_FATAL("%s: logprobs is NULL", who);
+		if (total > 0 && c.lp.k > 0 && (!c.lp.top_ids || !c.lp.top_logprobs)) CALM_FATAL("%s: top_ids or top_logprobs is NULL", who);
 	}
-	if (pen) { // bounds that keep every processed logit finite
-		const float big = 1e6f;
-		const int vocab = g.cfg.vocab_size;
-		if (pen->n_bias < 0) CALM_FATAL("%s: negative n_bias %d", who, pen->n_bias);
-		if (!pen->bias_off != !pen->bias_len || (!pen->bias_off && pen->n_bias > 0)) CALM_FATAL("%s: bias_off or bias_len is NULL", who);
-		if (pen->n_bias > 0 && (!pen->bias_ids || !pen->bias_val)) CALM_FATAL("%s: bias_ids or bias_val is NULL", who);
-		std::vector<int> listed(vocab, -1); // the request whose list last named the id
-		for (int i = 0; i < nreq; ++i) {
-			const float p = pen->p(i), f = pen->f(i), r = pen->r(i);
-			if (!std::isfinite(p) || !std::isfinite(f) || !std::isfinite(r) || fabsf(p) > big || fabsf(f) > big || !(r >= 1e-6f && r <= big))
-				CALM_FATAL("%s: request %d's presence %g, frequency %g or repetition %g is not finite or out of bounds", who, i, p, f, r);
-			if (!pen->bias_off) continue;
-			const int bo = pen->bias_off[i], bl = pen->bias_len[i];
-			if (bo < 0 || bl < 0 || (long)bo + bl > pen->n_bias) CALM_FATAL("%s: bias list %d (off %d, len %d) outside the %d entries", who, i, bo, bl, pen->n_bias);
-			for (int e = bo; e < bo + bl; ++e) {
-				const int id = pen->bias_ids[e];
-				const float b = pen->bias_val[e];
-				if (id < 0 || id >= vocab) CALM_FATAL("%s: request %d's bias id %d outside [0, %d)", who, i, id, vocab);
-				if (listed[id] == i) CALM_FATAL("%s: request %d's bias list repeats id %d", who, i, id);
-				if (!std::isfinite(b) || fabsf(b) > big) CALM_FATAL("%s: request %d's bias %g for id %d is not finite or out of bounds", who, i, b, id);
-				listed[id] = i;
-			}
-		}
-	}
-	if (aut) sq_check_automaton(who, *aut, nreq, max_new, g.cfg.vocab_size);
-	auto truncated = [&](int i) { // a sampled request with top-k or top-p (sample() is greedy at T 0 or minp >= 1)
-		return tr && !(temperature[i] == 0.0f || minp[i] >= 1.0f) && (tr->k(i) > 0 || tr->p(i) < 1.0f);
-	};
-	for (int i = 0; tr && i < nreq; ++i) {
-		trunc_check(who, i, tr->k(i), tr->p(i));
-		if (max_new[i] > 0 && truncated(i) && g.cfg.vocab_size > TRUNC_VOCAB_MAX)
-			CALM_FATAL("%s: request %d is truncated, and truncation serves vocabularies up to %d tokens, not %d", who, i, TRUNC_VOCAB_MAX, g.cfg.vocab_size);
-	}
-	if (lk && (lk->max_draft < 0 || lk->max_draft > SQ_ROWS - 1)) CALM_FATAL("%s: max_draft %d outside [0, %d]", who, lk->max_draft, SQ_ROWS - 1);
-	check_tokens(tokens, n);
-	check_tokens(stop, n_stop);
-	if (steps) *steps = 0;
-	if (prompt_rows) *prompt_rows = 0;
-	if (lk && lk->drafted) *lk->drafted = 0;
-	if (lk && lk->accepted) *lk->accepted = 0;
-	std::vector<int> cur(nreq, -1); // a constrained request's automaton state after its tokens so far
-	for (int i = 0; aut && i < nreq; ++i) cur[i] = aut->s0(i);
-	auto ends = [&](int i) { return cur[i] >= 0 && aut->fin[cur[i]]; }; // the request's last token led to a final state
-	std::vector<char> is_stop(g.cfg.vocab_size, 0);
-	for (int k = 0; k < n_stop; ++k) is_stop[stop[k]] = 1;
-	std::vector<size_t> O(nreq + 1, 0); // request i's tokens go to out_tokens[O[i] ..]
-	for (int i = 0; i < nreq; ++i) O[i + 1] = O[i] + max_new[i];
-	for (int i = 0; i < nreq; ++i)
-		if (max_new[i] == 0) out_len[i] = 0; // never admitted
-	if (aut && aut->out_state) std::copy(cur.begin(), cur.end(), aut->out_state); // (each request's final value below)
-	if (total == 0) return 1;
-	auto is_greedy = [&](int i) { return temperature[i] == 0.0f || minp[i] >= 1.0f; }; // sample() is greedy there
-	bool fits = true;
-	int P = 0, chunks = 0;
+	const float big = 1e6f; // bounds that keep every processed logit finite
+	if (pen.n_bias < 0) CALM_FATAL("%s: negative n_bias %d", who, pen.n_bias);
+	if (!pen.bias_off != !pen.bias_len || (!pen.bias_off && pen.n_bias > 0)) CALM_FATAL("%s: bias_off or bias_len is NULL", who);
+	if (pen.n_bias > 0 && (!pen.bias_ids || !pen.bias_val)) CALM_FATAL("%s: bias_ids or bias_val is NULL", who);
+	std::vector<int> listed(pen.bias_off ? vocab : 0, -1); // the request whose list last named the id
 	for (int i = 0; i < nreq; ++i) {
-		if (max_new[i] == 0) continue;
-		const int Rc = cdiv(ctx_len[i], 8) * 8, L = ctx_len[i] + len[i] - 1;
-		fits = fits && (long long)Rc + cdiv(len[i] - 1, 8) * 8 + max_new[i] <= g.cfg.seq_len;
-		P = imin(P + Rc + cdiv(len[i] - 1, 8) * 8, SB_BLOCK), chunks = std::max(chunks, cdiv(L + max_new[i], SN_CHUNK));
-	}
-	if (!pf_supported() || !fits) { // each request alone over ctx ++ prompt: decode_sample's stream, cut at its first stop token
-		for (int i = 0; i < nreq; ++i) {
-			std::vector<int> p(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
-			p.insert(p.end(), tokens + off[i], tokens + off[i] + len[i]);
-			const int L = (int)p.size() - 1;
-			int tok = p[L], k = 0;
-			if (max_new[i] > 0) forward_prefill_cuda(transformer, p.data(), L, 0);
-			const bool processed = pen && !pen->neutral(i), masked = cur[i] >= 0, cut = truncated(i);
-			std::vector<float> logits(lp || processed || masked || cut ? g.cfg.vocab_size : 0);
-			std::vector<int> cnt(processed ? g.cfg.vocab_size : 0);
-			std::vector<float> bias(processed ? g.cfg.vocab_size : 0);
-			std::vector<char> seen(processed ? g.cfg.vocab_size : 0);
-			if (processed) {
-				for (int t : p) seen[t] = 1;
-				for (int e = 0; e < pen->nb(i); ++e) bias[pen->bias_ids[pen->bias_off[i] + e]] = pen->bias_val[pen->bias_off[i] + e];
-			}
-			while (k < max_new[i]) {
-				if (processed || masked || cut) { // the decode path's device logits (its argmax discarded), processed, masked and sampled on the host
-					unsigned long long unused = 1;
-					calm_b200_forward_sample(transformer, tok, L + k, 0.0f, 0.0f, &unused);
-					calm_b200_read_device_logits(logits.data());
-					for (int v = 0; processed && v < g.cfg.vocab_size; ++v)
-						logits[v] = sq_pen_logit_host(logits[v], cnt[v], seen[v] || cnt[v] > 0, bias[v], pen->p(i), pen->f(i), pen->r(i));
-					for (int v = 0; masked && v < g.cfg.vocab_size; ++v)
-						if (!aut->allowed(cur[i], v)) logits[v] = -INFINITY;
-					// (greedy: the first maximum; sampled: through k_sample_scan_rows_masked where the row is masked, after
-					// k_sample_trunc_rows where it is truncated)
-					tok = sample_logits(logits.data(), g.cfg.vocab_size, temperature[i], minp[i], &rng_states[i], nullptr, masked, cut ? tr->k(i) : 0,
-					                    cut ? tr->p(i) : 1.0f);
-					if (processed) ++cnt[tok];
-					if (lp) {
-						const size_t o = O[i] + k;
-						host_logprobs(logits.data(), g.cfg.vocab_size, tok, lp->k, lp->logprobs + o, lp->top_ids + o * lp->k, lp->top_logprobs + o * lp->k);
-						for (size_t e = o * lp->k; masked && e < (o + 1) * lp->k; ++e) // ranks past the allowed tokens
-							if (lp->top_logprobs[e] == -INFINITY) lp->top_ids[e] = -1;
-					}
-					out_tokens[O[i] + k++] = tok;
-					if (masked) cur[i] = aut->next(cur[i], tok);
-					if (is_stop[tok] || ends(i)) break;
-					continue;
-				}
-				tok = calm_b200_forward_sample(transformer, tok, L + k, temperature[i], minp[i], &rng_states[i]);
-				if (lp) { // the step's device logits, through pf_score_one's decode-path log-softmax
-					const size_t o = O[i] + k;
-					calm_b200_read_device_logits(logits.data());
-					host_logprobs(logits.data(), g.cfg.vocab_size, tok, lp->k, lp->logprobs + o, lp->top_ids + o * lp->k, lp->top_logprobs + o * lp->k);
-				}
-				out_tokens[O[i] + k++] = tok;
-				if (is_stop[tok]) break;
-			}
-			out_len[i] = k;
-			if (aut && aut->out_state) aut->out_state[i] = cur[i];
+		const float p = pen.p(i), f = pen.f(i), r = pen.r(i);
+		if (!std::isfinite(p) || !std::isfinite(f) || !std::isfinite(r) || fabsf(p) > big || fabsf(f) > big || !(r >= 1e-6f && r <= big))
+			CALM_FATAL("%s: request %d's presence %g, frequency %g or repetition %g is not finite or out of bounds", who, i, p, f, r);
+		if (!pen.bias_off) continue;
+		const int bo = pen.bias_off[i], bl = pen.bias_len[i];
+		if (bo < 0 || bl < 0 || (long)bo + bl > pen.n_bias) CALM_FATAL("%s: bias list %d (off %d, len %d) outside the %d entries", who, i, bo, bl, pen.n_bias);
+		for (int e = bo; e < bo + bl; ++e) {
+			const int id = pen.bias_ids[e];
+			const float b = pen.bias_val[e];
+			if (id < 0 || id >= vocab) CALM_FATAL("%s: request %d's bias id %d outside [0, %d)", who, i, id, vocab);
+			if (listed[id] == i) CALM_FATAL("%s: request %d's bias list repeats id %d", who, i, id);
+			if (!std::isfinite(b) || fabsf(b) > big) CALM_FATAL("%s: request %d's bias %g for id %d is not finite or out of bounds", who, i, b, id);
+			listed[id] = i;
 		}
-		return 0;
 	}
-	sn_reserve(std::max(P, VF_TOK), chunks);
+	sq_check_automaton(who, c.aut, nreq, c.max_new, vocab);
+	for (int i = 0; i < nreq; ++i) {
+		trunc_check(who, i, c.tr.k(i), c.tr.p(i));
+		if (c.max_new[i] > 0 && c.truncated(i) && vocab > TRUNC_VOCAB_MAX)
+			CALM_FATAL("%s: request %d is truncated, and truncation serves vocabularies up to %d tokens, not %d", who, i, TRUNC_VOCAB_MAX, vocab);
+	}
+	if (c.lk.max_draft < 0 || c.lk.max_draft > SQ_ROWS - 1) CALM_FATAL("%s: max_draft %d outside [0, %d]", who, c.lk.max_draft, SQ_ROWS - 1);
+	check_tokens(c.tokens, n);
+	check_tokens(c.stop, c.n_stop);
+	return total;
+}
+
+// The host path (MoE, tensor parallelism, a request past seq_len): each request alone, decode_sample's stream cut at a stop
+static int sq_fallback(const SqCall& c, std::vector<int>& cur, const std::vector<char>& is_stop, const std::vector<size_t>& O) {
+	for (int i = 0; i < c.nreq; ++i) {
+		std::vector<int> p(c.tokens + c.ctx.off(i), c.tokens + c.ctx.off(i) + c.ctx.len(i));
+		p.insert(p.end(), c.tokens + c.off[i], c.tokens + c.off[i] + c.len[i]);
+		const int L = (int)p.size() - 1;
+		int tok = p[L], k = 0;
+		if (c.max_new[i] > 0) forward_prefill_cuda(c.transformer, p.data(), L, 0);
+		const bool processed = !c.pen.neutral(i), masked = cur[i] >= 0, cut = c.truncated(i);
+		std::vector<float> logits(c.lp.on || processed || masked || cut ? g.cfg.vocab_size : 0);
+		std::vector<int> cnt(processed ? g.cfg.vocab_size : 0);
+		std::vector<float> bias(processed ? g.cfg.vocab_size : 0);
+		std::vector<char> seen(processed ? g.cfg.vocab_size : 0);
+		if (processed) {
+			for (int t : p) seen[t] = 1;
+			for (int e = 0; e < c.pen.nb(i); ++e) bias[c.pen.bias_ids[c.pen.bias_off[i] + e]] = c.pen.bias_val[c.pen.bias_off[i] + e];
+		}
+		while (k < c.max_new[i]) {
+			if (processed || masked || cut) { // the decode path's device logits (its argmax discarded), processed, masked and sampled on the host
+				unsigned long long unused = 1;
+				calm_b200_forward_sample(c.transformer, tok, L + k, 0.0f, 0.0f, &unused);
+				calm_b200_read_device_logits(logits.data());
+				for (int v = 0; processed && v < g.cfg.vocab_size; ++v)
+					logits[v] = sq_pen_logit_host(logits[v], cnt[v], seen[v] || cnt[v] > 0, bias[v], c.pen.p(i), c.pen.f(i), c.pen.r(i));
+				for (int v = 0; masked && v < g.cfg.vocab_size; ++v)
+					if (!c.aut.allowed(cur[i], v)) logits[v] = -INFINITY;
+				// (greedy: the first maximum; sampled: through k_sample_scan_rows_masked where the row is masked, after
+				// k_sample_trunc_rows where it is truncated)
+				tok = sample_logits(logits.data(), g.cfg.vocab_size, c.temperature[i], c.minp[i], &c.rng_states[i], nullptr, masked, cut ? c.tr.k(i) : 0,
+				                    cut ? c.tr.p(i) : 1.0f);
+				if (processed) ++cnt[tok];
+				if (c.lp.on) {
+					const size_t o = O[i] + k;
+					host_logprobs(logits.data(), g.cfg.vocab_size, tok, c.lp.k, c.lp.logprobs + o, c.lp.top_ids + o * c.lp.k, c.lp.top_logprobs + o * c.lp.k);
+					for (size_t e = o * c.lp.k; masked && e < (o + 1) * c.lp.k; ++e) // ranks past the allowed tokens
+						if (c.lp.top_logprobs[e] == -INFINITY) c.lp.top_ids[e] = -1;
+				}
+				c.out_tokens[O[i] + k++] = tok;
+				if (masked) cur[i] = c.aut.next(cur[i], tok);
+				if (is_stop[tok] || c.aut.ends(cur[i])) break;
+				continue;
+			}
+			tok = calm_b200_forward_sample(c.transformer, tok, L + k, c.temperature[i], c.minp[i], &c.rng_states[i]);
+			if (c.lp.on) { // the step's device logits, through pf_score_one's decode-path log-softmax
+				const size_t o = O[i] + k;
+				calm_b200_read_device_logits(logits.data());
+				host_logprobs(logits.data(), g.cfg.vocab_size, tok, c.lp.k, c.lp.logprobs + o, c.lp.top_ids + o * c.lp.k, c.lp.top_logprobs + o * c.lp.k);
+			}
+			c.out_tokens[O[i] + k++] = tok;
+			if (is_stop[tok]) break;
+		}
+		c.out_len[i] = k;
+		if (c.aut.out_state) c.aut.out_state[i] = cur[i];
+	}
+	return 0;
+}
+
+// The device buffers of a call of `total` tokens and its uploads, once per call: the lanes' rows, tokens and bias lists
+// when a request is not neutral, the automaton's bitmasks when one is constrained (cur: each request's start state)
+static void sq_reserve(const SqCall& c, size_t total, const std::vector<int>& cur) {
+	const size_t vocab = g.cfg.vocab_size, nvt = cdiv(g.cfg.vocab_size, PF_BM);
 	if (!pf.sqrows) {
 		pf.sqrows = (SqRows*)dev_alloc(sizeof(SqRows));
 		pf.sqgroups = (SqGroups*)dev_alloc(sizeof(SqGroups));
 		pf.sqtok = (int*)dev_alloc(2 * VF_TOK * sizeof(int));
+		pf.sqlanes = (int*)dev_alloc(2 * SQ_ROWS * sizeof(int));
 	}
-	if (total > pf.sqout_cap || (size_t)nreq > pf.sqst_cap) { // (no step of an earlier call is still reading them)
-		CUDA_CHECK(cudaStreamSynchronize(g.stream));
-		cudaFree(pf.sqout), cudaFree(pf.sqst);
-		pf.sqout_cap = std::max(total, pf.sqout_cap), pf.sqst_cap = std::max((size_t)nreq, pf.sqst_cap);
-		pf.sqout = (int*)dev_alloc(pf.sqout_cap * sizeof(int));
-		pf.sqst = (unsigned long long*)dev_alloc(pf.sqst_cap * sizeof(unsigned long long));
+	sq_grow(pf.sqout_cap, total, pf.sqout);
+	sq_grow(pf.sqst_cap, c.nreq, pf.sqst);
+	if (c.lp.on && !pf.sqtopv) {
+		pf.sqtopv = (float*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(float));
+		pf.sqtopi = (int*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
+		pf.sqtid = (int*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(int));
+		pf.sqtlp = (float*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(float));
 	}
-	if (lp) sq_lp_reserve(total, lp->k);
-	bool any_pen = false; // a request with max_new > 0 is not neutral: the lanes are used
-	for (int i = 0; pen && i < nreq; ++i) any_pen = any_pen || (max_new[i] > 0 && !pen->neutral(i));
-	if (any_pen) { // the call's tokens and bias lists, once
-		sq_pen_reserve(n, pen->n_bias);
-		CUDA_CHECK(cudaMemcpyAsync(pf.sqptok, tokens, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-		if (pen->n_bias) {
-			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbid, pen->bias_ids, (size_t)pen->n_bias * sizeof(int), cudaMemcpyHostToDevice, g.stream));
-			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbval, pen->bias_val, (size_t)pen->n_bias * sizeof(float), cudaMemcpyHostToDevice, g.stream));
+	if (c.lp.on) sq_grow(pf.sqlp_cap, total, pf.sqlp), sq_grow(pf.sqtop_cap, total * c.lp.k, pf.sqoid, pf.sqolp);
+	bool any_pen = false, any_aut = false; // a request with max_new > 0 is not neutral / is constrained
+	for (int i = 0; i < c.nreq; ++i) any_pen = any_pen || (c.max_new[i] > 0 && !c.pen.neutral(i));
+	for (int i = 0; i < c.nreq; ++i) any_aut = any_aut || (c.max_new[i] > 0 && cur[i] >= 0);
+	if (any_pen) {
+		if (!pf.sqpcnt) {
+			pf.sqpcnt = (int*)dev_alloc(SQ_ROWS * vocab * sizeof(int));
+			pf.sqpbias = (float*)dev_alloc(SQ_ROWS * vocab * sizeof(float));
+			pf.sqppar = (float4*)dev_alloc(SQ_ROWS * sizeof(float4));
+		}
+		sq_grow(pf.sqptok_cap, c.n, pf.sqptok);
+		sq_grow(pf.sqpb_cap, c.pen.n_bias, pf.sqpbid, pf.sqpbval);
+		CUDA_CHECK(cudaMemcpyAsync(pf.sqptok, c.tokens, (size_t)c.n * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+		if (c.pen.n_bias) {
+			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbid, c.pen.bias_ids, (size_t)c.pen.n_bias * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+			CUDA_CHECK(cudaMemcpyAsync(pf.sqpbval, c.pen.bias_val, (size_t)c.pen.n_bias * sizeof(float), cudaMemcpyHostToDevice, g.stream));
 		}
 	}
-	bool any_aut = false; // a request with max_new > 0 is constrained: the automaton is uploaded, once
-	for (int i = 0; aut && i < nreq; ++i) any_aut = any_aut || (max_new[i] > 0 && cur[i] >= 0);
 	if (any_aut) {
-		const size_t words = (size_t)aut->n_states * aut->words;
-		if (!pf.sqlanes) pf.sqlanes = (int*)dev_alloc(2 * SQ_ROWS * sizeof(int));
-		if (words > pf.sqallow_cap) { // (no step of an earlier call is still reading it)
-			CUDA_CHECK(cudaStreamSynchronize(g.stream));
-			cudaFree(pf.sqallow);
-			pf.sqallow_cap = words;
-			pf.sqallow = (uint32_t*)dev_alloc(words * sizeof(uint32_t));
-		}
-		CUDA_CHECK(cudaMemcpyAsync(pf.sqallow, aut->allow, words * sizeof(uint32_t), cudaMemcpyHostToDevice, g.stream));
+		const size_t words = (size_t)c.aut.n_states * c.aut.words;
+		sq_grow(pf.sqallow_cap, words, pf.sqallow);
+		CUDA_CHECK(cudaMemcpyAsync(pf.sqallow, c.aut.allow, words * sizeof(uint32_t), cudaMemcpyHostToDevice, g.stream));
 	}
-	std::vector<int> lane_of(nreq, -1); // a non-neutral request's lane while it is in flight
-	const bool drafting = lk && lk->max_draft > 0;
-	std::vector<std::vector<int>> corpus(drafting ? nreq : 0); // (drafting) ctx ++ prompt ++ tokens so far: the lookup's sequence
-	std::vector<unsigned long long> hst(rng_states, rng_states + nreq); // a sampled request's state after its tokens so far
-	int ndrafted = 0, naccepted = 0;
-	unsigned lanes_free = (1u << SQ_ROWS) - 1;
+}
 
-	SqSlots slots(g.cfg.seq_len);
+// One step's tables, as SqLoop::build leaves them for launch and retire
+struct SqStep {
+	SqRows r = {};
+	SqGroups grp = {};
+	SqLanes lanes;          // each row's penalty lane and automaton state
+	TruncRows trows = {};   // the step's truncated rows
+	SqNext nx = {};         // the draft each row's successor is fed, -1 after a request's last row
+	int first[SQ_ROWS + 1]; // live request k's rows are first[k] .. first[k + 1] - 1
+	int ntrunc = 0, nsampled = 0, lmax = 0, nsuf = 0;
+	bool pen = false, mask = false, mask_sampled = false; // a row is a non-neutral request's; a constrained one's; .. that samples
+};
+
+// The step loop of a call that the batched path serves, and what it keeps across steps
+struct SqLoop {
+	const SqCall& c;
+	std::vector<int>& cur; // a constrained request's automaton state after its tokens so far
+	const std::vector<char>& is_stop;
+	const std::vector<size_t>& O;
+	const bool drafting;
+	std::vector<int> lane_of;                 // a non-neutral request's lane while it is in flight
+	std::vector<std::vector<int>> corpus;     // (drafting) ctx ++ prompt ++ tokens so far: the lookup's sequence
+	std::vector<unsigned long long> hst;      // a sampled request's state after its tokens so far
+	unsigned lanes_free = (1u << SQ_ROWS) - 1;
+	SqSlots slots;
 	std::map<SqCtx, int> resident; // contexts in the cache, at their first slot
-	std::vector<SqPlace> place(nreq);
-	std::vector<int> done(nreq, 0), row_of(nreq, -1); // tokens so far; row in the last step
-	std::vector<int> live;                            // requests in flight, in admission order
-	int head = 0, nsteps = 0, last_sampled = 0, rows_computed = 0, tok_host[2 * VF_TOK]; // last_sampled: the last step's rows if it sampled
-	std::vector<int> round;
-	std::vector<SqPlace> rp;
-	int rbase = 0; // the round's prompt extent's first slot
-	// admission: the requests at the head of the queue, in input order, while a row is free and the round's placement
-	// (recomputed with each newcomer, from the slots free before the round) fits
-	auto admit = [&]() {
+	std::vector<int> done, row_of, live; // tokens so far; row in the last step; requests in flight, in admission order
+	std::vector<int> round;              // the requests admitted before this step, their placement rp and its first slot rbase
+	std::vector<SqPlace> place, rp;      // (place: every admitted request's)
+	int rbase = 0, head = 0, nsteps = 0, rows_computed = 0, ndrafted = 0, naccepted = 0;
+	int last_sampled = 0, tok_host[2 * VF_TOK]; // the last step's rows if it sampled; its tokens, read back
+
+	SqLoop(const SqCall& c, std::vector<int>& cur, const std::vector<char>& is_stop, const std::vector<size_t>& O)
+	    : c(c), cur(cur), is_stop(is_stop), O(O), drafting(c.lk.max_draft > 0), lane_of(c.nreq, -1), corpus(drafting ? c.nreq : 0),
+	      hst(c.rng_states, c.rng_states + c.nreq), slots(g.cfg.seq_len), done(c.nreq, 0), row_of(c.nreq, -1), place(c.nreq) {}
+
+	// A round: the requests at the head of the queue, in input order, while a row is free and their placement fits
+	void take_round() {
 		round.clear(), rp.clear();
 		SqSlots after = slots;
-		while (head < nreq && (int)(live.size() + round.size()) < max_rows) {
-			if (max_new[head] == 0) {
+		while (head < c.nreq && (int)(live.size() + round.size()) < c.max_rows) {
+			if (c.max_new[head] == 0) {
 				++head;
 				continue;
 			}
@@ -2696,16 +2674,19 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			SqSlots a = slots;
 			std::vector<SqPlace> tp;
 			int tb;
-			if (!sq_place(a, trial, ctx_off, ctx_len, len, max_new, resident, tp, tb)) break;
+			if (!sq_place(a, trial, c.ctx, c.len, c.max_new, resident, tp, tb)) break;
 			round.swap(trial), rp.swap(tp), after = a, rbase = tb, ++head;
 		}
 		slots = after;
-	};
-	// release: a resident context that no request in flight or of the round names frees its slots
-	auto release = [&]() {
+	}
+
+	// Admission before a step: a round, the resident contexts no request in flight or of the round names released, the
+	// round's prompts through the packed prompt pass and a lane for each non-neutral request of it; false when none is left
+	bool admit() {
+		take_round();
 		std::set<SqCtx> named;
-		for (int i : live) named.insert(SqCtx(ctx_off[i], ctx_len[i]));
-		for (int i : round) named.insert(SqCtx(ctx_off[i], ctx_len[i]));
+		for (int i : live) named.insert(c.ctx.key(i));
+		for (int i : round) named.insert(c.ctx.key(i));
 		for (auto it = resident.begin(); it != resident.end();) {
 			if (named.count(it->first)) {
 				++it;
@@ -2714,231 +2695,271 @@ static int sq_run(const char* who, struct Transformer* transformer, const int* t
 			slots.give(it->second, cdiv(it->first.second, 8) * 8);
 			it = resident.erase(it);
 		}
-	};
-
-	for (;;) {
-		admit();
-		release();
 		if (live.empty() && round.empty()) { // the cache is empty now: the head fits
-			admit();
-			if (round.empty()) break;
+			take_round();
+			if (round.empty()) return false;
 		}
-		if (!round.empty()) {
-			PfPackedBlock pb;
-			for (size_t k = 0; k < round.size(); ++k) {
-				const int i = round[k];
-				const SqPlace& q = rp[k];
-				place[i] = q;
-				const SqCtx key(ctx_off[i], ctx_len[i]);
-				if (q.nc && !resident.count(key)) { // placed by this round, at the extent's next rows
-					resident[key] = q.c;
-					pb.add(tokens + ctx_off[i], q.nc, q.nc - 1, 0, make_int2(0, 0));
-				}
-				pb.add(tokens + off[i], len[i] - 1, len[i] - 1, q.nc, make_int2(q.c, q.nc));
-				if (drafting) {
-					corpus[i].assign(tokens + ctx_off[i], tokens + ctx_off[i] + ctx_len[i]);
-					corpus[i].insert(corpus[i].end(), tokens + off[i], tokens + off[i] + len[i]);
-				}
-				if (pen && !pen->neutral(i)) { // the lowest free lane, cleared and filled for the request
-					const int ln = __builtin_ctz(lanes_free);
-					lanes_free &= ~(1u << ln), lane_of[i] = ln;
-					const SqPenAdmit qa = {ln, ctx_off[i], ctx_len[i], off[i], len[i], pen->bias_off ? pen->bias_off[i] : 0, pen->nb(i),
-					                       make_float4(pen->p(i), pen->f(i), pen->r(i), 0.0f)};
-					launch_pdl(k_sq_pen_admit, cdiv(g.cfg.vocab_size, SQ_PEN_SPAN), 256, 0, qa, (const int*)pf.sqptok, (const int*)pf.sqpbid,
-					           (const float*)pf.sqpbval, g.cfg.vocab_size, pf.sqpcnt, pf.sqpbias, pf.sqppar);
-				}
+		if (round.empty()) return true;
+		PfPackedBlock pb;
+		for (size_t k = 0; k < round.size(); ++k) {
+			const int i = round[k];
+			const SqPlace& q = rp[k];
+			place[i] = q;
+			const SqCtx key = c.ctx.key(i);
+			if (q.nc && !resident.count(key)) { // placed by this round, at the extent's next rows
+				resident[key] = q.c;
+				pb.add(c.tokens + c.ctx.off(i), q.nc, q.nc - 1, 0, make_int2(0, 0));
 			}
-			if (pb.rows()) sb_prefill(pb, rbase);
-			rows_computed += pb.rows();
-			live.insert(live.end(), round.begin(), round.end());
+			pb.add(c.tokens + c.off[i], c.len[i] - 1, c.len[i] - 1, q.nc, make_int2(q.c, q.nc));
+			if (drafting) {
+				corpus[i].assign(c.tokens + c.ctx.off(i), c.tokens + c.ctx.off(i) + c.ctx.len(i));
+				corpus[i].insert(corpus[i].end(), c.tokens + c.off[i], c.tokens + c.off[i] + c.len[i]);
+			}
+			if (!c.pen.neutral(i)) { // the lowest free lane
+				const int ln = __builtin_ctz(lanes_free);
+				lanes_free &= ~(1u << ln), lane_of[i] = ln;
+				const SqPenAdmit qa = {ln, c.ctx.off(i), c.ctx.len(i), c.off[i], c.len[i], c.pen.bias_off ? c.pen.bias_off[i] : 0,
+				                       c.pen.nb(i), make_float4(c.pen.p(i), c.pen.f(i), c.pen.r(i), 0.0f)};
+				launch_pdl(k_sq_pen_admit, cdiv(g.cfg.vocab_size, SQ_PEN_SPAN), 256, 0, qa, (const int*)pf.sqptok, (const int*)pf.sqpbid,
+				           (const float*)pf.sqpbval, g.cfg.vocab_size, pf.sqpcnt, pf.sqpbias, pf.sqppar);
+			}
 		}
-		// the step: the rows in flight, in admission order, each request's draft rows after its row
-		SqRows r = {};
-		SqGroups grp = {};
-		SqLanes lanes;
-		SqMaskLanes ml;
-		bool pen_step = false;     // a row of the step is a non-neutral request's
-		bool mask_step = false;    // a row of the step is a constrained request's
-		bool mask_sampled = false; // .. that samples
-		TruncRows trows = {};      // the step's truncated rows
-		int ntrunc = 0;
+		if (pb.rows()) sb_prefill(pb, rbase);
+		rows_computed += pb.rows();
+		live.insert(live.end(), round.begin(), round.end());
+		return true;
+	}
+
+	// The step's rows in flight in admission order, each request's draft rows after its row in the rows left free: draft row
+	// d at step j + d, fed the draft's d-th token, the generator advanced d times and the state advanced through the draft
+	SqStep build() {
+		SqStep s;
+		SqRows& r = s.r;
 		const int nlive = (int)live.size();
-		int nsampled = 0, lmax = 0, nsuf = 0, nfree = SQ_ROWS - nlive; // nfree: rows left for drafts
-		int first[SQ_ROWS + 1]; // request k's rows are first[k] .. first[k + 1] - 1
-		SqNext nx = {};         // the draft each row's successor is fed, -1 after a request's last row
+		int nfree = SQ_ROWS - nlive;            // rows left for drafts
 		std::map<int, std::vector<int>> groups; // rows by their context's first slot
 		std::vector<int> gorder;                // group slots in order of their first row
 		for (int k = 0; k < nlive; ++k) {
 			const int i = live[k], j = done[i];
 			const SqPlace& q = place[i];
-			const bool gr = is_greedy(i);
+			const bool gr = c.greedy(i);
 			int draft[SQ_ROWS], sd[SQ_ROWS]; // the draft, and a constrained request's state before each of its rows
 			int nd = 0;
 			sd[0] = cur[i];
-			if (drafting && !(pen && !pen->neutral(i))) {
-				nd = vf_lookup(corpus[i], nullptr, 0, imin(imin(lk->max_draft, max_new[i] - j - 1), nfree), draft);
+			if (drafting && c.pen.neutral(i)) {
+				nd = vf_lookup(corpus[i], nullptr, 0, imin(imin(c.lk.max_draft, c.max_new[i] - j - 1), nfree), draft);
 				// no draft row follows its request's end: the draft stops before a stop token, a token the state disallows
 				// and a token that leads to a final state
 				for (int d = 0; d < nd; ++d) {
 					const int v = draft[d];
-					if (is_stop[v] || (sd[d] >= 0 && (!aut->allowed(sd[d], v) || aut->fin[aut->next(sd[d], v)]))) {
+					if (is_stop[v] || (sd[d] >= 0 && (!c.aut.allowed(sd[d], v) || c.aut.fin[c.aut.next(sd[d], v)]))) {
 						nd = d;
 						break;
 					}
-					sd[d + 1] = sd[d] >= 0 ? aut->next(sd[d], v) : -1;
+					sd[d + 1] = sd[d] >= 0 ? c.aut.next(sd[d], v) : -1;
 				}
 				nfree -= nd;
 			}
-			first[k] = r.n;
-			unsigned long long s = hst[i]; // row d draws the coin after the d coins before it
-			for (int d = 0; d <= nd; ++d, s = xorshift_step(s)) {
+			s.first[k] = r.n;
+			unsigned long long st = hst[i]; // row d draws the coin after the d coins before it
+			for (int d = 0; d <= nd; ++d, st = xorshift_step(st)) {
 				const int b = r.n++;
 				r.q[b] = make_int4(q.s, q.L, q.t, j + d), r.pos[b] = q.L + j + d, r.slot[b] = q.t + j + d;
-				r.src[b] = d ? -1 : row_of[i], r.tok0[b] = d ? draft[d - 1] : tokens[off[i] + len[i] - 1];
+				r.src[b] = d ? -1 : row_of[i], r.tok0[b] = d ? draft[d - 1] : c.tokens[c.off[i] + c.len[i] - 1];
 				// (a greedy row's sampler state is never read back: any valid one will do)
-				r.st0[b].rng = gr ? 1 : d ? s : rng_states[i], r.st0[b].temperature = gr ? 1.0f : temperature[i];
-				r.st0[b].cut_delta = gr ? 0.0f : logf(minp[i]) * temperature[i];
+				r.st0[b].rng = gr ? 1 : d ? st : c.rng_states[i], r.st0[b].temperature = gr ? 1.0f : c.temperature[i];
+				r.st0[b].cut_delta = gr ? 0.0f : logf(c.minp[i]) * c.temperature[i];
 				r.out[b] = (int)(O[i] + j + d), r.req[b] = i, r.greedy[b] = gr;
-				lanes.lane[b] = lane_of[i], pen_step = pen_step || lane_of[i] >= 0;
-				ml.lane[b] = lane_of[i], ml.state[b] = sd[d], mask_step = mask_step || sd[d] >= 0, mask_sampled = mask_sampled || (sd[d] >= 0 && !gr);
-				if (truncated(i)) trows.row[ntrunc] = b, trows.top_k[ntrunc] = tr->k(i), trows.top_p[ntrunc++] = tr->p(i);
-				nsampled += !gr, lmax = std::max(lmax, q.L + j + d);
-				grp.ctx[b] = make_int2(q.c, q.nc);
-				nsuf = std::max(nsuf, cdiv(q.L + j + d + 1, SN_CHUNK) - q.nc / SN_CHUNK);
+				s.lanes.lane[b] = lane_of[i], s.lanes.state[b] = sd[d];
+				s.pen = s.pen || lane_of[i] >= 0, s.mask = s.mask || sd[d] >= 0, s.mask_sampled = s.mask_sampled || (sd[d] >= 0 && !gr);
+				if (c.truncated(i)) s.trows.row[s.ntrunc] = b, s.trows.top_k[s.ntrunc] = c.tr.k(i), s.trows.top_p[s.ntrunc++] = c.tr.p(i);
+				s.nsampled += !gr, s.lmax = std::max(s.lmax, q.L + j + d);
+				s.grp.ctx[b] = make_int2(q.c, q.nc);
+				s.nsuf = std::max(s.nsuf, cdiv(q.L + j + d + 1, SN_CHUNK) - q.nc / SN_CHUNK);
 				if (q.nc) {
 					if (!groups.count(q.c)) gorder.push_back(q.c);
 					groups[q.c].push_back(b);
 				}
-				nx.tok[b] = d < nd ? draft[d] : -1;
+				s.nx.tok[b] = d < nd ? draft[d] : -1;
 			}
 		}
-		first[nlive] = r.n;
-		const bool draft_step = r.n > nlive;
-		std::fill(lanes.lane + r.n, lanes.lane + SQ_ROWS, -1);
-		std::fill(ml.lane + r.n, ml.lane + SQ_ROWS, -1), std::fill(ml.state + r.n, ml.state + SQ_ROWS, -1);
-		launch_pdl(k_sq_begin, 1, 32, 0, r, pf.sqrows, (const int*)pf.sqtok, pf.tokens, pf.vstate);
-		if (mask_step) launch_pdl(k_sq_mask_lanes, 1, 32, 0, ml, pf.sqlanes);
-		else if (pen_step) launch_pdl(k_sq_lanes, 1, 32, 0, lanes, pf.sqlanes);
-		PfSampleStep ss = {0, 0, r.n, lmax};
-		if (!gorder.empty()) { // rows with contexts: the groups table, and the GROUPS attention
-			for (int c : gorder) {
-				const std::vector<int>& rows = groups[c];
-				grp.first[grp.ng + 1] = grp.first[grp.ng] + (int)rows.size();
-				grp.chunk0[grp.ng + 1] = grp.chunk0[grp.ng] + grp.ctx[rows[0]].y / SN_CHUNK;
-				std::copy(rows.begin(), rows.end(), grp.rows + grp.first[grp.ng]);
-				++grp.ng;
-			}
-			launch_pdl(k_sq_groups, 1, 32, 0, grp, pf.sqgroups);
-			ss.nshared = grp.chunk0[grp.ng], ss.nsuf = nsuf;
+		s.first[nlive] = r.n;
+		std::fill(s.lanes.lane + r.n, s.lanes.lane + SQ_ROWS, -1), std::fill(s.lanes.state + r.n, s.lanes.state + SQ_ROWS, -1);
+		SqGroups& grp = s.grp; // rows with contexts: the groups table of the GROUPS attention
+		for (int cs : gorder) {
+			const std::vector<int>& rows = groups[cs];
+			grp.first[grp.ng + 1] = grp.first[grp.ng] + (int)rows.size();
+			grp.chunk0[grp.ng + 1] = grp.chunk0[grp.ng] + grp.ctx[rows[0]].y / SN_CHUNK;
+			std::copy(rows.begin(), rows.end(), grp.rows + grp.first[grp.ng]);
+			++grp.ng;
+		}
+		return s;
+	}
+
+	// The step's kernels: its tables, the pass over its rows, the classifier and the sampler, and its tokens' stores
+	void launch(const SqStep& s) {
+		launch_pdl(k_sq_begin, 1, 32, 0, s.r, pf.sqrows, (const int*)pf.sqtok, pf.tokens, pf.vstate);
+		if (s.pen || s.mask) launch_pdl(k_sq_lanes, 1, 32, 0, s.lanes, pf.sqlanes);
+		PfSampleStep ss = {0, 0, s.r.n, s.lmax};
+		if (s.grp.ng) {
+			launch_pdl(k_sq_groups, 1, 32, 0, s.grp, pf.sqgroups);
+			ss.nshared = s.grp.chunk0[s.grp.ng], ss.nsuf = s.nsuf;
 		}
 		with_formats([&](auto f) {
-			pf_run(f, r.n, 0, PF_QUEUE, &ss);
-			if (lp || pen_step || mask_step) sq_classify(f, r.n, lp ? lp->k : 0, nsampled > 0, pen_step || mask_step, mask_step);
-			else pf_score(f, r.n, PF_QUEUE, true, 0, nsampled > 0);
+			pf_run(f, s.r.n, 0, PF_QUEUE, &ss);
+			sq_classify(f, s.r.n, c.lp.k, s.nsampled > 0, s.pen || s.mask, s.mask);
 		});
-		if (lp) { // the sampler, then every row's target and the merge, whose argmax is the greedy rows' token as above
-			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled, ntrunc ? &trows : nullptr, ntrunc);
-			launch_pdl(k_sq_tgt, r.n, 32, 0, (const SqRows*)pf.sqrows, (const float2*)pf.part, cdiv(g.cfg.vocab_size, PF_BM), (const float*)pf.vlogits,
+		if (c.lp.on) { // the sampler, then every row's target and the merge, whose argmax is the greedy rows' token
+			if (s.nsampled > 0) vf_sample_rows(s.r.n, nullptr, s.mask_sampled, s.ntrunc ? &s.trows : nullptr, s.ntrunc);
+			launch_pdl(k_sq_tgt, s.r.n, 32, 0, (const SqRows*)pf.sqrows, (const float2*)pf.part, cdiv(g.cfg.vocab_size, PF_BM), (const float*)pf.vlogits,
 			           g.cfg.vocab_size, (const int*)pf.vsampled, pf.tgt);
-			sq_merge(r.n, lp->k);
+			sq_merge(s.r.n, c.lp.k);
 		} else {
-			if ((pen_step || mask_step) && nsampled == 0) pf_merge(r.n, true, 0); // pf_score's merge, which sq_classify leaves out
-			if (nsampled > 0 && nsampled < r.n) pf_merge(r.n, true, 0); // the greedy rows' argmax from the sampled classifier's records
-			if (nsampled > 0) vf_sample_rows(r.n, nullptr, mask_sampled, ntrunc ? &trows : nullptr, ntrunc);
+			if (s.nsampled < s.r.n) pf_merge(s.r.n, true, 0); // the greedy rows' argmax
+			if (s.nsampled > 0) vf_sample_rows(s.r.n, nullptr, s.mask_sampled, s.ntrunc ? &s.trows : nullptr, s.ntrunc);
 		}
-		if (draft_step)
-			launch_pdl(k_sq_accept, 1, 32, 0, (const SqRows*)pf.sqrows, nx, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate,
+		if (s.r.n > (int)live.size()) // a step with draft rows
+			launch_pdl(k_sq_accept, 1, 32, 0, (const SqRows*)pf.sqrows, s.nx, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate,
 			           pf.sqtok, pf.sqtok + VF_TOK, pf.sqout, pf.sqst);
 		else
 			launch_pdl(k_sq_end, 1, 32, 0, (const SqRows*)pf.sqrows, (const int*)pf.greedy, (const int*)pf.vsampled, (const SampleState*)pf.vstate, pf.sqtok, pf.sqout, pf.sqst);
-		if (lp)
-			launch_pdl(k_sq_lp, 1, 32, 0, (const SqRows*)pf.sqrows, (const float*)pf.logprob, (const int*)pf.sqtid, (const float*)pf.sqtlp, lp->k, pf.sqlp,
+		if (c.lp.on)
+			launch_pdl(k_sq_lp, 1, 32, 0, (const SqRows*)pf.sqrows, (const float*)pf.logprob, (const int*)pf.sqtid, (const float*)pf.sqtlp, c.lp.k, pf.sqlp,
 			           pf.sqoid, pf.sqolp);
-		if (pen_step) launch_pdl(k_sq_pen_step, 1, 32, 0, (const int*)pf.sqlanes, (const int*)pf.sqtok, g.cfg.vocab_size, pf.sqpcnt);
-		++nsteps, last_sampled = nsampled > 0 ? r.n : 0;
-		// the step's tokens decide which rows stop, the constrained rows' next states and the next drafts; with drafts, one
-		// copy also brings the emitted flags
-		if (n_stop || mask_step || drafting) {
-			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, (drafting ? 2 * VF_TOK : r.n) * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+		if (s.pen) launch_pdl(k_sq_pen_step, 1, 32, 0, (const int*)pf.sqlanes, (const int*)pf.sqtok, g.cfg.vocab_size, pf.sqpcnt);
+		++nsteps, last_sampled = s.nsampled > 0 ? s.r.n : 0;
+	}
+
+	// The step's tokens, read back where they decide stops, the constrained rows' states or the next drafts (with drafts, the
+	// emitted flags too), advance each request; one that ends frees its own slots and lane, the others keep their order
+	void retire(const SqStep& s) {
+		if (c.n_stop || s.mask || drafting) {
+			CUDA_CHECK(cudaMemcpyAsync(tok_host, pf.sqtok, (drafting ? 2 * VF_TOK : s.r.n) * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
 			sync_stream();
 		}
-		// retire: requests that reached max_new or emitted a stop token free their own slots; the others keep their order
 		std::vector<int> keep;
-		for (int k = 0; k < nlive; ++k) {
-			const int i = live[k], f = first[k], nr = first[k + 1] - f;
+		for (int k = 0; k < (int)live.size(); ++k) {
+			const int i = live[k], f = s.first[k], nr = s.first[k + 1] - f;
 			int a = 0; // accepted drafts: the request emits its rows 0 .. a
-			while (a < nr - 1 && tok_host[f + a] == nx.tok[f + a]) ++a;
+			while (a < nr - 1 && tok_host[f + a] == s.nx.tok[f + a]) ++a;
 			for (int d = 1; d < nr; ++d)
-				if (tok_host[VF_TOK + f + d] != (d <= a)) CALM_FATAL("%s: row %d's emitted flag disagrees with the step's tokens", who, f + d);
+				if (tok_host[VF_TOK + f + d] != (d <= a)) CALM_FATAL("%s: row %d's emitted flag disagrees with the step's tokens", c.who, f + d);
 			ndrafted += nr - 1, naccepted += a;
 			for (int d = 0; d <= a; ++d) {
 				++done[i];
-				if (cur[i] >= 0) cur[i] = aut->next(cur[i], tok_host[f + d]);
+				if (cur[i] >= 0) cur[i] = c.aut.next(cur[i], tok_host[f + d]);
 				if (drafting) corpus[i].push_back(tok_host[f + d]);
-				if (!is_greedy(i)) hst[i] = xorshift_step(hst[i]);
+				if (!c.greedy(i)) hst[i] = xorshift_step(hst[i]);
 			}
 			row_of[i] = f + a;
-			if (done[i] < max_new[i] && !(n_stop && is_stop[tok_host[f + a]]) && !ends(i)) {
+			if (done[i] < c.max_new[i] && !(c.n_stop && is_stop[tok_host[f + a]]) && !c.aut.ends(cur[i])) {
 				keep.push_back(i);
 				continue;
 			}
-			out_len[i] = done[i];
-			slots.give(place[i].s, cdiv(len[i] - 1, 8) * 8), slots.give(place[i].t, max_new[i]);
+			c.out_len[i] = done[i];
+			slots.give(place[i].s, cdiv(c.len[i] - 1, 8) * 8), slots.give(place[i].t, c.max_new[i]);
 			if (lane_of[i] >= 0) lanes_free |= 1u << lane_of[i], lane_of[i] = -1;
-			if (aut && aut->out_state) aut->out_state[i] = cur[i];
+			if (c.aut.out_state) c.aut.out_state[i] = cur[i];
 		}
 		live.swap(keep);
 	}
-	std::vector<int> all(total);
-	std::vector<unsigned long long> st(nreq);
-	CUDA_CHECK(cudaMemcpyAsync(all.data(), pf.sqout, total * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-	CUDA_CHECK(cudaMemcpyAsync(st.data(), pf.sqst, nreq * sizeof(unsigned long long), cudaMemcpyDeviceToHost, g.stream));
-	const size_t k = lp ? lp->k : 0;
-	std::vector<float> lps(lp ? total : 0), tlp(total * k);
-	std::vector<int> tid(total * k);
-	if (lp) {
-		CUDA_CHECK(cudaMemcpyAsync(lps.data(), pf.sqlp, total * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
-		if (k) {
-			CUDA_CHECK(cudaMemcpyAsync(tid.data(), pf.sqoid, total * k * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-			CUDA_CHECK(cudaMemcpyAsync(tlp.data(), pf.sqolp, total * k * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+
+	// Every request's tokens, final generator state and log-probabilities, copied out, and the call's counts
+	void finish(size_t total) {
+		std::vector<int> all(total);
+		std::vector<unsigned long long> st(c.nreq);
+		CUDA_CHECK(cudaMemcpyAsync(all.data(), pf.sqout, total * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+		CUDA_CHECK(cudaMemcpyAsync(st.data(), pf.sqst, c.nreq * sizeof(unsigned long long), cudaMemcpyDeviceToHost, g.stream));
+		const size_t k = c.lp.k;
+		std::vector<float> lps(c.lp.on ? total : 0), tlp(total * k);
+		std::vector<int> tid(total * k);
+		if (c.lp.on) {
+			CUDA_CHECK(cudaMemcpyAsync(lps.data(), pf.sqlp, total * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+			if (k) {
+				CUDA_CHECK(cudaMemcpyAsync(tid.data(), pf.sqoid, total * k * sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+				CUDA_CHECK(cudaMemcpyAsync(tlp.data(), pf.sqolp, total * k * sizeof(float), cudaMemcpyDeviceToHost, g.stream));
+			}
 		}
-	}
-	sync_stream();
-	CUDA_CHECK(cudaGetLastError());
-	for (int i = 0; i < nreq; ++i) {
-		std::copy(all.begin() + O[i], all.begin() + O[i] + out_len[i], out_tokens + O[i]);
-		if (out_len[i] > 0 && !is_greedy(i)) rng_states[i] = st[i];
-		if (lp) { // (slots past out_len[i] are left untouched)
-			std::copy(lps.begin() + O[i], lps.begin() + O[i] + out_len[i], lp->logprobs + O[i]);
-			std::copy(tid.begin() + O[i] * k, tid.begin() + (O[i] + out_len[i]) * k, lp->top_ids + O[i] * k);
-			std::copy(tlp.begin() + O[i] * k, tlp.begin() + (O[i] + out_len[i]) * k, lp->top_logprobs + O[i] * k);
-			if (aut && aut->s0(i) >= 0) // the merge's entry past a list's allowed tokens is (-inf, INT_MAX): id -1 there
-				for (size_t e = O[i] * k; e < (O[i] + out_len[i]) * k; ++e)
-					if (lp->top_ids[e] == INT_MAX) lp->top_ids[e] = -1;
+		sync_stream();
+		CUDA_CHECK(cudaGetLastError());
+		for (int i = 0; i < c.nreq; ++i) {
+			const size_t o = O[i], e = O[i] + c.out_len[i];
+			std::copy(all.begin() + o, all.begin() + e, c.out_tokens + o);
+			if (c.out_len[i] > 0 && !c.greedy(i)) c.rng_states[i] = st[i];
+			if (c.lp.on) { // (slots past out_len[i] are left untouched)
+				std::copy(lps.begin() + o, lps.begin() + e, c.lp.logprobs + o);
+				std::copy(tid.begin() + o * k, tid.begin() + e * k, c.lp.top_ids + o * k);
+				std::copy(tlp.begin() + o * k, tlp.begin() + e * k, c.lp.top_logprobs + o * k);
+				if (c.aut.s0(i) >= 0) // the merge's entry past a list's allowed tokens is (-inf, INT_MAX): id -1 there
+					for (size_t x = o * k; x < e * k; ++x)
+						if (c.lp.top_ids[x] == INT_MAX) c.lp.top_ids[x] = -1;
+			}
 		}
+		if (last_sampled) pf.vrows = last_sampled;
+		if (c.steps) *c.steps = nsteps;
+		if (c.prompt_rows) *c.prompt_rows = rows_computed;
+		if (c.lk.drafted) *c.lk.drafted = ndrafted;
+		if (c.lk.accepted) *c.lk.accepted = naccepted;
 	}
-	if (last_sampled) pf.vrows = last_sampled;
-	if (steps) *steps = nsteps;
-	if (prompt_rows) *prompt_rows = rows_computed;
-	if (lk && lk->drafted) *lk->drafted = ndrafted;
-	if (lk && lk->accepted) *lk->accepted = naccepted;
+};
+
+// Every queue call, after its checks, either on the per-request fallback or as a loop of admit -> build -> launch ->
+// retire.  Admission runs each round's extent through the packed prompt pass (sb_prefill), each request's own rows
+// continuing its context at positions ctx_len ...  A step is one short block over the rows in flight (PF_QUEUE), with
+// k_sn_attn's GROUPS variant where rows have contexts; with log-probabilities the TOPK epilogue (k > 0), and the merge
+// after the sampler with each row's target set to its token (k_sq_tgt); the PEN classifier where a row is not neutral
+// (its lane held from k_sq_pen_admit to retirement, counted by k_sq_pen_step) and MASK where one is constrained, their
+// lanes and states kept by k_sq_lanes; the masked and truncating samplers where such rows sample; and k_sq_accept in
+// place of k_sq_end where draft rows run.  A step without such rows launches what it would without those options.
+static int sq_run(SqCall c) {
+	const size_t total = sq_check(c);
+	if (c.steps) *c.steps = 0;
+	if (c.prompt_rows) *c.prompt_rows = 0;
+	if (c.lk.drafted) *c.lk.drafted = 0;
+	if (c.lk.accepted) *c.lk.accepted = 0;
+	std::vector<int> cur(c.nreq); // a constrained request's automaton state after its tokens so far (-1: unconstrained)
+	for (int i = 0; i < c.nreq; ++i) cur[i] = c.aut.s0(i);
+	std::vector<char> is_stop(g.cfg.vocab_size, 0);
+	for (int k = 0; k < c.n_stop; ++k) is_stop[c.stop[k]] = 1;
+	std::vector<size_t> O(c.nreq + 1, 0); // request i's tokens go to out_tokens[O[i] ..]
+	for (int i = 0; i < c.nreq; ++i) O[i + 1] = O[i] + c.max_new[i];
+	for (int i = 0; i < c.nreq; ++i)
+		if (c.max_new[i] == 0) c.out_len[i] = 0; // never admitted
+	if (c.aut.out_state) std::copy(cur.begin(), cur.end(), c.aut.out_state); // (each request's final value below)
+	if (total == 0) return 1;
+	bool fits = true;
+	int P = 0, chunks = 0;
+	for (int i = 0; i < c.nreq; ++i) {
+		if (c.max_new[i] == 0) continue;
+		const int Rc = cdiv(c.ctx.len(i), 8) * 8, L = c.ctx.len(i) + c.len[i] - 1;
+		fits = fits && (long long)Rc + cdiv(c.len[i] - 1, 8) * 8 + c.max_new[i] <= g.cfg.seq_len;
+		P = imin(P + Rc + cdiv(c.len[i] - 1, 8) * 8, SB_BLOCK), chunks = std::max(chunks, cdiv(L + c.max_new[i], SN_CHUNK));
+	}
+	if (!pf_supported() || !fits) return sq_fallback(c, cur, is_stop, O);
+	sn_reserve(std::max(P, VF_TOK), chunks);
+	sq_reserve(c, total, cur);
+	SqLoop q(c, cur, is_stop, O);
+	while (q.admit()) {
+		const SqStep s = q.build();
+		q.launch(s), q.retire(s);
+	}
+	q.finish(total);
 	return 1;
 }
 
 extern "C" int calm_b200_decode_sample_queue(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nreq,
                                              const int* max_new, const float* temperature, const float* minp, const int* stop, int n_stop,
                                              int max_rows, unsigned long long* rng_states, int* out_tokens, int* out_len, int* steps) {
-	const std::vector<int> empty(nreq > 0 ? nreq : 0);
-	return sq_run("decode_sample_queue", transformer, tokens, n, empty.data(), empty.data(), off, len, nreq, max_new, temperature, minp, stop, n_stop,
-	              max_rows, rng_states, out_tokens, out_len, steps, nullptr);
+	return sq_run({"decode_sample_queue", transformer, tokens, n, {nullptr, nullptr}, off, len, nreq, max_new, temperature, minp, stop, n_stop, max_rows,
+	                rng_states, out_tokens, out_len, steps, nullptr});
 }
 
 extern "C" int calm_b200_decode_sample_queue_context(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
                                                      const int* off, const int* len, int nreq, const int* max_new, const float* temperature,
                                                      const float* minp, const int* stop, int n_stop, int max_rows, unsigned long long* rng_states,
                                                      int* out_tokens, int* out_len, int* steps, int* prompt_rows) {
-	return sq_run("decode_sample_queue_context", transformer, tokens, n, ctx_off, ctx_len, off, len, nreq, max_new, temperature, minp, stop, n_stop,
-	              max_rows, rng_states, out_tokens, out_len, steps, prompt_rows);
+	return sq_run({"decode_sample_queue_context", transformer, tokens, n, {ctx_off, ctx_len, true}, off, len, nreq, max_new, temperature, minp, stop,
+	                n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows});
 }
 
 extern "C" int calm_b200_decode_sample_queue_logprobs(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
@@ -2946,11 +2967,8 @@ extern "C" int calm_b200_decode_sample_queue_logprobs(struct Transformer* transf
                                                       const float* minp, const int* stop, int n_stop, int max_rows, unsigned long long* rng_states,
                                                       int* out_tokens, int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
                                                       float* top_logprobs) {
-	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
-	const bool none = !ctx_off && !ctx_len;
-	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
-	return sq_run("decode_sample_queue_logprobs", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
-	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, &lp);
+	return sq_run({"decode_sample_queue_logprobs", transformer, tokens, n, {ctx_off, ctx_len}, off, len, nreq, max_new, temperature, minp, stop, n_stop,
+	                max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, {true, k, logprobs, top_ids, top_logprobs}});
 }
 
 extern "C" int calm_b200_decode_sample_queue_penalties(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
@@ -2960,13 +2978,9 @@ extern "C" int calm_b200_decode_sample_queue_penalties(struct Transformer* trans
                                                        const int* stop, int n_stop, int max_rows, unsigned long long* rng_states, int* out_tokens,
                                                        int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
                                                        float* top_logprobs) {
-	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
-	const bool none = !ctx_off && !ctx_len;
-	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
-	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
-	return sq_run("decode_sample_queue_penalties", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
-	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
-	              logprobs || k ? &lp : nullptr, &pen);
+	return sq_run({"decode_sample_queue_penalties", transformer, tokens, n, {ctx_off, ctx_len}, off, len, nreq, max_new, temperature, minp, stop, n_stop,
+	                max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, {logprobs || k, k, logprobs, top_ids, top_logprobs},
+	                {presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias}});
 }
 
 extern "C" int calm_b200_decode_sample_queue_constrained(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
@@ -2977,14 +2991,10 @@ extern "C" int calm_b200_decode_sample_queue_constrained(struct Transformer* tra
                                                          int* out_len, int* steps, int* prompt_rows, int k, float* logprobs, int* top_ids,
                                                          float* top_logprobs, int n_states, const uint32_t* allow, const int* next_default,
                                                          const int* exc_off, const int* exc_tok, const int* exc_next, const int* start, int* out_state) {
-	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
-	const bool none = !ctx_off && !ctx_len;
-	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
-	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
-	SqAutomaton aut{n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state, 0, {}};
-	return sq_run("decode_sample_queue_constrained", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len,
-	              nreq, max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
-	              logprobs || k ? &lp : nullptr, &pen, &aut);
+	return sq_run({"decode_sample_queue_constrained", transformer, tokens, n, {ctx_off, ctx_len}, off, len, nreq, max_new, temperature, minp, stop, n_stop,
+	                max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, {logprobs || k, k, logprobs, top_ids, top_logprobs},
+	                {presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias},
+	                {n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state}});
 }
 
 extern "C" int calm_b200_decode_sample_queue_truncated(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
@@ -2996,15 +3006,10 @@ extern "C" int calm_b200_decode_sample_queue_truncated(struct Transformer* trans
                                                        float* top_logprobs, int n_states, const uint32_t* allow, const int* next_default,
                                                        const int* exc_off, const int* exc_tok, const int* exc_next, const int* start, int* out_state,
                                                        const int* top_k, const float* top_p) {
-	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
-	const bool none = !ctx_off && !ctx_len;
-	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
-	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
-	SqAutomaton aut{n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state, 0, {}};
-	const SqTrunc tr{top_k, top_p};
-	return sq_run("decode_sample_queue_truncated", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len,
-	              nreq, max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows,
-	              logprobs || k ? &lp : nullptr, &pen, &aut, &tr);
+	return sq_run({"decode_sample_queue_truncated", transformer, tokens, n, {ctx_off, ctx_len}, off, len, nreq, max_new, temperature, minp, stop, n_stop,
+	                max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, {logprobs || k, k, logprobs, top_ids, top_logprobs},
+	                {presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias},
+	                {n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state}, {top_k, top_p}});
 }
 
 extern "C" int calm_b200_decode_sample_queue_lookup(struct Transformer* transformer, const int* tokens, int n, const int* ctx_off, const int* ctx_len,
@@ -3016,16 +3021,10 @@ extern "C" int calm_b200_decode_sample_queue_lookup(struct Transformer* transfor
                                                     float* top_logprobs, int n_states, const uint32_t* allow, const int* next_default,
                                                     const int* exc_off, const int* exc_tok, const int* exc_next, const int* start, int* out_state,
                                                     const int* top_k, const float* top_p, int max_draft, int* drafted, int* accepted) {
-	const std::vector<int> empty(nreq > 0 ? nreq : 0); // both NULL: no request has a context
-	const bool none = !ctx_off && !ctx_len;
-	const SqLogprobs lp{k, logprobs, top_ids, top_logprobs};
-	const SqPenalties pen{presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias};
-	SqAutomaton aut{n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state, 0, {}};
-	const SqTrunc tr{top_k, top_p};
-	const SqLookup lk{max_draft, drafted, accepted};
-	return sq_run("decode_sample_queue_lookup", transformer, tokens, n, none ? empty.data() : ctx_off, none ? empty.data() : ctx_len, off, len, nreq,
-	              max_new, temperature, minp, stop, n_stop, max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, logprobs || k ? &lp : nullptr,
-	              &pen, &aut, &tr, &lk);
+	return sq_run({"decode_sample_queue_lookup", transformer, tokens, n, {ctx_off, ctx_len}, off, len, nreq, max_new, temperature, minp, stop, n_stop,
+	                max_rows, rng_states, out_tokens, out_len, steps, prompt_rows, {logprobs || k, k, logprobs, top_ids, top_logprobs},
+	                {presence, frequency, repetition, bias_off, bias_len, bias_ids, bias_val, n_bias},
+	                {n_states, allow, next_default, exc_off, exc_tok, exc_next, start, out_state}, {top_k, top_p}, {max_draft, drafted, accepted}});
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests

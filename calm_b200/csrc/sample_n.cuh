@@ -390,15 +390,19 @@ __global__ void __launch_bounds__(32) k_sq_lp(const SqRows* tab, const float* lo
 
 // ---------------------------------------------------------------- calm_b200_decode_sample_queue_penalties
 
-// A step's penalty lane of each row (-1: a neutral request's row), passed by value to k_sq_lanes
+// A step's penalty lane (-1: a neutral request's row) and automaton state (-1: an unconstrained request's row) of each
+// row, passed by value to k_sq_lanes
 struct SqLanes {
 	int lane[SQ_ROWS];
+	int state[SQ_ROWS];
 };
+static_assert(sizeof(SqLanes) == 32 * sizeof(int), "one word per thread of k_sq_lanes' warp");
 
-// one warp, before a step with non-neutral rows: keep the step's lanes where k_vf_gemm<.., PEN> and k_sq_pen_step read them
+// one warp, before a step with a non-neutral or constrained row: keep the step's lanes and states, lanes[0 .. 16) and
+// lanes[16 .. 32), where k_vf_gemm<.., PEN> (and <.., PEN, MASK>) and k_sq_pen_step read them
 __global__ void __launch_bounds__(32) k_sq_lanes(const SqLanes l, int* lanes) {
 	pdl_enter();
-	if (threadIdx.x < SQ_ROWS) lanes[threadIdx.x] = l.lane[threadIdx.x];
+	lanes[threadIdx.x] = reinterpret_cast<const int*>(&l)[threadIdx.x];
 }
 
 // What k_sq_pen_admit needs of the request it admits to a lane: where its context, prompt and bias list lie in the
@@ -439,21 +443,4 @@ __global__ void __launch_bounds__(32) k_sq_pen_step(const int* lanes, const int*
 	pdl_enter();
 	const int i = threadIdx.x;
 	if (i < SQ_ROWS && lanes[i] >= 0) ++cnt[(size_t)lanes[i] * vocab + step_tok[i]];
-}
-
-// ---------------------------------------------------------------- calm_b200_decode_sample_queue_constrained
-
-// A step's penalty lane (-1: none) and automaton state (-1: an unconstrained request's row) of each row, passed by value
-// to k_sq_mask_lanes
-struct SqMaskLanes {
-	int lane[SQ_ROWS];
-	int state[SQ_ROWS];
-};
-static_assert(sizeof(SqMaskLanes) == 32 * sizeof(int), "one word per thread of k_sq_mask_lanes' warp");
-
-// one warp, before a step with a constrained row: keep the step's lanes and states, lanes[0 .. 16) and lanes[16 .. 32),
-// where k_vf_gemm<.., PEN, MASK> and k_sq_pen_step read them
-__global__ void __launch_bounds__(32) k_sq_mask_lanes(const SqMaskLanes l, int* lanes) {
-	pdl_enter();
-	lanes[threadIdx.x] = reinterpret_cast<const int*>(&l)[threadIdx.x];
 }

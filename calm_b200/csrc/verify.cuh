@@ -59,7 +59,7 @@ struct VfArgs {
 	const float* pbias; // [16][vocab] b(v): the request's logit bias, 0 off its list
 	const float4* ppar; // [16] (presence, frequency, repetition, 0)
 	// MASK: row t's automaton state, or -1 for a row left as it is, and the states' bitmasks
-	const int* mstate;       // [VF_TOK] (k_sq_mask_lanes)
+	const int* mstate;       // [VF_TOK] (k_sq_lanes)
 	const uint32_t* allow;   // [n_states][ceil(vocab / 32)] bit v % 32 of word v / 32: token v is allowed
 };
 
