@@ -71,19 +71,25 @@ STAGES = {
 @pytest.mark.parametrize("case", sorted(STAGES))
 def test_last_step_every_stage(case, capfd):
     spec, kvbits, lens, n_tokens, seq_len = STAGES[case]
-    nseq, j = len(lens), n_tokens - 1
     tensors, w = make_model(spec, 4)
+    with lib.DeviceModel(spec, tensors, seq_len=seq_len, kvbits=kvbits) as dm, capfd.disabled():
+        check_last_step(dm, w, kvbits, lens, n_tokens, case)
+
+
+def check_last_step(dm, w, kvbits, lens, n_tokens, case):
+    """decode_sample_batch of prompts of these lengths for n_tokens, then the last step's stages against float64."""
+    spec = w.spec
+    nseq, j = len(lens), n_tokens - 1
     prompts = prompts_of(spec.vocab_size, lens, start=3)
     starts, G = layout(lens)
     L = np.asarray(lens) - 1
     hd, kv_mul = spec.head_dim, spec.n_heads // spec.n_kv_heads
-    with lib.DeviceModel(spec, tensors, seq_len=seq_len, kvbits=kvbits) as dm, capfd.disabled():
-        toks, states, served = dm.decode_sample_batch(prompts, n_tokens, *DEFAULT, SEEDS[:nseq])
-        X = dm.read_state("pf_x").reshape(-1, spec.dim)[:nseq]
-        Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:nseq]
-        A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:nseq]
-        H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:nseq]
-        keys, values = layer_cache(dm, spec)
+    toks, states, served = dm.decode_sample_batch(prompts, n_tokens, *DEFAULT, SEEDS[:nseq])
+    X = dm.read_state("pf_x").reshape(-1, spec.dim)[:nseq]
+    Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:nseq]
+    A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:nseq]
+    H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:nseq]
+    keys, values = layer_cache(dm, spec)
     assert served == 1, f"{case}: the packed path did not serve this shape"
     assert states == [xs_advance(s, n_tokens) for s in SEEDS[:nseq]]
     label = f"sample_batch {case} kv{kvbits}"

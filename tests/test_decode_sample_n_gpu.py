@@ -61,22 +61,28 @@ STAGES = {
 def test_last_step_every_stage(case, capfd):
     spec, kvbits, nseq, n_tokens, pos0 = STAGES[case]
     tensors, w = make_model(spec, 4)
-    token0 = 3
-    hd, kv_mul, j = spec.head_dim, spec.n_heads // spec.n_kv_heads, n_tokens - 1
     with lib.DeviceModel(spec, tensors, seq_len=1024, kvbits=kvbits) as dm, capfd.disabled():
         dm.fill_kv(pos0, seed=6)
-        toks, states, served = dm.decode_sample_n(token0, pos0, n_tokens, *DEFAULT, SEEDS[:nseq])
-        X = dm.read_state("pf_x").reshape(-1, spec.dim)[:nseq]
-        Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:nseq]
-        A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:nseq]
-        H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:nseq]
-        keys, values = layer_cache(dm, spec)
+        check_last_step(dm, w, kvbits, nseq, n_tokens, pos0, case)
+
+
+def check_last_step(dm, w, kvbits, nseq, n_tokens, pos0, case, layer=0):
+    """decode_sample_n(3, pos0, n_tokens) for the first nseq SEEDS over the prompt in slots [0, pos0), then the last step's
+    stages of `layer` (whose input must be the embedding rows) against float64."""
+    spec, token0 = w.spec, 3
+    hd, kv_mul, j = spec.head_dim, spec.n_heads // spec.n_kv_heads, n_tokens - 1
+    toks, states, served = dm.decode_sample_n(token0, pos0, n_tokens, *DEFAULT, SEEDS[:nseq])
+    X = dm.read_state("pf_x").reshape(-1, spec.dim)[:nseq]
+    Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:nseq]
+    A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:nseq]
+    H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:nseq]
+    keys, values = layer_cache(dm, spec, layer)
     assert served == 1, f"{case}: the shared-prompt path did not serve this shape"
     assert states == [xs_advance(s, n_tokens) for s in SEEDS[:nseq]]
     label = f"sample_n {case} kv{kvbits}"
     inputs = toks[:, j - 1] if j > 0 else np.full(nseq, token0)
     X0 = w.mat("model.embed.weight")[inputs].astype(np.float64)
-    q_ref, k_ref, v_ref, xn = sr.qkv(w, 0, X0, np.full(nseq, pos0 + j))
+    q_ref, k_ref, v_ref, xn = sr.qkv(w, layer, X0, np.full(nseq, pos0 + j))
     report(label, "Q", "k_vf_gemm QKV", Q, q_ref, np.abs(q_ref).max(), lambda i: f"row {i[0]} head {i[1] // hd} dim {i[1] % hd}", "vf_q", pf_tol(spec.dim))
     slots = pos0 + j * nseq + np.arange(nseq)
     for name, dev, ref in (("K", keys, k_ref), ("V", values, v_ref)):
@@ -88,11 +94,12 @@ def test_last_step_every_stage(case, capfd):
         a_ref.append(sr.attention(spec, Q[b], K, V, pos0 + j + 1))
         vmax.append(np.repeat(np.abs(V).max((1, 2)), kv_mul * hd))
     report(label, "A", "k_sn_attn", A, np.stack(a_ref), np.stack(vmax), lambda i: f"row {i[0]} head {i[1] // hd} dim {i[1] % hd}", "pf_att")
-    x1 = sr.wo(w, 0, X0, A)
-    h_ref = sr.ffn_up(w, 0, sr.ffn_input(w, 0, x1, xn))
+    x1 = sr.wo(w, layer, X0, A)
+    h_ref = sr.ffn_up(w, layer, sr.ffn_input(w, layer, x1, xn))
     report(label, "H", "k_vf_gemm WO+UP", H, h_ref, np.abs(h_ref).max(), lambda i: f"row {i[0]} hidden row {i[1]}", "vf_hb", pf_tol(max(spec.dim, spec.q_dim)))
-    x_ref = sr.ffn_down(w, 0, x1, H)
+    x_ref = sr.ffn_down(w, layer, x1, H)
     report(label, "X", "k_vf_gemm DOWN", X, x_ref, np.abs(x_ref).max(), lambda i: f"row {i[0]} row {i[1]}", "vf_x", pf_tol(spec.hidden_dim))
+    return toks
 
 
 # ---- 2 + 3. batch invariance, the prompt's cache, each row's draw

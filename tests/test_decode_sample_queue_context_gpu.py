@@ -299,23 +299,28 @@ STAGES = {  # (spec, kvbits, contexts, ctx_of, own lengths, max_new, max_rows): 
 @pytest.mark.parametrize("case", sorted(STAGES))
 def test_last_step_every_stage(case, capfd):
     spec, kvbits, ctx_lens, ctx_of, lens, max_new, max_rows = STAGES[case]
-    nreq, seq_len = len(lens), 8192
     tensors, w = make_model(spec, 4)
+    with lib.DeviceModel(spec, tensors, seq_len=8192, kvbits=kvbits) as dm, capfd.disabled():
+        check_last_step(dm, w, kvbits, ctx_lens, ctx_of, lens, max_new, max_rows, case)
+
+
+def check_last_step(dm, w, kvbits, ctx_lens, ctx_of, lens, max_new, max_rows, case):
+    """The queue over contexts and own prompts of these lengths, then the last step's stages against float64."""
+    spec, nreq, seq_len = w.spec, len(lens), dm.seq_len
     contexts = prompts_of(spec.vocab_size, ctx_lens, start=61)
     prompts = prompts_of(spec.vocab_size, lens, start=3)
     key, clen = layout(contexts, ctx_of, prompts)
     hd, kv_mul = spec.head_dim, spec.n_heads // spec.n_kv_heads
     sets = [SETTINGS[i % len(SETTINGS)] for i in range(nreq)]
-    with lib.DeviceModel(spec, tensors, seq_len=seq_len, kvbits=kvbits) as dm, capfd.disabled():
-        toks, _, served, steps, _ = qctx(dm, contexts, ctx_of, prompts, max_new, sets, SEEDS[:nreq], [], max_rows)
-        sched, place, _, _, _, _ = simulate(key, clen, lens, max_new, max_new, max_rows, seq_len)
-        rows = sched[-1]
-        n = len(rows)
-        X = dm.read_state("pf_x").reshape(-1, spec.dim)[:n]
-        Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:n]
-        A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:n]
-        H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:n]
-        keys, values = layer_cache(dm, spec)
+    toks, _, served, steps, _ = qctx(dm, contexts, ctx_of, prompts, max_new, sets, SEEDS[:nreq], [], max_rows)
+    sched, place, _, _, _, _ = simulate(key, clen, lens, max_new, max_new, max_rows, seq_len)
+    rows = sched[-1]
+    n = len(rows)
+    X = dm.read_state("pf_x").reshape(-1, spec.dim)[:n]
+    Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:n]
+    A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:n]
+    H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:n]
+    keys, values = layer_cache(dm, spec)
     assert served == 1 and steps == len(sched)
     assert n >= 2 and len({j for _, j in rows}) >= 2, f"{case}: the last step's rows {rows} are not at different own steps"
     assert any(clen[i] >= CHUNK for i, _ in rows), f"{case}: no row of the last step has a shared chunk"

@@ -69,10 +69,11 @@ def rows_checked(m):
     return np.array(sorted(r))
 
 
-def check_pass(dm, w, toks, pos0, kvbits, label):
+def check_pass(dm, w, toks, pos0, kvbits, label, layer=0):
     """forward_prefill_cuda(toks, pos0) on a one-layer model, then every cache entry it wrote and the last block's Q,
     attention output, hidden and residual rows against float64.  Returns the float64 normed inputs and the device's hidden
-    rows, for the cases that check their own premise."""
+    rows, for the cases that check their own premise.  The stages are those of `layer`, whose input must be the embedding
+    rows: layer 0, or the last layer behind layers that pass them through."""
     s = w.spec
     n, hd, kv_mul = len(toks), s.head_dim, s.n_heads // s.n_kv_heads
     m = n - BLOCK * ((n - 1) // BLOCK)
@@ -83,12 +84,12 @@ def check_pass(dm, w, toks, pos0, kvbits, label):
     A = dm.read_state("pf_att").reshape(-1, s.q_dim)[:m]
     H = dm.read_state("pf_hb").reshape(-1, s.hidden_dim)[:m]
     X = dm.read_state("pf_x").reshape(-1, s.dim)[:m]
-    keys, values = layer_cache(dm, s)
+    keys, values = layer_cache(dm, s, layer)
     blocks = " + ".join(str(min(BLOCK, n - o)) for o in range(0, n, BLOCK))
     label = f"{label} kv{kvbits} pos0 {pos0} n {n} ({blocks})"
 
     X0 = w.mat("model.embed.weight")[toks].astype(np.float64)
-    q_ref, k_ref, v_ref, xn = sr.qkv(w, 0, X0, pos0 + np.arange(n))
+    q_ref, k_ref, v_ref, xn = sr.qkv(w, layer, X0, pos0 + np.arange(n))
     for name, dev, ref in (("K", keys, k_ref), ("V", values, v_ref)):
         got = dev[:, pos0:pos0 + n].transpose(1, 0, 2).reshape(n, -1)
         check_entries(label, name, "k_pf_gemm QKV", got, ref, kvbits, lambda i: f"slot {pos0 + i[0]} kv head {i[1] // hd} dim {i[1] % hd}", "pf_kv", pf_tol(s.dim))
@@ -101,11 +102,11 @@ def check_pass(dm, w, toks, pos0, kvbits, label):
     a_ref = np.stack([sr.attention(s, Q[t], k64, v64, b0 + t + 1) for t in R])
     vmax = np.maximum.accumulate(np.abs(values[:, :b0 + m]).max(2), 1)[:, b0 + R].T  # [rows, kv heads]: max |V| of the head so far
     report(label, "A", "k_pf_attn", A[R], a_ref, np.repeat(vmax, kv_mul * hd, 1), lambda i: f"{row(i)} head {i[1] // hd} dim {i[1] % hd}, keys 0..{b0 + R[i[0]]}", "pf_att")
-    x1 = sr.wo(w, 0, X0, A[R])
-    xn2 = sr.ffn_input(w, 0, x1, xn)
-    h_ref = sr.ffn_up(w, 0, xn2)
+    x1 = sr.wo(w, layer, X0, A[R])
+    xn2 = sr.ffn_input(w, layer, x1, xn)
+    h_ref = sr.ffn_up(w, layer, xn2)
     report(label, "H", "k_pf_gemm WO+UP", H[R], h_ref, np.abs(h_ref).max(), lambda i: f"{row(i)} hidden row {i[1]}", "pf_hb", pf_tol(max(s.dim, s.q_dim)))
-    x_ref = sr.ffn_down(w, 0, x1, H[R])
+    x_ref = sr.ffn_down(w, layer, x1, H[R])
     report(label, "X", "k_pf_gemm DOWN", X[R], x_ref, np.abs(x_ref).max(), lambda i: f"{row(i)} row {i[1]}", "pf_x", pf_tol(s.hidden_dim))
     return np.concatenate([xn.reshape(-1), xn2.reshape(-1)]), H
 

@@ -102,27 +102,28 @@ def make_model(spec, seed):
     return tensors, sr.Weights(spec, {k: v.cpu() for k, v in tensors.items()})
 
 
-def layer_cache(dm, spec):
+def layer_cache(dm, spec, layer=0):
     shape = (spec.n_kv_heads, dm.seq_len, spec.head_dim)
-    return dm.read_state("keys").reshape(shape), dm.read_state("values").reshape(shape)
+    return dm.read_state("keys", layer).reshape(shape), dm.read_state("values", layer).reshape(shape)
 
 
-def check_decode_step(dm, w, token, pos, kvbits, plan, label, fill_seed=5):
-    """fill_kv below `pos`, one forward_cuda, then every stage against float64 on the device's own inputs."""
+def check_decode_step(dm, w, token, pos, kvbits, plan, label, fill_seed=5, layer=0):
+    """fill_kv below `pos`, one forward_cuda, then every stage against float64 on the device's own inputs.  The stages are
+    those of `layer`, whose input must be the embedding row: layer 0, or a later one behind layers that pass it through."""
     s = w.spec
     attn_kernel, _, mv = plan
     slot, kv_len, sinks = sr.kv_slot(pos, dm.seq_len)
     dm.fill_kv(min(pos, dm.seq_len), seed=fill_seed)
-    keys_before = dm.read_state("keys").reshape(s.n_kv_heads, dm.seq_len, s.head_dim)[:, :sr.KV_SINKS].copy() if sinks else None
+    keys_before = dm.read_state("keys", layer).reshape(s.n_kv_heads, dm.seq_len, s.head_dim)[:, :sr.KV_SINKS].copy() if sinks else None
     logits = dm.forward(token, pos)
     q, att, x = dm.read_state("q"), dm.read_state("att"), dm.read_state("x")
     hb = dm.read_state("hb").reshape(-1, s.hidden_dim)
-    keys, values = layer_cache(dm, s)
+    keys, values = layer_cache(dm, s, layer)
     hd, kv_mul = s.head_dim, s.n_heads // s.n_kv_heads
     label = f"{label} pos {pos} slot {slot}"
 
     x0 = sr.embed(w, token)
-    q_ref, k_ref, v_ref, xn = sr.qkv(w, 0, x0, pos)
+    q_ref, k_ref, v_ref, xn = sr.qkv(w, layer, x0, pos)
     head_dim_of = lambda i: f"head {i[0] // hd} dim {i[0] % hd}"  # noqa: E731
     report(label, "q", "k_qkv", q, q_ref, np.abs(q_ref).max(), head_dim_of)
     for name, dev, ref in (("K", keys, k_ref), ("V", values, v_ref)):
@@ -136,10 +137,10 @@ def check_decode_step(dm, w, token, pos, kvbits, plan, label, fill_seed=5):
     vmax = np.repeat(np.abs(values[:, :kv_len]).max((1, 2)), kv_mul * hd)
     report(label, "att", attn_kernel, att, att_ref, vmax, lambda i: f"head {i[0] // hd} dim {i[0] % hd}, kv_len {kv_len}")
 
-    x1 = sr.wo(w, 0, x0, att)
-    xn2 = sr.ffn_input(w, 0, x1, xn)
+    x1 = sr.wo(w, layer, x0, att)
+    xn2 = sr.ffn_input(w, layer, x1, xn)
     if s.n_experts:
-        experts, weights, glog = sr.router(w, 0, xn2)
+        experts, weights, glog = sr.router(w, layer, xn2)
         sel = dm.read_state("moe_sel")
         dev_experts, dev_weights = [int(e) for e in sel[:len(experts)]], sel[len(experts):]
         srt = np.sort(glog)[::-1]
@@ -149,11 +150,11 @@ def check_decode_step(dm, w, token, pos, kvbits, plan, label, fill_seed=5):
         e = np.exp(glog[experts] - glog.max())
         weights = e / e.sum()
         report(label, "moe_w", mv["up"], dev_weights, weights, 1.0, lambda i: f"active expert {i[0]} (expert {experts[i[0]]})")
-        hb_ref = np.stack([sr.ffn_up(w, 0, xn2, e) for e in experts])
-        x_ref = sr.ffn_down(w, 0, x1, hb, experts, dev_weights)
+        hb_ref = np.stack([sr.ffn_up(w, layer, xn2, e) for e in experts])
+        x_ref = sr.ffn_down(w, layer, x1, hb, experts, dev_weights)
     else:
-        hb_ref = sr.ffn_up(w, 0, xn2)[None]
-        x_ref = sr.ffn_down(w, 0, x1, hb[0])
+        hb_ref = sr.ffn_up(w, layer, xn2)[None]
+        x_ref = sr.ffn_down(w, layer, x1, hb[0])
     report(label, "hb", mv["up"] + "+wo", hb, hb_ref, np.abs(hb_ref).max(), lambda i: f"expert slot {i[0]} hidden row {i[1]} (wo: {mv['wo']}, weight rows of {s.q_dim * s.dbits // 8} bytes)")
     report(label, "x", mv["down"], x, x_ref, np.abs(x_ref).max(), lambda i: f"row {i[0]} (weight rows of {s.hidden_dim * s.dbits // 8} bytes, sliced by 1 KB / 2 KB chunk)")
     logits_ref = sr.classifier(w, x)

@@ -50,16 +50,22 @@ VERIFY = {
 def test_verify_every_stage(case, capfd):
     spec, kvbits, n, pos0 = VERIFY[case]
     tensors, w = make_model(spec, 4)
-    toks = mg.teacher_tokens(spec.vocab_size, n, start=3)
-    hd, kv_mul = spec.head_dim, spec.n_heads // spec.n_kv_heads
     with lib.DeviceModel(spec, tensors, seq_len=2048, kvbits=kvbits) as dm, capfd.disabled():
         dm.fill_kv(pos0, seed=6)
-        greedy, served = dm.verify_greedy(toks, pos0)
-        X = dm.read_state("pf_x").reshape(-1, spec.dim)[:n]
-        Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:n]
-        A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:n]
-        H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:n]
-        keys, values = layer_cache(dm, spec)
+        check_block(dm, w, kvbits, n, pos0, case)
+
+
+def check_block(dm, w, kvbits, n, pos0, case):
+    """verify_greedy of n tokens at pos0 over the cache below it, then every stage of the block against float64."""
+    spec = w.spec
+    toks = mg.teacher_tokens(spec.vocab_size, n, start=3)
+    hd, kv_mul = spec.head_dim, spec.n_heads // spec.n_kv_heads
+    greedy, served = dm.verify_greedy(toks, pos0)
+    X = dm.read_state("pf_x").reshape(-1, spec.dim)[:n]
+    Q = dm.read_state("pf_q").reshape(-1, spec.q_dim)[:n]
+    A = dm.read_state("pf_att").reshape(-1, spec.q_dim)[:n]
+    H = dm.read_state("pf_hb").reshape(-1, spec.hidden_dim)[:n]
+    keys, values = layer_cache(dm, spec)
     assert served == 1, f"{case}: the short-block path did not serve this shape"
     label = f"verify {case} kv{kvbits}"
     X0 = w.mat("model.embed.weight")[toks].astype(np.float64)
