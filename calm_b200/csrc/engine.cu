@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <iterator>
 #include <map>
 #include <set>
@@ -218,6 +219,15 @@ struct Prefill {
 	// call with a constrained request and regrown like pf.sqout
 	uint32_t* sqallow = nullptr; // [sqallow_cap]
 	size_t sqallow_cap = 0;
+	// beam search (calm_b200_decode_beam), allocated on its first call and regrown when a call needs more: the ancestry
+	// tables (double-buffered), the per-step backpointers and candidate lists, the pool; and the last call's shape
+	int* bmanc[2] = {nullptr, nullptr}; // [bmanc_cap] each: [B][max_new]
+	BmBack* bmback = nullptr;           // [bmback_cap]: [max_new][B]
+	int* bmtid = nullptr;               // [bmtrace_cap]: [max_new][B][K]
+	float* bmtlp = nullptr;
+	BmState* bmst = nullptr;
+	size_t bmanc_cap = 0, bmback_cap = 0, bmtrace_cap = 0;
+	int bm_steps = 0, bm_beams = 0, bm_k = 0, bm_max_new = 0, bm_last = 0; // bm_last: the bmanc table the last step read
 };
 Prefill pf;
 
@@ -234,6 +244,7 @@ void pf_free() {
 	cudaFree(pf.sqtopv), cudaFree(pf.sqtopi), cudaFree(pf.sqtid), cudaFree(pf.sqtlp), cudaFree(pf.sqlp), cudaFree(pf.sqoid), cudaFree(pf.sqolp);
 	cudaFree(pf.sqpcnt), cudaFree(pf.sqpbias), cudaFree(pf.sqppar), cudaFree(pf.sqlanes), cudaFree(pf.sqptok), cudaFree(pf.sqpbid), cudaFree(pf.sqpbval);
 	cudaFree(pf.sqallow);
+	cudaFree(pf.bmanc[0]), cudaFree(pf.bmanc[1]), cudaFree(pf.bmback), cudaFree(pf.bmtid), cudaFree(pf.bmtlp), cudaFree(pf.bmst);
 	pf = Prefill();
 }
 
@@ -1361,11 +1372,13 @@ enum PfRows {
 	PF_PACKED,   // a packed block that holds no context (the scoring calls at pos0 = 0, and decode_sample_batch's prompts at
 	             // any slot base): per-row RoPE positions in pf.rowpos, each row's sequence start (its cache slot) in pf.seg
 	PF_CONTEXTS, // PF_PACKED, and sequences continue contexts placed in the same block: each row's context in pf.ctx
+	PF_BEAM,     // a step of calm_b200_decode_beam (PfSampleStep): PF_SAMPLES, but every row reads its generated keys through
+	             // its ancestry (sample_n.cuh's BEAM attention)
 };
 
 // a short block: at most VF_TOK rows whose GEMMs run on k_vf_gemm
 static bool pf_short(PfRows layout) {
-	return layout == PF_SHORT || layout == PF_SAMPLES || layout == PF_BATCH || layout == PF_QUEUE;
+	return layout == PF_SHORT || layout == PF_SAMPLES || layout == PF_BATCH || layout == PF_QUEUE || layout == PF_BEAM;
 }
 
 // A layer GEMM of the pass over `rows` output rows of `a` (UP: of w1 and of w3 each), whose activations are the f16 pair
@@ -1381,16 +1394,19 @@ static void pf_layer_gemm(PfRows layout, const CUtensorMap* tm, const __half* hi
 // same slots from pos0 = G, the end of the packed prompts, and row b at RoPE position L_b + step; lmax = max_b L_b.  A
 // step of calm_b200_decode_sample_queue: nseq rows, step 0, and lmax = the largest L + j of its rows (pf.sqrows).  A queue
 // step whose rows have contexts (pf.sqgroups): nshared shared chunks and nsuf > 0 per-row chunks per row (sample_n.cuh,
-// GROUPS); nsuf = 0 on every other step.
+// GROUPS); nsuf = 0 on every other step.  A step of calm_b200_decode_beam: nseq rows (1 at step 0) at slots pos0 + step *
+// nbeam + b, reading their keys through the ancestry `anc` (sample_n.cuh, BEAM).
 struct PfSampleStep {
 	int pos0, step, nseq, lmax;
 	int nshared = 0, nsuf = 0;
+	const int* anc = nullptr;
+	int nbeam = 0, anc_stride = 0;
 };
 
 // The attention of a PF_SAMPLES step (shared prompt) or, with BATCH, of a PF_BATCH step (a prompt per row), or with
 // QUEUE as well, of a PF_QUEUE step (sample_n.cuh), with GROUPS of one whose rows have contexts: chunk partials, then
 // their fold into pf.Ahi / pf.Alo
-template <typename KVT, int HD, bool BATCH, bool QUEUE = false, bool GROUPS = false>
+template <typename KVT, int HD, bool BATCH, bool QUEUE = false, bool GROUPS = false, bool BEAM = false>
 static void sn_attn(const SnAttnArgs& a, const PfSampleStep& ss) {
 	const int nkeys = a.pos0 + a.step + 1, npre = a.pos0 / SN_CHUNK, nsuf = cdiv(nkeys, SN_CHUNK) - npre;
 	const dim3 grid(GROUPS ? ss.nshared + a.nseq * ss.nsuf : BATCH ? a.nseq * cdiv(ss.lmax + a.step + 1, SN_CHUNK) : npre + a.nseq * nsuf, g.cfg.n_kv_heads);
@@ -1398,9 +1414,9 @@ static void sn_attn(const SnAttnArgs& a, const PfSampleStep& ss) {
 		smem_optin(kernel, smem);
 		launch_pdl(kernel, grid, SN_WARPS * 32, smem, a);
 	};
-	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4, BATCH, QUEUE, GROUPS>, sn_smem_bytes<KVT, HD, 4>());
-	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2, BATCH, QUEUE, GROUPS>, sn_smem_bytes<KVT, HD, 2>());
-	else run(k_sn_attn<KVT, HD, 1, BATCH, QUEUE, GROUPS>, sn_smem_bytes<KVT, HD, 1>());
+	if (g.kv_mul % 4 == 0) run(k_sn_attn<KVT, HD, 4, BATCH, QUEUE, GROUPS, BEAM>, sn_smem_bytes<KVT, HD, 4>());
+	else if (g.kv_mul % 2 == 0) run(k_sn_attn<KVT, HD, 2, BATCH, QUEUE, GROUPS, BEAM>, sn_smem_bytes<KVT, HD, 2>());
+	else run(k_sn_attn<KVT, HD, 1, BATCH, QUEUE, GROUPS, BEAM>, sn_smem_bytes<KVT, HD, 1>());
 	launch_pdl(k_sn_fold<HD, BATCH, QUEUE>, dim3(cdiv(g.cfg.n_heads, SN_WARPS), a.nseq), SN_WARPS * 32, 0, a);
 }
 
@@ -1413,7 +1429,7 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 	const Weights& w = g.w;
 	const size_t kv_layer = (size_t)c.n_kv_heads * c.seq_len * c.head_dim;
 	launch_pdl(k_pf_embed<DBITS>, n, 256, 0, pf.X, (const void*)w.token_embedding_table, (const int*)pf.tokens, n, c.dim);
-	if (layout == PF_SAMPLES || layout == PF_BATCH) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.snpos + (size_t)ss->step * n, n, c.head_dim / 2);
+	if (layout == PF_SAMPLES || layout == PF_BATCH || layout == PF_BEAM) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.snpos + (size_t)ss->step * n, n, c.head_dim / 2);
 	else if (layout == PF_QUEUE) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.sqrows->pos, n, c.head_dim / 2);
 	else if (packed) launch_pdl(k_pf_rope_rows, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, (const int*)pf.rowpos, n, c.head_dim / 2);
 	else launch_pdl(k_pf_rope, cdiv(n * (c.head_dim / 2), 256), 256, 0, pf.rope, (const float*)g.rope_freq, n, c.head_dim / 2, pos0);
@@ -1433,7 +1449,7 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 		aa.Q = pf.Q, aa.kc = a.kc, aa.vc = a.vc, aa.Ohi = pf.Ahi, aa.Olo = pf.Alo;
 		aa.n_tokens = n, aa.pos0 = pos0, aa.seq_len = c.seq_len, aa.q_dim = g.q_dim, aa.kv_mul = g.kv_mul, aa.inv_sqrt_hd = 1.0f / sqrtf((float)c.head_dim);
 		aa.seg = pf.seg, aa.ctx = pf.ctx;
-		if (layout == PF_SAMPLES || layout == PF_BATCH || layout == PF_QUEUE) {
+		if (layout == PF_SAMPLES || layout == PF_BATCH || layout == PF_QUEUE || layout == PF_BEAM) {
 			SnAttnArgs sa = {};
 			sa.Q = pf.Q, sa.kc = a.kc, sa.vc = a.vc, sa.part = pf.snpart, sa.Ohi = pf.Ahi, sa.Olo = pf.Alo;
 			sa.pos0 = ss->pos0, sa.step = ss->step, sa.nseq = ss->nseq, sa.seq_len = c.seq_len, sa.q_dim = g.q_dim, sa.kv_mul = g.kv_mul;
@@ -1446,6 +1462,10 @@ static void pf_run(Formats<DBITS, KVT>, int n, int pos0, PfRows layout, const Pf
 				sa.qrows = pf.sqrows->q;
 				if (c.head_dim == 128) sn_attn<KVT, 128, true, true>(sa, *ss);
 				else sn_attn<KVT, 64, true, true>(sa, *ss);
+			} else if (layout == PF_BEAM) {
+				sa.anc = ss->anc, sa.nbeam = ss->nbeam, sa.anc_stride = ss->anc_stride;
+				if (c.head_dim == 128) sn_attn<KVT, 128, false, false, false, true>(sa, *ss);
+				else sn_attn<KVT, 64, false, false, false, true>(sa, *ss);
 			} else if (layout == PF_BATCH) {
 				if (c.head_dim == 128) sn_attn<KVT, 128, true>(sa, *ss);
 				else sn_attn<KVT, 64, true>(sa, *ss);
@@ -2582,10 +2602,20 @@ static int sq_fallback(const SqCall& c, std::vector<int>& cur, const std::vector
 	return 0;
 }
 
+// A step's top-k tile lists and merged lists for VF_TOK rows and the largest k (sq_classify / sq_merge with k > 0)
+static void sq_topk_reserve() {
+	if (pf.sqtopv) return;
+	const size_t nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	pf.sqtopv = (float*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(float));
+	pf.sqtopi = (int*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
+	pf.sqtid = (int*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(int));
+	pf.sqtlp = (float*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(float));
+}
+
 // The device buffers of a call of `total` tokens and its uploads, once per call: the lanes' rows, tokens and bias lists
 // when a request is not neutral, the automaton's bitmasks when one is constrained (cur: each request's start state)
 static void sq_reserve(const SqCall& c, size_t total, const std::vector<int>& cur) {
-	const size_t vocab = g.cfg.vocab_size, nvt = cdiv(g.cfg.vocab_size, PF_BM);
+	const size_t vocab = g.cfg.vocab_size;
 	if (!pf.sqrows) {
 		pf.sqrows = (SqRows*)dev_alloc(sizeof(SqRows));
 		pf.sqgroups = (SqGroups*)dev_alloc(sizeof(SqGroups));
@@ -2594,12 +2624,7 @@ static void sq_reserve(const SqCall& c, size_t total, const std::vector<int>& cu
 	}
 	sq_grow(pf.sqout_cap, total, pf.sqout);
 	sq_grow(pf.sqst_cap, c.nreq, pf.sqst);
-	if (c.lp.on && !pf.sqtopv) {
-		pf.sqtopv = (float*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(float));
-		pf.sqtopi = (int*)dev_alloc(VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
-		pf.sqtid = (int*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(int));
-		pf.sqtlp = (float*)dev_alloc(VF_TOK * PF_TOPK_MAX * sizeof(float));
-	}
+	if (c.lp.on) sq_topk_reserve();
 	if (c.lp.on) sq_grow(pf.sqlp_cap, total, pf.sqlp), sq_grow(pf.sqtop_cap, total * c.lp.k, pf.sqoid, pf.sqolp);
 	bool any_pen = false, any_aut = false; // a request with max_new > 0 is not neutral / is constrained
 	for (int i = 0; i < c.nreq; ++i) any_pen = any_pen || (c.max_new[i] > 0 && !c.pen.neutral(i));
@@ -3028,6 +3053,107 @@ extern "C" int calm_b200_decode_sample_queue_lookup(struct Transformer* transfor
 }
 
 // the logits of the last device-resident step (decode_greedy / decode_sample keep them in HBM): copy for tests
+// ---------------------------------------------------------------------------------------------
+// calm_b200_decode_beam: num_beams beams of one prompt, one short block per step whose rows are the live beams (PF_BEAM),
+// the prompt's keys read once per step for all of them and each beam's generated keys through its ancestry
+// (sample_n.cuh, BEAM); the classifier's top-K epilogue and merge give each row its K best tokens, and k_bm_select walks
+// them into the next beams, the pool and the next ancestry.  Nothing is copied back before the end but, with a stop list,
+// the 4-byte done flag after each step.
+
+static_assert(BM_MAX == CALM_B200_BEAM_MAX, "the pool and the sums hold the most beams a call takes");
+
+// a finished hypothesis's tokens and log-probabilities: row `row` of step `step`'s history through the backpointers, then
+// its own token if it has one
+static void bm_tokens(const std::vector<BmBack>& back, int B, const BmHyp& h, std::vector<int>& tok, std::vector<float>& lp) {
+	tok.assign(h.step + (h.token >= 0), 0), lp.assign(tok.size(), 0.0f);
+	if (h.token >= 0) tok[h.step] = h.token, lp[h.step] = h.lp;
+	for (int s = h.step - 1, r = h.row; s >= 0; --s) {
+		const BmBack& b = back[(size_t)s * B + r];
+		tok[s] = b.token, lp[s] = b.lp, r = b.parent;
+	}
+}
+
+extern "C" int calm_b200_decode_beam(struct Transformer* transformer, int token0, int pos0, int max_new, int num_beams, const int* stop, int n_stop,
+                                     float length_penalty, int early_stopping, int num_return, int* out_tokens, int* out_len, float* out_logprobs,
+                                     float* out_scores, int* steps) {
+	if (!g.ready) CALM_FATAL("decode_beam before prepare_cuda");
+	const int B = num_beams;
+	if (B < 1 || B > CALM_B200_BEAM_MAX) CALM_FATAL("decode_beam: num_beams %d outside [1, %d]", B, CALM_B200_BEAM_MAX);
+	if (max_new < 0 || n_stop < 0) CALM_FATAL("decode_beam: negative max_new %d or n_stop %d", max_new, n_stop);
+	const long long K = (long long)std::max(2, 1 + n_stop) * B;
+	if (K > CALM_B200_TOPK_MAX) CALM_FATAL("decode_beam: %lld candidates per beam (max(2, 1 + n_stop) x num_beams) exceed %d", K, CALM_B200_TOPK_MAX);
+	if (num_return < 1 || num_return > B) CALM_FATAL("decode_beam: num_return %d outside [1, %d]", num_return, B);
+	if (n_stop > 0 && !stop) CALM_FATAL("decode_beam: stop is NULL");
+	for (int i = 0; i < n_stop; ++i)
+		if (stop[i] < 0 || stop[i] >= g.cfg.vocab_size) CALM_FATAL("decode_beam: stop token %d out of range", stop[i]);
+	if (!std::isfinite(length_penalty)) CALM_FATAL("decode_beam: length_penalty is not finite");
+	if (early_stopping != 0 && early_stopping != 1) CALM_FATAL("decode_beam: early_stopping %d is not 0 or 1", early_stopping);
+	if (!out_tokens || !out_len || !out_scores || !steps) CALM_FATAL("decode_beam: out_tokens, out_len, out_scores or steps is NULL");
+	check_call(transformer, token0, pos0);
+	if (max_new == 0) return 1;
+	if (!pf_supported() || (long long)pos0 + (long long)B * max_new > g.cfg.seq_len) {
+		*steps = 0;
+		return 0;
+	}
+	sn_reserve(B, cdiv(pos0 + max_new, SN_CHUNK));
+	sq_topk_reserve();
+	const size_t nanc = (size_t)B * max_new, nback = (size_t)max_new * B, ntrace = nback * K;
+	if (!pf.bmst) pf.bmst = (BmState*)dev_alloc(sizeof(BmState));
+	sq_grow(pf.bmanc_cap, nanc, pf.bmanc[0], pf.bmanc[1]);
+	sq_grow(pf.bmback_cap, nback, pf.bmback);
+	sq_grow(pf.bmtrace_cap, ntrace, pf.bmtid, pf.bmtlp);
+	std::vector<float> norm(max_new + 1); // norm[L] = L^length_penalty, in double, rounded once
+	for (int L = 1; L <= max_new; ++L) norm[L] = (float)pow((double)L, (double)length_penalty);
+	std::vector<int> pos(nanc);
+	for (size_t r = 0; r < nanc; ++r) pos[r] = pos0 + (int)(r / B); // step j's rows at [j B, j B + rows)
+	CUDA_CHECK(cudaMemcpyAsync(pf.snpos, pos.data(), nanc * sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(pf.tokens, &token0, sizeof(int), cudaMemcpyHostToDevice, g.stream));
+	CUDA_CHECK(cudaMemsetAsync(pf.bmanc[0], 0, nanc * sizeof(int), g.stream)); // step 0's one row reads its own key
+	CUDA_CHECK(cudaMemsetAsync(pf.bmst, 0, sizeof(BmState), g.stream));
+	BmArgs ba = {};
+	ba.tid = pf.sqtid, ba.tlp = pf.sqtlp, ba.st = pf.bmst, ba.back = pf.bmback, ba.trace_id = pf.bmtid, ba.trace_lp = pf.bmtlp, ba.tokens = pf.tokens;
+	std::copy(stop, stop + n_stop, ba.stop);
+	ba.n_stop = n_stop, ba.B = B, ba.K = (int)K, ba.max_new = max_new, ba.early = early_stopping;
+	int done = 0, j = 0, cur = 0;
+	for (; j < max_new && !done; ++j, cur ^= 1) {
+		const int rows = j ? B : 1;
+		PfSampleStep ss = {pos0, j, rows, 0};
+		ss.anc = pf.bmanc[cur], ss.nbeam = B, ss.anc_stride = max_new;
+		with_formats([&](auto f) {
+			pf_run(f, rows, pos0 + j * B, PF_BEAM, &ss);
+			sq_classify(f, rows, (int)K, false, false, false);
+		});
+		sq_merge(rows, (int)K);
+		ba.anc = pf.bmanc[cur], ba.anc_next = pf.bmanc[cur ^ 1], ba.j = j, ba.rows = rows;
+		ba.norm_j = norm[std::max(1, j)], ba.norm_next = norm[j + 1];
+		launch_pdl(k_bm_select, 1, BM_THREADS, 0, ba);
+		if (n_stop) {
+			CUDA_CHECK(cudaMemcpyAsync(&done, &pf.bmst->done, sizeof(int), cudaMemcpyDeviceToHost, g.stream));
+			sync_stream();
+		}
+	}
+	pf.bm_steps = j, pf.bm_beams = B, pf.bm_k = (int)K, pf.bm_max_new = max_new, pf.bm_last = cur ^ 1;
+	BmState st;
+	std::vector<BmBack> back((size_t)j * B);
+	CUDA_CHECK(cudaMemcpyAsync(&st, pf.bmst, sizeof(BmState), cudaMemcpyDeviceToHost, g.stream));
+	CUDA_CHECK(cudaMemcpyAsync(back.data(), pf.bmback, back.size() * sizeof(BmBack), cudaMemcpyDeviceToHost, g.stream));
+	sync_stream();
+	CUDA_CHECK(cudaGetLastError());
+	if (!st.done) // the live beams, in beam order, after the last step
+		for (int b = 0; b < B; ++b) bm_add(st, B, BmHyp{st.sum[b] / norm[max_new], st.sum[b], 0.0f, max_new, b, -1, 0});
+	std::sort(st.pool, st.pool + st.npool, [](const BmHyp& x, const BmHyp& y) { return x.score > y.score || (x.score == y.score && x.order < y.order); });
+	std::vector<int> tok;
+	std::vector<float> lp;
+	for (int r = 0; r < num_return && r < st.npool; ++r) {
+		bm_tokens(back, B, st.pool[r], tok, lp);
+		std::copy(tok.begin(), tok.end(), out_tokens + (size_t)r * max_new);
+		if (out_logprobs) std::copy(lp.begin(), lp.end(), out_logprobs + (size_t)r * max_new);
+		out_len[r] = (int)tok.size(), out_scores[r] = st.pool[r].score;
+	}
+	*steps = j;
+	return 1;
+}
+
 extern "C" void calm_b200_read_device_logits(float* out) {
 	CUDA_CHECK(cudaMemcpy(out, g.logits_dev, (size_t)g.cfg.vocab_size * sizeof(float), cudaMemcpyDeviceToHost));
 }
@@ -3084,6 +3210,7 @@ extern "C" int calm_b200_read_state(int which, int layer, float* out, int cap) {
 	CUDA_CHECK(cudaStreamSynchronize(g.stream));
 	const float* f32 = nullptr;           // a float buffer, copied as it is
 	const __half *hi = nullptr, *lo = nullptr; // a prompt-pass activation pair, summed in float
+	const int* i32 = nullptr;                 // an int buffer, converted to float
 	size_t count = 0;
 	switch (which) {
 	case CALM_B200_STATE_X: f32 = g.x, count = c.dim; break;
@@ -3102,12 +3229,19 @@ extern "C" int calm_b200_read_state(int which, int layer, float* out, int cap) {
 	case CALM_B200_STATE_PF_ATT: hi = pf.Ahi, lo = pf.Alo, count = (size_t)pf.cap * g.q_dim; break;
 	case CALM_B200_STATE_PF_HB: hi = pf.Hhi, lo = pf.Hlo, count = (size_t)pf.cap * c.hidden_dim; break;
 	case CALM_B200_STATE_PF_LOGITS: f32 = pf.vlogits, count = (size_t)pf.vrows * c.vocab_size; break;
+	case CALM_B200_STATE_BEAM_IDS: i32 = pf.bmtid, count = (size_t)pf.bm_steps * pf.bm_beams * pf.bm_k; break;
+	case CALM_B200_STATE_BEAM_LOGPROBS: f32 = pf.bmtlp, count = (size_t)pf.bm_steps * pf.bm_beams * pf.bm_k; break;
+	case CALM_B200_STATE_BEAM_ANC: i32 = pf.bmanc[pf.bm_last], count = (size_t)pf.bm_beams * pf.bm_max_new; break;
 	default: CALM_FATAL("read_state: unknown selector %d", which);
 	}
 	if (count > 0x7fffffff) CALM_FATAL("read_state: %zu values do not fit the int the call returns", count);
 	if (!out || (size_t)cap < count || count == 0) return (int)count; // (no prompt pass yet: its matrices are empty)
 	if (f32) {
 		CUDA_CHECK(cudaMemcpy(out, f32, count * sizeof(float), cudaMemcpyDeviceToHost));
+	} else if (i32) {
+		std::vector<int> v(count);
+		CUDA_CHECK(cudaMemcpy(v.data(), i32, count * sizeof(int), cudaMemcpyDeviceToHost));
+		for (size_t i = 0; i < count; ++i) out[i] = (float)v[i];
 	} else if (hi) {
 		std::vector<__half> h(count), l(count);
 		CUDA_CHECK(cudaMemcpy(h.data(), hi, count * sizeof(__half), cudaMemcpyDeviceToHost));
@@ -3196,6 +3330,10 @@ extern "C" void calm_b200_poison_state(struct Transformer* transformer, int kv_f
 		nan(pf.sqtopv, VF_TOK * nvt * PF_TOPK_MAX * sizeof(float)), nan(pf.sqtopi, VF_TOK * nvt * PF_TOPK_MAX * sizeof(int));
 		nan(pf.sqtid, VF_TOK * PF_TOPK_MAX * sizeof(int)), nan(pf.sqtlp, VF_TOK * PF_TOPK_MAX * sizeof(float));
 		nan(pf.sqlp, pf.sqlp_cap * sizeof(float)), nan(pf.sqoid, pf.sqtop_cap * sizeof(int)), nan(pf.sqolp, pf.sqtop_cap * sizeof(float));
+		// decode_beam's candidate lists, backpointers and pool, which every call writes before it reads them (its ancestry
+		// tables, read as key slots, are index buffers)
+		nan(pf.bmtid, pf.bmtrace_cap * sizeof(int)), nan(pf.bmtlp, pf.bmtrace_cap * sizeof(float)), nan(pf.bmback, pf.bmback_cap * sizeof(BmBack));
+		nan(pf.bmst, sizeof(BmState));
 		// and its penalty call's lanes, which k_sq_pen_admit rewrites whole for each request it admits (a poisoned count
 		// word reads as seen with count 0x3fffffff), and its uploaded bias values (the uploaded tokens and bias ids and the
 		// step's lanes, pf.sqlanes, read as addresses into the lanes, are index buffers)

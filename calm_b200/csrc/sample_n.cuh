@@ -42,6 +42,12 @@
 // nseq x nsuf, kv heads): CTA x < the shared chunks' count is shared chunk x - chunk0[g] of the group g that holds it, the
 // others are per-row chunk nc / SN_CHUNK + x' % nsuf of row x' / nsuf.  Which chunks are shared depends on nc alone and a
 // query's arithmetic does not depend on the CTA or warp that runs it, so a row gives what QUEUE gives it over the same keys.
+//
+// BEAM (calm_b200_decode_beam): the plain layout, but a row reads its generated keys through its ancestry.  Step j writes
+// row b to slot pos0 + j * nbeam + b (step 0 runs one row), and anc[b * anc_stride + i] is the row of step i whose key
+// row b reads as its virtual key pos0 + i, so v >= pos0 is slot pos0 + (v - pos0) * nbeam + anc[b][v - pos0].  With
+// anc[b][i] = b and nbeam = nseq that is the plain mapping, and grid, chunking and every floating-point operation are
+// the plain kernels', so a beam's row gives what decode_sample_n gives a sequence over the same keys.
 #pragma once
 
 #include "prefill.cuh"
@@ -72,6 +78,8 @@ struct SnAttnArgs {
 	const int2* rows; // [nseq] (BATCH) row b's prompt: its first slot s_b and its length L_b; read by no other variant
 	const int4* qrows; // [nseq] (QUEUE) row b's (s, L, t, j); read by no other variant
 	const SqGroups* groups; // (GROUPS) the step's contexts and groups; read by no other variant
+	const int* anc;   // (BEAM) [nseq][anc_stride] each row's ancestor row at every step; read by no other variant
+	int nbeam, anc_stride; // (BEAM) the slot stride of a step and anc's row length
 };
 
 // dynamic shared memory of k_sn_attn: the K tile (padded rows), the V tile, each warp's KM queries
@@ -83,10 +91,11 @@ constexpr size_t sn_smem_bytes() {
 // grid (prompt chunks + nseq x suffix chunks, kv heads): CTA x < pos0 / SN_CHUNK is prompt chunk x for every row, the
 // others are suffix chunk x' % nsuf of row x' / nsuf (x' = x - prompt chunks).  BATCH (and QUEUE): grid (nseq x nch, kv
 // heads).  GROUPS: the grid above its header comment says.
-template <typename KVT, int HD, int KM, bool BATCH = false, bool QUEUE = false, bool GROUPS = false>
+template <typename KVT, int HD, int KM, bool BATCH = false, bool QUEUE = false, bool GROUPS = false, bool BEAM = false>
 __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 	static_assert(BATCH || !QUEUE, "a queue step is a batch step with per-row step counts");
 	static_assert(QUEUE || !GROUPS, "context groups are rows of a queue step");
+	static_assert(!(BEAM && BATCH), "beams share one prompt");
 	pdl_enter();
 	constexpr int DPL = HD / 32, KPL = SN_CHUNK / 32;
 	constexpr int VSTR = HD * sizeof(KVT), KSTR = VSTR + 16; // padded key row, as k_pf_attn's
@@ -148,6 +157,8 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_sn_attn(const SnAttnArgs a) {
 		} else if constexpr (BATCH) { // (read per key: held in registers through the score pass, they add spills)
 			const int2 pr = __ldg(a.rows + b0);
 			slot = v < pr.y ? pr.x + v : a.pos0 + (v - pr.y) * a.nseq + b0;
+		} else if constexpr (BEAM) { // (only a key the chunk holds reads its ancestor: anc ends at the row's last key)
+			slot = v < a.pos0 || !in ? v : a.pos0 + (v - a.pos0) * a.nbeam + __ldg(a.anc + (size_t)b0 * a.anc_stride + (v - a.pos0));
 		} else slot = v < a.pos0 ? v : a.pos0 + (v - a.pos0) * a.nseq + b0;
 		const uint4 z = make_uint4(0, 0, 0, 0);
 		*reinterpret_cast<uint4*>(ks + row * KSTR + cc * 16) = in ? __ldcg(reinterpret_cast<const uint4*>(kbase + (size_t)slot * HD) + cc) : z;
@@ -443,4 +454,117 @@ __global__ void __launch_bounds__(32) k_sq_pen_step(const int* lanes, const int*
 	pdl_enter();
 	const int i = threadIdx.x;
 	if (i < SQ_ROWS && lanes[i] >= 0) ++cnt[(size_t)lanes[i] * vocab + step_tok[i]];
+}
+
+// ---------------------------------------------------------------- calm_b200_decode_beam
+
+#define BM_MAX 10      // CALM_B200_BEAM_MAX
+#define BM_THREADS 256 // k_bm_select: one thread per candidate, at most BM_MAX x PF_TOPK_MAX of them
+
+// A finished hypothesis: the tokens of row `row` of step `step` (its history), then `token` with log-probability `lp`
+// (-1: none, a live beam entering the pool after the last step); `order` counts the call's entries into the pool
+struct BmHyp {
+	float score, sum, lp;
+	int step, row, token, order;
+};
+
+// The pool of at most B finished hypotheses, and each live beam's running sum; zeroed before a call's first step
+struct BmState {
+	float sum[BM_MAX];
+	BmHyp pool[BM_MAX];
+	int npool, nadded, done;
+};
+
+// The row and token a live beam of step j + 1 continues, and the token's log-probability
+struct BmBack {
+	int parent, token;
+	float lp;
+};
+
+// The pool rule of calm_b200_decode_beam (include/calm_b200.h): h enters while the pool holds fewer than B, or when its
+// score is strictly greater than the worst; past B the worst leaves, the earliest added among equal worst scores.  The
+// device's walk and the host's last step share it, so both keep the same pool.
+__host__ __device__ inline int bm_worst(const BmState& s) {
+	int w = 0;
+	for (int i = 1; i < s.npool; ++i)
+		if (s.pool[i].score < s.pool[w].score || (s.pool[i].score == s.pool[w].score && s.pool[i].order < s.pool[w].order)) w = i;
+	return w;
+}
+__host__ __device__ inline void bm_add(BmState& s, int B, BmHyp h) {
+	if (s.npool == B && !(h.score > s.pool[bm_worst(s)].score)) return;
+	h.order = s.nadded++;
+	if (s.npool < B) {
+		s.pool[s.npool++] = h;
+		return;
+	}
+	s.pool[bm_worst(s)] = h; // (one in, the worst out: the pool never holds more than B)
+}
+
+// What k_bm_select needs of one step
+struct BmArgs {
+	const int* tid;    // [rows][K] the step's merged top-K ids and log-probabilities (pf.sqtid / pf.sqtlp)
+	const float* tlp;
+	const int* anc;    // [B][max_new] the ancestry the step read, and the one the next step reads
+	int* anc_next;
+	BmState* st;
+	BmBack* back;      // [max_new][B]
+	int* trace_id;     // [max_new][B][K] every step's lists (rows past `rows`: id -1, -inf)
+	float* trace_lp;
+	int* tokens;       // [B] the next step's tokens (pf.tokens)
+	int stop[PF_TOPK_MAX];
+	int n_stop, j, rows, B, K, max_new, early;
+	float norm_j, norm_next; // norm[max(1, j)] and norm[j + 1]
+};
+
+// one CTA, after the merge of step j: each candidate's score c = S_b + lp and its place in the walk order (c descending,
+// beam ascending, rank ascending, found by counting the candidates before it), then the walk on one thread, then the next
+// ancestry: anc'[b'][i] = anc[parent][i] for i <= j, and b' at j + 1
+__global__ void __launch_bounds__(BM_THREADS) k_bm_select(const BmArgs a) {
+	pdl_enter();
+	__shared__ float cs[BM_MAX * PF_TOPK_MAX];
+	__shared__ int walk[PF_TOPK_MAX], par[BM_MAX];
+	__shared__ float S[BM_MAX]; // the next beams' sums
+	const int n = a.rows * a.K, t = threadIdx.x;
+	BmState* st = a.st;
+	if (t < a.K) walk[t] = 0; // (places in the walk are distinct unless a score is NaN: no entry is left unset)
+	if (t < a.B) par[t] = 0;
+	for (int e = t; e < a.B * a.K; e += blockDim.x) {
+		const bool in = e < n;
+		const size_t o = ((size_t)a.j * a.B) * a.K + e;
+		a.trace_id[o] = in ? a.tid[e] : -1, a.trace_lp[o] = in ? a.tlp[e] : -INFINITY;
+		if (in) cs[e] = st->sum[e / a.K] + a.tlp[e];
+	}
+	__syncthreads();
+	for (int e = t; e < n; e += blockDim.x) {
+		const float c = cs[e];
+		int q = 0; // (e / K, e % K) order as e does: beam, then rank
+		for (int f = 0; f < n; ++f) q += cs[f] > c || (cs[f] == c && f < e);
+		if (q < a.K) walk[q] = e;
+	}
+	__syncthreads();
+	if (t == 0) {
+		for (int b = 0; b < a.B; ++b) S[b] = -INFINITY;
+		int taken = 0;
+		for (int q = 0; q < a.K && taken < a.B; ++q) {
+			const int e = walk[q], tok = a.tid[e];
+			const float lp = a.tlp[e], c = cs[e];
+			bool stop = false;
+			for (int i = 0; i < a.n_stop; ++i) stop = stop || tok == a.stop[i];
+			if (stop) {
+				if (q < a.B) bm_add(*st, a.B, BmHyp{c / a.norm_j, c, lp, a.j, e / a.K, tok, 0});
+				continue;
+			}
+			S[taken] = c, par[taken] = e / a.K, a.tokens[taken] = tok;
+			a.back[(size_t)a.j * a.B + taken] = BmBack{e / a.K, tok, lp};
+			++taken;
+		}
+		for (int b = 0; b < a.B; ++b) st->sum[b] = S[b];
+		st->done = st->npool == a.B && (a.early || st->pool[bm_worst(*st)].score >= S[0] / a.norm_next);
+	}
+	__syncthreads();
+	if (a.j + 1 >= a.max_new) return;
+	for (int x = t; x < a.B * (a.j + 2); x += blockDim.x) {
+		const int b = x / (a.j + 2), i = x % (a.j + 2);
+		a.anc_next[(size_t)b * a.max_new + i] = i <= a.j ? a.anc[(size_t)par[b] * a.max_new + i] : b;
+	}
 }

@@ -27,7 +27,7 @@ SYMBOLS = [
     "calm_b200_score_topk", "calm_b200_score_batch_topk", "calm_b200_score_context_topk",
     "calm_b200_abi_version", "calm_b200_set_device", "calm_b200_free", "calm_b200_release",
     "calm_b200_forward_argmax", "calm_b200_decode_greedy", "calm_b200_verify_greedy", "calm_b200_decode_lookup", "calm_b200_verify_sample", "calm_b200_decode_lookup_sample",
-    "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_sample_queue",
+    "calm_b200_decode_sample_n", "calm_b200_decode_sample_batch", "calm_b200_decode_beam", "calm_b200_decode_sample_queue",
     "calm_b200_decode_sample_queue_context", "calm_b200_decode_sample_queue_logprobs", "calm_b200_decode_sample_queue_penalties",
     "calm_b200_decode_sample_queue_constrained", "calm_b200_decode_sample_queue_truncated", "calm_b200_decode_sample_queue_lookup",
     "calm_b200_timer_start", "calm_b200_timer_stop",
@@ -51,8 +51,12 @@ VERIFY_MAX = 16
 # calm_b200_decode_sample_queue keeps in flight (CALM_B200_SAMPLE_N_MAX)
 SAMPLE_N_MAX = 16
 
+# the most beams calm_b200_decode_beam takes (CALM_B200_BEAM_MAX)
+BEAM_MAX = 10
+
 # calm_b200_read_state selectors (include/calm_b200.h)
-STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11, "pf_logits": 12}
+STATE = {"x": 0, "xb": 1, "q": 2, "att": 3, "hb": 4, "moe_sel": 5, "keys": 6, "values": 7, "pf_x": 8, "pf_q": 9, "pf_att": 10, "pf_hb": 11, "pf_logits": 12,
+         "beam_ids": 13, "beam_logprobs": 14, "beam_anc": 15}
 
 _lib = None
 
@@ -126,6 +130,8 @@ def load() -> C.CDLL:
     L.calm_b200_decode_sample_queue_truncated.restype = C.c_int
     L.calm_b200_decode_sample_queue_lookup.argtypes = L.calm_b200_decode_sample_queue_truncated.argtypes + [C.c_int, _iptr, _iptr]
     L.calm_b200_decode_sample_queue_lookup.restype = C.c_int
+    L.calm_b200_decode_beam.argtypes = [T, C.c_int, C.c_int, C.c_int, C.c_int, _iptr, C.c_int, C.c_float, C.c_int, C.c_int, _iptr, _iptr, _fptr, _fptr, _iptr]
+    L.calm_b200_decode_beam.restype = C.c_int
     L.calm_b200_timer_start.argtypes, L.calm_b200_timer_start.restype = [], None
     L.calm_b200_timer_stop.argtypes, L.calm_b200_timer_stop.restype = [], C.c_float
     L.calm_b200_stream.argtypes, L.calm_b200_stream.restype = [], C.c_void_p
@@ -561,6 +567,48 @@ class DeviceModel:
         served = self.lib.calm_b200_decode_sample_n(C.byref(self.transformer), int(token0), int(pos0), int(n_tokens), nseq, temperature, minp, rng,
                                                     out.ctypes.data_as(C.POINTER(C.c_int)))
         return out, [int(s) for s in rng], served
+
+    def decode_beam(self, token0: int, pos0: int, max_new: int, num_beams: int, stop=(), length_penalty: float = 1.0, early_stopping: bool = False,
+                    num_return: Optional[int] = None):
+        """calm_b200_decode_beam: beam search over the prompt in cache slots [0, pos0), feeding token0 at pos0, with
+        include/calm_b200.h's rules (Hugging Face's num_beams, length_penalty, early_stopping, num_return_sequences and
+        eos_token_id = stop).  Returns (hypotheses, served, steps): hypotheses is a list of num_return (default num_beams)
+        tuples (tokens int32[len], logprobs float32[len], score), best first, or [] when served is 0 (MoE, tensor-parallel
+        or unserved shapes, or pos0 + num_beams * max_new > seq_len).  Raises ValueError wherever the C call would abort."""
+        def whole(name, x, lo, hi):
+            if isinstance(x, bool) or not isinstance(x, (int, np.integer)) or not lo <= x <= hi:
+                raise ValueError(f"decode_beam: {name} must be an integer in [{lo}, {hi}], got {x!r}")
+            return int(x)
+
+        B = whole("num_beams", num_beams, 1, BEAM_MAX)
+        max_new = whole("max_new", max_new, 0, 1 << 31)
+        pos0 = whole("pos0", pos0, 0, 1 << 31)
+        token0 = whole("token0", token0, 0, self.vocab - 1)
+        R = B if num_return is None else whole("num_return", num_return, 1, B)
+        if early_stopping not in (0, 1):  # (True and False included)
+            raise ValueError(f"decode_beam: early_stopping must be 0 or 1, got {early_stopping!r}")
+        try:
+            stop = np.ascontiguousarray(np.asarray(list(stop), np.int64).reshape(-1))
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"decode_beam: bad stop list: {e}") from None
+        if ((stop < 0) | (stop >= self.vocab)).any():
+            raise ValueError(f"decode_beam: stop ids must be in [0, {self.vocab})")
+        K = max(2, 1 + len(stop)) * B
+        if K > TOPK_MAX:
+            raise ValueError(f"decode_beam: max(2, 1 + len(stop)) * num_beams = {K} candidates per beam exceed {TOPK_MAX}")
+        if not np.isfinite(np.float32(length_penalty)):
+            raise ValueError(f"decode_beam: length_penalty must be finite, got {length_penalty!r}")
+        stop = stop.astype(np.int32)
+        ip = C.POINTER(C.c_int)
+        toks = np.full((R, max(max_new, 1)), -1, np.int32)
+        lps = np.zeros((R, max(max_new, 1)), np.float32)
+        lens, scores, steps = np.zeros(R, np.int32), np.zeros(R, np.float32), C.c_int(0)
+        served = self.lib.calm_b200_decode_beam(C.byref(self.transformer), token0, pos0, max_new, B, stop.ctypes.data_as(ip), len(stop),
+                                                float(length_penalty), int(early_stopping), R, toks.ctypes.data_as(ip), lens.ctypes.data_as(ip),
+                                                lps.ctypes.data_as(_fptr), scores.ctypes.data_as(_fptr), C.byref(steps))
+        if not served or max_new == 0:
+            return [], served, 0
+        return [(toks[r, :lens[r]].copy(), lps[r, :lens[r]].copy(), float(scores[r])) for r in range(R)], served, steps.value
 
     def decode_sample_batch(self, prompts, n_tokens: int, temperature: float, minp: float, rng_states):
         """calm_b200_decode_sample_batch: len(prompts) = nseq sequences, sequence b continuing prompts[b] (a sequence of at

@@ -284,6 +284,48 @@ int calm_b200_decode_sample_n(struct Transformer* transformer, int token0, int p
 int calm_b200_decode_sample_batch(struct Transformer* transformer, const int* tokens, int n, const int* off, const int* len, int nseq,
                                   int n_tokens, float temperature, float minp, unsigned long long* rng_states, int* out_tokens);
 
+/* Beam search over one prompt: num_beams = B beams advance together, every step one pass over the weights for all of
+ * them, the prompt's cache entries read once per step for all of them and each beam's generated entries read through its
+ * ancestry, so no cache entry is ever copied (DESIGN.md s.6).  Hugging Face's generate(num_beams, length_penalty,
+ * early_stopping, num_return_sequences) with eos_token_id = stop, at temperature 1 and without logit processors
+ * (INTEGRATION.md).  The cache holds the prompt at slots [0, pos0); token0 is fed at pos0.
+ *   Rows and slots.  Step j runs every live beam at RoPE position pos0 + j, row b writing cache slot pos0 + j * B + b;
+ *     step 0 runs one row, fed token0, and every later step B rows.  The call needs pos0 + B * max_new <= seq_len; slots
+ *     [0, pos0) are never written and slots from pos0 on are scratch afterwards.
+ *   Candidates.  K = max(2, 1 + n_stop) * B (Hugging Face's, which leaves B candidates that are not stop tokens).  Each
+ *     row takes its K best tokens, logit descending and the lowest id on ties, each with lp = l - M - ln S of the step's
+ *     fp32 logits (calm_b200_decode_sample_queue_logprobs' log-probability, at temperature 1).  Beam b has a running fp32
+ *     sum S_b, 0 at the start, and a candidate's score is c = S_b + lp, one fp32 add.  All rows' candidates are ordered
+ *     by c descending, then beam ascending, then rank ascending, and the first K are walked in that order, q being the
+ *     place in the walk.
+ *   Walk.  A candidate whose token is in stop becomes a finished hypothesis when q < B and is skipped otherwise: the
+ *     parent's tokens plus the stop token, raw sum c, score c / norm[max(1, j)] (the tokens before the stop).  Any other
+ *     candidate becomes the next live beam, in walk order, until B are taken.  norm[L] = (float)pow((double)L,
+ *     (double)length_penalty), computed on the host; every division is one IEEE fp32 division.
+ *   Pool.  At most B finished hypotheses.  A new one enters while the pool holds fewer than B, or when its score is
+ *     strictly greater than the worst; when the pool exceeds B the worst leaves, the earliest added among equal scores.
+ *   Done.  After each step's walk, when the pool holds B: early_stopping 1 is done; early_stopping 0 is done when
+ *     worst >= S_best / norm[j + 1], S_best the first live beam's sum (Hugging Face's default heuristic).  After max_new
+ *     steps, if the call is not done, each live beam enters the pool, in beam order, with score S_b / norm[max_new].
+ *   Outputs.  The pool sorted by score descending, the earliest added first among equal scores; for r < num_return,
+ *     out_tokens[r * max_new ..] gets hypothesis r's tokens (stop token included), out_len[r] its length, out_scores[r]
+ *     its score and, unless out_logprobs is NULL, out_logprobs[r * max_new ..] each token's lp; summed left to right in
+ *     fp32 from 0 they give its raw sum bit for bit.  *steps gets the number of steps run.  Slots past out_len[r] and
+ *     rows from num_return on are left untouched.
+ * Returns 1 on this path.  MoE and tensor-parallel models, shapes the prompt pass does not serve (as for
+ * calm_b200_verify_greedy) and calls past seq_len return 0, set *steps = 0 and do nothing else: a per-token fallback
+ * would need a cache per beam (DESIGN.md s.8).  The call aborts before any device work when num_beams is outside
+ * [1, CALM_B200_BEAM_MAX], K > CALM_B200_TOPK_MAX, num_return is outside [1, num_beams], max_new or n_stop is negative,
+ * a stop id or token0 is outside the vocabulary, pos0 is negative, length_penalty is not finite, early_stopping is not
+ * 0 or 1, or stop (with n_stop > 0), out_tokens, out_len, out_scores or steps is NULL.  max_new == 0 does nothing else
+ * and returns 1.  The first call allocates what calm_b200_decode_sample_n allocates for ceil((pos0 + max_new) / 128)
+ * chunks, the queue's top-k lists (calm_b200_decode_sample_queue_logprobs) and, regrown when a later call needs more,
+ * 4 x B x max_new x (2 + 3 + 2 K) bytes of ancestry, backpointers and candidate lists. */
+#define CALM_B200_BEAM_MAX 10
+int calm_b200_decode_beam(struct Transformer* transformer, int token0, int pos0, int max_new, int num_beams, const int* stop, int n_stop,
+                          float length_penalty, int early_stopping, int num_return, int* out_tokens, int* out_len, float* out_logprobs,
+                          float* out_scores, int* steps);
+
 /* Generate for a queue of nreq requests, at most max_rows (1 .. CALM_B200_SAMPLE_N_MAX) in flight, each with its own
  * length, sampling settings and generator, and admit new requests as rows finish (DESIGN.md s.6).  Request i's prompt is
  * tokens[off[i] .. off[i] + len[i]), len[i] >= 1, as in calm_b200_decode_sample_batch; it generates at most
@@ -609,14 +651,19 @@ void calm_b200_read_kv(struct Transformer* transformer, int layer, int kv_pos, f
  *            sampler drew from, or of the last step of a calm_b200_decode_sample_queue call on its new path if that step
  *            sampled any row (n = the rows in flight).  After calm_b200_decode_sample_queue_penalties the rows of
  *            non-neutral requests hold their processed logits l2, the values the sampler drew from
+ *   BEAM_IDS, BEAM_LOGPROBS  float[steps][B][K]   the last calm_b200_decode_beam call on its path: each step's rows'
+ *            K best ids and their lp, as the walk read them (step 0's rows past row 0: id -1, lp -inf)
+ *   BEAM_ANC  float[B][max_new]   that call's ancestry as its last step read it: entry [b][i] is the row of step i whose
+ *            key row b read as its key pos0 + i (i <= steps - 1; the rest unspecified)
  *   After calm_b200_decode_sample_n or calm_b200_decode_sample_batch on its new path, the PF_* matrices hold the last
  *   step, row b = sequence b.  After calm_b200_decode_sample_queue on its new path, the PF_* matrices and PF_LOGITS hold
- *   the last step, with the rows in flight in admission order. */
+ *   the last step, with the rows in flight in admission order.  After calm_b200_decode_beam on its path, the PF_*
+ *   matrices hold the last step, row b = live beam b. */
 enum {
 	CALM_B200_STATE_X = 0, CALM_B200_STATE_XB = 1, CALM_B200_STATE_Q = 2, CALM_B200_STATE_ATT = 3, CALM_B200_STATE_HB = 4,
 	CALM_B200_STATE_MOE_SEL = 5, CALM_B200_STATE_KEYS = 6, CALM_B200_STATE_VALUES = 7,
 	CALM_B200_STATE_PF_X = 8, CALM_B200_STATE_PF_Q = 9, CALM_B200_STATE_PF_ATT = 10, CALM_B200_STATE_PF_HB = 11,
-	CALM_B200_STATE_PF_LOGITS = 12
+	CALM_B200_STATE_PF_LOGITS = 12, CALM_B200_STATE_BEAM_IDS = 13, CALM_B200_STATE_BEAM_LOGPROBS = 14, CALM_B200_STATE_BEAM_ANC = 15
 };
 int calm_b200_read_state(int which, int layer, float* out, int cap);
 
